@@ -1,7 +1,7 @@
 #!/usr/bin/env python
 """Benchmark of the OmniVGGT hot path (BASELINE.json metric: view-sets/sec, N-view 518^2 batches).
 
-    python bench.py [--gpus N] [--steps K] [--warmup W] [--impl b200|reference] [--config cfg1..cfg5]
+    python bench.py [--gpus N] [--steps K] [--warmup W] [--impl b200|reference] [--config cfg1..cfg5] [--dump-outputs DIR]
 
 One "step" = the full OmniVGGT.forward over this rank's share of the workload.  Workloads (BASELINE.json configs[0..4]):
   cfg1  1 scene x 4 views @ 518^2, images only
@@ -11,6 +11,8 @@ One "step" = the full OmniVGGT.forward over this rank's share of the workload.  
   cfg5  1 scene x 24 views @ 518^2, partial depth_gt_index / camera_gt_index
 cfg1/2/3/5 under torchrun: weak scaling, one independent view-set per rank per step; weights broadcast once from rank 0 (NCCL).
 Prints ONE JSON line on rank 0 (DESIGN.md section "Measurement" defines the fields).
+--dump-outputs DIR writes what the last timed step returned as DIR/<name>.npy (float32; inputs are seeded, so two builds of the
+project can be compared output for output).
 """
 from __future__ import annotations
 
@@ -46,8 +48,43 @@ def measured_peaks():
     p = os.path.join(ROOT, "MEASURED_PEAKS.json")
     if os.path.exists(p):
         d = json.load(open(p))
-        return d.get("bf16_tflops_sustained", 1393.7), d.get("hbm_gbs", 6489.9), "measured (MEASURED_PEAKS.json, sustained bf16)"
-    return 1400.0, 6650.0, "fallback (B200_PROFILING.md)"
+        if "bf16_tflops_sustained" in d and "hbm_gbs" in d:
+            return d["bf16_tflops_sustained"], d["hbm_gbs"], "measured (MEASURED_PEAKS.json, sustained bf16)"
+    return 989.0, 3350.0, "H100 SXM data sheet (dense bf16, HBM3; not reached in practice)"
+
+
+DUMP_BYTES = 64 << 20          # all files of --dump-outputs together
+DUMP_WHOLE_BYTES = 1 << 20     # arrays up to this size (pose encodings) are always written whole
+
+
+def dump_outputs(d, outs):
+    """Write the tensors of the forward results `outs` (one dict per forward call of the step) as float32 .npy files, at most
+    DUMP_BYTES in all.  Small arrays are written whole; when the rest does not fit, each larger array is replaced by a fixed,
+    seeded strided sample of its flattened values (the same indices on every run with the same shapes)."""
+    import numpy as np
+    import torch
+    arrays = {}
+    for c, out in enumerate(outs):
+        sfx = "" if len(outs) == 1 else f"_call{c}"
+        for k, v in out.items():
+            if k == "images":                       # the input, passed through
+                continue
+            if isinstance(v, (list, tuple)):
+                v = torch.stack(list(v))
+            if torch.is_tensor(v):
+                arrays[k + sfx] = v.detach().float().cpu().numpy()
+    small = {k for k, a in arrays.items() if a.size * 4 <= DUMP_WHOLE_BYTES}
+    budget = DUMP_BYTES - 4096 * len(arrays) - sum(arrays[k].size * 4 for k in small)   # .npy headers, whole arrays
+    large = sum(a.size * 4 for k, a in arrays.items() if k not in small)
+    keep = 1.0 if large <= budget else max(budget, 4 * len(arrays)) / large
+    rng = np.random.default_rng(0)
+    os.makedirs(d, exist_ok=True)
+    for k in sorted(arrays):
+        a = arrays[k]
+        if k not in small and keep < 1.0:
+            stride = int(np.ceil(1.0 / keep)) + 1       # + 1: the ceil of the sample length stays within the share
+            a = a.reshape(-1)[int(rng.integers(stride))::stride]
+        np.save(os.path.join(d, k + ".npy"), np.ascontiguousarray(a, dtype=np.float32))
 
 
 def synth_inputs(B, S, seed):
@@ -185,7 +222,7 @@ def run_reference(args, rank, world):
 
 # ------------------------------------------------------------------------------------------------ GPU library baseline
 def gpu_torch_baseline(model, inputs, cfg, dev, ours):
-    """The real competitor (SURVEY.md section 8d): the UNMODIFIED reference on the same B200 through the library kernels
+    """The real competitor (SURVEY.md section 8d): the UNMODIFIED reference on the same GPU through the library kernels
     PyTorch dispatches to (cuBLAS, cuDNN, SDPA), fp32 as inference.py runs it and under torch.autocast(bf16), with OUR
     weights loaded (same 1 505 keys).  Runs after the product arm's timed regions.  Also reports output deviations:
     ours vs reference fp32, and reference-bf16-autocast vs reference fp32 (the yardstick of SURVEY.md section 8d)."""
@@ -247,6 +284,7 @@ def main():
     ap.add_argument("--cp", action="store_true", help="context parallelism: ONE scene per step, its views sharded over the ranks")
     ap.add_argument("--no-cpu-baseline", action="store_true")
     ap.add_argument("--no-gpu-torch-baseline", action="store_true")
+    ap.add_argument("--dump-outputs", metavar="DIR", help="write the outputs of the last timed step as DIR/<name>.npy")
     args = ap.parse_args()
     rank = int(os.environ.get("RANK", 0))
     world = int(os.environ.get("WORLD_SIZE", 1))
@@ -300,11 +338,13 @@ def main():
     dev_in = [{k: v.to(dev) for k, v in h.items()} for h in host_in]
     idx_kw = dict(depth_gt_index=list(cfg["depth_idx"]), camera_gt_index=list(cfg["cam_idx"]))
     host_out = [None] * calls
+    last_out = [None] * calls
 
     def step_resident():
         out = None
         for c in range(calls):
             out = model(**dev_in[c], **idx_kw)
+            last_out[c] = out
         return out
 
     from omnivggt_official_b200.pipeline import StreamingPipeline
@@ -347,6 +387,8 @@ def main():
     with ClockSampler(local) as cs:
         total_ms = timed(step_resident, args.steps)
     clocks = cs.summary()
+    if args.dump_outputs and rank == 0:
+        dump_outputs(args.dump_outputs, last_out)
     ms_step = total_ms / args.steps
     value = total_scenes * 1e3 / ms_step
 
@@ -394,12 +436,8 @@ def main():
         att_flops /= world                            # a rank's own queries (L / world rows) against all L keys
     att_avg = sum(att_ms) / max(len(att_ms), 1)
     achieved = att_flops / (att_avg * 1e-3) / 1e12
-    traffic = None
-    tp = os.path.join(ROOT, "profiles", "attn_traffic.json")
-    if os.path.exists(tp):
-        traffic = json.load(open(tp)).get(f"S{S}") if Bm == 1 else None
     roofline = {"kernel": "ovg::attn1_kernel (global attention)", "bound": "tensor", "achieved": achieved, "peak": peak_tf,
-                "unit": "TFLOP/s", "frac": achieved / peak_tf, "traffic": traffic, "peak_source": peak_src,
+                "unit": "TFLOP/s", "frac": achieved / peak_tf, "traffic": None, "peak_source": peak_src,
                 "launches_timed": len(att_ms), "avg_launch_ms": att_avg,
                 "share_of_step": sum(att_ms) / args.steps / ms_step,
                 "timed_in": "separate eager pass of the same K steps (launches inside the replayed CUDA graph cannot be bracketed)"}
@@ -416,7 +454,7 @@ def main():
                                        f"epilogue + flag barrier, no collective on the data path" if args.cp else
                                        f"dp{world} (scene-sharded, NCCL weight broadcast {bcast_bytes} B at start-up)"),
                        "weights": "random-init, full architecture (1217.5 M params)",
-                       "l2": "no flush needed: each step streams >2 GB of weights+activations, far beyond the 126 MB L2",
+                       "l2": "no flush needed: each step streams >2 GB of weights+activations, far beyond the 50 MB L2",
                        "dino": "frozen DINOv2 patchifier on the libovg kernels",
                        "launch": "CUDA graph replay" if model.use_cuda_graph else "eager (C++ runtime sequences)"},
             "clocks": clocks,

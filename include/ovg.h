@@ -1,4 +1,4 @@
-/* libovg -- C ABI of the B200-native OmniVGGT hot path (sm_100a).
+/* libovg -- C ABI of the H100-native OmniVGGT hot path (sm_90a).
  *
  * The reference has no FFI / plugin layer (SURVEY.md section 8b): its boundary is the Python nn.Module API of
  * omnivggt/models/omnivggt.py:10-68.  The drop-in module `omnivggt-official_b200.OmniVGGT` keeps that API and
@@ -24,10 +24,10 @@ extern "C" {
 /* Library / device ------------------------------------------------------------------------------------- */
 int ovg_version(void);               /* ABI version, currently 2 */
 const char* ovg_last_error(void);    /* thread-local message of the last failing call */
-int ovg_device_check(void);          /* OVG_OK iff the current device is sm_100 (B200); OVG_E_NODEVICE otherwise */
+int ovg_device_check(void);          /* OVG_OK iff the current device is sm_90 (H100); OVG_E_NODEVICE otherwise */
 long long ovg_launch_count(void);    /* kernels launched by this library since load (bench.py "gpu_launches") */
 
-/* Fused tcgen05 GEMM ------------------------------------------------------------------------------------
+/* Fused wgmma GEMM ---------------------------------------------------------------------------------------
  *   acc[m, n] = sum_{t < num_taps} sum_{c < a_cols} A[m + tap_off[t], c] * B[n, t * a_cols + c]
  * A: bf16 [a_rows, a_cols] row stride lda; B: bf16 [n, num_taps * a_cols] row stride ldb (nn.Linear / flattened
  * conv weight layout).  Rows of A outside [0, a_rows) read as zero, which makes a 3x3 conv over a zero-bordered
@@ -72,7 +72,7 @@ typedef struct ovg_gemm_args {
   const float* rope_cos; const float* rope_sin; float qscale;
   /* OVG_EPI_HEADTAIL */
   const float* w2; const float* b2; int outc; int head_act; float* preds; float* conf;
-  /* tuning: 0 = auto, else 64/128/256, 512 = CTA-pair kernel (256 x 256 tile per 2-SM cluster) */
+  /* tuning: 0 = auto, else 32/64/128 (tile width; larger requests run as 128) */
   int block_n;
   /* OVG_EPI_QKV switches: q/k LayerNorm(64) and 2-D RoPE (both 1 for aggregator blocks, 0 for DINOv2 blocks) */
   int qk_norm; int rope;
@@ -289,7 +289,7 @@ int ovg_dpt_forward(ovg_dpt* h, const void* const* slots, int T, int nspecial, i
                     void* workspace, long long workspace_bytes, void* stream);
 
 /* Camera head: iterative pose refinement on the camera tokens; reference heads/camera_head.py:83-154.  The weight-streaming
- * GEMMs run on the tcgen05 GEMM; AdaLN, the S-token attention (head_dim D / heads) and the 9-wide pose update are small fp32
+ * GEMMs run on the wgmma GEMM; AdaLN, the S-token attention (head_dim D / heads) and the 9-wide pose update are small fp32
  * kernels. */
 typedef struct ovg_camera_desc {
   int D; int heads; int trunk_depth;                           /* 2*embed_dim (2048), 16, 4 */

@@ -1,5 +1,5 @@
 """ctypes binding of libovg.so (include/ovg.h).  There is NO fallback: if the shared library is missing or the
-device is not a B200 the import / first call fails loudly."""
+device is not an H100 (sm_90) the import / first call fails loudly."""
 from __future__ import annotations
 
 import ctypes as C
@@ -174,12 +174,12 @@ def load() -> C.CDLL:
 
 
 def lib() -> C.CDLL:
-    """Library handle for compute calls: additionally requires a B200 as the current device."""
+    """Library handle for compute calls: additionally requires an H100 (sm_90) as the current device."""
     global _device_ok
     l = load()
     if not _device_ok:
         if not torch.cuda.is_available():
-            raise OvgError("libovg needs a CUDA device (B200); torch.cuda.is_available() is False")
+            raise OvgError("libovg needs a CUDA device (H100); torch.cuda.is_available() is False")
         torch.cuda.current_device()          # make sure the primary context exists
         check(l.ovg_device_check())
         _device_ok = True

@@ -1,4 +1,4 @@
-"""Build libovg.so for sm_100a with nvcc (cross-compiles without a GPU).  In-tree output so the .so travels with the
+"""Build libovg.so for sm_90a (H100) with nvcc (cross-compiles without a GPU).  In-tree output so the .so travels with the
 repo snapshot to the GPU box."""
 from __future__ import annotations
 
@@ -11,7 +11,7 @@ SRC = os.path.join(HERE, "csrc", "ovg.cu")
 OUT = os.path.join(HERE, "libovg.so")
 DEPS = sorted(os.path.join(HERE, "csrc", f) for f in os.listdir(os.path.join(HERE, "csrc"))
               if f.endswith((".cu", ".cuh", ".inc", ".h"))) + [os.path.join(os.path.dirname(HERE), "include", "ovg.h")]
-NVCC_FLAGS = ["-gencode", "arch=compute_100a,code=sm_100a", "-O3", "-std=c++17", "-lineinfo", "-shared",
+NVCC_FLAGS = ["-gencode", "arch=compute_90a,code=sm_90a", "-O3", "-std=c++17", "-lineinfo", "-shared",
               "-Xcompiler", "-fPIC", "-Xptxas", "-v"]
 
 

@@ -1,13 +1,9 @@
-// Fused softmax(Q K^T) V for head_dim 64, non-causal, ragged sequence length (sm_100a, tcgen05 + TMA).
+// Fused softmax(Q K^T) V for head_dim 64, non-causal, ragged sequence length (sm_90a, wgmma + TMA).
 // Replaces F.scaled_dot_product_attention at reference layers/attention.py:61-66 for both the frame-wise
 // (batch = B*S, N = 1374) and the global (batch = B, N = S*1374) attention of models/aggregator.py:312-341.
 //
 // q is pre-scaled by (1/sqrt(64))*log2(e) in the QKV GEMM epilogue, so probabilities are exp2(s - m).
-//
-// Online softmax with a stale reference and lazy rescaling: P(j) = exp2(S - m_ref) is computed against the reference left
-// by earlier steps; no running maximum is tracked.  bf16 P and the fp32 O / l accumulators carry the full fp32 exponent
-// range, so a stale reference costs no precision (it cancels in O / l) until exp2 comes near overflow: only then -- detected
-// on the row sum -- O / l are rescaled and the step is redone exactly from the S row still held in registers.
+// Online softmax with a running row maximum; S, P and O stay in registers (P is the A operand of the PV wgmma).
 #pragma once
 #include "ptx.cuh"
 
@@ -19,7 +15,6 @@ struct AttnParams {
   int heads;
   int C;        // heads * 64 (row stride of `out`)
   __nv_bfloat16* out;  // [batch, n, C]
-  long long* prof;     // optional [2][8] cycle counters (OVG_ATT_PROFILE builds only)
   int q_tiles;         // ceil(n / 128)
   int items;           // work items: (batch, head, q tile) tiles -- item = bh * q_tiles + q tile -- walked by the persistent grid, or,
                        // with parts > 1 (one CTA per item), n_full whole tiles followed by the LAST tiles cut into `parts` KV ranges
@@ -27,91 +22,48 @@ struct AttnParams {
   float* part_o;       // [(tile - n_full) * parts + part][128][64] un-normalised O of a KV range
   float2* part_ml;     // ... [128] (softmax reference, row sum) of that range; attn_merge_kernel combines them
 };
-#ifdef OVG_ATT_PROFILE
-#define ATT_T(var) const long long var = clock64()
-#define ATT_ACC(slot, a, b) do { if (prof_on) prof_acc[slot] += (b) - (a); } while (0)
-#else
-#define ATT_T(var)
-#define ATT_ACC(slot, a, b)
-#endif
 
 constexpr int ATT_TILE_BYTES = 128 * 64 * 2;
 
-template <int N>
-__device__ __forceinline__ void reg_alloc() { asm volatile("setmaxnreg.inc.sync.aligned.u32 %0;" ::"n"(N)); }
-template <int N>
-__device__ __forceinline__ void reg_dealloc() { asm volatile("setmaxnreg.dec.sync.aligned.u32 %0;" ::"n"(N)); }
-// exp2 on the FMA pipes for a pair of values (x <= ~8): Cody-Waite split x = n + r, r in [-0.5, 0.5], 2^r by a
-// degree-3 minimax polynomial (max rel. error 1.0e-4, far below bf16 resolution of P), exponent inserted with one IMAD.
-// At head_dim 64 the softmax needs 16 384 exp2 per 128x128 tile against 512 tensor-pipe clocks; the MUFU unit alone
-// (16/clk/SM) caps the kernel at 50% tensor utilisation, so a fraction of the exponentials is moved here.
-__device__ __forceinline__ float2 exp2_poly2(float2 x) {
-  const float kMagic = 12582912.0f;   // 1.5 * 2^23: adding it rounds x to the nearest integer in the low mantissa bits
-  x.x = fmaxf(x.x, -126.0f);
-  x.y = fmaxf(x.y, -126.0f);
-  const float2 t = fadd2(x, make_float2(kMagic, kMagic));
-  const float2 n = fadd2(t, make_float2(-kMagic, -kMagic));
-  const float2 r = fadd2(x, make_float2(-n.x, -n.y));
-  float2 p = ffma2(make_float2(0.05500871f, 0.05500871f), r, make_float2(0.24221068f, 0.24221068f));
-  p = ffma2(p, r, make_float2(0.69328292f, 0.69328292f));
-  p = ffma2(p, r, make_float2(1.0f, 1.0f));
-  float2 o;
-  o.x = __int_as_float(__float_as_int(t.x) * 8388608 + __float_as_int(p.x));
-  o.y = __int_as_float(__float_as_int(t.y) * 8388608 + __float_as_int(p.y));
-  return o;
-}
-#ifndef OVG_ATT_LATE_WAIT
-#define OVG_ATT_LATE_WAIT 1   // P chunks computed before the wait for PV(j-1) (0: wait before the first store, as in round 1)
-#endif
-#ifndef OVG_ATT_EMU_PAIRS
-#define OVG_ATT_EMU_PAIRS 2   // of every 16 element pairs, how many take the polynomial path (0..4): 4 is fastest for the isolated
-                              // kernel (603 us), 2 inside the power-capped forward (profiles/r02_step_ab.txt)
-#endif
 __device__ __forceinline__ float ex2_approx(float x) {
   float y;
   asm("ex2.approx.ftz.f32 %0, %1;" : "=f"(y) : "f"(x));
   return y;
 }
 
-// ---------------------------------------------------------------------------------------------------------------------
-// Single-tile variant: CTA = 128 query rows, 256 threads, TWO CTAs per SM (256 TMEM columns, ~112 KB smem and half of
-// the register file each).  The two tiles that share an SM are
-// independent CTAs: their phases drift freely, one CTA's prologue (barrier init, TMEM alloc, Q / first K loads) and
-// epilogue (O read-out, global stores, TMEM free) run under the other CTA's main loop, and the grid quantises in
-// 128-row units.  Cost: every CTA streams K/V for itself (2x the L2->SM bytes of the paired kernel).
-//   warp 0 TMA producer, warp 1 MMA issuer + TMEM owner, warps 2-3 idle, warps 4-7 softmax (one query row per thread).
-// TMEM (256 cols): S [0,128) P [128,192) O [192,256).
-constexpr int ATT1_THREADS = 256;
+// CTA = 128 query rows of one (batch, head), 384 threads, one CTA per SM (~112 KB smem):
+//   warpgroup 0: TMA producer (one thread) -- Q once per work item, K / V tiles of 128 keys through a 3-stage ring;
+//   warpgroups 1, 2: 64 query rows each -- S = Q K^T (wgmma, 64 x 128 fp32 in registers), softmax, O += P V (wgmma with P
+//   from registers, V MN-major from smem).  Each warpgroup waits for its own MMAs before its softmax (wgmma_wait<0> after
+//   S and after P V), and nothing schedules the two warpgroups against each other: any overlap of one's softmax with the
+//   other's MMAs is incidental.  Known limit: this reaches about a third of the data-sheet bf16 rate on the global attention
+//   (DESIGN.md, "Measurement"); an enforced ping-pong between the warpgroups and issuing S(j+1) before the softmax of step j
+//   are the next steps.
+constexpr int ATT1_THREADS = 384;
 constexpr int ATT1_KV_STAGES = 3;
-constexpr int ATT1_SMEM_BYTES = (1 + 2 * ATT1_KV_STAGES) * ATT_TILE_BYTES + 256;   // base must be 1024-aligned (checked)
+constexpr int ATT1_SMEM_BYTES = (1 + 2 * ATT1_KV_STAGES) * ATT_TILE_BYTES + 1024 + 256;
 
-__global__ void __launch_bounds__(ATT1_THREADS, 2)
+__global__ void __launch_bounds__(ATT1_THREADS, 1)
 attn1_kernel(const __grid_constant__ CUtensorMap tmQ, const __grid_constant__ CUtensorMap tmK,
              const __grid_constant__ CUtensorMap tmV, const AttnParams p) {
   constexpr int NS = ATT1_KV_STAGES;
-  extern __shared__ __align__(1024) uint8_t smem[];
+  extern __shared__ uint8_t smem_raw[];
+  uint8_t* smem = reinterpret_cast<uint8_t*>((reinterpret_cast<uintptr_t>(smem_raw) + 1023) & ~uintptr_t(1023));
   uint8_t* sQ = smem;
   uint8_t* sK = smem + ATT_TILE_BYTES;
   uint8_t* sV = sK + NS * ATT_TILE_BYTES;
   uint64_t* bars = reinterpret_cast<uint64_t*>(sV + NS * ATT_TILE_BYTES);
   uint64_t* q_full = bars;             // [1]
-  uint64_t* k_full = bars + 1;         // [NS]
+  uint64_t* q_empty = bars + 1;        // [1] both consumer warpgroups have finished their last S MMA of the item
+  uint64_t* k_full = bars + 2;         // [NS]
   uint64_t* k_empty = k_full + NS;     // [NS]
   uint64_t* v_full = k_empty + NS;     // [NS]
   uint64_t* v_empty = v_full + NS;     // [NS]
-  uint64_t* s_full = v_empty + NS;     // [1]
-  uint64_t* p_full = s_full + 1;       // [1]
-  uint64_t* o_ready = p_full + 1;      // [1]
-  uint64_t* s_taken = o_ready + 1;     // [1]
-  uint64_t* q_empty = s_taken + 1;     // [1] the last S MMA of a work item has been issued: Q may be overwritten
-  uint64_t* o_taken = q_empty + 1;     // [1] the softmax warps hold the finished O tile in registers: O may be overwritten
-  uint32_t* tmem_slot = reinterpret_cast<uint32_t*>(o_taken + 1);
 
   const int warp = threadIdx.x >> 5;
   const int lane = threadIdx.x & 31;
   // KV tile range [jb, jb + nkv) of this CTA's work items: everything, or -- tail tiles of a long sequence, one CTA per item --
   // one of `parts` ranges whose partial results attn_merge_kernel combines (fills the last, partly empty wave of CTAs).
-  // Every role derives what it needs from blockIdx when it needs it (nothing of this stays live across the softmax loop).
   const bool is_part = p.parts > 1 && static_cast<int>(blockIdx.x) >= p.n_full;
   auto part_of = [&]() { const int i = blockIdx.x - p.n_full; return i - (i / p.parts) * p.parts; };
   auto split_tile_of = [&]() { return p.n_full + static_cast<int>(blockIdx.x - p.n_full) / p.parts; };
@@ -122,48 +74,31 @@ attn1_kernel(const __grid_constant__ CUtensorMap tmQ, const __grid_constant__ CU
     nkv = (part + 1) * nkv / p.parts - jb;
   }
 
-  if (warp == 0 && lane == 0) {
-    if (smem_u32(smem) & 1023u) {
-      printf("ovg attn1: dynamic shared memory base is not 1024-byte aligned\n");
-      __trap();
-    }
+  if (threadIdx.x == 0) {
     tma_prefetch_desc(&tmQ);
     tma_prefetch_desc(&tmK);
     tma_prefetch_desc(&tmV);
     mbar_init(q_full, 1);
-    mbar_init(s_full, 1);
-    mbar_init(p_full, 4);
-    mbar_init(o_ready, 1);
-    mbar_init(s_taken, 4);
-    mbar_init(q_empty, 1);
-    mbar_init(o_taken, 4);
+    mbar_init(q_empty, 8);             // one arrive per consumer warp
     for (int i = 0; i < NS; ++i) {
       mbar_init(&k_full[i], 1);
-      mbar_init(&k_empty[i], 1);
+      mbar_init(&k_empty[i], 8);
       mbar_init(&v_full[i], 1);
-      mbar_init(&v_empty[i], 1);
+      mbar_init(&v_empty[i], 8);
     }
     fence_barrier_init();
   }
-  if (warp == 1) {
-    tmem_alloc(tmem_slot, 256);
-    tmem_relinquish();
-  }
-  tc_fence_before();
   __syncthreads();
-  tc_fence_after();
-  const uint32_t tmem_base = *tmem_slot;
 
-  // register budget: launch allocation 128 * 256 = 32768 per CTA; after the split 128*40 + 128*208 = 31744
-  if (warp < 4) reg_dealloc<40>();
-  if (warp == 0) {
-    if (lane == 0) {
+  if (warp < 4) {
+    reg_dealloc<24>();
+    if (threadIdx.x == 0) {
       int s = 0;
       uint32_t ph = 0, iph = 0;
       for (int item = blockIdx.x; item < p.items; item += gridDim.x, iph ^= 1) {
         const int tile = is_part ? split_tile_of() : item;
         const int bh = tile / p.q_tiles, q0 = (tile - bh * p.q_tiles) * 128;
-        mbar_wait_quiet(q_empty, iph ^ 1);          // (first item: passes) the previous item's last S MMA has been issued
+        mbar_wait_quiet(q_empty, iph ^ 1);          // (first item: passes) the previous item's last S MMAs have completed
         mbar_expect_tx(q_full, ATT_TILE_BYTES);
         tma_load_3d(sQ, &tmQ, q_full, 0, q0, bh);
         for (int j = 0; j < nkv; ++j) {
@@ -180,253 +115,109 @@ attn1_kernel(const __grid_constant__ CUtensorMap tmQ, const __grid_constant__ CU
         }
       }
     }
-  } else if (warp == 1) {
-    if (lane == 0) {
-      constexpr uint32_t idesc_s = make_idesc_bf16(128, 128, 0, 0);
-      constexpr uint32_t idesc_pv = make_idesc_bf16(128, 64, 0, 1);  // B (=V) is MN-major
-      const uint32_t tS = tmem_base;
-      const uint32_t tP = tmem_base + 128;
-      const uint32_t tO = tmem_base + 192;
-      const uint64_t qdesc = make_sw128_desc(smem_u32(sQ));
-      const uint64_t kdesc0 = make_sw128_desc(smem_u32(sK));
-      const uint64_t vdesc0 = make_sw128_desc(smem_u32(sV));
-      constexpr uint64_t kStageStep = ATT_TILE_BYTES >> 4;
-      auto issue_S = [&](int stage) {
-        const uint64_t bdesc = kdesc0 + stage * kStageStep;
+  } else {
+    reg_alloc<240>();
+    const int cw = (warp >> 2) - 1;                       // consumer warpgroup: query rows [64 cw, 64 cw + 64) of the tile
+    const int row0 = cw * 64 + (warp & 3) * 16 + (lane >> 2);   // this thread's rows: row0, row0 + 8
+    const int fcol = 2 * (lane & 3);                      // and columns 8 j + fcol, + 1 of every accumulator
+    const uint64_t qdesc = make_sw128_desc(smem_u32(sQ + cw * 64 * 128));
+    int s = 0;
+    uint32_t ph = 0, iph = 0;
+    for (int item = blockIdx.x; item < p.items; item += gridDim.x, iph ^= 1) {
+      const int tile = is_part ? split_tile_of() : item;
+      const int bh = tile / p.q_tiles;
+      const int q0 = (tile - bh * p.q_tiles) * 128;
+      const int kv_rem = p.nkv - jb * 128;           // keys from this item's first KV tile to the end of the sequence
+      float m_run[2] = {-INFINITY, -INFINITY}, l_run[2] = {0.f, 0.f};
+      float o[32];
 #pragma unroll
-        for (int k = 0; k < 4; ++k) umma_ss(tS, qdesc + 2 * k, bdesc + 2 * k, idesc_s, k > 0 ? 1u : 0u);
-        umma_commit(s_full);
-      };
-      auto issue_PV = [&](int stage, int j) {
-        const uint64_t bdesc = vdesc0 + stage * kStageStep;
+      for (int i = 0; i < 32; ++i) o[i] = 0.f;
+      mbar_wait_quiet(q_full, iph);
+      for (int j = 0; j < nkv; ++j) {
+        const int kv_valid = min(128, kv_rem - j * 128);
+        float sc[64];
+        mbar_wait_quiet(&k_full[s], ph);
+        const uint64_t kdesc = make_sw128_desc(smem_u32(sK + s * ATT_TILE_BYTES));
+        wgmma_fence();
 #pragma unroll
-        for (int k = 0; k < 8; ++k)
-          umma_ts(tO, tP + 8 * k, bdesc + static_cast<uint64_t>(k) * (2048 >> 4), idesc_pv, (j > 0 || k > 0) ? 1u : 0u);
-        umma_commit(o_ready);
-      };
-      // One flat sequence of KV iterations over all work items of this CTA (`it` counts them: the per-iteration barriers
-      // complete once per iteration).  S of the NEXT iteration -- also across an item boundary, then with the next item's Q --
-      // is issued as soon as the softmax warps hold the current S in registers.
-      int n_items = 0;
-      for (int item = blockIdx.x; item < p.items; item += gridDim.x) ++n_items;
-      if (n_items > 0) {
-        mbar_wait_quiet(q_full, 0);
-        mbar_wait_quiet(&k_full[0], 0);
-        tc_fence_after();
-        issue_S(0);
-        umma_commit(&k_empty[0]);
-        if (nkv == 1) umma_commit(q_empty);
+        for (int k = 0; k < 4; ++k) wgmma_ss<128, false>(sc, qdesc + 2 * k, kdesc + 2 * k, k > 0);
+        wgmma_commit();
+        wgmma_wait<0>();
+        fence_regs<64>(sc);
+        __syncwarp();
+        if (lane == 0) {
+          mbar_arrive(&k_empty[s]);
+          if (j + 1 == nkv) mbar_arrive(q_empty);
+        }
+        if (kv_valid < 128) {
+#pragma unroll
+          for (int i = 0; i < 64; ++i)
+            if (8 * (i >> 2) + fcol + (i & 1) >= kv_valid) sc[i] = -INFINITY;
+        }
+        // online softmax: row maxima over the quad of threads that share a row
+        float mx[2] = {-INFINITY, -INFINITY};
+#pragma unroll
+        for (int i = 0; i < 64; ++i) mx[(i >> 1) & 1] = fmaxf(mx[(i >> 1) & 1], sc[i]);
+        float alpha[2];
+#pragma unroll
+        for (int h = 0; h < 2; ++h) {
+          mx[h] = fmaxf(mx[h], __shfl_xor_sync(0xffffffffu, mx[h], 1));
+          mx[h] = fmaxf(mx[h], __shfl_xor_sync(0xffffffffu, mx[h], 2));
+          const float m_new = fmaxf(m_run[h], mx[h]);
+          alpha[h] = ex2_approx(m_run[h] - m_new);         // first tile: exp2(-inf) = 0
+          m_run[h] = m_new;
+          l_run[h] *= alpha[h];
+        }
+        uint32_t pa[32];                                  // P as bf16 A fragments: 8 k-steps of 16 keys x 4 registers
+#pragma unroll
+        for (int i = 0; i < 64; i += 2) {
+          const int h = (i >> 1) & 1;
+          const float e0 = ex2_approx(sc[i] - m_run[h]), e1 = ex2_approx(sc[i + 1] - m_run[h]);
+          l_run[h] += e0 + e1;
+          pa[i >> 1] = pack_bf16(e0, e1);
+        }
+#pragma unroll
+        for (int i = 0; i < 32; ++i) o[i] *= alpha[(i >> 1) & 1];
+        mbar_wait_quiet(&v_full[s], ph);
+        const uint64_t vdesc = make_sw128_desc(smem_u32(sV + s * ATT_TILE_BYTES));
+        wgmma_fence();
+#pragma unroll
+        for (int kk = 0; kk < 8; ++kk) wgmma_rs64_bf16_tb(o, pa + 4 * kk, vdesc + static_cast<uint64_t>(kk) * (2048 >> 4), 1);
+        wgmma_commit();
+        wgmma_wait<0>();
+        fence_regs<32>(o);
+        __syncwarp();
+        if (lane == 0) mbar_arrive(&v_empty[s]);
+        if (++s == NS) {
+          s = 0;
+          ph ^= 1;
+        }
       }
-      int s = 0, sn = 1 % NS;
-      uint32_t ph = 0, phn = (NS == 1) ? 1u : 0u;
-      uint32_t it = 0;
-      for (int ii = 0; ii < n_items; ++ii) {
-        for (int j = 0; j < nkv; ++j, ++it) {
-          const bool next_in_item = j + 1 < nkv;
-          if (next_in_item || ii + 1 < n_items) {   // S(next) as soon as the softmax warps hold S(it) in registers
-            if (!next_in_item) mbar_wait_quiet(q_full, (ii + 1) & 1);      // Q of the next work item
-            mbar_wait_quiet(&k_full[sn], phn);
-            mbar_wait_quiet(s_taken, it & 1);
-            tc_fence_after();
-            issue_S(sn);
-            umma_commit(&k_empty[sn]);
-            // that was the last S of its item: Q may be replaced
-            if (next_in_item ? (j + 2 == nkv) : (nkv == 1)) umma_commit(q_empty);
-          }
-          mbar_wait_quiet(&v_full[s], ph);
-          mbar_wait_quiet(p_full, it & 1);
-          if (j == 0 && ii > 0) mbar_wait_quiet(o_taken, (ii - 1) & 1);   // the previous item's O has been read out
-          tc_fence_after();
-          issue_PV(s, j);
-          umma_commit(&v_empty[s]);
-          s = sn;
-          ph = phn;
-          if (++sn == NS) {
-            sn = 0;
-            phn ^= 1;
-          }
+      // ---- epilogue: O / l -> bf16 -> out[b, qrow, head*64 .. +64)
+#pragma unroll
+      for (int h = 0; h < 2; ++h) {
+        l_run[h] += __shfl_xor_sync(0xffffffffu, l_run[h], 1);
+        l_run[h] += __shfl_xor_sync(0xffffffffu, l_run[h], 2);
+      }
+      const int head = bh % p.heads, bz = bh / p.heads;
+#pragma unroll
+      for (int h = 0; h < 2; ++h) {
+        const int r = row0 + 8 * h;
+        if (is_part) {     // one KV range of a split tile: un-normalised O, reference and row sum for attn_merge_kernel
+          const long long sidx = static_cast<long long>(blockIdx.x) - p.n_full;     // == (tile - n_full) * parts + part
+          float* dst = p.part_o + (sidx * 128 + r) * 64 + fcol;
+#pragma unroll
+          for (int j = 0; j < 8; ++j) *reinterpret_cast<float2*>(dst + 8 * j) = make_float2(o[4 * j + 2 * h], o[4 * j + 2 * h + 1]);
+          if ((lane & 3) == 0) p.part_ml[sidx * 128 + r] = make_float2(m_run[h], l_run[h]);
+        } else if (q0 + r < p.n) {
+          const float inv = 1.0f / l_run[h];
+          __nv_bfloat16* dst = p.out + (static_cast<long long>(bz) * p.n + q0 + r) * p.C + head * 64 + fcol;
+#pragma unroll
+          for (int j = 0; j < 8; ++j)
+            *reinterpret_cast<uint32_t*>(dst + 8 * j) = pack_bf16(o[4 * j + 2 * h] * inv, o[4 * j + 2 * h + 1] * inv);
         }
       }
     }
-  } else if (warp >= 4) {
-    reg_alloc<208>();
-    const int quarter = warp & 3;
-    const int r = quarter * 32 + lane;
-    const uint32_t lane_off = static_cast<uint32_t>(quarter * 32) << 16;
-    const uint32_t tS = tmem_base + lane_off;
-    const uint32_t tP = tmem_base + 128 + lane_off;
-    const uint32_t tO = tmem_base + 192 + lane_off;
-    uint32_t it = 0;
-    for (int item = blockIdx.x; item < p.items; item += gridDim.x) {
-    const int tile = is_part ? split_tile_of() : item;
-    const int bh = tile / p.q_tiles;
-    const int qrow = (tile - bh * p.q_tiles) * 128 + r;
-    const int kv_rem = p.nkv - jb * 128;           // keys from this item's first KV tile to the end of the sequence
-    const int head = bh % p.heads, bz = bh / p.heads;
-    float m_used = -INFINITY;
-    float l = 0.f;
-    for (int j = 0; j < nkv; ++j, ++it) {
-      const int kv_valid = min(128, kv_rem - j * 128);
-      mbar_wait_quiet(s_full, it & 1);
-      tc_fence_after();
-      uint32_t raw[128];
-      tmem_ld32(tS, raw);
-      tmem_ld32(tS + 32, raw + 32);
-      tmem_ld32(tS + 64, raw + 64);
-      tmem_ld32(tS + 96, raw + 96);
-      tmem_ld_wait();
-      tc_fence_before();
-      __syncwarp();
-      if (lane == 0) mbar_arrive(s_taken);
-      if (kv_valid != 128) {
-#pragma unroll
-        for (int i = 0; i < 128; ++i)
-          if (i >= kv_valid) raw[i] = 0xff800000u;
-      }
-      // stale-reference softmax step (see the file header)
-      float2 acc = make_float2(0.f, 0.f);
-      bool slow = (j == 0);
-      float m_new = m_used;
-      if (j > 0) {
-        const float2 negm = make_float2(-m_used, -m_used);
-        float mx0 = -INFINITY, mx1 = -INFINITY;
-        // The P buffer may only be overwritten once PV(j-1) has read it (o_ready).  PV(j-1) is issued when this step
-        // starts, so waiting before the first P store exposed its whole latency: ncu attributed 24% of the fast pass to
-        // that wait.  The packed results of the first OVG_ATT_LATE_WAIT chunks are held in registers instead and the wait
-        // is taken one or two chunks (~500 - 1000 clocks) later, when the MMA has long finished.
-        uint32_t held[OVG_ATT_LATE_WAIT > 0 ? 16 * OVG_ATT_LATE_WAIT : 1];
-#pragma unroll
-        for (int c = 0; c < 4; ++c) {
-          uint32_t pk[16];
-#pragma unroll
-          for (int i = 0; i < 16; ++i) {
-            const float r0 = __uint_as_float(raw[c * 32 + 2 * i]), r1 = __uint_as_float(raw[c * 32 + 2 * i + 1]);
-            // every 4th pair goes through the FMA-pipe polynomial (interleaved with the MUFU pairs: 607 vs 624 us clustered)
-            const bool poly = (i & 3) == 3 && (i >> 2) < OVG_ATT_EMU_PAIRS;
-            if (poly) mx0 = fmaxf(fmaxf(mx0, r0), r1);     // the polynomial's exponent insertion wraps above 2^127: watch its inputs
-            float2 x = fadd2(make_float2(r0, r1), negm);
-            if (poly) {
-              x = exp2_poly2(x);
-            } else {
-              x.x = ex2_approx(x.x);
-              x.y = ex2_approx(x.y);
-            }
-            acc = fadd2(acc, x);
-            pk[i] = pack_bf16(x.x, x.y);
-          }
-          if (c < OVG_ATT_LATE_WAIT) {
-#pragma unroll
-            for (int i = 0; i < 16; ++i) held[c * 16 + i] = pk[i];
-            continue;
-          }
-          if (c == OVG_ATT_LATE_WAIT) {
-            mbar_wait_quiet(o_ready, (it - 1) & 1);   // PV(j-1) complete: P buffer reusable, O stable
-            tc_fence_after();
-#pragma unroll
-            for (int h = 0; h < OVG_ATT_LATE_WAIT; ++h) tmem_st16(tP + h * 16, held + h * 16);
-          }
-          tmem_st16(tP + c * 16, pk);
-        }
-        // No running maximum (612 vs 624 us): bf16 P and the fp32 O / l accumulators carry the full fp32 exponent range, so a stale reference
-        // costs no precision until exp2 overflows.  The step is redone (exactly, from the S row in registers) only if the row
-        // sum says a probability came near the top of that range, or a polynomial lane saw an input it cannot represent.
-        slow = __any_sync(0xffffffffu, !(acc.x + acc.y < 1e30f) || (mx0 - m_used) > 100.0f);
-        if (slow) {
-#pragma unroll
-          for (int i = 0; i < 128; i += 4) {
-            mx0 = fmaxf(fmaxf(mx0, __uint_as_float(raw[i])), __uint_as_float(raw[i + 1]));
-            mx1 = fmaxf(fmaxf(mx1, __uint_as_float(raw[i + 2])), __uint_as_float(raw[i + 3]));
-          }
-          m_new = fmaxf(m_used, fmaxf(mx0, mx1));
-        }
-      }
-      if (slow) {
-        if (j == 0) {
-          float mx0 = -INFINITY, mx1 = -INFINITY;
-#pragma unroll
-          for (int i = 0; i < 128; i += 4) {
-            mx0 = fmaxf(fmaxf(mx0, __uint_as_float(raw[i])), __uint_as_float(raw[i + 1]));
-            mx1 = fmaxf(fmaxf(mx1, __uint_as_float(raw[i + 2])), __uint_as_float(raw[i + 3]));
-          }
-          m_used = fmaxf(mx0, mx1);
-        } else {
-          const bool need = (m_new - m_used) > 8.0f;
-          const float alpha = need ? ex2_approx(m_used - m_new) : 1.0f;
-          if (need) {
-            m_used = m_new;
-            l *= alpha;
-          }
-          tmem_st_wait();
-#pragma unroll
-          for (int c = 0; c < 2; ++c) {
-            uint32_t o[32];
-            tmem_ld32(tO + c * 32, o);
-            tmem_ld_wait();
-#pragma unroll
-            for (int i = 0; i < 32; ++i) o[i] = __float_as_uint(__uint_as_float(o[i]) * alpha);
-            tmem_st32(tO + c * 32, o);
-          }
-        }
-        const float2 negm = make_float2(-m_used, -m_used);
-        acc = make_float2(0.f, 0.f);
-#pragma unroll
-        for (int c = 0; c < 4; ++c) {
-          uint32_t pk[16];
-#pragma unroll
-          for (int i = 0; i < 16; ++i) {
-            float2 x = make_float2(__uint_as_float(raw[c * 32 + 2 * i]), __uint_as_float(raw[c * 32 + 2 * i + 1]));
-            x = fadd2(x, negm);
-            x.x = ex2_approx(x.x);
-            x.y = ex2_approx(x.y);
-            acc = fadd2(acc, x);
-            pk[i] = pack_bf16(x.x, x.y);
-          }
-          tmem_st16(tP + c * 16, pk);
-        }
-      }
-      l += acc.x + acc.y;
-      tmem_st_wait();
-      tc_fence_before();
-      __syncwarp();
-      if (lane == 0) mbar_arrive(p_full);
-    }
-    // ---- epilogue: O / l -> bf16 -> out[b, qrow, head*64 .. +64)
-    mbar_wait_quiet(o_ready, (it - 1) & 1);
-    tc_fence_after();
-    const float inv = 1.0f / l;
-    uint32_t o[64];
-    tmem_ld32(tO, o);
-    tmem_ld32(tO + 32, o + 32);
-    tmem_ld_wait();
-    tc_fence_before();
-    __syncwarp();
-    if (lane == 0) mbar_arrive(o_taken);             // the next item's first PV may overwrite O
-    if (is_part) {         // one KV range of a split tile: un-normalised O, reference and row sum for attn_merge_kernel
-      const long long sidx = static_cast<long long>(blockIdx.x) - p.n_full;     // == (tile - n_full) * parts + part
-      float4* dst = reinterpret_cast<float4*>(p.part_o + (sidx * 128 + r) * 64);
-#pragma unroll
-      for (int i = 0; i < 16; ++i)
-        dst[i] = make_float4(__uint_as_float(o[4 * i]), __uint_as_float(o[4 * i + 1]), __uint_as_float(o[4 * i + 2]), __uint_as_float(o[4 * i + 3]));
-      p.part_ml[sidx * 128 + r] = make_float2(m_used, l);
-    } else if (qrow < p.n) {
-      uint4* dst = reinterpret_cast<uint4*>(p.out + (static_cast<long long>(bz) * p.n + qrow) * p.C + head * 64);
-#pragma unroll
-      for (int i = 0; i < 8; ++i) {
-        uint4 w;
-        w.x = pack_bf16(__uint_as_float(o[8 * i + 0]) * inv, __uint_as_float(o[8 * i + 1]) * inv);
-        w.y = pack_bf16(__uint_as_float(o[8 * i + 2]) * inv, __uint_as_float(o[8 * i + 3]) * inv);
-        w.z = pack_bf16(__uint_as_float(o[8 * i + 4]) * inv, __uint_as_float(o[8 * i + 5]) * inv);
-        w.w = pack_bf16(__uint_as_float(o[8 * i + 6]) * inv, __uint_as_float(o[8 * i + 7]) * inv);
-        dst[i] = w;
-      }
-    }
-    }   // work items
-  }
-  tc_fence_before();
-  __syncthreads();
-  if (warp == 1) {
-    tc_fence_after();
-    tmem_dealloc(tmem_base, 256);
   }
 }
 

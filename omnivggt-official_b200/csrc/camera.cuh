@@ -1,5 +1,5 @@
 // Small kernels of the camera head (reference heads/camera_head.py:83-154): M = B*S rows (8 .. a few dozen), so everything
-// except the weight-streaming GEMMs (which run on the tcgen05 GEMM of gemm.cuh) is a one-warp-per-row kernel in fp32.
+// except the weight-streaming GEMMs (which run on the wgmma GEMM of gemm.cuh) is a one-warp-per-row kernel in fp32.
 #pragma once
 #include "elem.cuh"
 

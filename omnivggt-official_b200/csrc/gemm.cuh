@@ -1,14 +1,16 @@
-// Persistent warp-specialised tcgen05 GEMM for sm_100a with fused epilogues.
+// Persistent warp-specialised wgmma GEMM for sm_90a with fused epilogues.
 //
-//   D[M,N] = sum_taps A[m + tap_off[t], 0:Kc] * B[n, t*Kc:(t+1)*Kc]^T      (bf16 x bf16 -> fp32 in TMEM)
+//   D[M,N] = sum_taps A[m + tap_off[t], 0:Kc] * B[n, t*Kc:(t+1)*Kc]^T      (bf16 x bf16 -> fp32 in registers)
 //
 // One kernel serves every dense contraction on the hot path:
 //   * aggregator linears  (reference layers/attention.py:52,:75, layers/mlp.py:35-38)  -- 1 tap
 //   * DPT 1x1 / transposed convs (heads/dpt_head.py:69-96)                              -- 1 tap
 //   * DPT 3x3 convs as 9 row-shifted GEMMs over a zero-bordered ("padded-linear") NHWC
 //     layout (heads/dpt_head.py:326-354,:379-399,:115-126)                              -- 9 taps
-// Roles: warp0 = TMA producer, warp1 = MMA issuer (+TMEM alloc), warps 2..9 = epilogue.
-// Pipelines: smem full/empty ring (TMA<->MMA), 2 TMEM accumulator stages (MMA<->epilogue).
+// Roles: warpgroup 0 = TMA producer (one thread), warpgroups 1-2 = wgmma (64 rows of the 128-row tile each) + epilogue.
+// Pipeline: smem full/empty ring (TMA<->MMA).  The finished accumulator tile goes through an fp32 smem tile so that the
+// epilogue works on whole rows (one row per thread), as the QKV head LayerNorm and the row remaps need; the producer keeps
+// loading the next tile's K blocks meanwhile.
 #pragma once
 #include "ptx.cuh"
 
@@ -39,8 +41,6 @@ struct GemmParams {
   // ---- EPI_RESID:  out(fp32)[row,n] += gamma[n] * (acc + bias[n]),  row = row_index ? row_index[m] : m
   const float* gamma;
   const int* row_index;
-  int split_tail;  // pair kernel, BN = 256: the tiles of the last (partial) wave are issued as two 256 x 128 halves
-  int staged;  // 1: epilogue output goes through smem + TMA (store for EPI_BF16, fp32 reduce-add for EPI_RESID)
   // ---- EPI_QKV (layers/attention.py:52-58 fused: bias, q/k LayerNorm(64), 2-D RoPE, head-major bf16)
   __nv_bfloat16* q_out;
   __nv_bfloat16* k_out;
@@ -73,24 +73,26 @@ struct GemmParams {
 
 constexpr int GEMM_BM = 128;
 constexpr int GEMM_BK = 64;
-constexpr int GEMM_THREADS = 320;
+constexpr int GEMM_THREADS = 384;
 constexpr int GEMM_A_BYTES = GEMM_BM * GEMM_BK * 2;
 
 constexpr int GEMM_QKV_TABLE_BYTES = 3 * 64 * 18 * 4 + 1024;   // QKV epilogue: rope cos / sin / -sin + q,k LayerNorm affine
+// BN <= 128: a 128 x 256 tile would need 128 accumulator registers per thread plus a 128 KB fp32 smem tile, which leaves room
+// for only two K stages within the 227 KB of an H100 SM.
 template <int BN>
 struct GemmCfg {
+  static_assert(BN == 32 || BN == 64 || BN == 128, "block_n");
   static constexpr int B_BYTES = BN * GEMM_BK * 2;
   static constexpr int STAGE_BYTES = GEMM_A_BYTES + B_BYTES;
-  static constexpr int STAGES = (BN >= 256) ? 4 : (BN >= 128 ? 6 : 8);
-  static constexpr int TMEM_COLS = (2 * BN < 32) ? 32 : 2 * BN;
-  static constexpr int SMEM_BYTES = STAGES * STAGE_BYTES + 1024 /*align*/ + 256 /*barriers*/ + GEMM_QKV_TABLE_BYTES;
+  static constexpr int STAGES = BN >= 128 ? 4 : 6;
+  static constexpr int ACC_LD = BN + 4;   // fp32 row pitch of the accumulator tile: row-wise float4 reads are conflict-free
+  static constexpr int ACC_BYTES = GEMM_BM * ACC_LD * 4;
+  static constexpr int SMEM_BYTES = STAGES * STAGE_BYTES + ACC_BYTES + 1024 /*align*/ + 256 /*barriers*/ + GEMM_QKV_TABLE_BYTES;
 };
 
 // Exact-erf GELU (nn.GELU() default, reference layers/mlp.py:22,:36) with erf evaluated by Abramowitz-Stegun 7.1.26
 // (|abs err| <= 1.5e-7, three orders below the bf16 output resolution): 2 MUFU (rcp, ex2) + FMA-pipe work per element;
 // erff() costs ~3x more and made the fc1 epilogue longer than its K = 1024 mainloop.
-// Two values at a time on the packed fp32x2 pipes (FFMA2 / FMUL2): ~9 instead of ~16 issue slots per element for the
-// scalar form.  The epilogue warps of the fc1 GEMM are issue-bound (2 warps per SM sub-partition, 32 768 GELUs per tile).
 __device__ __forceinline__ float2 gelu_erf2(const float2 x) {
   const float2 z = make_float2(fabsf(x.x) * 0.70710678118654752f, fabsf(x.y) * 0.70710678118654752f);
   const float2 d = ffma2(make_float2(0.3275911f, 0.3275911f), z, make_float2(1.0f, 1.0f));
@@ -113,13 +115,21 @@ __device__ __forceinline__ float2 gelu_erf2(const float2 x) {
   return ffma2(hax, w, hx);
 }
 
-// One 128 x BN accumulator tile: TMEM -> registers -> fused epilogue -> global.  `trow` addresses this warp's TMEM lane
-// quarter of the accumulator stage, `m` is this thread's global row, `colhalf` selects which column chunks this warp owns.
+// 32 consecutive fp32 accumulator values of this thread's row (16-byte aligned smem)
+__device__ __forceinline__ void acc_ld32(const float* src, uint32_t* r) {
+#pragma unroll
+  for (int i = 0; i < 8; ++i) {
+    const float4 v = reinterpret_cast<const float4*>(src)[i];
+    r[4 * i] = __float_as_uint(v.x); r[4 * i + 1] = __float_as_uint(v.y);
+    r[4 * i + 2] = __float_as_uint(v.z); r[4 * i + 3] = __float_as_uint(v.w);
+  }
+}
+
+// One 128 x BN accumulator tile: smem -> registers -> fused epilogue -> global.  `arow` is this thread's row of the fp32
+// accumulator tile, `m` its global row, `colhalf` selects which column chunks this warp owns.
 template <int BN, int EPI>
-__device__ __forceinline__ void epilogue_tile(const GemmParams& p, const uint32_t trow, const int m, const int n0,
-                                              const int colhalf, const float* s_rope, uint8_t* stg = nullptr,
-                                              const CUtensorMap* tmO = nullptr, const CUtensorMap* tmO2 = nullptr,
-                                              const CUtensorMap* tmO3 = nullptr) {
+__device__ __forceinline__ void epilogue_tile(const GemmParams& p, const float* arow, const int m, const int n0,
+                                              const int colhalf, const float* s_rope) {
   if constexpr (EPI == EPI_QKV) {
     // ---- per-row RoPE position (reference omnivggt_aggregator.py:215-224; layers/rope.py:39-59)
     int py = 0, px = 0;
@@ -145,13 +155,11 @@ __device__ __forceinline__ void epilogue_tile(const GemmParams& p, const uint32_
     const int heads = p.C >> 6;
     for (int c = colhalf; c < BN / 64; c += 2) {
       const int n = n0 + c * 64;
-      uint32_t raw[64];
-      tmem_ld32(trow + c * 64, raw);
-      tmem_ld32(trow + c * 64 + 32, raw + 32);
-      tmem_ld_wait();
-      if (n >= p.N || m - static_cast<int>(threadIdx.x & 31) >= p.M) continue;   // warp-uniform
-      const long long tok0 = __shfl_sync(0xffffffffu, tok, 0);   // all 32 lanes are converged here
-      if (p.staged || m < p.M) {                               // staged: every lane of the warp takes part
+      if (n >= p.N) continue;                                   // warp-uniform
+      if (m < p.M) {
+        uint32_t raw[64];
+        acc_ld32(arow + c * 64, raw);
+        acc_ld32(arow + c * 64 + 32, raw + 32);
         // all arithmetic on packed fp32 pairs (FADD2 / FMUL2 / FFMA2): v2[i] = elements (2i, 2i+1) of this head
         float2 v2[32];
         {
@@ -210,34 +218,6 @@ __device__ __forceinline__ void epilogue_tile(const GemmParams& p, const uint32_
             v2[24 + k] = ffma2(a1, sx[k], fmul2(b1, cx[k]));
           }
         }
-        // 32 rows x 128 B (one head of 32 tokens) -> 128B-swizzled smem tile -> one bulk tensor store into the
-        // head-major [batch*heads, ntok, 64] output.  Direct stores (every lane a different 128 B row) kept the LSU
-        // busy for ~20% of the kernel.  The few warps whose 32 rows straddle two sequences (or the end of the problem)
-        // keep the direct path: a second bulk store at a negative token coordinate faults on sm_100.
-        if (p.staged && tok0 + 32 <= p.ntok) {
-          const int lane = threadIdx.x & 31;
-          if (lane == 0) tma_store_wait_read0();
-          __syncwarp();
-#pragma unroll
-          for (int i = 0; i < 8; ++i) {
-            uint4 o;
-            o.x = pack_bf16(v2[4 * i + 0].x, v2[4 * i + 0].y);
-            o.y = pack_bf16(v2[4 * i + 1].x, v2[4 * i + 1].y);
-            o.z = pack_bf16(v2[4 * i + 2].x, v2[4 * i + 2].y);
-            o.w = pack_bf16(v2[4 * i + 3].x, v2[4 * i + 3].y);
-            *reinterpret_cast<uint4*>(stg + lane * 128 + ((i ^ (lane & 7)) << 4)) = o;
-          }
-          fence_proxy_async();
-          __syncwarp();
-          if (lane == 0) {
-            const CUtensorMap* tm = which == 0 ? tmO : (which == 1 ? tmO2 : tmO3);
-            const int bh = static_cast<int>(seq) * heads + h;     // lane 0: seq / tok of the warp's first row
-            tma_store_3d(tm, stg, 0, static_cast<int>(tok), bh);
-            tma_store_commit();
-          }
-          continue;
-        }
-        if (m >= p.M) continue;
         uint4 o8[8];
 #pragma unroll
         for (int i = 0; i < 8; ++i) {
@@ -292,38 +272,14 @@ __device__ __forceinline__ void epilogue_tile(const GemmParams& p, const uint32_
     }
     for (int c = colhalf; c < BN / 32; c += 2) {
       const int n = n0 + c * 32;
+      if (n >= p.N || !row_ok) continue;
       uint32_t raw[32];
-      tmem_ld32(trow + c * 32, raw);
-      tmem_ld_wait();
-      if (n >= p.N) continue;                       // warp-uniform
-      if (!p.staged && !row_ok) continue;           // staged: all lanes take part (TMA clips rows >= M)
+      acc_ld32(arow + c * 32, raw);
       float v[32];
 #pragma unroll
       for (int i = 0; i < 32; ++i) v[i] = __uint_as_float(raw[i]);
 
       if constexpr (EPI == EPI_RESID) {
-        if (p.staged) {
-          // gamma * (acc + bias) -> swizzled fp32 smem tile [32 rows x 32 cols] of this warp -> TMA reduce-add into x.
-          // The SM never reads x: the read-modify-write happens in L2, and the stores leave as whole 128 B rows.
-          const int lane = threadIdx.x & 31;
-          if (lane == 0) tma_store_wait_read0();      // previous chunk's bulk read of this buffer has finished
-          __syncwarp();
-#pragma unroll
-          for (int i = 0; i < 8; ++i) {
-            const float4 g = __ldg(reinterpret_cast<const float4*>(p.gamma + n) + i);
-            const float4 b = __ldg(reinterpret_cast<const float4*>(p.bias + n) + i);
-            const float2 o01 = fmul2(make_float2(g.x, g.y), fadd2(make_float2(v[4 * i + 0], v[4 * i + 1]), make_float2(b.x, b.y)));
-            const float2 o23 = fmul2(make_float2(g.z, g.w), fadd2(make_float2(v[4 * i + 2], v[4 * i + 3]), make_float2(b.z, b.w)));
-            *reinterpret_cast<float4*>(stg + lane * 128 + ((i ^ (lane & 7)) << 4)) = make_float4(o01.x, o01.y, o23.x, o23.y);
-          }
-          fence_proxy_async();
-          __syncwarp();
-          if (lane == 0) {
-            tma_reduce_add_2d(tmO, stg, n, m - lane);
-            tma_store_commit();
-          }
-          continue;
-        }
         float* x = reinterpret_cast<float*>(p.out) + drow * p.ldo + n;
 #pragma unroll
         for (int i = 0; i < 8; ++i) {
@@ -418,27 +374,6 @@ __device__ __forceinline__ void epilogue_tile(const GemmParams& p, const uint32_
 #pragma unroll
           for (int i = 0; i < 32; ++i) v[i] = 0.f;
         }
-        if (p.staged) {
-          const int lane = threadIdx.x & 31;
-          if (lane == 0) tma_store_wait_read0();
-          __syncwarp();
-#pragma unroll
-          for (int i = 0; i < 4; ++i) {
-            uint4 o;
-            o.x = pack_h(v[8 * i + 0], v[8 * i + 1], p.f16);
-            o.y = pack_h(v[8 * i + 2], v[8 * i + 3], p.f16);
-            o.z = pack_h(v[8 * i + 4], v[8 * i + 5], p.f16);
-            o.w = pack_h(v[8 * i + 6], v[8 * i + 7], p.f16);
-            *reinterpret_cast<uint4*>(stg + lane * 64 + ((i ^ ((lane >> 1) & 3)) << 4)) = o;   // 64B-swizzled tile
-          }
-          fence_proxy_async();
-          __syncwarp();
-          if (lane == 0) {
-            tma_store_2d(tmO, stg, n, m - lane);
-            tma_store_commit();
-          }
-          continue;
-        }
         uint4* d4 = reinterpret_cast<uint4*>(reinterpret_cast<__nv_bfloat16*>(p.out) + off);
 #pragma unroll
         for (int i = 0; i < 4; ++i) {
@@ -463,13 +398,11 @@ gemm_kernel(const __grid_constant__ CUtensorMap tmA, const __grid_constant__ CUt
   uint8_t* smem = reinterpret_cast<uint8_t*>((reinterpret_cast<uintptr_t>(smem_raw) + 1023) & ~uintptr_t(1023));
   uint8_t* sA = smem;
   uint8_t* sB = smem + STAGES * GEMM_A_BYTES;
-  uint64_t* bars = reinterpret_cast<uint64_t*>(smem + STAGES * Cfg::STAGE_BYTES);
+  float* sAcc = reinterpret_cast<float*>(smem + STAGES * Cfg::STAGE_BYTES);
+  uint64_t* bars = reinterpret_cast<uint64_t*>(smem + STAGES * Cfg::STAGE_BYTES + Cfg::ACC_BYTES);
   uint64_t* full = bars;
   uint64_t* empty = bars + STAGES;
-  uint64_t* tfull = bars + 2 * STAGES;
-  uint64_t* tempty = bars + 2 * STAGES + 2;
-  uint32_t* tmem_slot = reinterpret_cast<uint32_t*>(bars + 2 * STAGES + 4);
-  float* s_rope = reinterpret_cast<float*>(smem + STAGES * Cfg::STAGE_BYTES + 256);  // [3][64][18] + [4][64]
+  float* s_rope = reinterpret_cast<float*>(reinterpret_cast<uint8_t*>(bars) + 256);  // [3][64][18] + [4][64]
 
   const int warp = threadIdx.x >> 5;
   const int lane = threadIdx.x & 31;
@@ -477,53 +410,43 @@ gemm_kernel(const __grid_constant__ CUtensorMap tmA, const __grid_constant__ CUt
   const int n_tiles = (p.N + BN - 1) / BN;
   const int num_tiles = m_tiles * n_tiles;
 
-  if (warp == 0 && lane == 0) {
+  if (threadIdx.x == 0) {
     tma_prefetch_desc(&tmA);
     tma_prefetch_desc(&tmB);
     for (int i = 0; i < STAGES; ++i) {
       mbar_init(&full[i], 1);
-      mbar_init(&empty[i], 1);
-    }
-    for (int i = 0; i < 2; ++i) {
-      mbar_init(&tfull[i], 1);
-      mbar_init(&tempty[i], 8);
+      mbar_init(&empty[i], 8);     // one arrive per consumer warp
     }
     fence_barrier_init();
   }
-  if (warp == 1) {
-    tmem_alloc(tmem_slot, Cfg::TMEM_COLS);
-    tmem_relinquish();
-  }
-  if (EPI == EPI_QKV && warp >= 2) {
-    for (int i = threadIdx.x - 64; i < p.maxpos * 16; i += GEMM_THREADS - 64) {
+  if (EPI == EPI_QKV && warp >= 4) {
+    for (int i = threadIdx.x - 128; i < p.maxpos * 16; i += GEMM_THREADS - 128) {
       s_rope[(i >> 4) * 18 + (i & 15)] = p.rope_cos[i];
       s_rope[64 * 18 + (i >> 4) * 18 + (i & 15)] = p.rope_sin[i];
       s_rope[128 * 18 + (i >> 4) * 18 + (i & 15)] = -p.rope_sin[i];
     }
-    if (p.qk_norm && threadIdx.x >= 64 && threadIdx.x < 128) {
+    if (p.qk_norm && threadIdx.x >= 128 && threadIdx.x < 192) {
       float* s_ln = s_rope + 3 * 64 * 18;
-      const int i = threadIdx.x - 64;
+      const int i = threadIdx.x - 128;
       s_ln[i] = p.qn_w[i] * p.qscale;          // q is pre-scaled by log2(e)/sqrt(head_dim): fold it into the affine
       s_ln[64 + i] = p.qn_b[i] * p.qscale;
       s_ln[128 + i] = p.kn_w[i];
       s_ln[192 + i] = p.kn_b[i];
     }
   }
-  tc_fence_before();
   __syncthreads();
-  tc_fence_after();
-  const uint32_t tmem_base = *tmem_slot;
 
-  if (warp == 0) {
+  if (warp < 4) {
     // ===================== TMA producer =====================
-    if (lane == 0) {
+    reg_dealloc<40>();
+    if (threadIdx.x == 0) {
       int s = 0;
       uint32_t ph = 0;
       for (int tile = blockIdx.x; tile < num_tiles; tile += gridDim.x) {
         const int m0 = (tile / n_tiles) * GEMM_BM;
         const int n0 = (tile % n_tiles) * BN;
         for (int kb = 0; kb < p.k_blocks; ++kb) {
-          mbar_wait(&empty[s], ph ^ 1);
+          mbar_wait_quiet(&empty[s], ph ^ 1);
           mbar_expect_tx(&full[s], Cfg::STAGE_BYTES);
           const int tap = kb / p.kc_blocks;
           const int c0 = (kb - tap * p.kc_blocks) * GEMM_BK;
@@ -536,93 +459,69 @@ gemm_kernel(const __grid_constant__ CUtensorMap tmA, const __grid_constant__ CUt
         }
       }
     }
-  } else if (warp == 1) {
-    // ===================== MMA issuer =====================
-    if (lane == 0) {
-      const uint32_t idesc = make_idesc_bf16(GEMM_BM, BN, 0, 0) & ~(p.f16 ? IDESC_BF16_BITS : 0u);
-      int s = 0;
-      uint32_t ph = 0;
-      int as = 0;
-      uint32_t aph = 0;
-      for (int tile = blockIdx.x; tile < num_tiles; tile += gridDim.x) {
-        mbar_wait(&tempty[as], aph ^ 1);
-        tc_fence_after();
-        const uint32_t d_tmem = tmem_base + as * BN;
-        for (int kb = 0; kb < p.k_blocks; ++kb) {
-          mbar_wait(&full[s], ph);
-          tc_fence_after();
-          const uint64_t adesc = make_sw128_desc(smem_u32(sA + s * GEMM_A_BYTES));
-          const uint64_t bdesc = make_sw128_desc(smem_u32(sB + s * Cfg::B_BYTES));
-#pragma unroll
-          for (int k = 0; k < GEMM_BK / 16; ++k) {
-            umma_ss(d_tmem, adesc + 2 * k, bdesc + 2 * k, idesc, (kb | k) != 0 ? 1u : 0u);
-          }
-          umma_commit(&empty[s]);
-          if (++s == STAGES) {
-            s = 0;
-            ph ^= 1;
-          }
-        }
-        umma_commit(&tfull[as]);
-        if (++as == 2) {
-          as = 0;
-          aph ^= 1;
-        }
-      }
-    }
   } else {
-    // ===================== epilogue (8 warps) =====================
-    const int e = warp - 2;
-    const int quarter = warp & 3;  // TMEM lanes accessible to this warp: 32*(warp%4)..+31
+    // ===================== wgmma + epilogue (2 warpgroups, 8 warps) =====================
+    reg_alloc<232>();
+    const int cw = (warp >> 2) - 1;      // consumer warpgroup: rows [64 cw, 64 cw + 64) of the tile
+    const int e = warp - 4;              // epilogue warp 0..7
+    const int quarter = e & 3;           // epilogue rows 32 * quarter .. + 31
     const int colhalf = e >> 2;
     const int r = quarter * 32 + lane;
-    int as = 0;
-    uint32_t aph = 0;
+    const int frow = cw * 64 + (warp & 3) * 16 + (lane >> 2);   // accumulator fragment rows frow, frow + 8
+    const int fcol = 2 * (lane & 3);
+    int s = 0;
+    uint32_t ph = 0;
+    float acc[BN / 2];
     for (int tile = blockIdx.x; tile < num_tiles; tile += gridDim.x) {
       const int m0 = (tile / n_tiles) * GEMM_BM;
       const int n0 = (tile % n_tiles) * BN;
-      const int m = m0 + r;
-      mbar_wait(&tfull[as], aph);
-      tc_fence_after();
-      const uint32_t trow = tmem_base + as * BN + (static_cast<uint32_t>(quarter * 32) << 16);
-
-      epilogue_tile<BN, EPI>(p, trow, m, n0, colhalf, s_rope);
-      tc_fence_before();
-      __syncwarp();
-      if (lane == 0) mbar_arrive(&tempty[as]);
-      if (++as == 2) {
-        as = 0;
-        aph ^= 1;
+      int prev = -1;
+      for (int kb = 0; kb < p.k_blocks; ++kb) {
+        mbar_wait_quiet(&full[s], ph);      // no printf call site: it would serialise the wgmma pipeline
+        const uint64_t adesc = make_sw128_desc(smem_u32(sA + s * GEMM_A_BYTES + cw * 64 * 128));
+        const uint64_t bdesc = make_sw128_desc(smem_u32(sB + s * Cfg::B_BYTES));
+        wgmma_fence();
+#pragma unroll
+        for (int k = 0; k < GEMM_BK / 16; ++k) {
+          if (p.f16) wgmma_ss<BN, true>(acc, adesc + 2 * k, bdesc + 2 * k, (kb | k) != 0);
+          else wgmma_ss<BN, false>(acc, adesc + 2 * k, bdesc + 2 * k, (kb | k) != 0);
+        }
+        wgmma_commit();
+        wgmma_wait<1>();                 // the previous K block's MMAs are done: release its stage
+        if (prev >= 0 && lane == 0) mbar_arrive(&empty[prev]);
+        prev = s;
+        if (++s == STAGES) {
+          s = 0;
+          ph ^= 1;
+        }
       }
+      wgmma_wait<0>();
+      fence_regs<BN / 2>(acc);
+      if (lane == 0) mbar_arrive(&empty[prev]);
+      named_sync(1, 256);                // every epilogue thread is done with the previous tile's accumulators
+#pragma unroll
+      for (int j = 0; j < BN / 8; ++j) {
+        *reinterpret_cast<float2*>(sAcc + frow * Cfg::ACC_LD + 8 * j + fcol) = make_float2(acc[4 * j], acc[4 * j + 1]);
+        *reinterpret_cast<float2*>(sAcc + (frow + 8) * Cfg::ACC_LD + 8 * j + fcol) = make_float2(acc[4 * j + 2], acc[4 * j + 3]);
+      }
+      named_sync(1, 256);
+      epilogue_tile<BN, EPI>(p, sAcc + r * Cfg::ACC_LD, m0 + r, n0, colhalf, s_rope);
     }
-  }
-  tc_fence_before();
-  __syncthreads();
-  if (warp == 1) {
-    tc_fence_after();
-    tmem_dealloc(tmem_base, Cfg::TMEM_COLS);
   }
 }
 
-
-// =====================================================================================================================
-// CTA-pair variant (cta_group::2): one 256 x 256 output tile per 2-SM cluster.  Each CTA stages its own 128 rows of A and
-// 128 of the 256 B rows per K block (32 KB/stage instead of 48 KB for the same FLOPs), which is what matters here: a
-// 128 x 256 single-CTA tile needs ~87 FLOP per L2->SM byte and saturates the L2 fabric (~10-12 TB/s) near 1 PFLOP/s;
-// the paired tile needs 131 FLOP/B.  The pair leader issues M=256 MMAs that write both CTAs' TMEM; every CTA runs its own
-// TMA producer and epilogue (rows [128*rank, 128*rank+128) of the tile).
-// ---------------------------------------------------------------------------------------------------------------------
-// DPT output tail at full resolution (heads/dpt_head.py:121-126,:255-260): 3x3 conv 128 -> 32 over the zero-bordered NHWC
-// map + ReLU + 1x1 conv + activations.  With N = 32 the generic 9-tap path is bound by L2->SM traffic: it re-loads the
-// 128 x 64 A tile for every tap (18 loads of 16 KB per 128 output pixels).  Here the three horizontal taps of one kernel
-// row read ONE smem block of 136 rows through row-shifted UMMA descriptors (start address + kx * 128 B), so a tile needs 6
-// A loads instead of 18, and the 72 KB of weights are loaded once per CTA and stay resident.
+// DPT output tail at full resolution (heads/dpt_head.py:121-126,:255-260) for the shapes the fused tail (tail.cuh) does not take:
+// 3x3 conv 128 -> 32 over the zero-bordered NHWC map + ReLU + 1x1 conv + activations.  With N = 32 the generic 9-tap path is bound
+// by L2->SM traffic: it re-loads the 128 x 64 A tile for every tap (18 loads of 16 KB per 128 output pixels).  Here the three
+// horizontal taps of one kernel row read ONE smem block of 136 rows through row-shifted wgmma descriptors (start address +
+// kx * 128 B), so a tile needs 6 A loads instead of 18, and the 72 KB of weights are loaded once per CTA and stay resident.
 constexpr int HT_A_ROWS = 136;
 constexpr int HT_A_BYTES = HT_A_ROWS * 128;          // 17 408 = 17 swizzle atoms
 constexpr int HT_STAGES = 6;
-constexpr int HT_B_TILE = 32 * 128;                  // one [32 x 64] bf16 weight tile
+constexpr int HT_B_TILE = 32 * 128;                  // one [32 x 64] 16-bit weight tile
 constexpr int HT_B_BYTES = 18 * HT_B_TILE;           // 9 taps x 2 K blocks
-constexpr int HT_SMEM_BYTES = HT_STAGES * HT_A_BYTES + HT_B_BYTES + 1024 + 256;
+constexpr int HT_ACC_LD = 36;
+constexpr int HT_SMEM_BYTES = HT_STAGES * HT_A_BYTES + HT_B_BYTES + GEMM_BM * HT_ACC_LD * 4 + 1024 + 256;
 
 __global__ void __launch_bounds__(GEMM_THREADS, 1)
 headtail_kernel(const __grid_constant__ CUtensorMap tmA, const __grid_constant__ CUtensorMap tmB, const GemmParams p) {
@@ -630,43 +529,32 @@ headtail_kernel(const __grid_constant__ CUtensorMap tmA, const __grid_constant__
   uint8_t* smem = reinterpret_cast<uint8_t*>((reinterpret_cast<uintptr_t>(smem_raw) + 1023) & ~uintptr_t(1023));
   uint8_t* sA = smem;
   uint8_t* sB = smem + HT_STAGES * HT_A_BYTES;
-  uint64_t* bars = reinterpret_cast<uint64_t*>(sB + HT_B_BYTES);
+  float* sAcc = reinterpret_cast<float*>(sB + HT_B_BYTES);
+  uint64_t* bars = reinterpret_cast<uint64_t*>(sAcc + GEMM_BM * HT_ACC_LD);
   uint64_t* full = bars;
   uint64_t* empty = bars + HT_STAGES;
-  uint64_t* tfull = bars + 2 * HT_STAGES;
-  uint64_t* tempty = tfull + 2;
-  uint64_t* bfull = tempty + 2;
-  uint32_t* tmem_slot = reinterpret_cast<uint32_t*>(bfull + 1);
+  uint64_t* bfull = bars + 2 * HT_STAGES;
 
   const int warp = threadIdx.x >> 5;
   const int lane = threadIdx.x & 31;
   const int num_tiles = (p.M + GEMM_BM - 1) / GEMM_BM;
 
-  if (warp == 0 && lane == 0) {
+  if (threadIdx.x == 0) {
     tma_prefetch_desc(&tmA);
     tma_prefetch_desc(&tmB);
     for (int i = 0; i < HT_STAGES; ++i) {
       mbar_init(&full[i], 1);
-      mbar_init(&empty[i], 1);
-    }
-    for (int i = 0; i < 2; ++i) {
-      mbar_init(&tfull[i], 1);
-      mbar_init(&tempty[i], 4);
+      mbar_init(&empty[i], 8);     // one arrive per consumer warp
     }
     mbar_init(bfull, 1);
     fence_barrier_init();
   }
-  if (warp == 1) {
-    tmem_alloc(tmem_slot, 64);
-    tmem_relinquish();
-  }
-  tc_fence_before();
   __syncthreads();
-  tc_fence_after();
-  const uint32_t tmem_base = *tmem_slot;
 
-  if (warp == 0) {
-    if (lane == 0) {
+  if (warp < 4) {
+    // ===================== TMA producer: weights once, then 3 kernel rows x 2 K blocks of 136 A rows per tile =====================
+    reg_dealloc<40>();
+    if (threadIdx.x == 0) {
       mbar_expect_tx(bfull, HT_B_BYTES);
       for (int t = 0; t < 18; ++t) tma_load_2d(sB + t * HT_B_TILE, &tmB, bfull, t * GEMM_BK, 0);
       int s = 0;
@@ -676,7 +564,7 @@ headtail_kernel(const __grid_constant__ CUtensorMap tmA, const __grid_constant__
         for (int ky = 0; ky < 3; ++ky) {
           const int row0 = m0 + p.tap_off[ky * 3 + 1] - 1;     // first row the kx = 0 tap reads
           for (int kb = 0; kb < 2; ++kb) {
-            mbar_wait(&empty[s], ph ^ 1);
+            mbar_wait_quiet(&empty[s], ph ^ 1);
             mbar_expect_tx(&full[s], HT_A_BYTES);
             tma_load_2d(sA + s * HT_A_BYTES, &tmA, &full[s], kb * GEMM_BK, row0);
             if (++s == HT_STAGES) {
@@ -687,276 +575,58 @@ headtail_kernel(const __grid_constant__ CUtensorMap tmA, const __grid_constant__
         }
       }
     }
-  } else if (warp == 1) {
-    if (lane == 0) {
-      const uint32_t idesc = make_idesc_bf16(GEMM_BM, 32, 0, 0) & ~(p.f16 ? IDESC_BF16_BITS : 0u);
-      int s = 0;
-      uint32_t ph = 0;
-      int as = 0;
-      uint32_t aph = 0;
-      mbar_wait(bfull, 0);
-      for (int tile = blockIdx.x; tile < num_tiles; tile += gridDim.x) {
-        mbar_wait(&tempty[as], aph ^ 1);
-        tc_fence_after();
-        const uint32_t d_tmem = tmem_base + as * 32;
-        for (int ky = 0; ky < 3; ++ky) {
-          for (int kb = 0; kb < 2; ++kb) {
-            mbar_wait(&full[s], ph);
-            tc_fence_after();
-            const uint32_t a_atom = smem_u32(sA + s * HT_A_BYTES);
+  } else {
+    // ===================== wgmma (64 rows per warpgroup) + HEADTAIL epilogue =====================
+    reg_alloc<232>();
+    const int cw = (warp >> 2) - 1;
+    const int e = warp - 4;
+    const int r = (e & 3) * 32 + lane;
+    const int frow = cw * 64 + (warp & 3) * 16 + (lane >> 2);
+    const int fcol = 2 * (lane & 3);
+    mbar_wait_quiet(bfull, 0);
+    int s = 0;
+    uint32_t ph = 0;
+    float acc[16];
+    for (int tile = blockIdx.x; tile < num_tiles; tile += gridDim.x) {
+      const int m0 = tile * GEMM_BM;
+      int prev = -1;
+      for (int ky = 0; ky < 3; ++ky) {
+        for (int kb = 0; kb < 2; ++kb) {
+          mbar_wait_quiet(&full[s], ph);
+          const uint32_t a_atom = smem_u32(sA + s * HT_A_BYTES + cw * 64 * 128);
+          wgmma_fence();
 #pragma unroll
-            for (int kx = 0; kx < 3; ++kx) {
-              const uint64_t adesc = make_sw128_desc_rows(a_atom, kx);
-              const uint64_t bdesc = make_sw128_desc(smem_u32(sB + ((ky * 3 + kx) * 2 + kb) * HT_B_TILE));
+          for (int kx = 0; kx < 3; ++kx) {
+            const uint64_t adesc = make_sw128_desc_rows(a_atom, kx);
+            const uint64_t bdesc = make_sw128_desc(smem_u32(sB + ((ky * 3 + kx) * 2 + kb) * HT_B_TILE));
 #pragma unroll
-              for (int k = 0; k < GEMM_BK / 16; ++k)
-                umma_ss(d_tmem, adesc + 2 * k, bdesc + 2 * k, idesc, (ky | kb | kx | k) != 0 ? 1u : 0u);
-            }
-            umma_commit(&empty[s]);
-            if (++s == HT_STAGES) {
-              s = 0;
-              ph ^= 1;
+            for (int k = 0; k < GEMM_BK / 16; ++k) {
+              if (p.f16) wgmma_ss<32, true>(acc, adesc + 2 * k, bdesc + 2 * k, (ky | kb | kx | k) != 0);
+              else wgmma_ss<32, false>(acc, adesc + 2 * k, bdesc + 2 * k, (ky | kb | kx | k) != 0);
             }
           }
-        }
-        umma_commit(&tfull[as]);
-        if (++as == 2) {
-          as = 0;
-          aph ^= 1;
-        }
-      }
-    }
-  } else {
-    // The tile is only 32 columns wide, so a column split would leave half of the epilogue warps idle; instead the two
-    // warp sets (2-5, 6-9) own one accumulator stage each and take alternate tiles (the per-row 1x1 conv + activations
-    // + strided fp32 stores are latency-bound).
-    const int quarter = warp & 3;
-    const int eset = (warp - 2) >> 2;          // == accumulator stage this warp set serves
-    const int r = quarter * 32 + lane;
-    uint32_t aph = 0;
-    int seq = 0;
-    for (int tile = blockIdx.x; tile < num_tiles; tile += gridDim.x, ++seq) {
-      if ((seq & 1) != eset) continue;
-      const int m = tile * GEMM_BM + r;
-      mbar_wait(&tfull[eset], aph);
-      tc_fence_after();
-      const uint32_t trow = tmem_base + eset * 32 + (static_cast<uint32_t>(quarter * 32) << 16);
-      epilogue_tile<32, EPI_HEADTAIL>(p, trow, m, 0, 0, nullptr);
-      tc_fence_before();
-      __syncwarp();
-      if (lane == 0) mbar_arrive(&tempty[eset]);
-      aph ^= 1;
-    }
-  }
-  tc_fence_before();
-  __syncthreads();
-  if (warp == 1) {
-    tc_fence_after();
-    tmem_dealloc(tmem_base, 64);
-  }
-}
-
-constexpr int GEMM2_STG_BYTES = 8 * 4096;   // one 32 x 32 fp32 (or bf16) staging tile per epilogue warp; followed by the QKV tables
-template <int BN>
-struct Gemm2Cfg {
-#ifndef OVG_GEMM2_STAGES
-#define OVG_GEMM2_STAGES 5
-#endif
-  static constexpr int STAGES = BN >= 256 ? OVG_GEMM2_STAGES : 7;
-  static constexpr int B_BYTES = (BN / 2) * GEMM_BK * 2;       // each CTA stages half of the B rows
-  static constexpr int STAGE_BYTES = GEMM_A_BYTES + B_BYTES;
-  static constexpr int SMEM_BYTES = STAGES * STAGE_BYTES + 1024 + 256 + 1024 + GEMM2_STG_BYTES + GEMM_QKV_TABLE_BYTES;
-};
-
-template <int BN, int EPI>
-__global__ void __cluster_dims__(2, 1, 1) __launch_bounds__(GEMM_THREADS, 1)
-gemm2_kernel(const __grid_constant__ CUtensorMap tmA, const __grid_constant__ CUtensorMap tmB,
-             const __grid_constant__ CUtensorMap tmBh, const __grid_constant__ CUtensorMap tmO,
-             const __grid_constant__ CUtensorMap tmO2, const __grid_constant__ CUtensorMap tmO3, const GemmParams p) {
-  using Cfg2 = Gemm2Cfg<BN>;
-  constexpr int STAGES = Cfg2::STAGES;
-  constexpr int GEMM2_B_BYTES = Cfg2::B_BYTES;
-  constexpr int GEMM2_STAGE_BYTES = Cfg2::STAGE_BYTES;
-  extern __shared__ uint8_t smem_raw[];
-  uint8_t* smem = reinterpret_cast<uint8_t*>((reinterpret_cast<uintptr_t>(smem_raw) + 1023) & ~uintptr_t(1023));
-  uint8_t* sA = smem;
-  uint8_t* sB = smem + STAGES * GEMM_A_BYTES;
-  uint64_t* bars = reinterpret_cast<uint64_t*>(smem + STAGES * GEMM2_STAGE_BYTES);
-  uint64_t* full = bars;                    // used in the leader only: its arrive.expect_tx covers both CTAs' bytes
-  uint64_t* empty = bars + STAGES;          // per CTA: multicast MMA commit
-  uint64_t* tfull = bars + 2 * STAGES;      // per CTA: multicast MMA commit
-  uint64_t* tempty = bars + 2 * STAGES + 2; // used in the leader only: 8 epilogue warps x 2 CTAs
-  uint32_t* tmem_slot = reinterpret_cast<uint32_t*>(bars + 2 * STAGES + 4);
-  uint8_t* s_stage = smem + STAGES * GEMM2_STAGE_BYTES + 1024;     // 1024-aligned: swizzled TMA-store tiles
-  float* s_rope = reinterpret_cast<float*>(s_stage + GEMM2_STG_BYTES);   // QKV epilogue tables
-
-  const int warp = threadIdx.x >> 5;
-  const int lane = threadIdx.x & 31;
-  const uint32_t rank = cluster_ctarank();
-  const bool leader = rank == 0;
-  const int cluster_id = blockIdx.x >> 1;
-  const int num_clusters = gridDim.x >> 1;
-  const int m_tiles = (p.M + 255) / 256;
-  const int n_tiles = (p.N + BN - 1) / BN;
-  const int num_tiles = m_tiles * n_tiles;
-  // Wave quantisation: with T tiles on G clusters the last wave holds T mod G tiles and the other clusters idle for a
-  // whole tile time (proj / fc2 at cfg2: 172 tiles on 74 clusters = 2.32 waves, paid as 3).  When that remainder fits
-  // twice into the machine its tiles are issued as two 256 x 128 halves (tmBh: 64 B rows per CTA, N = 128 MMAs, the
-  // BN = 128 epilogue), so the tail costs half a tile time.  All three roles walk the same sequence `it`.
-  const int full_tiles = (BN == 256 && p.split_tail) ? (num_tiles / num_clusters) * num_clusters : num_tiles;
-  const int num_items = full_tiles + 2 * (num_tiles - full_tiles);
-#define OVG_GEMM2_ITEM(it)                                                          \
-  const bool half_tile = (it) >= full_tiles;                                        \
-  const int tile = half_tile ? full_tiles + (((it) - full_tiles) >> 1) : (it);      \
-  const int hsel = half_tile ? (((it) - full_tiles) & 1) : 0;
-
-  if (warp == 0 && lane == 0) {
-    tma_prefetch_desc(&tmA);
-    tma_prefetch_desc(&tmB);
-    if (BN == 256 && p.split_tail) tma_prefetch_desc(&tmBh);
-    if (p.staged) {
-      tma_prefetch_desc(&tmO);
-      if (EPI == EPI_QKV) {
-        tma_prefetch_desc(&tmO2);
-        tma_prefetch_desc(&tmO3);
-      }
-    }
-    for (int i = 0; i < STAGES; ++i) {
-      mbar_init(&full[i], 1);
-      mbar_init(&empty[i], 1);
-    }
-    for (int i = 0; i < 2; ++i) {
-      mbar_init(&tfull[i], 1);
-      mbar_init(&tempty[i], 16);
-    }
-    fence_barrier_init();
-  }
-  if (warp == 1) {
-    tmem_alloc_2sm(tmem_slot, 2 * BN);
-    tmem_relinquish_2sm();
-  }
-  if (EPI == EPI_QKV && warp >= 2) {
-    for (int i = threadIdx.x - 64; i < p.maxpos * 16; i += GEMM_THREADS - 64) {
-      s_rope[(i >> 4) * 18 + (i & 15)] = p.rope_cos[i];
-      s_rope[64 * 18 + (i >> 4) * 18 + (i & 15)] = p.rope_sin[i];
-      s_rope[128 * 18 + (i >> 4) * 18 + (i & 15)] = -p.rope_sin[i];
-    }
-    if (p.qk_norm && threadIdx.x >= 64 && threadIdx.x < 128) {
-      float* s_ln = s_rope + 3 * 64 * 18;
-      const int i = threadIdx.x - 64;
-      s_ln[i] = p.qn_w[i] * p.qscale;          // q is pre-scaled by log2(e)/sqrt(head_dim): fold it into the affine
-      s_ln[64 + i] = p.qn_b[i] * p.qscale;
-      s_ln[128 + i] = p.kn_w[i];
-      s_ln[192 + i] = p.kn_b[i];
-    }
-  }
-  tc_fence_before();
-  cluster_sync();
-  tc_fence_after();
-  const uint32_t tmem_base = *tmem_slot;
-
-  if (warp == 0) {
-    // ===================== TMA producer (both CTAs) =====================
-    if (lane == 0) {
-      int s = 0;
-      uint32_t ph = 0;
-      for (int it = cluster_id; it < num_items; it += num_clusters) {
-        OVG_GEMM2_ITEM(it)
-        const int m0 = (tile / n_tiles) * 256 + static_cast<int>(rank) * 128;
-        const int n0 = half_tile ? (tile % n_tiles) * BN + hsel * (BN / 2) + static_cast<int>(rank) * (BN / 4)
-                                 : (tile % n_tiles) * BN + static_cast<int>(rank) * (BN / 2);
-        const uint32_t stage_tx = half_tile ? GEMM_A_BYTES + GEMM2_B_BYTES / 2 : GEMM2_STAGE_BYTES;
-        for (int kb = 0; kb < p.k_blocks; ++kb) {
-          mbar_wait(&empty[s], ph ^ 1);
-          const uint32_t lead_full = mapa_u32(smem_u32(&full[s]), 0);
-          // Only the leader arrives; the peer's TMA bytes are accounted for by the leader's expect_tx (the transaction
-          // count may go transiently negative, which mbarrier allows).  The peer cannot run a phase ahead: it refills
-          // stage s only after the MMA that consumed the previous fill has committed to its empty[s].
-          if (leader) mbar_expect_tx(&full[s], 2 * stage_tx);
-          const int tap = kb / p.kc_blocks;
-          const int c0 = (kb - tap * p.kc_blocks) * GEMM_BK;
-          tma_load_2d_2sm(sA + s * GEMM_A_BYTES, &tmA, lead_full, c0, m0 + p.tap_off[tap]);
-          tma_load_2d_2sm(sB + s * GEMM2_B_BYTES, half_tile ? &tmBh : &tmB, lead_full, kb * GEMM_BK, n0);
-          if (++s == STAGES) {
+          wgmma_commit();
+          wgmma_wait<1>();               // the previous A stage has been read: release it
+          if (prev >= 0 && lane == 0) mbar_arrive(&empty[prev]);
+          prev = s;
+          if (++s == HT_STAGES) {
             s = 0;
             ph ^= 1;
           }
         }
       }
-    }
-  } else if (warp == 1) {
-    // ===================== MMA issuer (pair leader only) =====================
-    if (leader && lane == 0) {
-      const uint32_t fmt_clear = ~(p.f16 ? IDESC_BF16_BITS : 0u);
-      const uint32_t idesc_full = make_idesc_bf16(256, BN, 0, 0) & fmt_clear;
-      const uint32_t idesc_half = make_idesc_bf16(256, BN / 2, 0, 0) & fmt_clear;
-      int s = 0;
-      uint32_t ph = 0;
-      int as = 0;
-      uint32_t aph = 0;
-      for (int it = cluster_id; it < num_items; it += num_clusters) {
-        const uint32_t idesc = it >= full_tiles ? idesc_half : idesc_full;
-        mbar_wait(&tempty[as], aph ^ 1);
-        tc_fence_after();
-        const uint32_t d_tmem = tmem_base + as * BN;
-        for (int kb = 0; kb < p.k_blocks; ++kb) {
-          mbar_wait(&full[s], ph);
-          tc_fence_after();
-          const uint64_t adesc = make_sw128_desc(smem_u32(sA + s * GEMM_A_BYTES));
-          const uint64_t bdesc = make_sw128_desc(smem_u32(sB + s * GEMM2_B_BYTES));
+      wgmma_wait<0>();
+      fence_regs<16>(acc);
+      if (lane == 0) mbar_arrive(&empty[prev]);
+      named_sync(1, 256);
 #pragma unroll
-          for (int k = 0; k < GEMM_BK / 16; ++k)
-            umma_ss_2sm(d_tmem, adesc + 2 * k, bdesc + 2 * k, idesc, (kb | k) != 0 ? 1u : 0u);
-          umma_commit_2sm(&empty[s], 3);
-          if (++s == STAGES) {
-            s = 0;
-            ph ^= 1;
-          }
-        }
-        umma_commit_2sm(&tfull[as], 3);
-        if (++as == 2) {
-          as = 0;
-          aph ^= 1;
-        }
+      for (int j = 0; j < 4; ++j) {
+        *reinterpret_cast<float2*>(sAcc + frow * HT_ACC_LD + 8 * j + fcol) = make_float2(acc[4 * j], acc[4 * j + 1]);
+        *reinterpret_cast<float2*>(sAcc + (frow + 8) * HT_ACC_LD + 8 * j + fcol) = make_float2(acc[4 * j + 2], acc[4 * j + 3]);
       }
+      named_sync(1, 256);
+      epilogue_tile<32, EPI_HEADTAIL>(p, sAcc + r * HT_ACC_LD, m0 + r, 0, e >> 2, nullptr);
     }
-  } else {
-    // ===================== epilogue (8 warps per CTA) =====================
-    const int quarter = warp & 3;
-    const int colhalf = (warp - 2) >> 2;
-    const int r = quarter * 32 + lane;
-    int as = 0;
-    uint32_t aph = 0;
-    for (int it = cluster_id; it < num_items; it += num_clusters) {
-      OVG_GEMM2_ITEM(it)
-      const int m = (tile / n_tiles) * 256 + static_cast<int>(rank) * 128 + r;
-      const int n0 = (tile % n_tiles) * BN + hsel * (BN / 2);
-      mbar_wait(&tfull[as], aph);
-      tc_fence_after();
-      const uint32_t trow = tmem_base + as * BN + (static_cast<uint32_t>(quarter * 32) << 16);
-      if (half_tile)
-        epilogue_tile<BN / 2, EPI>(p, trow, m, n0, colhalf, s_rope, s_stage + (warp - 2) * 4096, &tmO, &tmO2, &tmO3);
-      else
-        epilogue_tile<BN, EPI>(p, trow, m, n0, colhalf, s_rope, s_stage + (warp - 2) * 4096, &tmO, &tmO2, &tmO3);
-      tc_fence_before();
-      __syncwarp();
-      if (lane == 0) {
-        if (leader) mbar_arrive(&tempty[as]);
-        else mbar_arrive_cluster(mapa_u32(smem_u32(&tempty[as]), 0));
-      }
-      if (++as == 2) {
-        as = 0;
-        aph ^= 1;
-      }
-    }
-  }
-#undef OVG_GEMM2_ITEM
-  if (p.staged && warp >= 2 && lane == 0) tma_store_wait_all();   // bulk stores issued by this thread have completed
-  tc_fence_before();
-  cluster_sync();   // the peer may still signal barriers / read smem of this CTA until both are done
-  if (warp == 1) {
-    tc_fence_after();
-    tmem_dealloc_2sm(tmem_base, 2 * BN);
   }
 }
 

@@ -109,42 +109,6 @@ int get_map(const void* ptr, unsigned long long d0, unsigned long long d1, unsig
   return OVG_OK;
 }
 
-// Output map for the staged epilogue: [rows, cols] row-major (row stride ld elements), box 32 cols x 32 rows;
-// bf16 -> 64 B inner box, SWIZZLE_64B; fp32 -> 128 B inner box, SWIZZLE_128B.
-int get_out_map(const void* ptr, bool f32, unsigned long long cols, unsigned long long rows, unsigned long long ld,
-                CUtensorMap* out) {
-  MapKey key{ptr, cols, rows, 0, ld, (f32 ? 2ull : 1ull) << 32};
-  {
-    std::lock_guard<std::mutex> g(g_map_mu);
-    auto it = g_maps.find(key);
-    if (it != g_maps.end()) {
-      *out = it->second;
-      return OVG_OK;
-    }
-  }
-  auto enc = get_encode();
-  if (!enc) return fail(OVG_E_CUDA, "cuTensorMapEncodeTiled entry point not available");
-  const unsigned esz = f32 ? 4 : 2;
-  if ((reinterpret_cast<uintptr_t>(ptr) & 15) || ((ld * esz) & 15))
-    return fail(OVG_E_INVALID, "TMA store target must be 16-byte aligned with a 16-byte multiple row stride");
-  cuuint64_t gdim[2] = {cols, rows};
-  cuuint64_t gstr[1] = {ld * esz};
-  cuuint32_t box[2] = {32, 32};
-  cuuint32_t estr[2] = {1, 1};
-  CUtensorMap m;
-  CUresult r = enc(&m, f32 ? CU_TENSOR_MAP_DATA_TYPE_FLOAT32 : CU_TENSOR_MAP_DATA_TYPE_BFLOAT16, 2, const_cast<void*>(ptr),
-                   gdim, gstr, box, estr, CU_TENSOR_MAP_INTERLEAVE_NONE,
-                   f32 ? CU_TENSOR_MAP_SWIZZLE_128B : CU_TENSOR_MAP_SWIZZLE_64B, CU_TENSOR_MAP_L2_PROMOTION_NONE,
-                   CU_TENSOR_MAP_FLOAT_OOB_FILL_NONE);
-  if (r != CUDA_SUCCESS) return fail(OVG_E_CUDA, "cuTensorMapEncodeTiled(out) failed (" + std::to_string(int(r)) + ")");
-  {
-    std::lock_guard<std::mutex> g(g_map_mu);
-    g_maps.emplace(key, m);
-  }
-  *out = m;
-  return OVG_OK;
-}
-
 // Function attributes and the SM count are per device: one process may drive several GPUs (or several host threads).
 constexpr int kMaxDevices = 64;
 int current_device() {
@@ -184,48 +148,19 @@ int launch_gemm(const CUtensorMap& ta, const CUtensorMap& tb, const ovg::GemmPar
   return post_launch("ovg_gemm");
 }
 
-template <int BN, int EPI>
-int launch_gemm2(const CUtensorMap& ta, const CUtensorMap& tb, const CUtensorMap& tbh, const CUtensorMap (&to)[3],
-                 ovg::GemmParams& p, cudaStream_t st) {
-  using Cfg = ovg::Gemm2Cfg<BN>;
-  static PerDeviceOnce once;
-  auto kern = ovg::gemm2_kernel<BN, EPI>;
-  if (once.needed()) {
-    OVG_CUDA(cudaFuncSetAttribute(kern, cudaFuncAttributeMaxDynamicSharedMemorySize, Cfg::SMEM_BYTES));
-    once.mark_done();
-  }
-  const int tiles = ((p.M + 255) / 256) * ((p.N + BN - 1) / BN);
-  const int pairs = num_sms() / 2;
-  const int grid = 2 * (tiles < pairs ? tiles : pairs);
-  // last partial wave as half tiles when both halves of every leftover tile find a free cluster (gemm.cuh)
-  const int tail = tiles > pairs ? tiles % pairs : 0;
-#ifndef OVG_GEMM_SPLIT_TAIL
-#define OVG_GEMM_SPLIT_TAIL 1
-#endif
-  p.split_tail = (OVG_GEMM_SPLIT_TAIL && BN == 256 && tail > 0 && 2 * tail <= pairs) ? 1 : 0;
-  kern<<<grid, ovg::GEMM_THREADS, Cfg::SMEM_BYTES, st>>>(ta, tb, tbh, to[0], to[1], to[2], p);
-  return post_launch("ovg_gemm(2sm)");
-}
-
 template <int EPI>
 int dispatch_bn(int bn, const CUtensorMap& ta, const CUtensorMap& tb, const ovg::GemmParams& p, cudaStream_t st) {
   switch (bn) {
-    case 256: return launch_gemm<256, EPI>(ta, tb, p, st);
     case 128: return launch_gemm<128, EPI>(ta, tb, p, st);
     case 64: return launch_gemm<64, EPI>(ta, tb, p, st);
+    case 32: return launch_gemm<32, EPI>(ta, tb, p, st);
     default: return fail(OVG_E_INVALID, "ovg_gemm: unsupported block_n");
   }
 }
 
 }  // namespace
 
-long long* g_attn_prof = nullptr;   // set through ovg_debug_set_attn_profile (profiling builds)
-long long* g_tail_prof = nullptr;   // ovg_debug_set_tail_profile: clock64 stamps of the fused DPT tail (csrc/tail.cuh)
-
 extern "C" {
-
-void ovg_debug_set_attn_profile(long long* buf) { g_attn_prof = buf; }
-void ovg_debug_set_tail_profile(long long* buf) { g_tail_prof = buf; }
 
 int ovg_version(void) { return 3; }
 const char* ovg_last_error(void) { return g_err.c_str(); }
@@ -236,8 +171,8 @@ int ovg_device_check(void) {
   if (cudaGetDevice(&dev) != cudaSuccess) return fail(OVG_E_NODEVICE, "no CUDA device");
   cudaDeviceProp prop;
   if (cudaGetDeviceProperties(&prop, dev) != cudaSuccess) return fail(OVG_E_NODEVICE, "cannot query device");
-  if (prop.major != 10)
-    return fail(OVG_E_NODEVICE, std::string("libovg requires sm_100 (B200); found sm_") + std::to_string(prop.major) +
+  if (prop.major != 9 || prop.minor != 0)
+    return fail(OVG_E_NODEVICE, std::string("libovg requires sm_90 (H100); found sm_") + std::to_string(prop.major) +
                                     std::to_string(prop.minor));
   return OVG_OK;
 }
@@ -309,24 +244,17 @@ int ovg_gemm(const ovg_gemm_args* a, void* stream) {
   if (p.n_peers > 0) OVG_REQUIRE(a->peer_ntok >= a->ntok && a->peer_tok_off >= 0 && a->peer_tok_off + a->ntok <= a->peer_ntok,
                                  "peer token window");
 
-  int bn = a->block_n;
+  // block_n: 0 picks the tile width; any request above 128 (the widest tile on sm_90) runs as 128.
+  int bn = a->block_n > 128 ? 128 : a->block_n;
   if (a->epi == OVG_EPI_HEADTAIL) {
     OVG_REQUIRE(a->n == 32, "HEADTAIL epilogue needs n == 32");
     OVG_REQUIRE(a->w2 && a->b2 && a->bias && a->preds && a->conf && a->outc >= 2 && a->outc <= 4, "HEADTAIL args");
     OVG_REQUIRE(a->rowmap == OVG_ROWS_PAD, "HEADTAIL runs on the zero-bordered grid");
     bn = 32;
   } else if (bn == 0) {
-    bn = a->n >= 256 ? 256 : (a->n >= 128 ? 128 : 64);
-    if (a->epi != OVG_EPI_QKV && bn == 256) {
-      // prefer 128-wide tiles when 256-wide ones leave a badly quantised last wave
-      const long long mt = (a->m + 127) / 128;
-      const long long t256 = mt * ((a->n + 255) / 256), t128 = mt * ((a->n + 127) / 128);
-      const int sms = num_sms();
-      const double e256 = double(t256) / double(((t256 + sms - 1) / sms) * sms);
-      const double e128 = double(t128) / double(((t128 + sms - 1) / sms) * sms);
-      if (e128 > e256 + 0.08) bn = 128;
-    }
+    bn = a->n >= 128 ? 128 : 64;
   }
+  OVG_REQUIRE(bn == 32 || bn == 64 || bn == 128, "block_n must be 0, 32, 64 or >= 128");
   if (a->epi == OVG_EPI_QKV) {
     OVG_REQUIRE(a->q_out && a->bias && ((a->k_out && a->v_out) || a->n_peers > 0), "QKV args");
     if (a->qk_norm) OVG_REQUIRE(a->qn_w && a->qn_b && a->kn_w && a->kn_b, "QKV q/k norm weights");
@@ -353,51 +281,6 @@ int ovg_gemm(const ovg_gemm_args* a, void* stream) {
   int rc = get_map(a->a, a->a_cols, a->a_rows, 0, a->lda, 128, &ta);
   if (rc) return rc;
   const unsigned long long ktot = static_cast<unsigned long long>(a->a_cols) * a->num_taps;
-  // block_n 512 / 384 select the CTA-pair kernels (256 x 256 / 256 x 128 tile per 2-SM cluster).  They stage 33% fewer
-  // L2->SM bytes per FLOP than the single-CTA tiles, which is what bounds these GEMMs; auto-selected for large problems.
-  const bool pair = (a->block_n == 512 || a->block_n == 384) ||
-                    (a->block_n == 0 && a->epi != OVG_EPI_HEADTAIL && a->n >= 128 && a->m >= 1024);
-  if (pair) {
-    OVG_REQUIRE(a->epi != OVG_EPI_HEADTAIL, "pair kernel has no HEADTAIL epilogue");
-    const int pbn = (a->block_n == 384 || (a->block_n == 0 && a->n < 256)) ? 128 : 256;
-    rc = get_map(a->b, ktot, a->n, 0, a->ldb, pbn / 2, &tb);
-    if (rc) return rc;
-    CUtensorMap tbh;
-    rc = get_map(a->b, ktot, a->n, 0, a->ldb, pbn / 4, &tbh);     // half tiles of the last wave: N/4 rows of B per CTA
-    if (rc) return rc;
-    // staged epilogue (smem -> TMA store / fp32 reduce-add) whenever output rows are the GEMM rows
-    CUtensorMap to[3] = {ta, ta, ta};
-    const bool stage_ok = (a->epi == OVG_EPI_RESID && !a->row_index) ||
-                          (a->epi == OVG_EPI_BF16 && (a->rowmap == OVG_ROWS_IDENT || a->rowmap == OVG_ROWS_PAD));
-    if (stage_ok) {
-      rc = get_out_map(a->out, a->epi == OVG_EPI_RESID, a->n, a->m, a->ldo, &to[0]);
-      if (rc) return rc;
-      p.staged = 1;
-    } else if (a->epi == OVG_EPI_QKV && a->n_peers == 0) {
-      // head-major q / k / v [batch * heads, ntok, 64]: one 32-token x 64 box per bulk store
-      const unsigned long long bh = static_cast<unsigned long long>(a->m / a->ntok) * (a->C / 64);
-      const void* outs[3] = {a->q_out, a->k_out, a->v_out};
-      for (int i = 0; i < 3; ++i) {
-        rc = get_map(outs[i], 64, a->ntok, bh, 64, 32, &to[i]);
-        if (rc) return rc;
-      }
-      p.staged = 1;
-    }
-    if (pbn == 256) {
-      switch (a->epi) {
-        case OVG_EPI_BF16: return launch_gemm2<256, ovg::EPI_BF16>(ta, tb, tbh, to, p, st);
-        case OVG_EPI_RESID: return launch_gemm2<256, ovg::EPI_RESID>(ta, tb, tbh, to, p, st);
-        case OVG_EPI_QKV: return launch_gemm2<256, ovg::EPI_QKV>(ta, tb, tbh, to, p, st);
-        default: return fail(OVG_E_INVALID, "ovg_gemm: unknown epilogue");
-      }
-    }
-    switch (a->epi) {
-      case OVG_EPI_BF16: return launch_gemm2<128, ovg::EPI_BF16>(ta, tb, tbh, to, p, st);
-      case OVG_EPI_RESID: return launch_gemm2<128, ovg::EPI_RESID>(ta, tb, tbh, to, p, st);
-      case OVG_EPI_QKV: return launch_gemm2<128, ovg::EPI_QKV>(ta, tb, tbh, to, p, st);
-      default: return fail(OVG_E_INVALID, "ovg_gemm: unknown epilogue");
-    }
-  }
   rc = get_map(a->b, ktot, a->n, 0, a->ldb, bn, &tb);
   if (rc) return rc;
 
@@ -411,10 +294,8 @@ int ovg_gemm(const ovg_gemm_args* a, void* stream) {
       for (int ky = 0; ky < 3 && shape_ok; ++ky)
         shape_ok = a->tap_off[ky * 3 + 1] - a->tap_off[ky * 3] == 1 && a->tap_off[ky * 3 + 2] - a->tap_off[ky * 3 + 1] == 1;
       if (!shape_ok) return launch_gemm<32, ovg::EPI_HEADTAIL>(ta, tb, p, st);
-      CUtensorMap ta136, tb32;
+      CUtensorMap ta136;
       rc = get_map(a->a, a->a_cols, a->a_rows, 0, a->lda, ovg::HT_A_ROWS, &ta136);
-      if (rc) return rc;
-      rc = get_map(a->b, ktot, a->n, 0, a->ldb, 32, &tb32);
       if (rc) return rc;
       static PerDeviceOnce once;
       if (once.needed()) {
@@ -423,14 +304,14 @@ int ovg_gemm(const ovg_gemm_args* a, void* stream) {
       }
       const int tiles = (p.M + ovg::GEMM_BM - 1) / ovg::GEMM_BM;
       const int grid = tiles < num_sms() ? tiles : num_sms();
-      ovg::headtail_kernel<<<grid, ovg::GEMM_THREADS, ovg::HT_SMEM_BYTES, st>>>(ta136, tb32, p);
+      ovg::headtail_kernel<<<grid, ovg::GEMM_THREADS, ovg::HT_SMEM_BYTES, st>>>(ta136, tb, p);
       return post_launch("ovg_gemm(headtail)");
     }
     default: return fail(OVG_E_INVALID, "ovg_gemm: unknown epilogue");
   }
 }
 
-long long ovg_attention_scratch_bytes(void) { return 4LL * 2 * num_sms() * 128 * (64 * 4 + 8) + 256; }   // <= 4 parts of < one wave of tiles
+long long ovg_attention_scratch_bytes(void) { return 4LL * num_sms() * 128 * (64 * 4 + 8) + 256; }   // <= 4 parts of < one wave of tiles
 
 int ovg_attention_kv_ws(const void* q, const void* k, const void* v, void* out, int batch, int heads, int nq, int nkv,
                         void* scratch, long long scratch_bytes, void* stream) {
@@ -448,13 +329,12 @@ int ovg_attention_kv_ws(const void* q, const void* k, const void* v, void* out, 
   static PerDeviceOnce once;
   if (once.needed()) {
     OVG_CUDA(cudaFuncSetAttribute(ovg::attn1_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, ovg::ATT1_SMEM_BYTES));
-    OVG_CUDA(cudaFuncSetAttribute(ovg::attn1_kernel, cudaFuncAttributePreferredSharedMemoryCarveout, 100));
     once.mark_done();
   }
   const int q_tiles = (nq + 127) / 128;
   const long long tiles = static_cast<long long>(q_tiles) * heads * batch;
   OVG_REQUIRE(tiles < (1LL << 28), "too many tiles");
-  ovg::AttnParams p{nq, nkv, heads, heads * 64, reinterpret_cast<__nv_bfloat16*>(out), g_attn_prof, q_tiles, static_cast<int>(tiles),
+  ovg::AttnParams p{nq, nkv, heads, heads * 64, reinterpret_cast<__nv_bfloat16*>(out), q_tiles, static_cast<int>(tiles),
                     static_cast<int>(tiles), 1, nullptr, nullptr};
 #ifndef OVG_ATT_PERSISTENT
 #define OVG_ATT_PERSISTENT 1    // 0: always one CTA per work item (A/B builds)
@@ -462,15 +342,14 @@ int ovg_attention_kv_ws(const void* q, const void* k, const void* v, void* out, 
 #ifndef OVG_ATT_SPLIT_TAIL
 #define OVG_ATT_SPLIT_TAIL 1    // 0: never split the tiles of the last wave over the keys (A/B builds)
 #endif
-  // Short sequences (frame / DINOv2 attention: 11 KV tiles per item): two resident CTAs per SM walk the items, so barrier /
-  // TMEM set-up is paid once and the next item's Q, K, V stream in under the current item's tail (0.1126 -> 0.1085 ms at
-  // 8 x 16 x 1374).  Long sequences keep one CTA per item: the hardware's dynamic CTA placement balances the 4.65 "waves" of
-  // the global attention better than a static round robin (0.619 vs 0.649 ms), profiles/r02_attn_ab.jsonl.
-  const int resident = 2 * num_sms();
+  // Short sequences (frame / DINOv2 attention: 11 KV tiles per item): one resident CTA per SM walks the items, so barrier
+  // set-up is paid once and the next item's Q, K, V stream in under the current item's tail.  Long sequences keep one CTA
+  // per item: the hardware's dynamic CTA placement balances the partial waves of the global attention.
+  const int resident = num_sms();
   const int kv_tiles = (nkv + 127) / 128;
   const bool persistent = OVG_ATT_PERSISTENT && tiles > resident && kv_tiles <= 16;
   // Long sequences: the tiles of the last, partly empty wave are cut into 2-4 KV ranges (one CTA each, issued after the whole
-  // tiles) whose partial (O, reference, row sum) a small kernel merges: 1 376 tiles on 296 slots cost 4.67 instead of 5 waves.
+  // tiles) whose partial (O, reference, row sum) a small kernel merges.
   int parts = 1;
   const int tail = static_cast<int>(tiles % resident);
   if (OVG_ATT_SPLIT_TAIL && !persistent && scratch && tiles > resident && tail > 0 && kv_tiles >= 24) {
@@ -699,7 +578,6 @@ int ovg_dpt_tail(const void* src, const float* tx, const float* ty, const void* 
   if (p.seg_rows < 8 && H >= 8) p.seg_rows = 8;
   p.n_segs = (H + p.seg_rows - 1) / p.seg_rows;
   p.n_items = F * p.n_strips * p.n_segs;
-  p.prof = g_tail_prof;
   static PerDeviceOnce once;
   if (once.needed()) {
     OVG_CUDA(cudaFuncSetAttribute(ovg::fusedtail_kernel<true>, cudaFuncAttributeMaxDynamicSharedMemorySize, ovg::FT_SMEM_BYTES));

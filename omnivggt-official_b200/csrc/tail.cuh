@@ -5,17 +5,17 @@
 // image row of a 128-pixel column strip at a time straight into the swizzled shared-memory A operand of the tensor core.
 //
 // One CTA walks DOWN a strip, one input row per step.  An input row r contributes to the three output rows r-1, r, r+1 (kernel rows
-// ky = 2, 1, 0), so the accumulators of 16 consecutive output rows live in a ring of 32-column TMEM blocks and ONE N = 96 MMA per
-// (kx, k-step) adds [W_ky=2 | W_ky=1 | W_ky=0] x row r into the three neighbouring blocks: the A row block (136 x 64 halves) is read
-// from shared memory once per kx instead of once per (ky, kx), which is what bounds the N = 32 formulation (5 KB of operand reads
-// per 16-clock MMA).  Blocks are zeroed by the epilogue warps when they drain them, so every MMA accumulates.
+// ky = 2, 1, 0), so ONE N = 96 wgmma per (kx, k-step) computes [W_ky=2 | W_ky=1 | W_ky=0] x row r: the A row block (136 x 64 halves)
+// is read from shared memory once per kx instead of once per (ky, kx).  The three 32-column blocks of that product go into three
+// register accumulators: output row r-1 is finished (and drained by the epilogue), the partial sums of rows r and r+1 move up.
 //
-// Roles (512 threads, one CTA per SM, 222 KB of shared memory, all 512 TMEM columns):
-//   warp 0        loads the 72 KB of weights once (TMA), issues the MMAs, commits "A stage free" / "output row finished";
-//   warps 1-3, 8-15 (352 threads) producers: one thread bulk-copies the strip's source rows into a 4-row ring two rows ahead of use,
-//                 all of them blend vertically + horizontally (fp32, packed f32x2) and write the swizzled A stage (2 stages);
-//   warps 4-7     epilogue: TMEM block -> + bias + conv(position embedding) tables (the convolution is linear: its image under the
-//                 3x3 kernel separates into gx[row class][x] + gy[column class][y], tail_tables_kernel) -> ReLU -> 1x1 -> activations.
+// Roles (640 threads, one CTA per SM, 222 KB of shared memory):
+//   warp 0        loads the 72 KB of weights once (TMA);
+//   warps 1-3, 12-19 (352 threads) producers: one thread bulk-copies the strip's source rows into a 4-row ring two rows ahead of use,
+//                 all of them blend vertically + horizontally (fp32) and write the swizzled A stage (2 stages);
+//   warps 4-11    two consumer warpgroups, 64 strip pixels each: wgmma, then the epilogue on the finished row in registers:
+//                 + bias + conv(position embedding) tables (the convolution is linear: its image under the 3x3 kernel separates into
+//                 gx[row class][x] + gy[column class][y], tail_tables_kernel) -> ReLU -> 1x1 (quad shuffles) -> activations.
 // Work items: (frame, strip, segment of rows) with two halo rows per segment, about three per SM.
 #pragma once
 #include "ptx.cuh"
@@ -35,14 +35,9 @@ struct TailParams {
   float sy, sx;
   int outc, head_act, f16;
   int n_strips, n_segs, seg_rows, n_items;
-  long long* prof;      // debug: clock64 stamps of CTA 0's first 192 rows, 8 slots per row (nullptr: off)
 };
-#define OVG_FT_STAMP(cnt, slot)                                                                   \
-  do {                                                                                            \
-    if (p.prof && blockIdx.x == 0 && (cnt) < 192) p.prof[(cnt) * 8 + (slot)] = clock64();         \
-  } while (0)
 
-constexpr int FT_THREADS = 512;                 // warp 0: MMA; warps 4-7: epilogue; warps 1-3 and 8-15: producers
+constexpr int FT_THREADS = 640;                 // warp 0: weights; warps 4-11: wgmma + epilogue; warps 1-3 and 12-19: producers
 constexpr int FT_PROD_THREADS = 352;
 constexpr int FT_PROD_GROUPS = FT_PROD_THREADS / 16;   // 22 groups of 16 channel vectors
 constexpr int FT_IPT = 4;                       // consecutive source intervals per producer thread (22 x 4 >= 80)
@@ -80,6 +75,62 @@ __device__ __forceinline__ void ft_wait_idle(uint64_t* bar, uint32_t parity) {
   }
 }
 
+// Epilogue of one finished output row y for this thread's two pixels (rows h = 0, 1 of its accumulator fragment) and eight
+// channels (8 jj + fcol + c): + bias + position-embedding tables -> ReLU -> 1x1 conv (partial dots reduced over the quad of
+// threads that share a pixel) -> activations; lane fcol / 2 == h writes pixel h.
+__device__ __forceinline__ void ft_epilogue_row(const TailParams& p, const float* acc, const float* sw,
+                                                const int y, const int f, const int (&X)[2], const int fcol, const int lane) {
+  const int q = lane & 3;
+  float res[2][4];
+#pragma unroll
+  for (int h = 0; h < 2; ++h) {
+    const int Xc = X[h] < p.W ? X[h] : p.W - 1;
+    float v[8];
+#pragma unroll
+    for (int jj = 0; jj < 4; ++jj)
+#pragma unroll
+      for (int c = 0; c < 2; ++c) v[2 * jj + c] = acc[4 * jj + 2 * h + c] + sw[8 * jj + fcol + c];
+    if (p.gx) {
+      const int xcls = Xc == 0 ? 0 : (Xc == p.W - 1 ? 2 : 1);
+      const float* gy = p.gy + (static_cast<size_t>(xcls) * p.H + y) * 32 + fcol;
+      const int ycls = y == 0 ? 0 : (y == p.H - 1 ? 2 : 1);
+      const float* gx = p.gx + (static_cast<size_t>(ycls) * p.W + Xc) * 32 + fcol;   // interior rows: the same row for every y (L1)
+#pragma unroll
+      for (int jj = 0; jj < 4; ++jj) {
+        const float2 t = __ldg(reinterpret_cast<const float2*>(gy + 8 * jj));
+        const float2 u = __ldg(reinterpret_cast<const float2*>(gx + 8 * jj));
+        v[2 * jj] += t.x + u.x;
+        v[2 * jj + 1] += t.y + u.y;
+      }
+    }
+#pragma unroll
+    for (int o = 0; o < 4; ++o) {
+      float a = 0.f;
+#pragma unroll
+      for (int jj = 0; jj < 4; ++jj)
+#pragma unroll
+        for (int c = 0; c < 2; ++c) a = fmaf(sw[32 + o * 32 + 8 * jj + fcol + c], fmaxf(v[2 * jj + c], 0.f), a);
+      a += __shfl_xor_sync(0xffffffffu, a, 1);
+      a += __shfl_xor_sync(0xffffffffu, a, 2);
+      res[h][o] = a + sw[160 + o];
+    }
+  }
+  if (q >= 2) return;
+  if (X[q] >= p.W) return;                               // columns past the image
+  const long long pix = (static_cast<long long>(f) * p.H + y) * p.W + X[q];
+#pragma unroll
+  for (int o = 0; o < 4; ++o) {
+    if (o < p.outc) {
+      const float a = res[q][o];
+      if (o == p.outc - 1) {
+        p.conf[pix] = 1.0f + expf(a);
+      } else {
+        p.preds[pix * (p.outc - 1) + o] = p.head_act == 0 ? expf(a) : copysignf(expm1f(fabsf(a)), a);
+      }
+    }
+  }
+}
+
 template <bool F16>
 __global__ void __launch_bounds__(FT_THREADS, 1)
 fusedtail_kernel(const __grid_constant__ CUtensorMap tmB, const TailParams p) {
@@ -91,44 +142,33 @@ fusedtail_kernel(const __grid_constant__ CUtensorMap tmB, const TailParams p) {
   int* itab = reinterpret_cast<int*>(ring + FT_RING * FT_RAW_ROW);
   float* sw = reinterpret_cast<float*>(reinterpret_cast<uint8_t*>(itab) + FT_ITAB_BYTES);
   uint64_t* bars = reinterpret_cast<uint64_t*>(reinterpret_cast<uint8_t*>(sw) + FT_W_BYTES);
-  uint64_t* a_full = bars;         // [2]  producers (8 warps) -> MMA
-  uint64_t* a_empty = bars + 2;    // [2]  MMA commit -> producers
-  uint64_t* o_full = bars + 4;     // [16] MMA commit -> epilogue: block holds a finished output row
-  uint64_t* o_free = bars + 20;    // [16] epilogue (4 warps) -> MMA: block drained and zeroed
-  uint64_t* bfull = bars + 36;
-  uint64_t* r_full = bars + 37;    // [FT_RING] bulk copies of source rows
-  uint32_t* tmem_slot = reinterpret_cast<uint32_t*>(bars + 37 + FT_RING);
+  uint64_t* a_full = bars;         // [2]  producers (11 warps) -> consumers
+  uint64_t* a_empty = bars + 2;    // [2]  consumers (8 warps) -> producers
+  uint64_t* bfull = bars + 4;
+  uint64_t* r_full = bars + 5;     // [FT_RING] bulk copies of source rows
 
   const int warp = threadIdx.x >> 5;
   const int lane = threadIdx.x & 31;
 
-  if (warp == 0) {
-    if (lane == 0) {
-      tma_prefetch_desc(&tmB);
-      for (int i = 0; i < 2; ++i) {
-        mbar_init(&a_full[i], FT_PROD_THREADS / 32);
-        mbar_init(&a_empty[i], 1);
-      }
-      for (int i = 0; i < 16; ++i) {
-        mbar_init(&o_full[i], 1);
-        mbar_init(&o_free[i], 4);
-      }
-      mbar_init(bfull, 1);
-      for (int i = 0; i < FT_RING; ++i) mbar_init(&r_full[i], 1);
-      fence_barrier_init();
+  if (threadIdx.x == 0) {
+    tma_prefetch_desc(&tmB);
+    for (int i = 0; i < 2; ++i) {
+      mbar_init(&a_full[i], FT_PROD_THREADS / 32);
+      mbar_init(&a_empty[i], 8);
     }
-    __syncwarp();
-    tmem_alloc(tmem_slot, 512);
-    tmem_relinquish();
+    mbar_init(bfull, 1);
+    for (int i = 0; i < FT_RING; ++i) mbar_init(&r_full[i], 1);
+    fence_barrier_init();
   }
   if (threadIdx.x >= 128 && threadIdx.x < 128 + 32 + 4 * 32 + 4) {
     const int i = threadIdx.x - 128;
     sw[i] = i < 32 ? p.bias[i] : (i < 160 ? (i - 32 < p.outc * 32 ? p.w2[i - 32] : 0.f) : (i - 160 < p.outc ? p.b2[i - 160] : 0.f));
   }
-  tc_fence_before();
   __syncthreads();
-  tc_fence_after();
-  const uint32_t tmem_base = *tmem_slot;
+  // Registers: 96 per thread for every role (640 threads; no setmaxnreg).  The consumers hold 80 accumulator registers (this
+  // row's product and the partial sums of the next two output rows), and ptxas spills about 180 B per thread at this budget.
+  // Moving registers to the consumers does not remove that: the producers then need more than the 64-72 registers left for them
+  // (ptxas ignores the split) or spill themselves at 80, and a 512-thread layout with 128 registers for everyone still spills.
 
 #define OVG_FT_ITEM(item)                                        \
   const int seg = (item) % p.n_segs;                             \
@@ -139,180 +179,66 @@ fusedtail_kernel(const __grid_constant__ CUtensorMap tmB, const TailParams p) {
   const int x0 = strip * 128;
 
   if (warp == 0) {
-    // ===================== weights (once) + MMA issue =====================
+    // ===================== weights (once) =====================
     if (lane == 0) {
       mbar_expect_tx(bfull, FT_B_BYTES);
       for (int kx = 0; kx < 3; ++kx)
         for (int kb = 0; kb < 2; ++kb)
           for (int s = 0; s < 3; ++s)        // slot s holds kernel row ky = 2 - s
             tma_load_2d(sB + (kx * 2 + kb) * FT_B_TILE + s * 4096, &tmB, bfull, ((2 - s) * 3 + kx) * 128 + kb * 64, 0);
-      const uint32_t fmt_clear = ~(F16 ? IDESC_BF16_BITS : 0u);
-      const uint32_t idesc96 = make_idesc_bf16(128, 96, 0, 0) & fmt_clear;
-      const uint32_t idesc64 = make_idesc_bf16(128, 64, 0, 0) & fmt_clear;
-      const uint32_t idesc32 = make_idesc_bf16(128, 32, 0, 0) & fmt_clear;
-      mbar_wait_quiet(bfull, 0);
-      mbar_wait_quiet(&o_free[0], 0);
-      mbar_wait_quiet(&o_free[1], 0);
-      int st = 0;
-      uint32_t aph = 0;
-      int mcnt = 0;
-      int g = 1;                              // running input-row index: row g accumulates into blocks g-1, g, g+1 (mod 16)
-      for (int item = blockIdx.x; item < p.n_items; item += gridDim.x) {
-        OVG_FT_ITEM(item)
-        (void)f; (void)x0;
-        for (int r = ya - 1; r <= yb; ++r, ++g) {
-          ft_wait_idle(&o_free[(g + 1) & 15], ((g + 1) >> 4) & 1);
-          tc_fence_after();
-          if (r >= 0 && r < p.H) {
-            ft_wait_idle(&a_full[st], aph);
-            tc_fence_after();
-            OVG_FT_STAMP(mcnt, 5);
-            const int c0 = (g - 1) & 15;
-#pragma unroll
-            for (int kb = 0; kb < 2; ++kb) {
-              const uint32_t a_atom = smem_u32(sA + st * FT_A_STAGE + kb * FT_A_KB_BYTES);
-#pragma unroll
-              for (int kx = 0; kx < 3; ++kx) {
-                const uint64_t adesc = make_sw128_desc_rows(a_atom, kx);
-                const uint32_t bt = smem_u32(sB + (kx * 2 + kb) * FT_B_TILE);
-                if (c0 <= 13) {
-                  const uint64_t bdesc = make_sw128_desc(bt);
-#pragma unroll
-                  for (int k = 0; k < 4; ++k) umma_ss(tmem_base + c0 * 32, adesc + 2 * k, bdesc + 2 * k, idesc96, 1u);
-                } else if (c0 == 14) {       // blocks 14, 15 | 0
-                  const uint64_t b0 = make_sw128_desc(bt), b1 = make_sw128_desc(bt + 64 * 128);
-#pragma unroll
-                  for (int k = 0; k < 4; ++k) {
-                    umma_ss(tmem_base + 448, adesc + 2 * k, b0 + 2 * k, idesc64, 1u);
-                    umma_ss(tmem_base, adesc + 2 * k, b1 + 2 * k, idesc32, 1u);
-                  }
-                } else {                     // blocks 15 | 0, 1
-                  const uint64_t b0 = make_sw128_desc(bt), b1 = make_sw128_desc(bt + 32 * 128);
-#pragma unroll
-                  for (int k = 0; k < 4; ++k) {
-                    umma_ss(tmem_base + 480, adesc + 2 * k, b0 + 2 * k, idesc32, 1u);
-                    umma_ss(tmem_base, adesc + 2 * k, b1 + 2 * k, idesc64, 1u);
-                  }
-                }
-              }
-            }
-            umma_commit(&a_empty[st]);
-            OVG_FT_STAMP(mcnt, 6);
-            ++mcnt;
-            if (++st == FT_A_STAGES) {
-              st = 0;
-              aph ^= 1;
-            }
-          }
-          umma_commit(&o_full[(g - 1) & 15]);   // output row r-1 has received its three kernel rows
-        }
-      }
     }
-  } else if (warp >= 4 && warp < 8) {
-    // ===================== epilogue: drain + zero one TMEM block per input row =====================
-    const int quarter = warp & 3;
-    const uint32_t lane_base = tmem_base + (static_cast<uint32_t>(quarter * 32) << 16);
-    uint32_t zeros[32];
-#pragma unroll
-    for (int i = 0; i < 32; ++i) zeros[i] = 0u;
-    for (int b = 0; b < 16; ++b) tmem_st32(lane_base + b * 32, zeros);
-    tmem_st_wait();
-    tc_fence_before();
-    __syncwarp();
-    if (lane == 0)
-      for (int b = 0; b < 16; ++b) mbar_arrive(&o_free[b]);
-    int g = 1;
+  } else if (warp >= 4 && warp < 12) {
+    // ===================== wgmma + epilogue: 64 strip pixels per warpgroup =====================
+    const int cw = (warp >> 2) - 1;
+    const int prow = cw * 64 + (warp & 3) * 16 + (lane >> 2);   // strip pixels prow, prow + 8
+    const int fcol = 2 * (lane & 3);
+    mbar_wait_quiet(bfull, 0);
+    int st = 0;
+    uint32_t aph = 0;
     for (int item = blockIdx.x; item < p.n_items; item += gridDim.x) {
       OVG_FT_ITEM(item)
-      const int X = x0 + quarter * 32 + lane;
-      const int Xc = X < p.W ? X : p.W - 1;
-      // conv(position embedding) = gx[row class][x] + gy[column class][y]; the x part of interior rows stays in registers
-      float gxr[32];
+      const int X[2] = {x0 + prow, x0 + prow + 8};
+      float p1[16], p2[16];                   // partial sums of output rows r and r + 1
 #pragma unroll
-      for (int i = 0; i < 32; ++i) gxr[i] = 0.f;
-      if (p.gx) {
-        const float4* g4 = reinterpret_cast<const float4*>(p.gx + (static_cast<size_t>(p.W) + Xc) * 32);
+      for (int i = 0; i < 16; ++i) p1[i] = p2[i] = 0.f;
+      for (int r = ya - 1; r <= yb; ++r) {
+        float d[48];
+        if (r >= 0 && r < p.H) {
+          mbar_wait_quiet(&a_full[st], aph);
+          wgmma_fence();
 #pragma unroll
-        for (int i = 0; i < 8; ++i) {
-          const float4 t = __ldg(g4 + i);
-          gxr[4 * i] = t.x; gxr[4 * i + 1] = t.y; gxr[4 * i + 2] = t.z; gxr[4 * i + 3] = t.w;
+          for (int kb = 0; kb < 2; ++kb) {
+            const uint32_t a_atom = smem_u32(sA + st * FT_A_STAGE + kb * FT_A_KB_BYTES + cw * 64 * 128);
+#pragma unroll
+            for (int kx = 0; kx < 3; ++kx) {
+              const uint64_t adesc = make_sw128_desc_rows(a_atom, kx);
+              const uint64_t bdesc = make_sw128_desc(smem_u32(sB + (kx * 2 + kb) * FT_B_TILE));
+#pragma unroll
+              for (int k = 0; k < 4; ++k) wgmma_ss<96, F16>(d, adesc + 2 * k, bdesc + 2 * k, (kb | kx | k) != 0);
+            }
+          }
+          wgmma_commit();
+          wgmma_wait<0>();
+          fence_regs<48>(d);
+          __syncwarp();
+          if (lane == 0) mbar_arrive(&a_empty[st]);
+          if (++st == FT_A_STAGES) {
+            st = 0;
+            aph ^= 1;
+          }
+        } else {
+#pragma unroll
+          for (int i = 0; i < 48; ++i) d[i] = 0.f;   // zero padding above / below the image
         }
-      }
-      const int xcls = Xc == 0 ? 0 : (Xc == p.W - 1 ? 2 : 1);
-      const float* gyb = p.gx ? p.gy + static_cast<size_t>(xcls) * p.H * 32 : nullptr;
-      float4 gyn[8];                          // gy row of the NEXT finished output row (loaded one step ahead of its use)
+        // d = [ky = 2 -> row r-1 | ky = 1 -> row r | ky = 0 -> row r+1], 16 registers per 32-column block
 #pragma unroll
-      for (int i = 0; i < 8; ++i) gyn[i] = make_float4(0.f, 0.f, 0.f, 0.f);
-      auto load_gy = [&](int y) {
-        if (gyb && y >= ya && y < yb) {
-          const float4* g4 = reinterpret_cast<const float4*>(gyb + static_cast<size_t>(y) * 32);
-#pragma unroll
-          for (int i = 0; i < 8; ++i) gyn[i] = __ldg(g4 + i);
+        for (int i = 0; i < 16; ++i) {
+          d[i] += p1[i];
+          p1[i] = p2[i] + d[16 + i];
+          p2[i] = d[32 + i];
         }
-      };
-      load_gy(ya);                            // the first valid block of the item is output row ya
-      for (int r = ya - 1; r <= yb; ++r, ++g) {
-        const int e = g - 1;                  // block finished by input row r: output row r - 1
         const int y = r - 1;
-        ft_wait_idle(&o_full[e & 15], (e >> 4) & 1);
-        tc_fence_after();
-        if (warp == 4 && lane == 0) OVG_FT_STAMP(g - 1, 7);
-        uint32_t raw[32];
-        tmem_ld32(lane_base + (e & 15) * 32, raw);
-        tmem_ld_wait();
-        tmem_st32(lane_base + (e & 15) * 32, zeros);
-        tmem_st_wait();
-        tc_fence_before();
-        __syncwarp();
-        if (lane == 0) mbar_arrive(&o_free[e & 15]);
-        if (y < ya || y >= yb) continue;                 // halo rows of the segment (warp-uniform)
-        float v[32];
-#pragma unroll
-        for (int i = 0; i < 8; ++i) {
-          const float4 b4 = reinterpret_cast<const float4*>(sw)[i];
-          v[4 * i + 0] = __uint_as_float(raw[4 * i + 0]) + b4.x + gyn[i].x;
-          v[4 * i + 1] = __uint_as_float(raw[4 * i + 1]) + b4.y + gyn[i].y;
-          v[4 * i + 2] = __uint_as_float(raw[4 * i + 2]) + b4.z + gyn[i].z;
-          v[4 * i + 3] = __uint_as_float(raw[4 * i + 3]) + b4.w + gyn[i].w;
-        }
-        load_gy(y + 1);
-        if (p.gx) {
-          if (y == 0 || y == p.H - 1) {                  // first / last image row: the row class of gx changes (warp-uniform)
-            const float4* gx4 = reinterpret_cast<const float4*>(p.gx + (static_cast<size_t>(y == 0 ? 0 : 2) * p.W + Xc) * 32);
-#pragma unroll
-            for (int i = 0; i < 8; ++i) {
-              const float4 u = __ldg(gx4 + i);
-              v[4 * i + 0] += u.x; v[4 * i + 1] += u.y; v[4 * i + 2] += u.z; v[4 * i + 3] += u.w;
-            }
-          } else {
-#pragma unroll
-            for (int i = 0; i < 32; ++i) v[i] += gxr[i];
-          }
-        }
-#pragma unroll
-        for (int i = 0; i < 32; ++i) v[i] = fmaxf(v[i], 0.f);
-        if (X >= p.W) continue;                          // columns past the image
-        // 1x1 conv 32 -> outc: four independent accumulation chains (rows of w2 beyond outc are zero)
-        float acc[4] = {sw[160], sw[161], sw[162], sw[163]};
-#pragma unroll
-        for (int i = 0; i < 8; ++i) {
-#pragma unroll
-          for (int o = 0; o < 4; ++o) {
-            const float4 w = reinterpret_cast<const float4*>(sw + 32 + o * 32)[i];
-            acc[o] = fmaf(w.w, v[4 * i + 3], fmaf(w.z, v[4 * i + 2], fmaf(w.y, v[4 * i + 1], fmaf(w.x, v[4 * i + 0], acc[o]))));
-          }
-        }
-        const long long pix = (static_cast<long long>(f) * p.H + y) * p.W + X;
-#pragma unroll
-        for (int o = 0; o < 4; ++o) {
-          if (o < p.outc) {
-            if (o == p.outc - 1) {
-              p.conf[pix] = 1.0f + expf(acc[o]);
-            } else {
-              p.preds[pix * (p.outc - 1) + o] = p.head_act == 0 ? expf(acc[o]) : copysignf(expm1f(fabsf(acc[o])), acc[o]);
-            }
-          }
-        }
+        if (y >= ya && y < yb) ft_epilogue_row(p, d, sw, y, f, X, fcol, lane);
       }
     }
   } else {
@@ -324,7 +250,7 @@ fusedtail_kernel(const __grid_constant__ CUtensorMap tmB, const TailParams p) {
     // (itab): horizontal blend, pack to 16 bits, store with the 128-byte swizzle (row = pixel, chunk ^ (row & 7)).  The position
     // embedding is not added here: the convolution is linear, its image under the 3x3 kernel is a per-shape table that the
     // epilogue adds in fp32.
-    const int ptid = warp < 4 ? (warp - 1) * 32 + lane : (warp - 5) * 32 + lane;      // 0 .. 351
+    const int ptid = warp < 4 ? (warp - 1) * 32 + lane : (warp - 9) * 32 + lane;      // 0 .. 351
     const int v = ptid & 15, grp = ptid >> 4;
     int st = 0, pcnt = 0;
     uint32_t eph = 0, loaded = 0;                       // `loaded`: source rows copied so far (ring slot = index % FT_RING)
@@ -383,7 +309,6 @@ fusedtail_kernel(const __grid_constant__ CUtensorMap tmB, const TailParams p) {
         pk[j] = s_first + j < ns ? static_cast<int>(t) : 0;
       }
       for (int r = r_first; r <= r_last; ++r, ++pcnt) {
-        if (ptid == 0) OVG_FT_STAMP(pcnt, 0);
         const float fy = p.sy * r;
         const int y0 = static_cast<int>(fy);
         const int y1 = y0 + (y0 < p.h - 1 ? 1 : 0);
@@ -392,10 +317,8 @@ fusedtail_kernel(const __grid_constant__ CUtensorMap tmB, const TailParams p) {
         const uint32_t l0 = lbase + static_cast<uint32_t>(y0 - y_first), l1 = lbase + static_cast<uint32_t>(y1 - y_first);
         mbar_wait_quiet(&r_full[l0 % FT_RING], (l0 / FT_RING) & 1);
         mbar_wait_quiet(&r_full[l1 % FT_RING], (l1 / FT_RING) & 1);
-        if (ptid == 0) OVG_FT_STAMP(pcnt, 1);
         const uint32_t ra = ring_s + (l0 % FT_RING) * FT_RAW_ROW, rb = ring_s + (l1 % FT_RING) * FT_RAW_ROW;
         mbar_wait_quiet(&a_empty[st], eph ^ 1);     // the MMAs that read this stage two rows ago have completed
-        if (ptid == 0) OVG_FT_STAMP(pcnt, 2);
         const uint32_t stage = smem_u32(sA) + st * FT_A_STAGE + (v >> 3) * FT_A_KB_BYTES;
         // zero columns left / right of the image (conv padding)
         if (x0 == 0 && grp == 20) ft_sts128(stage + (vsw << 4), make_uint4(0, 0, 0, 0));
@@ -440,25 +363,17 @@ fusedtail_kernel(const __grid_constant__ CUtensorMap tmB, const TailParams p) {
         fence_proxy_async();
         __syncwarp();
         if (lane == 0) mbar_arrive(&a_full[st]);
-        if (ptid == 0) OVG_FT_STAMP(pcnt, 3);
         if (++st == FT_A_STAGES) {
           st = 0;
           eph ^= 1;
         }
         ft_prod_sync();                              // every thread has read the source rows of image row r
         if (ptid == 0 && r < r_last) copy_rows(static_cast<int>(p.sy * (r + 1)) + FT_RING - 1);   // slots below y0(r+1) are free
-        if (ptid == 0) OVG_FT_STAMP(pcnt, 4);
       }
       loaded = lbase + static_cast<uint32_t>(y_end - y_first + 1);
     }
   }
 #undef OVG_FT_ITEM
-  tc_fence_before();
-  __syncthreads();
-  if (warp == 0) {
-    tc_fence_after();
-    tmem_dealloc(tmem_base, 512);
-  }
 }
 
 // Image of the UV position embedding (heads/dpt_head.py:249-250, separable: channels [0, 64) depend on x, [64, 128) on y) under

@@ -1,5 +1,5 @@
 """Drop-in ``OmniVGGT`` module: the reference's constructor / forward / state-dict contract
-(reference omnivggt/models/omnivggt.py:10-68, consumed by inference.py:321-356) on the B200-native engine.
+(reference omnivggt/models/omnivggt.py:10-68, consumed by inference.py:321-356) on the H100-native engine.
 
     model = OmniVGGT().to("cuda").eval()
     model.load_state_dict(load_file("checkpoints/OmniVGGT.safetensors"))     # strict, same 1 505 keys
@@ -112,7 +112,7 @@ class OmniVGGT(nn.Module, PyTorchModelHubMixin):
         if self._engine is None:
             from .engine import Engine          # imports the CUDA library; fails loudly if it is missing
             if next(self.parameters()).device.type != "cuda":
-                raise RuntimeError("OmniVGGT (B200 engine) has no CPU path: move the module to a CUDA device")
+                raise RuntimeError("OmniVGGT (H100 engine) has no CPU path: move the module to a CUDA device")
             self._engine = Engine(self)
         return self._engine
 
@@ -299,7 +299,7 @@ class OmniVGGT(nn.Module, PyTorchModelHubMixin):
 
         # ---- heads.  The camera head and the two DPT heads only read the aggregator outputs: they run on three streams
         # (forked / joined with events, also inside a captured CUDA graph) so that their many small kernels -- 19^2 / 37^2
-        # feature maps, M = 8 GEMVs -- share the 148 SMs instead of running one after the other.
+        # feature maps, M = 8 GEMVs -- share the 132 SMs instead of running one after the other.
         predictions: Dict[str, object] = {}
         eng.warm_tables(H, W)
         d_out = eng.dpt_alloc("depth_head", K, H, W)

@@ -11,7 +11,7 @@ GOLDEN = os.path.join(ROOT, "tests", "golden")
 
 
 def pytest_configure(config):
-    config.addinivalue_line("markers", "gpu: needs a CUDA device (run on the B200 box with -m gpu)")
+    config.addinivalue_line("markers", "gpu: needs a CUDA device, an H100 (run with -m gpu)")
     # the PyTorch fp32 references of the kernel tests must be fp32: by default cuDNN runs fp32 convolutions in TF32 on a GPU
     import torch
     torch.backends.cudnn.allow_tf32 = False

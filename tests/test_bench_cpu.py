@@ -97,3 +97,37 @@ def test_reference_arm_ignores_torchrun_thread_cap():
     ncpu = len(os.sched_getaffinity(0)) if hasattr(os, "sched_getaffinity") else (os.cpu_count() or 1)
     if ncpu > 1:
         assert line["cpu_baseline"]["cores"] > 1, line["cpu_baseline"]
+
+
+def test_dump_outputs_whole_and_sampled(tmp_path, monkeypatch):
+    """--dump-outputs: float32 files per output (input images left out, lists stacked, per-call suffixes), everything whole
+    under the cap; over it, small arrays stay whole, the rest is a seeded sample that repeats exactly and fits the cap."""
+    import numpy as np
+    import torch
+    bench = _bench()
+    g = torch.Generator().manual_seed(0)
+    out = {"images": torch.rand(1, 2, 3, 8, 8, generator=g), "pose_enc": torch.rand(1, 2, 9, generator=g),
+           "depth": torch.rand(1, 2, 8, 8, 1, generator=g).half(), "pose_enc_list": [torch.rand(1, 2, 9, generator=g) for _ in range(4)]}
+    bench.dump_outputs(str(tmp_path / "a"), [out])
+    names = sorted(p.name for p in (tmp_path / "a").iterdir())
+    assert names == ["depth.npy", "pose_enc.npy", "pose_enc_list.npy"]
+    for k in ("depth", "pose_enc"):
+        a = np.load(tmp_path / "a" / f"{k}.npy")
+        assert a.dtype == np.float32 and np.array_equal(a, out[k].float().numpy())
+    assert np.load(tmp_path / "a" / "pose_enc_list.npy").shape == (4, 1, 2, 9)
+
+    big = {"pose_enc": torch.rand(1, 4, 9, generator=g), "world_points": torch.rand(1, 4, 300, 300, 3, generator=g),
+           "depth": torch.rand(1, 4, 300, 300, 1, generator=g)}
+    monkeypatch.setattr(bench, "DUMP_BYTES", 1 << 20)
+    monkeypatch.setattr(bench, "DUMP_WHOLE_BYTES", 64 << 10)
+    for d in ("b", "c"):
+        bench.dump_outputs(str(tmp_path / d), [big, big])
+    files = sorted((tmp_path / "b").iterdir())
+    assert [p.name for p in files] == [f"{k}_call{c}.npy" for k in ("depth", "pose_enc", "world_points") for c in (0, 1)]
+    assert sum(p.stat().st_size for p in files) <= 1 << 20
+    assert np.array_equal(np.load(tmp_path / "b" / "pose_enc_call1.npy"), big["pose_enc"].numpy())     # small: whole
+    for p in files:
+        a, b = np.load(p), np.load(tmp_path / "c" / p.name)
+        assert a.dtype == np.float32 and np.array_equal(a, b)                                           # same sample every run
+        if not p.name.startswith("pose_enc"):
+            assert 0 < a.size < big[p.name.rsplit("_", 1)[0]].numel() and np.isin(a, big[p.name.rsplit("_", 1)[0]].numpy()).all()

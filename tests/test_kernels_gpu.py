@@ -29,12 +29,11 @@ def randn(*s, scale=1.0, seed=0, dtype=F32):
 # ----------------------------------------------------------------------------------------------- GEMM
 @pytest.mark.parametrize("M,N,K,bn", [(128, 64, 64, 0), (300, 256, 128, 0), (1000, 384, 192, 128), (2748, 3072, 1024, 256),
                                       (515, 1024, 4096, 128), (77, 96, 392, 64),
-                                      # block_n = 512 selects the CTA-pair (cta_group::2) kernel, 256 x 256 tiles
+                                      # block_n above 128 (the widest tile) runs as 128
                                       (2748, 3072, 1024, 512), (515, 1024, 4096, 512), (300, 256, 128, 512), (129, 512, 64, 512),
                                       (10992, 1024, 1024, 512),
-                                      # > 74 tiles with a short last wave: its tiles run as two 256 x 128 halves
+                                      # many tiles with a short last wave
                                       (5000, 1024, 128, 512), (4000, 1280, 64, 512), (19000, 256, 64, 512),
-                                      # block_n = 384: CTA-pair kernel with 256 x 128 tiles
                                       (2748, 384, 192, 384), (1500, 128, 2048, 384), (300, 256, 128, 384)])
 def test_gemm_bf16_bias_gelu(M, N, K, bn):
     ops = _ops()
@@ -51,7 +50,7 @@ def test_gemm_bf16_bias_gelu(M, N, K, bn):
 
 @pytest.mark.parametrize("M,N,K,bn", [(5000, 1024, 128, 512), (10992, 1024, 256, 512)])
 def test_gemm_resid_split_tail(M, N, K, bn):
-    """Residual epilogue (bulk reduce-add) over a tile count whose last wave is split into half tiles."""
+    """Residual epilogue (fp32 read-modify-write) over a tile count with a short last wave."""
     ops = _ops()
     a = randn(M, K, seed=1, dtype=BF16)
     w = randn(N, K, scale=K ** -0.5, seed=2, dtype=BF16)
@@ -175,7 +174,7 @@ def _sdpa_fp32_chunked(qs, kb, vb, qchunk=4096):
 def test_attention_global_sizes_of_baseline_configs(heads, n):
     """BASELINE.json configs[1] / configs[4]: the global attention of 8 views (L = 10 992, 172 KV steps) and of 24 views
     (L = 32 976, 516 KV steps), 16 heads, against fp32 SDPA (reference layers/attention.py:61-66) -- same 1e-2 bar as the
-    small shapes; the long accumulation (fp32 O / l in TMEM, lazy rescaling) is what is under test."""
+    small shapes; the long accumulation (fp32 O / l in registers, online rescaling) is what is under test."""
     ops = _ops()
     q = randn(1, heads, n, 64, seed=1)
     k = randn(1, heads, n, 64, seed=2)
@@ -246,8 +245,8 @@ def test_attention_peaky_rows_rescale():
 
 @pytest.mark.parametrize("spike_at", [130, 650, 699])
 def test_attention_late_spike_overflow(spike_at):
-    """One key far down the sequence whose logit exceeds everything before it by > 2^128: exp2 against the stale
-    reference overflows, the kernel must redo that step against the new maximum (and keep earlier / later steps exact)."""
+    """One key far down the sequence whose logit exceeds everything before it by > 2^128: exp2 against the previous
+    maximum would overflow, the kernel must rescale O / l to the new maximum (and keep earlier / later steps exact)."""
     ops = _ops()
     batch, heads, n = 1, 2, 700
     q = randn(batch, heads, n, 64, seed=1) * 0.3 + 2.0

@@ -5,7 +5,7 @@ plus size-independent properties at the BASELINE image size.
 
 Tolerance.  The kernels compute with bf16 operands and fp32 accumulation (the reference runs fp32), so the bar is stated
 as relative L2 per output: 2e-2 on the reduced configs / full-width model (measured: <= 1.5e-2, recorded in
-profiles/ and DESIGN.md); pose_enc additionally max-abs 5e-2."""
+DESIGN.md); pose_enc additionally max-abs 5e-2."""
 import json
 import os
 

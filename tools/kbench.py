@@ -35,7 +35,7 @@ KB = os.environ.get("KB", "all")
 S, T, C = int(os.environ.get("S", 8)), 1374, 1024
 M = S * T
 a = torch.randn(M, C, device=dev).to(BF16)
-for name, N, K, bns in () if KB == "attn" else (("qkv", 3072, 1024, (256, 512)), ("proj", 1024, 1024, (384, 512)), ("fc1", 4096, 1024, (256, 512)), ("fc2", 1024, 4096, (384, 512))):
+for name, N, K, bns in () if KB == "attn" else (("qkv", 3072, 1024, (64, 128)), ("proj", 1024, 1024, (64, 128)), ("fc1", 4096, 1024, (64, 128)), ("fc2", 1024, 4096, (64, 128))):
     x = torch.randn(M, K, device=dev).to(BF16)
     w = (torch.randn(N, K, device=dev) * K ** -0.5).to(BF16)
     bias = torch.randn(N, device=dev)
@@ -61,7 +61,7 @@ ones, zeros = torch.ones(64, device=dev), torch.zeros(64, device=dev)
 cos, sin = ops.rope_tables(38, dev)
 q = torch.empty(1, 16, M, 64, device=dev, dtype=BF16)
 k, v = torch.empty_like(q), torch.empty_like(q)
-for bn in (256, 512) if KB != "attn" else (256,):
+for bn in (64, 128) if KB != "attn" else (128,):
     ms = timeit(lambda: ops.qkv_proj(a, w, bias, ones, zeros, ones, zeros, q, k, v, ntok=M, T=T, nspecial=5, wp=37, rope_cos=cos, rope_sin=sin, block_n=bn))
     res[f"gemm_qkv_fused_bn{bn}"] = dict(ms=ms, tflops=2 * M * 3 * C * C / ms / 1e9)
 # DPT-shaped 3x3 conv: 8 frames x 148^2, 256 -> 256
@@ -72,7 +72,7 @@ wc = (torch.randn(256, 9 * 256, device=dev) * (9 * 256) ** -0.5).to(BF16)
 outp = torch.empty_like(xp)
 taps = [(ky - 1) * (ww + 2) + (kx - 1) for ky in range(3) for kx in range(3)]
 bias256 = torch.randn(256, device=dev)
-for bn in (256, 512) if KB != "attn" else ():
+for bn in (64, 128) if KB != "attn" else ():
     ms = timeit(lambda: ops.gemm(xp.reshape(-1, 256), wc, taps=taps, epi=ops.L.EPI_BF16, bias=bias256, act=ops.L.ACT_RELU, out=outp, ldo=256, rowmap=ops.L.ROWS_PAD, gh=hh, gw=ww, block_n=bn), iters=5)
     res[f"conv3x3_148_bn{bn}"] = dict(ms=ms, tflops=2 * Fr * hh * ww * 256 * 256 * 9 / ms / 1e9)
 # attention: global and frame
@@ -89,7 +89,7 @@ if KB != "attn":
     oq = torch.empty(8, 298, 298, 128, device=dev, dtype=BF16)
     tq = [(ky - 1) * 298 + (kx - 1) for ky in range(3) for kx in range(3)]
     b128 = torch.randn(128, device=dev)
-    for bn in (128, 384):
+    for bn in (32, 64, 128):
         ms = timeit(lambda: ops.gemm(xq.reshape(-1, 256), wq, taps=tq, epi=ops.L.EPI_BF16, bias=b128, out=oq, ldo=128, rowmap=ops.L.ROWS_PAD, gh=296, gw=296, block_n=bn), iters=5)
         res[f"conv3x3_296_n128_bn{bn}"] = dict(ms=ms, tflops=2 * 8 * 296 * 296 * 256 * 128 * 9 / ms / 1e9)
     del xq, oq
