@@ -22,7 +22,7 @@ extern "C" {
 #define OVG_E_NODEVICE (-3)
 
 /* Library / device ------------------------------------------------------------------------------------- */
-int ovg_version(void);               /* ABI version, currently 2 */
+int ovg_version(void);               /* ABI version, currently 4 */
 const char* ovg_last_error(void);    /* thread-local message of the last failing call */
 int ovg_device_check(void);          /* OVG_OK iff the current device is sm_90 (H100); OVG_E_NODEVICE otherwise */
 long long ovg_launch_count(void);    /* kernels launched by this library since load (bench.py "gpu_launches") */
@@ -90,20 +90,16 @@ typedef struct ovg_gemm_args {
 int ovg_gemm(const ovg_gemm_args* args, void* stream);
 
 /* Fused attention: out[b, i, h*64:(h+1)*64] = softmax_j(q[b,h,i,:] . k[b,h,j,:]) v[b,h,j,:], q pre-scaled by
- * log2(e)/sqrt(64).  q,k,v: bf16 [batch, heads, n, 64]; out: bf16 [batch, n, heads*64].
- * Replaces F.scaled_dot_product_attention, layers/attention.py:61-66. */
-int ovg_attention(const void* q, const void* k, const void* v, void* out, int batch, int heads, int n, void* stream);
-/* Same with nq query rows and nkv keys / values per (batch, head): q [batch, heads, nq, 64], k, v [batch, heads, nkv, 64],
- * out [batch, nq, heads*64] (context parallelism: a rank's own queries against the keys / values of all ranks). */
-int ovg_attention_kv(const void* q, const void* k, const void* v, void* out, int batch, int heads, int nq, int nkv,
-                     void* stream);
-/* Same with a scratch buffer of ovg_attention_scratch_bytes() bytes (16-byte aligned): for long sequences whose 128-row query tiles
- * do not fill the last wave of resident CTAs (two per SM), the tiles of that wave are cut into 2-4 key ranges, one CTA each, and
- * a small kernel merges their (un-normalised O, softmax reference, row sum) -- e.g. 1 376 tiles on 296 slots: 4.67 instead of 5
- * waves.  Results are deterministic (fixed merge order); scratch NULL = no split. */
+ * log2(e)/sqrt(64).  q: bf16 [batch, heads, nq, 64]; k, v: bf16 [batch, heads, nkv, 64]; out: bf16 [batch, nq, heads*64].
+ * nq == nkv is self-attention; nq < nkv is what a context-parallel rank runs: its own queries against the keys / values of
+ * all ranks.  Replaces F.scaled_dot_product_attention, layers/attention.py:61-66.
+ * scratch: NULL, or ovg_attention_scratch_bytes() bytes (16-byte aligned).  With scratch, for long sequences whose 128-row query
+ * tiles do not fill the last wave of resident CTAs (two per SM), the tiles of that wave are cut into 2-4 key ranges, one CTA each,
+ * and a small kernel merges their (un-normalised O, softmax reference, row sum) -- e.g. 1 376 tiles on 296 slots: 4.67 instead of
+ * 5 waves.  Results are deterministic (fixed merge order); scratch NULL = no split. */
 long long ovg_attention_scratch_bytes(void);
-int ovg_attention_kv_ws(const void* q, const void* k, const void* v, void* out, int batch, int heads, int nq, int nkv,
-                        void* scratch, long long scratch_bytes, void* stream);
+int ovg_attention(const void* q, const void* k, const void* v, void* out, int batch, int heads, int nq, int nkv,
+                  void* scratch, long long scratch_bytes, void* stream);
 
 /* LayerNorm over the last dim, fp32 or bf16 in -> bf16 (out_is_f32 = 0), fp32 (1) or fp16 (2) out, optional affine, optional row gather
  * (out row m <- in row (m / grp_out) * grp_in + grp_off + m % grp_out; grp_out = 0: identity).
@@ -123,15 +119,13 @@ int ovg_inject_snapshot(float* x, const float* inj, void* slot, float* cam_out, 
 
 /* Depth modality: masked per-scene mean over the selected views, then [depth/(mean+1e-8)*mask, mask] im2col rows
  * (2*patch*patch wide, row stride ldc) for the patch-embedding GEMM (omnivggt_aggregator.py:107-128,:189-199;
- * layers/patch_embed.py:65-77).  scratch: OVG_DEPTH_SCRATCH_DOUBLES(B) doubles of device memory. */
+ * layers/patch_embed.py:65-77).  scratch: OVG_DEPTH_SCRATCH_DOUBLES(B) doubles of device memory.
+ * The normalisation mean is taken over the views idx_stats[0..n_stats) (ALL selected views of the scene,
+ * omnivggt_aggregator.py:118-126); rows are produced for the views idx_cols[0..n_cols) only (the same list on one GPU; the views
+ * this rank owns when a scene is sharded over ranks; n_cols may be 0). */
 #define OVG_DEPTH_SCRATCH_DOUBLES(B) ((B) * (2 * 1024 + 1))
-/* Same with separate view lists: the normalisation mean is taken over the views idx_stats[0..n_stats) (ALL selected views of
- * the scene, omnivggt_aggregator.py:118-126), rows are produced for the views idx_cols[0..n_cols) only (the views this rank
- * owns when a scene is sharded over ranks; n_cols may be 0). */
-int ovg_depth_im2col2(const float* depth, const float* mask, const int* idx_stats, int n_stats, const int* idx_cols, int n_cols,
-                      double* scratch, void* cols, int ldc, int B, int S, int H, int W, int patch, void* stream);
-int ovg_depth_im2col(const float* depth, const float* mask, const int* idx, double* scratch, void* cols, int ldc,
-                     int B, int S, int Sd, int H, int W, int patch, void* stream);
+int ovg_depth_im2col(const float* depth, const float* mask, const int* idx_stats, int n_stats, const int* idx_cols, int n_cols,
+                     double* scratch, void* cols, int ldc, int B, int S, int H, int W, int patch, void* stream);
 
 /* RGB patch im2col for the DINOv2 patch embedding (layers/patch_embed.py:65-77, conv k = s = patch): images fp32
  * [K,3,H,W] in [0,1] are normalised with (x - mean[c]) / std[c] (models/omnivggt_aggregator.py:143) and written as bf16
@@ -319,7 +313,7 @@ int ovg_peer_barrier(int* const* flag_peers, int* epoch_counter, int rank, int w
  * Every rank runs the per-token work (LayerNorm, QKV / proj / MLP GEMMs, frame attention) on its own S views; in the global
  * blocks (models/aggregator.py:312-341: one SDPA over all views) the QKV epilogue stores the K / V rows of the rank's tokens
  * straight into every rank's full-length K / V buffer over NVLink (ovg_gemm_args.k_peers), a flag barrier follows, and the
- * rank's own queries attend to all keys (ovg_attention_kv).  No collective library call on the data path; K / V buffers are
+ * rank's own queries attend to all keys (ovg_attention with nq < nkv).  No collective library call on the data path; K / V buffers are
  * double buffered so that one barrier per global block suffices. */
 typedef struct ovg_context_parallel {
   int rank; int world;
@@ -343,7 +337,7 @@ int ovg_aggregator_forward_cp(ovg_aggregator* h, const ovg_context_parallel* cp,
 /* Timing hook for bench.py: when enabled, every global-attention launch of ovg_aggregator_forward is bracketed by CUDA events
  * on its stream; after a synchronize, ovg_runtime_attention_times() returns the elapsed ms of the launches since the enable. */
 void ovg_runtime_time_attention(int enable);
-/* Process-wide switch (default on): the block runtimes hand ovg_attention_kv_ws their scratch, so long sequences may split the
+/* Process-wide switch (default on): the block runtimes hand ovg_attention their scratch, so long sequences may split the
  * tiles of the last CTA wave over the keys.  Off: every tile is computed by one CTA -- the summation order of a tile then does not
  * depend on how many tiles the launch has, which is what makes a context-parallel forward BIT-identical to the single-GPU one
  * (tests/test_cp_gpu.py checks that with the switch off, and agreement within 5e-3 of the dense outputs with it on). */

@@ -97,19 +97,16 @@ EXPORTS = {
     "ovg_device_check": (C.c_int, []),
     "ovg_launch_count": (C.c_longlong, []),
     "ovg_gemm": (C.c_int, [C.POINTER(GemmArgs), _vp]),
-    "ovg_attention": (C.c_int, [_vp, _vp, _vp, _vp, _i, _i, _i, _vp]),
-    "ovg_attention_kv": (C.c_int, [_vp, _vp, _vp, _vp, _i, _i, _i, _i, _vp]),
+    "ovg_attention": (C.c_int, [_vp, _vp, _vp, _vp, _i, _i, _i, _i, _vp, _ll, _vp]),
     "ovg_attention_scratch_bytes": (C.c_longlong, []),
-    "ovg_attention_kv_ws": (C.c_int, [_vp, _vp, _vp, _vp, _i, _i, _i, _i, _vp, _ll, _vp]),
     "ovg_peer_barrier": (C.c_int, [C.POINTER(_vp), _vp, _i, _i, _vp]),
     "ovg_aggregator_forward_cp": (C.c_int, [_vp, C.POINTER(ContextParallelDesc), _vp, _vp, _vp, _vp, _vp, _i, _vp, _i, _vp, _vp, _i,
                                             _i, _i, _i, _vp, _ll, _pp, _vp, _vp]),
-    "ovg_depth_im2col2": (C.c_int, [_vp, _vp, _vp, _i, _vp, _i, _vp, _vp, _i, _i, _i, _i, _i, _i, _vp]),
     "ovg_layernorm": (C.c_int, [_vp, _i, _ll, _vp, _i, _ll, _i, _i, _vp, _vp, _f, _i, _i, _i, _vp]),
     "ovg_image_im2col": (C.c_int, [_vp, _vp, _vp, _vp, _i, _i, _i, _i, _i, _vp]),
     "ovg_assemble_tokens": (C.c_int, [_vp, _vp, _vp, _vp, _vp, _vp, _vp, _i, _i, _i, _i, _i, _i, _vp]),
     "ovg_inject_snapshot": (C.c_int, [_vp, _vp, _vp, _vp, _i, _i, _i, _i, _vp]),
-    "ovg_depth_im2col": (C.c_int, [_vp, _vp, _vp, _vp, _vp, _i, _i, _i, _i, _i, _i, _i, _vp]),
+    "ovg_depth_im2col": (C.c_int, [_vp, _vp, _vp, _i, _vp, _i, _vp, _vp, _i, _i, _i, _i, _i, _i, _vp]),
     "ovg_im2col3x3s2": (C.c_int, [_vp, _vp, _i, _i, _i, _i, _vp]),
     "ovg_dpt_tail_supported": (C.c_int, [_i, _i, _i, _i, _i]),
     "ovg_dpt_tail_scratch_bytes": (C.c_longlong, [_i, _i]),

@@ -133,18 +133,25 @@ struct PerDeviceOnce {
   void mark_done() { done[current_device()].store(true, std::memory_order_release); }
 };
 
+// Lets Kernel launch with `bytes` of dynamic shared memory (more than the 48 KB default); set once per device.
+template <auto Kernel>
+int allow_dynamic_smem(int bytes) {
+  static PerDeviceOnce once;
+  if (once.needed()) {
+    OVG_CUDA(cudaFuncSetAttribute(Kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, bytes));
+    once.mark_done();
+  }
+  return OVG_OK;
+}
+
 template <int BN, int EPI>
 int launch_gemm(const CUtensorMap& ta, const CUtensorMap& tb, const ovg::GemmParams& p, cudaStream_t st) {
   using Cfg = ovg::GemmCfg<BN>;
-  static PerDeviceOnce once;
-  auto kern = ovg::gemm_kernel<BN, EPI>;
-  if (once.needed()) {
-    OVG_CUDA(cudaFuncSetAttribute(kern, cudaFuncAttributeMaxDynamicSharedMemorySize, Cfg::SMEM_BYTES));
-    once.mark_done();
-  }
+  const int rc = allow_dynamic_smem<ovg::gemm_kernel<BN, EPI>>(Cfg::SMEM_BYTES);
+  if (rc) return rc;
   const int tiles = ((p.M + 127) / 128) * ((p.N + BN - 1) / BN);
   const int grid = tiles < num_sms() ? tiles : num_sms();
-  kern<<<grid, ovg::GEMM_THREADS, Cfg::SMEM_BYTES, st>>>(ta, tb, p);
+  ovg::gemm_kernel<BN, EPI><<<grid, ovg::GEMM_THREADS, Cfg::SMEM_BYTES, st>>>(ta, tb, p);
   return post_launch("ovg_gemm");
 }
 
@@ -162,7 +169,7 @@ int dispatch_bn(int bn, const CUtensorMap& ta, const CUtensorMap& tb, const ovg:
 
 extern "C" {
 
-int ovg_version(void) { return 3; }
+int ovg_version(void) { return 4; }
 const char* ovg_last_error(void) { return g_err.c_str(); }
 long long ovg_launch_count(void) { return g_launches.load(); }
 
@@ -297,11 +304,8 @@ int ovg_gemm(const ovg_gemm_args* a, void* stream) {
       CUtensorMap ta136;
       rc = get_map(a->a, a->a_cols, a->a_rows, 0, a->lda, ovg::HT_A_ROWS, &ta136);
       if (rc) return rc;
-      static PerDeviceOnce once;
-      if (once.needed()) {
-        OVG_CUDA(cudaFuncSetAttribute(ovg::headtail_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, ovg::HT_SMEM_BYTES));
-        once.mark_done();
-      }
+      rc = allow_dynamic_smem<ovg::headtail_kernel>(ovg::HT_SMEM_BYTES);
+      if (rc) return rc;
       const int tiles = (p.M + ovg::GEMM_BM - 1) / ovg::GEMM_BM;
       const int grid = tiles < num_sms() ? tiles : num_sms();
       ovg::headtail_kernel<<<grid, ovg::GEMM_THREADS, ovg::HT_SMEM_BYTES, st>>>(ta136, tb, p);
@@ -313,8 +317,8 @@ int ovg_gemm(const ovg_gemm_args* a, void* stream) {
 
 long long ovg_attention_scratch_bytes(void) { return 4LL * num_sms() * 128 * (64 * 4 + 8) + 256; }   // <= 4 parts of < one wave of tiles
 
-int ovg_attention_kv_ws(const void* q, const void* k, const void* v, void* out, int batch, int heads, int nq, int nkv,
-                        void* scratch, long long scratch_bytes, void* stream) {
+int ovg_attention(const void* q, const void* k, const void* v, void* out, int batch, int heads, int nq, int nkv,
+                  void* scratch, long long scratch_bytes, void* stream) {
   OVG_REQUIRE(q && k && v && out, "null operand");
   OVG_REQUIRE(batch > 0 && heads > 0 && nq > 0 && nkv > 0, "empty problem");
   cudaStream_t st = reinterpret_cast<cudaStream_t>(stream);
@@ -326,33 +330,24 @@ int ovg_attention_kv_ws(const void* q, const void* k, const void* v, void* out, 
   if (rc) return rc;
   rc = get_map(v, 64, nkv, bh, 64, 128, &tv);
   if (rc) return rc;
-  static PerDeviceOnce once;
-  if (once.needed()) {
-    OVG_CUDA(cudaFuncSetAttribute(ovg::attn1_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, ovg::ATT1_SMEM_BYTES));
-    once.mark_done();
-  }
+  rc = allow_dynamic_smem<ovg::attn1_kernel>(ovg::ATT1_SMEM_BYTES);
+  if (rc) return rc;
   const int q_tiles = (nq + 127) / 128;
   const long long tiles = static_cast<long long>(q_tiles) * heads * batch;
   OVG_REQUIRE(tiles < (1LL << 28), "too many tiles");
   ovg::AttnParams p{nq, nkv, heads, heads * 64, reinterpret_cast<__nv_bfloat16*>(out), q_tiles, static_cast<int>(tiles),
                     static_cast<int>(tiles), 1, nullptr, nullptr};
-#ifndef OVG_ATT_PERSISTENT
-#define OVG_ATT_PERSISTENT 1    // 0: always one CTA per work item (A/B builds)
-#endif
-#ifndef OVG_ATT_SPLIT_TAIL
-#define OVG_ATT_SPLIT_TAIL 1    // 0: never split the tiles of the last wave over the keys (A/B builds)
-#endif
   // Short sequences (frame / DINOv2 attention: 11 KV tiles per item): one resident CTA per SM walks the items, so barrier
   // set-up is paid once and the next item's Q, K, V stream in under the current item's tail.  Long sequences keep one CTA
   // per item: the hardware's dynamic CTA placement balances the partial waves of the global attention.
   const int resident = num_sms();
   const int kv_tiles = (nkv + 127) / 128;
-  const bool persistent = OVG_ATT_PERSISTENT && tiles > resident && kv_tiles <= 16;
+  const bool persistent = tiles > resident && kv_tiles <= 16;
   // Long sequences: the tiles of the last, partly empty wave are cut into 2-4 KV ranges (one CTA each, issued after the whole
   // tiles) whose partial (O, reference, row sum) a small kernel merges.
   int parts = 1;
   const int tail = static_cast<int>(tiles % resident);
-  if (OVG_ATT_SPLIT_TAIL && !persistent && scratch && tiles > resident && tail > 0 && kv_tiles >= 24) {
+  if (!persistent && scratch && tiles > resident && tail > 0 && kv_tiles >= 24) {
     double best = 1.0;
     for (int c = 2; c <= 4; ++c) {
       const double cost = static_cast<double>((static_cast<long long>(tail) * c + resident - 1) / resident) / c + 0.04;   // + merge
@@ -381,15 +376,6 @@ int ovg_attention_kv_ws(const void* q, const void* k, const void* v, void* out, 
   return post_launch("ovg_attention(merge)");
 }
 
-int ovg_attention_kv(const void* q, const void* k, const void* v, void* out, int batch, int heads, int nq, int nkv,
-                     void* stream) {
-  return ovg_attention_kv_ws(q, k, v, out, batch, heads, nq, nkv, nullptr, 0, stream);
-}
-
-int ovg_attention(const void* q, const void* k, const void* v, void* out, int batch, int heads, int n, void* stream) {
-  return ovg_attention_kv(q, k, v, out, batch, heads, n, n, stream);
-}
-
 int ovg_layernorm(const void* in, int in_is_bf16, long long ld_in, void* out, int out_is_f32, long long ld_out, int rows,
                   int C, const float* w, const float* b, float eps, int grp_out, int grp_in, int grp_off, void* stream) {
   OVG_REQUIRE(in && out && rows > 0, "null operand");
@@ -400,10 +386,7 @@ int ovg_layernorm(const void* in, int in_is_bf16, long long ld_in, void* out, in
   ovg::LnParams p{in, in_is_bf16, ld_in, out, out_is_f32, ld_out, rows, C, w, b, eps,
                   grp_out, grp_in, grp_off};
   constexpr int ln_threads = 256;     // 8 rows per block
-#ifndef OVG_LN_PERSIST
-#define OVG_LN_PERSIST 2
-#endif
-  constexpr int ln_persist = OVG_LN_PERSIST;       // persistent grid: blocks per SM
+  constexpr int ln_persist = 2;       // persistent grid: blocks per SM
   OVG_REQUIRE((reinterpret_cast<uintptr_t>(w) & 15) == 0 && (reinterpret_cast<uintptr_t>(b) & 15) == 0, "w / b must be 16-byte aligned");
   const int rpb = ln_threads / 32;
   int blocks = (rows + rpb - 1) / rpb;
@@ -453,8 +436,8 @@ int ovg_inject_snapshot(float* x, const float* inj, void* slot, float* cam_out, 
   return post_launch("ovg_inject_snapshot");
 }
 
-int ovg_depth_im2col2(const float* depth, const float* mask, const int* idx_stats, int n_stats, const int* idx_cols, int n_cols,
-                      double* scratch, void* cols, int ldc, int B, int S, int H, int W, int patch, void* stream) {
+int ovg_depth_im2col(const float* depth, const float* mask, const int* idx_stats, int n_stats, const int* idx_cols, int n_cols,
+                     double* scratch, void* cols, int ldc, int B, int S, int H, int W, int patch, void* stream) {
   OVG_REQUIRE(depth && mask && idx_stats && scratch && (n_cols == 0 || (idx_cols && cols)), "null operand");
   OVG_REQUIRE(B > 0 && n_stats > 0 && n_stats <= S && n_cols >= 0 && n_cols <= S && H % patch == 0 && W % patch == 0 &&
                   patch % 2 == 0, "bad geometry");
@@ -475,12 +458,6 @@ int ovg_depth_im2col2(const float* depth, const float* mask, const int* idx_stat
   if (patch == 14) ovg::depth_im2col_kernel<14><<<B * n_cols * (H / patch), 256, 0, st>>>(pc);
   else ovg::depth_im2col_kernel<0><<<B * n_cols * (H / patch), 256, 0, st>>>(pc);
   return post_launch("ovg_depth_im2col");
-}
-
-int ovg_depth_im2col(const float* depth, const float* mask, const int* idx, double* scratch, void* cols, int ldc,
-                     int B, int S, int Sd, int H, int W, int patch, void* stream) {
-  OVG_REQUIRE(Sd > 0, "bad geometry");
-  return ovg_depth_im2col2(depth, mask, idx, Sd, idx, Sd, scratch, cols, ldc, B, S, H, W, patch, stream);
 }
 
 int ovg_image_im2col(const float* images, const float* mean3, const float* std3, void* cols, int ldc, int K, int H, int W,
@@ -578,12 +555,9 @@ int ovg_dpt_tail(const void* src, const float* tx, const float* ty, const void* 
   if (p.seg_rows < 8 && H >= 8) p.seg_rows = 8;
   p.n_segs = (H + p.seg_rows - 1) / p.seg_rows;
   p.n_items = F * p.n_strips * p.n_segs;
-  static PerDeviceOnce once;
-  if (once.needed()) {
-    OVG_CUDA(cudaFuncSetAttribute(ovg::fusedtail_kernel<true>, cudaFuncAttributeMaxDynamicSharedMemorySize, ovg::FT_SMEM_BYTES));
-    OVG_CUDA(cudaFuncSetAttribute(ovg::fusedtail_kernel<false>, cudaFuncAttributeMaxDynamicSharedMemorySize, ovg::FT_SMEM_BYTES));
-    once.mark_done();
-  }
+  rc = p.f16 ? allow_dynamic_smem<ovg::fusedtail_kernel<true>>(ovg::FT_SMEM_BYTES)
+             : allow_dynamic_smem<ovg::fusedtail_kernel<false>>(ovg::FT_SMEM_BYTES);
+  if (rc) return rc;
   const int grid = p.n_items < sms ? p.n_items : sms;
   if (p.f16) ovg::fusedtail_kernel<true><<<grid, ovg::FT_THREADS, ovg::FT_SMEM_BYTES, st>>>(tb, p);
   else ovg::fusedtail_kernel<false><<<grid, ovg::FT_THREADS, ovg::FT_SMEM_BYTES, st>>>(tb, p);

@@ -89,31 +89,20 @@ def qkv_proj(a, w, bias, qn_w, qn_b, kn_w, kn_b, q, k, v, *, ntok, T, nspecial=0
          qscale=(1.0 / math.sqrt(64.0)) * math.log2(math.e), block_n=block_n)
 
 
-def attention(q, k, v, out, batch: int, heads: int, n: int, scratch=None):
-    """scratch: uint8 buffer of ovg_attention_scratch_bytes() -> long sequences may split the tiles of the last CTA wave over the keys."""
+def attention(q, k, v, out, batch: int, heads: int, nq: int, nkv: Optional[int] = None, scratch=None):
+    """q [batch, heads, nq, 64] against k, v [batch, heads, nkv, 64] (nkv defaults to nq) -> out [batch, nq, heads*64].
+    scratch: uint8 buffer of ovg_attention_scratch_bytes() -> long sequences may split the tiles of the last CTA wave over the keys."""
     for t, nm in ((q, "q"), (k, "k"), (v, "v"), (out, "out")):
         _chk(t, BF16, nm)
         assert t.is_contiguous()
-    if scratch is None:
-        L.check(L.lib().ovg_attention(q.data_ptr(), k.data_ptr(), v.data_ptr(), out.data_ptr(), batch, heads, n, L.stream()))
-    else:
-        L.check(L.lib().ovg_attention_kv_ws(q.data_ptr(), k.data_ptr(), v.data_ptr(), out.data_ptr(), batch, heads, n, n,
-                                            scratch.data_ptr(), scratch.numel(), L.stream()))
+    L.check(L.lib().ovg_attention(q.data_ptr(), k.data_ptr(), v.data_ptr(), out.data_ptr(), batch, heads, nq,
+                                  nq if nkv is None else nkv, L.ptr(scratch), 0 if scratch is None else scratch.numel(),
+                                  L.stream()))
     return out
 
 
 def attention_scratch(device):
     return torch.empty(L.lib().ovg_attention_scratch_bytes(), device=device, dtype=torch.uint8)
-
-
-def attention_kv(q, k, v, out, batch: int, heads: int, nq: int, nkv: int, scratch=None):
-    """q [batch, heads, nq, 64] against k, v [batch, heads, nkv, 64] -> out [batch, nq, heads*64]."""
-    for t, nm in ((q, "q"), (k, "k"), (v, "v"), (out, "out")):
-        _chk(t, BF16, nm)
-        assert t.is_contiguous()
-    L.check(L.lib().ovg_attention_kv_ws(q.data_ptr(), k.data_ptr(), v.data_ptr(), out.data_ptr(), batch, heads, nq, nkv,
-                                        L.ptr(scratch), 0 if scratch is None else scratch.numel(), L.stream()))
-    return out
 
 
 def layernorm(x, out, w=None, b=None, eps=1e-5, rows=None, grp_out=0, grp_in=0, grp_off=0):
@@ -139,8 +128,9 @@ def inject_snapshot(x, inj, slot, cam_out, K, T, C, coff):
 
 
 def depth_im2col(depth, mask, idx, scratch, cols, B, S, Sd, H, W, patch):
-    L.check(L.lib().ovg_depth_im2col(depth.data_ptr(), mask.data_ptr(), idx.data_ptr(), scratch.data_ptr(),
-                                     cols.data_ptr(), cols.stride(0), B, S, Sd, H, W, patch, L.stream()))
+    """Normalisation mean and im2col rows over the same Sd views idx."""
+    L.check(L.lib().ovg_depth_im2col(depth.data_ptr(), mask.data_ptr(), idx.data_ptr(), Sd, idx.data_ptr(), Sd,
+                                     scratch.data_ptr(), cols.data_ptr(), cols.stride(0), B, S, H, W, patch, L.stream()))
 
 
 def image_im2col(images, mean3, std3, cols, K, H, W, patch):

@@ -30,7 +30,7 @@ def mini_model(variant="mini_conv"):
     return OmniVGGT(**kw)
 
 
-def test_library_exports_every_declared_symbol():
+def test_library_exports_every_declared_symbol_and_abi_version():
     from omnivggt_official_b200 import _lib
     lib = _lib.load()
     hdr = open(os.path.join(ROOT, "include", "ovg.h")).read()
@@ -39,7 +39,7 @@ def test_library_exports_every_declared_symbol():
     for name in declared:
         assert hasattr(lib, name), f"{name} declared in include/ovg.h but not exported by libovg.so"
     assert declared == set(_lib.EXPORTS), declared ^ set(_lib.EXPORTS)
-    assert lib.ovg_version() == 3
+    assert lib.ovg_version() == 4
 
 
 def test_ctypes_struct_matches_header():

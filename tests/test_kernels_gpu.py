@@ -194,7 +194,7 @@ def test_attention_global_sizes_of_baseline_configs(heads, n):
     ops.attention(qs, kb, vb, out2, 1, heads, n)
     torch.cuda.synchronize()
     assert torch.equal(out, out2)          # run-to-run bit-identical (no atomics, no ordering races)
-    # with scratch the tiles of the last CTA wave are split over the keys and merged (ovg_attention_kv_ws): same bar, deterministic
+    # with scratch the tiles of the last CTA wave are split over the keys and merged (ovg_attention scratch): same bar, deterministic
     scratch = ops.attention_scratch("cuda")
     out3, out4 = torch.zeros_like(out), torch.zeros_like(out)
     ops.attention(qs, kb, vb, out3, 1, heads, n, scratch=scratch)
@@ -613,9 +613,9 @@ def test_c_host_drives_the_runtime(tmp_path):
 
 
 # ----------------------------------------------------------------------------------------------- context-parallel pieces (one GPU)
-def test_attention_kv_own_queries_against_all_keys():
-    """ovg_attention_kv: a window of the query rows against ALL keys equals the same rows of the full self-attention bit for bit
-    (what a rank of the context-parallel global block computes)."""
+def test_attention_own_queries_against_all_keys():
+    """ovg_attention with nq < nkv: a window of the query rows against ALL keys equals the same rows of the full self-attention bit
+    for bit (what a rank of the context-parallel global block computes)."""
     ops = _ops()
     heads, n, lo, hi = 4, 1374 * 2, 1374, 1374 + 700
     q = randn(1, heads, n, 64, seed=1, dtype=BF16) * 0.18
@@ -624,7 +624,7 @@ def test_attention_kv_own_queries_against_all_keys():
     full = torch.zeros(1, n, heads * 64, device="cuda", dtype=BF16)
     ops.attention(q, k, v, full, 1, heads, n)
     part = torch.zeros(1, hi - lo, heads * 64, device="cuda", dtype=BF16)
-    ops.attention_kv(q[:, :, lo:hi].contiguous(), k, v, part, 1, heads, hi - lo, n)
+    ops.attention(q[:, :, lo:hi].contiguous(), k, v, part, 1, heads, hi - lo, n)
     torch.cuda.synchronize()
     assert torch.equal(part, full[:, lo:hi])
     # the shape a rank of a 2-GPU context-parallel forward runs (half of the query rows of 8 views against all keys): 688 tiles,
@@ -635,8 +635,8 @@ def test_attention_kv_own_queries_against_all_keys():
     v = randn(1, heads, n, 64, seed=6, dtype=BF16)
     plain = torch.zeros(1, n // 2, heads * 64, device="cuda", dtype=BF16)
     split = torch.zeros_like(plain)
-    ops.attention_kv(q, k, v, plain, 1, heads, n // 2, n)
-    ops.attention_kv(q, k, v, split, 1, heads, n // 2, n, scratch=ops.attention_scratch("cuda"))
+    ops.attention(q, k, v, plain, 1, heads, n // 2, n)
+    ops.attention(q, k, v, split, 1, heads, n // 2, n, scratch=ops.attention_scratch("cuda"))
     torch.cuda.synchronize()
     assert not torch.equal(plain, split) and rel(split, plain) < 4e-3
 

@@ -36,7 +36,7 @@ def timeit(fn, iters=7, warm=2):
 res = {"tag": sys.argv[1] if len(sys.argv) > 1 else "", "lib": os.environ.get("OVG_LIB_PATH", "libovg.so"),
        "split_tail": os.environ.get("ATTN_SPLIT", "1") != "0"}
 shapes = {"global8": (1, 16, 8 * 1374), "frame8": (8, 16, 1374), "global24": (1, 16, 24 * 1374), "global4": (1, 16, 4 * 1374)}
-scratch = ops.attention_scratch("cuda") if os.environ.get("ATTN_SPLIT", "1") != "0" else None     # KV-split tail tiles (ovg_attention_kv_ws)
+scratch = ops.attention_scratch("cuda") if os.environ.get("ATTN_SPLIT", "1") != "0" else None     # KV-split tail tiles (ovg_attention scratch)
 if os.environ.get("ATTN_SHAPES"):
     shapes = {k: shapes[k] for k in os.environ["ATTN_SHAPES"].split(",")}
 for name, (b, h, n) in shapes.items():
