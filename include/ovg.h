@@ -196,6 +196,34 @@ int ovg_unproject_depth(const float* depth, const float* intrinsic, const float*
 int ovg_conf_percentile_mask(const float* conf, long long n, float percent, float floor_, void* workspace,
                              unsigned char* mask, float* threshold_out, unsigned long long* count_out, void* stream);
 
+/* Point cloud: the filtering and compaction of visual_util.py:190-236 (predictions_to_glb) and inference.py:96-151 (viewer).
+ * Pixels are numbered (frame, row, column), numpy's boolean-indexing order; every result is deterministic (no atomics decide
+ * a position or a sum).  One workspace of ovg_point_cloud_workspace_bytes(F*H*W) bytes (16-byte aligned) serves all four calls
+ * of one cloud; run them in the order below on one stream.
+ * ovg_point_cloud_count: keep[i] = conf_mask[i] (from ovg_conf_percentile_mask over the same pixels)
+ *     && (!mask_black_bg || r + g + b >= 16) && (!mask_white_bg || !(r > 240 && g > 240 && b > 240)), with the colours
+ *     uint8(trunc(x * 255)) of images fp32 [F,3,H,W] (visual_util.py:202,:211-221); count_out: device u64, the number of kept
+ *     pixels.  Reading it back to size the outputs is the one host synchronisation of a cloud. */
+long long ovg_point_cloud_workspace_bytes(long long n);
+int ovg_point_cloud_count(const unsigned char* conf_mask, const float* images, int F, int H, int W, int mask_black_bg,
+                          int mask_white_bg, void* workspace, long long workspace_bytes, unsigned long long* count_out,
+                          void* stream);
+/* ovg_point_cloud_gather: the kept pixels in order (visual_util.py:223-224): points fp32 [F,H,W,3] -> points_out [n_kept,3],
+ * colors_out uint8 [n_kept,3], frame_out int32 [n_kept] = frame0 + frame, and xyz fp32 [3, ld] (ld >= n_kept, ld % 4 == 0,
+ * 16-byte aligned) = the same points as x / y / z columns for ovg_point_cloud_scale.  Same conf_mask, images, sizes, flags and
+ * workspace as the count. */
+int ovg_point_cloud_gather(const float* points, const unsigned char* conf_mask, const float* images, int F, int H, int W,
+                           int mask_black_bg, int mask_white_bg, int frame0, const void* workspace, long long workspace_bytes,
+                           float* points_out, unsigned char* colors_out, int* frame_out, float* xyz, long long ld,
+                           void* stream);
+/* ovg_point_cloud_center: center_out fp32 [3] = mean of points fp32 [n,3] (inference.py:111), fp64 sums in a fixed order. */
+int ovg_point_cloud_center(const float* points, long long n, void* workspace, long long workspace_bytes, float* center_out,
+                           void* stream);
+/* ovg_point_cloud_scale: scale_out fp32 = || percentile(p, 95) - percentile(p, 5) || per axis over the n_kept columns of xyz
+ * (visual_util.py:231-236), by the exact selection of ovg_conf_percentile_mask.  n_kept >= 1. */
+int ovg_point_cloud_scale(const float* xyz, long long n_kept, long long ld, void* workspace, long long workspace_bytes,
+                          float* scale_out, void* stream);
+
 /* ======================================================================================================================
  * Runtime: the launch SEQUENCES of the hot path behind handles, so that a host in any language runs the path with three
  * calls and raw device pointers (SURVEY.md section 8b).  Weight pointers refer to device memory in kernel layout (bf16

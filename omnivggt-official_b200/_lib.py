@@ -118,6 +118,11 @@ EXPORTS = {
     "ovg_pose_decode": (C.c_int, [_vp, _vp, _vp, _vp, _i, _i, _i, _vp]),
     "ovg_unproject_depth": (C.c_int, [_vp, _vp, _vp, _vp, _i, _i, _i, _vp]),
     "ovg_conf_percentile_mask": (C.c_int, [_vp, _ll, _f, _f, _vp, _vp, _vp, _vp, _vp]),
+    "ovg_point_cloud_workspace_bytes": (_ll, [_ll]),
+    "ovg_point_cloud_count": (C.c_int, [_vp, _vp, _i, _i, _i, _i, _i, _vp, _ll, _vp, _vp]),
+    "ovg_point_cloud_gather": (C.c_int, [_vp, _vp, _vp, _i, _i, _i, _i, _i, _i, _vp, _ll, _vp, _vp, _vp, _vp, _ll, _vp]),
+    "ovg_point_cloud_center": (C.c_int, [_vp, _ll, _vp, _ll, _vp, _vp]),
+    "ovg_point_cloud_scale": (C.c_int, [_vp, _ll, _ll, _vp, _ll, _vp, _vp]),
     # ---- runtime (handle-level sequences)
     "ovg_aggregator_create": (C.c_int, [C.POINTER(AggregatorDesc), _pp]),
     "ovg_aggregator_destroy": (None, [_vp]),

@@ -624,6 +624,78 @@ int ovg_unproject_depth(const float* depth, const float* intrinsic, const float*
   return post_launch("ovg_unproject_depth");
 }
 
+}  // extern "C"
+
+namespace {
+
+// Grid of the selection histograms and of the mask pass: one float4 per thread, at most 4 blocks per SM (grid-stride).
+int select_blocks(long long n) {
+  long long blocks = (n / 4 + 255) / 256;
+  if (blocks > num_sms() * 4) blocks = num_sms() * 4;
+  return blocks < 1 ? 1 : static_cast<int>(blocks);
+}
+
+// numpy.percentile(v[0, n), percent) (method "linear", exact) by radix select: one init launch, then 4 x (histogram, decide).
+// workspace: OVG_PERCENTILE_WORKSPACE_BYTES (6 x u64 state | 512 x u32 histograms | ...); out3: device float[3] = the two
+// neighbouring order statistics and the interpolated percentile.  count (optional) is zeroed by the init launch.
+int radix_percentile(const float* v, long long n, float percent, void* workspace, float* out3, unsigned long long* count,
+                     const std::string& what, cudaStream_t st) {
+  // virtual index p/100 * (n - 1), linear interpolation between its two neighbours
+  const double vi = static_cast<double>(percent) / 100.0 * static_cast<double>(n - 1);
+  const unsigned long long r0 = static_cast<unsigned long long>(vi);
+  const unsigned long long r1 = r0 + 1 < static_cast<unsigned long long>(n) ? r0 + 1 : r0;
+  const double frac = vi - static_cast<double>(r0);
+  unsigned long long* state = reinterpret_cast<unsigned long long*>(workspace);
+  unsigned int* hist = reinterpret_cast<unsigned int*>(state + 6);
+  ovg::select_init_kernel<<<1, 128, 0, st>>>(state, hist, r0, r1, count);
+  int rc = post_launch((what + "(init)").c_str());
+  if (rc) return rc;
+  const int blocks = select_blocks(n);
+  for (int pass = 0; pass < 4; ++pass) {
+    ovg::SelectParams sp{v, n, state, hist, pass, out3, static_cast<float>(frac)};
+    ovg::select_hist_kernel<<<blocks, 256, 0, st>>>(sp);
+    rc = post_launch((what + "(hist)").c_str());
+    if (rc) return rc;
+    ovg::select_decide_kernel<<<1, 32, 0, st>>>(sp);
+    rc = post_launch((what + "(decide)").c_str());
+    if (rc) return rc;
+  }
+  return OVG_OK;
+}
+
+// Point-cloud workspace, carved the same way by the size query and by every entry point.
+struct CloudWorkspace {
+  void* select;                      // OVG_PERCENTILE_WORKSPACE_BYTES
+  float* sel;                        // [6][3] selection results of the scale
+  double* center_partial;            // [CLOUD_CENTER_BLOCKS][3]
+  unsigned int* tile_count;          // [tiles]
+  unsigned long long* tile_offset;   // [tiles]
+  long long bytes;
+};
+
+CloudWorkspace cloud_workspace(void* base, long long n) {
+  const long long tiles = (n + ovg::CLOUD_TILE - 1) / ovg::CLOUD_TILE;
+  char* p = static_cast<char*>(base);
+  long long off = 0;
+  auto carve = [&](long long bytes) {
+    char* r = p ? p + off : nullptr;
+    off += (bytes + 255) / 256 * 256;
+    return r;
+  };
+  CloudWorkspace w;
+  w.select = carve(OVG_PERCENTILE_WORKSPACE_BYTES);
+  w.sel = reinterpret_cast<float*>(carve(18 * sizeof(float)));
+  w.center_partial = reinterpret_cast<double*>(carve(3LL * ovg::CLOUD_CENTER_BLOCKS * sizeof(double)));
+  w.tile_count = reinterpret_cast<unsigned int*>(carve(tiles * 4));
+  w.tile_offset = reinterpret_cast<unsigned long long*>(carve(tiles * 8));
+  w.bytes = off;
+  return w;
+}
+
+}  // namespace
+
+extern "C" {
+
 int ovg_conf_percentile_mask(const float* conf, long long n, float percent, float floor_, void* workspace,
                              unsigned char* mask, float* threshold_out, unsigned long long* count_out, void* stream) {
   OVG_REQUIRE(conf && workspace && mask && threshold_out && n > 0, "bad arguments");
@@ -632,36 +704,107 @@ int ovg_conf_percentile_mask(const float* conf, long long n, float percent, floa
                   (reinterpret_cast<uintptr_t>(workspace) & 15) == 0,
               "conf must be 16-byte, mask 4-byte, workspace 16-byte aligned");
   cudaStream_t st = reinterpret_cast<cudaStream_t>(stream);
-  // numpy.percentile(method="linear"): virtual index p/100 * (n - 1), linear interpolation between its two neighbours
-  const double vi = static_cast<double>(percent) / 100.0 * static_cast<double>(n - 1);
-  const unsigned long long r0 = static_cast<unsigned long long>(vi);
-  const unsigned long long r1 = r0 + 1 < static_cast<unsigned long long>(n) ? r0 + 1 : r0;
-  const double frac = vi - static_cast<double>(r0);
   // workspace: 6 x u64 state | 512 x u32 histograms | 3 x f32 results       (OVG_PERCENTILE_WORKSPACE_BYTES)
-  unsigned long long* state = reinterpret_cast<unsigned long long*>(workspace);
-  unsigned int* hist = reinterpret_cast<unsigned int*>(state + 6);
-  float* res = reinterpret_cast<float*>(hist + 512);
-  ovg::select_init_kernel<<<1, 128, 0, st>>>(state, hist, r0, r1, count_out);
-  {
-    int rc = post_launch("ovg_conf_percentile_mask(init)");
-    if (rc) return rc;
-  }
-  int blocks = static_cast<int>((n / 4 + 255) / 256);
-  if (blocks > num_sms() * 4) blocks = num_sms() * 4;
-  if (blocks < 1) blocks = 1;
-  for (int pass = 0; pass < 4; ++pass) {
-    ovg::SelectParams sp{conf, n, state, hist, pass, res, static_cast<float>(frac)};
-    ovg::select_hist_kernel<<<blocks, 256, 0, st>>>(sp);
-    int rc = post_launch("ovg_conf_percentile_mask(hist)");
-    if (rc) return rc;
-    ovg::select_decide_kernel<<<1, 32, 0, st>>>(sp);
-    rc = post_launch("ovg_conf_percentile_mask(decide)");
-    if (rc) return rc;
-  }
+  float* res = reinterpret_cast<float*>(reinterpret_cast<unsigned int*>(reinterpret_cast<unsigned long long*>(workspace) + 6) + 512);
+  int rc = radix_percentile(conf, n, percent, workspace, res, count_out, "ovg_conf_percentile_mask", st);
+  if (rc) return rc;
+  const int blocks = select_blocks(n);
   OVG_CUDA(cudaMemcpyAsync(threshold_out, res + 2, sizeof(float), cudaMemcpyDeviceToDevice, st));
   ovg::ConfMaskParams mp{conf, res + 2, mask, n, floor_, count_out};
   ovg::conf_mask_kernel<<<blocks, 256, 0, st>>>(mp);
   return post_launch("ovg_conf_percentile_mask");
+}
+
+long long ovg_point_cloud_workspace_bytes(long long n) { return n > 0 ? cloud_workspace(nullptr, n).bytes : -1; }
+
+}  // extern "C"
+
+namespace {
+
+int cloud_params(const unsigned char* conf_mask, const float* images, int F, int H, int W, int mask_black_bg, int mask_white_bg,
+                 void* workspace, long long workspace_bytes, ovg::CloudParams* p) {
+  OVG_REQUIRE(conf_mask && images && workspace && F > 0 && H > 0 && W > 0, "bad arguments");
+  const long long n = static_cast<long long>(F) * H * W;
+  const CloudWorkspace w = cloud_workspace(workspace, n);
+  OVG_REQUIRE((reinterpret_cast<uintptr_t>(workspace) & 15) == 0 && workspace_bytes >= w.bytes,
+              "workspace must be 16-byte aligned and ovg_point_cloud_workspace_bytes(F*H*W) long");
+  OVG_REQUIRE((n + ovg::CLOUD_TILE - 1) / ovg::CLOUD_TILE < (1LL << 31), "too many pixels");
+  *p = ovg::CloudParams{};
+  p->conf_mask = conf_mask; p->images = images; p->n = n; p->hw = static_cast<long long>(H) * W;
+  p->black_bg = mask_black_bg ? 1 : 0; p->white_bg = mask_white_bg ? 1 : 0;
+  p->tile_count = w.tile_count; p->tile_offset = w.tile_offset;
+  p->tiles = static_cast<int>((n + ovg::CLOUD_TILE - 1) / ovg::CLOUD_TILE);
+  return OVG_OK;
+}
+
+}  // namespace
+
+extern "C" {
+
+int ovg_point_cloud_count(const unsigned char* conf_mask, const float* images, int F, int H, int W, int mask_black_bg,
+                          int mask_white_bg, void* workspace, long long workspace_bytes, unsigned long long* count_out,
+                          void* stream) {
+  OVG_REQUIRE(count_out, "null count_out");
+  ovg::CloudParams p;
+  int rc = cloud_params(conf_mask, images, F, H, W, mask_black_bg, mask_white_bg, workspace, workspace_bytes, &p);
+  if (rc) return rc;
+  p.total = count_out;
+  cudaStream_t st = reinterpret_cast<cudaStream_t>(stream);
+  ovg::cloud_count_kernel<<<p.tiles, ovg::CLOUD_THREADS, 0, st>>>(p);
+  rc = post_launch("ovg_point_cloud_count");
+  if (rc) return rc;
+  ovg::cloud_scan_kernel<<<1, 1024, 0, st>>>(p);
+  return post_launch("ovg_point_cloud_count(scan)");
+}
+
+int ovg_point_cloud_gather(const float* points, const unsigned char* conf_mask, const float* images, int F, int H, int W,
+                           int mask_black_bg, int mask_white_bg, int frame0, const void* workspace, long long workspace_bytes,
+                           float* points_out, unsigned char* colors_out, int* frame_out, float* xyz, long long ld,
+                           void* stream) {
+  OVG_REQUIRE(points && points_out && colors_out && frame_out && xyz, "null operand");
+  ovg::CloudParams p;
+  int rc = cloud_params(conf_mask, images, F, H, W, mask_black_bg, mask_white_bg, const_cast<void*>(workspace),
+                        workspace_bytes, &p);
+  if (rc) return rc;
+  OVG_REQUIRE(ld >= 0 && (ld % 4) == 0 && (reinterpret_cast<uintptr_t>(xyz) & 15) == 0,
+              "xyz must be 16-byte aligned with a column stride ld % 4 == 0");
+  p.points = points; p.frame0 = frame0;
+  p.points_out = points_out; p.colors_out = colors_out; p.frame_out = frame_out; p.xyz = xyz; p.ld = ld;
+  ovg::cloud_gather_kernel<<<p.tiles, ovg::CLOUD_THREADS, 0, reinterpret_cast<cudaStream_t>(stream)>>>(p);
+  return post_launch("ovg_point_cloud_gather");
+}
+
+int ovg_point_cloud_center(const float* points, long long n, void* workspace, long long workspace_bytes, float* center_out,
+                           void* stream) {
+  OVG_REQUIRE(points && workspace && center_out && n > 0, "bad arguments");
+  const CloudWorkspace w = cloud_workspace(workspace, n);
+  OVG_REQUIRE((reinterpret_cast<uintptr_t>(workspace) & 15) == 0 && workspace_bytes >= w.bytes,
+              "workspace must be 16-byte aligned and ovg_point_cloud_workspace_bytes(n) long");
+  cudaStream_t st = reinterpret_cast<cudaStream_t>(stream);
+  ovg::CloudCenterParams p{points, n, w.center_partial, center_out};
+  ovg::cloud_center_partial_kernel<<<ovg::CLOUD_CENTER_BLOCKS, 256, 0, st>>>(p);
+  int rc = post_launch("ovg_point_cloud_center");
+  if (rc) return rc;
+  ovg::cloud_center_final_kernel<<<1, 32, 0, st>>>(p);
+  return post_launch("ovg_point_cloud_center(final)");
+}
+
+int ovg_point_cloud_scale(const float* xyz, long long n_kept, long long ld, void* workspace, long long workspace_bytes,
+                          float* scale_out, void* stream) {
+  OVG_REQUIRE(xyz && workspace && scale_out && n_kept > 0 && ld >= n_kept && ld % 4 == 0, "bad arguments");
+  OVG_REQUIRE((reinterpret_cast<uintptr_t>(xyz) & 15) == 0, "xyz must be 16-byte aligned");
+  const CloudWorkspace w = cloud_workspace(workspace, 1);   // the scale uses only the fixed-size head of the workspace
+  OVG_REQUIRE((reinterpret_cast<uintptr_t>(workspace) & 15) == 0 && workspace_bytes >= w.bytes,
+              "workspace must be 16-byte aligned and ovg_point_cloud_workspace_bytes() long");
+  cudaStream_t st = reinterpret_cast<cudaStream_t>(stream);
+  for (int q = 0; q < 2; ++q)
+    for (int a = 0; a < 3; ++a) {
+      const int rc = radix_percentile(xyz + a * ld, n_kept, q ? 95.f : 5.f, w.select, w.sel + (q * 3 + a) * 3, nullptr,
+                                      "ovg_point_cloud_scale", st);
+      if (rc) return rc;
+    }
+  ovg::cloud_scale_kernel<<<1, 32, 0, st>>>(w.sel, scale_out);
+  return post_launch("ovg_point_cloud_scale");
 }
 
 }  // extern "C"

@@ -4,6 +4,8 @@
 //                                                                    utils/rotation.py:14-44, utils/geometry.py:269-318)
 //   unproject_kernel          depth + cameras -> world points                                  (utils/geometry.py:151-264)
 //   percentile select + mask  conf >= percentile(conf, p) && conf > 0.1                        (inference.py:132-133)
+//   cloud_* kernels           background filters, ordered compaction, centre, scene scale      (visual_util.py:190-236,
+//                                                                    inference.py:96-151)
 // All HBM-bound: one coalesced pass per kernel, 16-byte accesses where the layout allows; the percentile is an exact
 // order statistic by 4 x 8-bit radix-select passes over the fp32 bit patterns (integer histograms: deterministic).
 #pragma once
@@ -264,6 +266,184 @@ __global__ void __launch_bounds__(256) conf_mask_kernel(const ConfMaskParams p) 
 #pragma unroll
     for (int o = 16; o > 0; o >>= 1) kept += __shfl_xor_sync(0xffffffffu, kept, o);
     if ((threadIdx.x & 31) == 0 && kept) atomicAdd(p.count, static_cast<unsigned long long>(kept));
+  }
+}
+
+// ---------------------------------------------------------------------------------------------------
+// Point cloud (visual_util.py:190-236 predictions_to_glb, inference.py:96-151 viewer): filter, compact, centre, scale.
+// Pixels are numbered i = (f * H + y) * W + x, the order of numpy boolean indexing.  Block b of the count / gather kernels
+// owns the tile [b * CLOUD_TILE, (b + 1) * CLOUD_TILE), walked in CLOUD_ITERS chunks of 256 consecutive pixels; the count
+// kernel stores the tile's kept count, a one-block scan turns the counts into tile offsets, and the gather kernel places
+// each kept pixel at its tile offset + its rank inside the tile (ballot / popc within a warp, a scan over the 8 warps).
+constexpr int CLOUD_THREADS = 256;
+constexpr int CLOUD_ITERS = 16;
+constexpr int CLOUD_TILE = CLOUD_THREADS * CLOUD_ITERS;
+constexpr int CLOUD_CENTER_BLOCKS = 256;   // fixed, so the fp64 summation order does not depend on the device
+
+struct CloudParams {
+  const unsigned char* conf_mask;   // [F*H*W] from conf_mask_kernel
+  const float* images;              // [F, 3, H, W] in [0, 1]
+  const float* points;              // [F*H*W, 3]
+  long long n;                      // F*H*W
+  long long hw;                     // H*W
+  int black_bg, white_bg, frame0;
+  unsigned int* tile_count;         // [tiles]
+  unsigned long long* tile_offset;  // [tiles] exclusive prefix of tile_count
+  unsigned long long* total;        // kept points
+  int tiles;
+  float* points_out;                // [n_kept, 3]
+  unsigned char* colors_out;        // [n_kept, 3]
+  int* frame_out;                   // [n_kept]
+  float* xyz;                       // [3, ld]: the kept x / y / z as columns (scratch of the scale's percentiles)
+  long long ld;
+};
+
+// colours as visual_util.py:202 computes them, (x * 255).astype(uint8): fp32 product, truncation (mod 256 like the x86
+// conversion numpy uses for values outside [0, 256)); background tests of :213-221 on those bytes.
+__device__ __forceinline__ bool cloud_keep(const CloudParams& p, long long i, int& f, uchar3& rgb) {
+  f = static_cast<int>(i / p.hw);
+  const float* img = p.images + f * 2 * p.hw + i;         // = images + (3 f) hw + (i - f hw)
+  rgb.x = static_cast<unsigned char>(__float2int_rz(__fmul_rn(img[0], 255.0f)));
+  rgb.y = static_cast<unsigned char>(__float2int_rz(__fmul_rn(img[p.hw], 255.0f)));
+  rgb.z = static_cast<unsigned char>(__float2int_rz(__fmul_rn(img[2 * p.hw], 255.0f)));
+  bool keep = p.conf_mask[i] != 0;
+  if (p.black_bg) keep = keep && static_cast<int>(rgb.x) + rgb.y + rgb.z >= 16;
+  if (p.white_bg) keep = keep && !(rgb.x > 240 && rgb.y > 240 && rgb.z > 240);
+  return keep;
+}
+
+__global__ void __launch_bounds__(CLOUD_THREADS) cloud_count_kernel(const CloudParams p) {
+  __shared__ unsigned int warp_sum[CLOUD_THREADS / 32];
+  const long long base = static_cast<long long>(blockIdx.x) * CLOUD_TILE;
+  unsigned int kept = 0;
+#pragma unroll 4
+  for (int it = 0; it < CLOUD_ITERS; ++it) {
+    const long long i = base + it * CLOUD_THREADS + threadIdx.x;
+    int f;
+    uchar3 rgb;
+    if (i < p.n && cloud_keep(p, i, f, rgb)) ++kept;
+  }
+#pragma unroll
+  for (int o = 16; o > 0; o >>= 1) kept += __shfl_xor_sync(0xffffffffu, kept, o);
+  if ((threadIdx.x & 31) == 0) warp_sum[threadIdx.x >> 5] = kept;
+  __syncthreads();
+  if (threadIdx.x == 0) {
+    unsigned int s = 0;
+#pragma unroll
+    for (int w = 0; w < CLOUD_THREADS / 32; ++w) s += warp_sum[w];
+    p.tile_count[blockIdx.x] = s;
+  }
+}
+
+// One block of 1024 threads: thread t sums a contiguous run of tile counts, the 1024 run sums are scanned in shared memory.
+__global__ void __launch_bounds__(1024) cloud_scan_kernel(const CloudParams p) {
+  __shared__ unsigned long long run[1024];
+  const int per = (p.tiles + 1023) / 1024;
+  const int b0 = threadIdx.x * per;
+  const int b1 = min(b0 + per, p.tiles);
+  unsigned long long s = 0;
+  for (int b = b0; b < b1; ++b) s += p.tile_count[b];
+  run[threadIdx.x] = s;
+  __syncthreads();
+  for (int o = 1; o < 1024; o <<= 1) {          // Hillis-Steele inclusive scan
+    const unsigned long long v = threadIdx.x >= o ? run[threadIdx.x - o] : 0ull;
+    __syncthreads();
+    run[threadIdx.x] += v;
+    __syncthreads();
+  }
+  unsigned long long off = run[threadIdx.x] - s;
+  for (int b = b0; b < b1; ++b) {
+    p.tile_offset[b] = off;
+    off += p.tile_count[b];
+  }
+  if (threadIdx.x == 1023) *p.total = run[1023];
+}
+
+__global__ void __launch_bounds__(CLOUD_THREADS) cloud_gather_kernel(const CloudParams p) {
+  __shared__ unsigned int warp_pre[CLOUD_THREADS / 32 + 1];
+  const int lane = threadIdx.x & 31, warp = threadIdx.x >> 5;
+  const long long base = static_cast<long long>(blockIdx.x) * CLOUD_TILE;
+  unsigned long long out = p.tile_offset[blockIdx.x];
+  for (int it = 0; it < CLOUD_ITERS; ++it) {
+    const long long i = base + it * CLOUD_THREADS + threadIdx.x;
+    int f = 0;
+    uchar3 rgb = make_uchar3(0, 0, 0);
+    const bool keep = i < p.n && cloud_keep(p, i, f, rgb);
+    const unsigned int ballot = __ballot_sync(0xffffffffu, keep);
+    if (lane == 0) warp_pre[warp + 1] = __popc(ballot);
+    __syncthreads();
+    if (threadIdx.x == 0) {
+      warp_pre[0] = 0;
+#pragma unroll
+      for (int w = 1; w <= CLOUD_THREADS / 32; ++w) warp_pre[w] += warp_pre[w - 1];
+    }
+    __syncthreads();
+    if (keep) {
+      const unsigned long long k = out + warp_pre[warp] + __popc(ballot & ((1u << lane) - 1u));
+      const float x = p.points[3 * i], y = p.points[3 * i + 1], z = p.points[3 * i + 2];
+      p.points_out[3 * k] = x;
+      p.points_out[3 * k + 1] = y;
+      p.points_out[3 * k + 2] = z;
+      p.colors_out[3 * k] = rgb.x;
+      p.colors_out[3 * k + 1] = rgb.y;
+      p.colors_out[3 * k + 2] = rgb.z;
+      p.frame_out[k] = p.frame0 + f;
+      p.xyz[k] = x;
+      p.xyz[p.ld + k] = y;
+      p.xyz[2 * p.ld + k] = z;
+    }
+    out += warp_pre[CLOUD_THREADS / 32];
+    __syncthreads();                               // warp_pre is rewritten by the next chunk
+  }
+}
+
+// Mean of n points (inference.py:111): fp64 partial sums per block in a fixed order, then one thread adds the partials.
+struct CloudCenterParams {
+  const float* points;   // [n, 3]
+  long long n;
+  double* partial;       // [CLOUD_CENTER_BLOCKS, 3]
+  float* center;         // [3]
+};
+
+__global__ void __launch_bounds__(256) cloud_center_partial_kernel(const CloudCenterParams p) {
+  __shared__ double sh[3][256];
+  double s[3] = {0.0, 0.0, 0.0};
+  for (long long i = blockIdx.x * 256LL + threadIdx.x; i < p.n; i += 256LL * CLOUD_CENTER_BLOCKS) {
+#pragma unroll
+    for (int a = 0; a < 3; ++a) s[a] += static_cast<double>(p.points[3 * i + a]);
+  }
+#pragma unroll
+  for (int a = 0; a < 3; ++a) sh[a][threadIdx.x] = s[a];
+  __syncthreads();
+  for (int o = 128; o > 0; o >>= 1) {
+    if (threadIdx.x < o) {
+#pragma unroll
+      for (int a = 0; a < 3; ++a) sh[a][threadIdx.x] += sh[a][threadIdx.x + o];
+    }
+    __syncthreads();
+  }
+  if (threadIdx.x < 3) p.partial[blockIdx.x * 3 + threadIdx.x] = sh[threadIdx.x][0];
+}
+
+__global__ void cloud_center_final_kernel(const CloudCenterParams p) {
+  if (threadIdx.x < 3) {
+    double s = 0.0;
+    for (int b = 0; b < CLOUD_CENTER_BLOCKS; ++b) s += p.partial[b * 3 + threadIdx.x];
+    p.center[threadIdx.x] = static_cast<float>(s / static_cast<double>(p.n));
+  }
+}
+
+// scene_scale = ||p95 - p5|| (visual_util.py:231-236).  sel: the three [lo, hi, interpolated] triples of the 5th percentiles
+// (x, y, z) followed by those of the 95th.  fp32 like numpy's norm of a float32 vector.
+__global__ void cloud_scale_kernel(const float* sel, float* scale) {
+  if (threadIdx.x == 0) {
+    float ss = 0.f;
+#pragma unroll
+    for (int a = 0; a < 3; ++a) {
+      const float d = __fsub_rn(sel[(3 + a) * 3 + 2], sel[a * 3 + 2]);
+      ss = __fadd_rn(ss, __fmul_rn(d, d));
+    }
+    *scale = sqrtf(ss);
   }
 }
 

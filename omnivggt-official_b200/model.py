@@ -206,6 +206,88 @@ class OmniVGGT(nn.Module, PyTorchModelHubMixin):
         predictions["conf_mask"], predictions["conf_threshold"], predictions["conf_kept"] = mask.bool(), thr, cnt
         return predictions
 
+    @staticmethod
+    @torch.no_grad()
+    def point_cloud(predictions: Dict[str, object], *, source: str = "depth", conf_percent: float = 50.0,
+                    conf_floor: float = 1e-5, frame: Optional[int] = None, mask_black_bg: bool = False,
+                    mask_white_bg: bool = False, scene: int = 0) -> Dict[str, torch.Tensor]:
+        """The filtered, coloured point cloud of one scene, built on the device (libovg kernels).
+
+        Replaces the host numpy of the reference's GLB export (visual_util.py:190-236,:320-358 predictions_to_glb) and
+        viewer (inference.py:96-151).  ``source="depth"``: ``world_points_from_depth`` (computed here when ``postprocess``
+        has not run) with ``depth_conf``, as ``--save_glb`` uses it; ``"pointmap"``: ``world_points`` with
+        ``world_points_conf``.  ``frame``: keep only that view, selected before the percentile (visual_util.py:190-194).
+        Kept: conf >= percentile(conf, conf_percent) (0 for conf_percent == 0, visual_util.py:206-207) and conf > conf_floor,
+        minus black / white background pixels when asked.  ``conf_floor=0.1`` reproduces the viewer's initial mask
+        (inference.py:132-133); its frame dropdown is ``cloud["frame"] == i`` on the ``frame=None`` cloud.
+
+        Returns ``points`` fp32 [n,3], ``colors`` uint8 [n,3], ``frame`` int32 [n] (numpy boolean-indexing order),
+        ``conf_threshold`` (0-d), ``center`` fp32 [3] (mean of all points of the selected views, inference.py:111),
+        ``scale`` (0-d, ||p95 - p5||, 1.0 when nothing is kept) and ``align`` fp64 [4,4] = inv(E0) diag(1,-1,-1,1) R_y(180)
+        with E0 the first selected camera (visual_util.py:320-341).  The kept count and E0 are the only device-to-host reads."""
+        from . import ops
+        if source not in ("depth", "pointmap"):
+            raise ValueError(f"source must be 'depth' or 'pointmap', got {source!r}")
+        if not 0.0 <= conf_percent <= 100.0:
+            raise ValueError("conf_percent must be in [0, 100]")
+        if conf_floor < 0.0:
+            raise ValueError("conf_floor must be >= 0")        # the reference's floors are 1e-5 and 0.1
+
+        def scene_of(t, trailing):                             # [B, S, ...] or [S, ...] -> [S, ...] of the scene
+            return t[scene] if t.dim() == trailing + 2 else t
+
+        images = scene_of(predictions["images"], 3).float()
+        S, _, H, W = images.shape
+        if "extrinsic" in predictions:
+            ext = scene_of(predictions["extrinsic"], 2).float()
+            c2w = None
+        else:
+            ext, intr, c2w = ops.pose_decode(scene_of(predictions["pose_enc"], 1).float().contiguous(), H, W)
+        if source == "pointmap":
+            points = scene_of(predictions["world_points"], 3)
+            conf = scene_of(predictions["world_points_conf"], 2)
+        else:
+            if "world_points_from_depth" in predictions:
+                points = scene_of(predictions["world_points_from_depth"], 3)
+            else:
+                if c2w is None:
+                    ext, intr, c2w = ops.pose_decode(scene_of(predictions["pose_enc"], 1).float().contiguous(), H, W)
+                depth = scene_of(predictions["depth"], 3).float().reshape(S, H, W)
+                points = ops.unproject_depth(depth, intr, c2w, H, W)
+            conf = scene_of(predictions["depth_conf"], 2)
+        f0 = 0
+        if frame is not None:
+            if not 0 <= frame < S:
+                raise IndexError(f"frame {frame} out of range for {S} views")
+            f0 = frame
+            images, points, conf = images[frame:frame + 1], points[frame:frame + 1], conf[frame:frame + 1]
+        images = images.contiguous()
+        points = points.float().contiguous()
+        conf = conf.float().contiguous()
+        F = images.shape[0]
+        dev = images.device
+
+        mask, thr, _ = ops.conf_percentile_mask(conf, conf_percent, conf_floor)
+        if conf_percent == 0.0:
+            thr = torch.zeros((), device=dev, dtype=torch.float32)   # same mask: conf > conf_floor >= 0 implies conf >= 0
+        ws = ops.point_cloud_workspace(F * H * W, dev)
+        cnt = ops.point_cloud_count(mask, images, ws, mask_black_bg, mask_white_bg)
+        center = ops.point_cloud_center(points, ws)
+        n = int(cnt.item())
+        e0 = torch.eye(4, dtype=torch.float64)
+        e0[:3, :4] = ext[f0].double().cpu()
+        gl = torch.diag(torch.tensor([1.0, -1.0, -1.0, 1.0], dtype=torch.float64))
+        rot_y = torch.diag(torch.tensor([-1.0, 1.0, -1.0, 1.0], dtype=torch.float64))
+        align = (torch.linalg.inv(e0) @ gl @ rot_y).to(dev)
+        if n == 0:
+            return {"points": torch.empty(0, 3, device=dev), "colors": torch.empty(0, 3, device=dev, dtype=torch.uint8),
+                    "frame": torch.empty(0, device=dev, dtype=torch.int32), "conf_threshold": thr, "center": center,
+                    "scale": torch.ones((), device=dev), "align": align}
+        pts, cols, fr, xyz = ops.point_cloud_gather(points, mask, images, ws, n, mask_black_bg, mask_white_bg, f0)
+        scale = ops.point_cloud_scale(xyz, n, ws)
+        return {"points": pts, "colors": cols, "frame": fr, "conf_threshold": thr, "center": center, "scale": scale,
+                "align": align}
+
     # ---------------------------------------------------------------------------------------------- CUDA graph replay
     def _forward_graphed(self, eng, impl, images, extrinsics, intrinsics, depth, mask, depth_idx, cam_idx):
         """Same computation, launched from a captured CUDA graph (a forward is >1000 kernel launches; issuing them from

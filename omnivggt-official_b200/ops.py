@@ -202,3 +202,59 @@ def conf_percentile_mask(conf, percent: float, floor: float = 0.1):
     L.check(L.lib().ovg_conf_percentile_mask(c.data_ptr(), c.numel(), float(percent), float(floor), ws.data_ptr(),
                                              mask.data_ptr(), thr.data_ptr(), cnt.data_ptr(), L.stream()))
     return mask, thr, cnt
+
+
+def point_cloud_workspace(n: int, device):
+    """uint8 workspace of ovg_point_cloud_workspace_bytes(n) for a cloud over n pixels (F*H*W)."""
+    return torch.empty(L.lib().ovg_point_cloud_workspace_bytes(n), device=device, dtype=torch.uint8)
+
+
+def point_cloud_count(conf_mask, images, ws, mask_black_bg: bool = False, mask_white_bg: bool = False):
+    """conf_mask uint8 [F,H,W], images fp32 [F,3,H,W] -> kept-pixel count (0-d int64 device tensor)."""
+    _chk(conf_mask, torch.uint8, "conf_mask")
+    _chk(images, F32, "images")
+    assert conf_mask.is_contiguous() and images.is_contiguous() and images.dim() == 4 and images.shape[1] == 3
+    F, _, H, W = images.shape
+    assert conf_mask.numel() == F * H * W
+    cnt = torch.empty((), device=images.device, dtype=torch.int64)
+    L.check(L.lib().ovg_point_cloud_count(conf_mask.data_ptr(), images.data_ptr(), F, H, W, int(mask_black_bg), int(mask_white_bg),
+                                          ws.data_ptr(), ws.numel(), cnt.data_ptr(), L.stream()))
+    return cnt
+
+
+def point_cloud_gather(points, conf_mask, images, ws, n_kept: int, mask_black_bg: bool = False, mask_white_bg: bool = False,
+                       frame0: int = 0):
+    """The n_kept pixels that point_cloud_count kept, in (frame, row, column) order: (points fp32 [n,3], colors uint8 [n,3],
+    frame int32 [n], xyz fp32 [3, ld] column copy of the points for point_cloud_scale)."""
+    _chk(points, F32, "points")
+    assert points.is_contiguous() and points.numel() == conf_mask.numel() * 3
+    F, _, H, W = images.shape
+    dev = images.device
+    ld = (n_kept + 3) // 4 * 4
+    pts = torch.empty(n_kept, 3, device=dev, dtype=F32)
+    cols = torch.empty(n_kept, 3, device=dev, dtype=torch.uint8)
+    frame = torch.empty(n_kept, device=dev, dtype=torch.int32)
+    xyz = torch.empty(3, ld, device=dev, dtype=F32)
+    L.check(L.lib().ovg_point_cloud_gather(points.data_ptr(), conf_mask.data_ptr(), images.data_ptr(), F, H, W, int(mask_black_bg),
+                                           int(mask_white_bg), int(frame0), ws.data_ptr(), ws.numel(), pts.data_ptr(),
+                                           cols.data_ptr(), frame.data_ptr(), xyz.data_ptr(), ld, L.stream()))
+    return pts, cols, frame, xyz
+
+
+def point_cloud_center(points, ws):
+    """Mean of points fp32 [..., 3] -> fp32 [3] (fp64 sums in a fixed order)."""
+    _chk(points, F32, "points")
+    assert points.is_contiguous()
+    center = torch.empty(3, device=points.device, dtype=F32)
+    L.check(L.lib().ovg_point_cloud_center(points.data_ptr(), points.numel() // 3, ws.data_ptr(), ws.numel(), center.data_ptr(),
+                                           L.stream()))
+    return center
+
+
+def point_cloud_scale(xyz, n_kept: int, ws):
+    """||percentile(p, 95) - percentile(p, 5)|| over the first n_kept columns of xyz [3, ld] -> 0-d fp32 tensor."""
+    _chk(xyz, F32, "xyz")
+    scale = torch.empty((), device=xyz.device, dtype=F32)
+    L.check(L.lib().ovg_point_cloud_scale(xyz.data_ptr(), n_kept, xyz.shape[1], ws.data_ptr(), ws.numel(), scale.data_ptr(),
+                                          L.stream()))
+    return scale
