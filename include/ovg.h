@@ -261,6 +261,15 @@ int ovg_aggregator_forward(ovg_aggregator* h, const float* patch_tokens, const f
                            const int* depth_idx, int n_depth, const float* rope_cos, const float* rope_sin, int maxpos, int B,
                            int S, int H, int W, void* workspace, long long workspace_bytes, void* const* slots, float* cam_out,
                            void* stream);
+/* As ovg_aggregator_forward, and additionally exports layers in fp32, as the reference's aggregator returns them
+ * (models/omnivggt_aggregator.py:248-256: aggregated_tokens_list, one [B, S, T, 2C] tensor per layer, frame half | global half).
+ * layers: host array of `depth` device pointers, fp32 [B*S, T, 2C] each; NULL entries are not exported.  Each layer is written in
+ * the same pass that makes its bf16 snapshot.  Entries of slots may be NULL (that slot is not written); with all four NULL and no
+ * layer exported, the call produces cam_out only (the input of the camera head, heads/camera_head.py:96-99). */
+int ovg_aggregator_forward_layers(ovg_aggregator* h, const float* patch_tokens, const float* inj, const float* depth,
+                                  const float* mask, const int* depth_idx, int n_depth, const float* rope_cos, const float* rope_sin,
+                                  int maxpos, int B, int S, int H, int W, void* workspace, long long workspace_bytes,
+                                  void* const* slots, float* cam_out, float* const* layers, void* stream);
 
 /* Frozen DINOv2 patchifier on the same kernels: reference layers/vision_transformer.py:214-271. */
 typedef struct ovg_dino_desc {
@@ -309,6 +318,13 @@ long long ovg_dpt_workspace_bytes(const ovg_dpt* h, int Fc, int H, int W);
 int ovg_dpt_forward(ovg_dpt* h, const void* const* slots, int T, int nspecial, int f0, int Fc, int H, int W,
                     const float* const* tables, const float* tx, const float* ty, int head_act, float* preds, float* conf,
                     void* workspace, long long workspace_bytes, void* stream);
+/* As ovg_dpt_forward on fp32 layers: layers is a host array of 4 device pointers, fp32 [K, T, C2] -- the layers the DPT head
+ * selects from an aggregated_tokens_list (heads/dpt_head.py:128-183,:212-229; DPTHead.forward).  The first LayerNorm rounds each
+ * element to bf16 (nearest even) as it loads it, so the results equal ovg_dpt_forward on the bf16 rounding of the same layers
+ * bit for bit. */
+int ovg_dpt_forward_f32(ovg_dpt* h, const float* const* layers, int T, int nspecial, int f0, int Fc, int H, int W,
+                        const float* const* tables, const float* tx, const float* ty, int head_act, float* preds, float* conf,
+                        void* workspace, long long workspace_bytes, void* stream);
 
 /* Camera head: iterative pose refinement on the camera tokens; reference heads/camera_head.py:83-154.  The weight-streaming
  * GEMMs run on the wgmma GEMM; AdaLN, the S-token attention (head_dim D / heads) and the 9-wide pose update are small fp32

@@ -17,9 +17,11 @@ __device__ __forceinline__ float warp_sum(float v) {
 // One warp per row; fp32 or bf16 input, bf16 output, optional affine.  Row gather: output row m reads
 // input row (m / grp_out) * grp_in + grp_off + (m % grp_out)   (grp_out == 0 -> identity); this drops the 5
 // special tokens of every frame for the DPT input (heads/dpt_head.py:219).
+enum { LN_IN_F32 = 0, LN_IN_BF16 = 1, LN_IN_F32_AS_BF16 = 2 };
 struct LnParams {
   const void* in;
-  int in_bf16;
+  int in_bf16;      // input type (LN_IN_*): fp32, bf16, or fp32 rounded to bf16 (nearest even) on load -- the values a bf16
+                    // snapshot of the same fp32 tensor (inject_snapshot_kernel) would hold
   long long ld_in;
   void* out;
   int out_f32;      // output type: 0 bf16, 1 fp32, 2 IEEE half (saturating)
@@ -36,7 +38,7 @@ __device__ __forceinline__ void ln_load_row(const LnParams& p, const int row, co
   long long src = row;
   if (p.grp_out > 0) src = static_cast<long long>(row / p.grp_out) * p.grp_in + p.grp_off + (row % p.grp_out);
   // lane handles chunks of 4 consecutive elements: element index = (i*32 + lane)*4 + e
-  if (p.in_bf16) {
+  if (p.in_bf16 == LN_IN_BF16) {
     const __nv_bfloat16* x = reinterpret_cast<const __nv_bfloat16*>(p.in) + src * p.ld_in;
 #pragma unroll
     for (int i = 0; i < VPL / 4; ++i) {
@@ -55,6 +57,14 @@ __device__ __forceinline__ void ln_load_row(const LnParams& p, const int row, co
       v[4 * i + 1] = f.y;
       v[4 * i + 2] = f.z;
       v[4 * i + 3] = f.w;
+    }
+    if (p.in_bf16 == LN_IN_F32_AS_BF16) {
+#pragma unroll
+      for (int i = 0; i < VPL / 2; ++i) {
+        const uint32_t u = pack_bf16(v[2 * i], v[2 * i + 1]);
+        v[2 * i] = bf16_lo(u);
+        v[2 * i + 1] = bf16_hi(u);
+      }
     }
   }
 }
@@ -168,6 +178,7 @@ __global__ void assemble_tokens_kernel(const AssembleParams p) {
 // Per-layer camera injection + intermediate snapshot (reference omnivggt_aggregator.py:273-303,:248-251).
 //   x[k,0,:] += inj[k,:]                                   (only token 0 of each frame receives a non-zero add)
 //   slot[k,t, coff:coff+C] = bf16(x[k,t,:])                (frame half coff=0 / global half coff=C)
+//   layer[k,t, coff:coff+C] = x[k,t,:]                     (fp32 export of the layer, as the reference returns it)
 //   cam_out[k, coff:coff+C] = x[k,0,:]                     (fp32 camera tokens for the camera head)
 struct InjectParams {
   float* x;                 // [K*T, C]
@@ -175,11 +186,12 @@ struct InjectParams {
   __nv_bfloat16* slot;      // [K*T, 2C] or nullptr
   float* cam_out;           // [K, 2C] or nullptr
   int K, T, C, coff;
+  float* layer;             // [K*T, 2C] or nullptr
 };
 
 __global__ void inject_snapshot_kernel(const InjectParams p) {
-  // with a snapshot slot: one block per token row; without: only the camera-token rows change (one block per frame)
-  const int row = p.slot ? blockIdx.x : blockIdx.x * p.T;
+  // with a snapshot slot or layer: one block per token row; without: only the camera-token rows change (one block per frame)
+  const int row = (p.slot || p.layer) ? blockIdx.x : blockIdx.x * p.T;
   const int k = row / p.T, t = row % p.T;
   for (int c = threadIdx.x * 4; c < p.C; c += blockDim.x * 4) {
     float4 v = *reinterpret_cast<const float4*>(p.x + static_cast<long long>(row) * p.C + c);
@@ -197,6 +209,7 @@ __global__ void inject_snapshot_kernel(const InjectParams p) {
       u.y = pack_bf16(v.z, v.w);
       *reinterpret_cast<uint2*>(p.slot + static_cast<long long>(row) * 2 * p.C + p.coff + c) = u;
     }
+    if (p.layer) *reinterpret_cast<float4*>(p.layer + static_cast<long long>(row) * 2 * p.C + p.coff + c) = v;
   }
 }
 

@@ -376,14 +376,15 @@ int ovg_attention(const void* q, const void* k, const void* v, void* out, int ba
   return post_launch("ovg_attention(merge)");
 }
 
-int ovg_layernorm(const void* in, int in_is_bf16, long long ld_in, void* out, int out_is_f32, long long ld_out, int rows,
-                  int C, const float* w, const float* b, float eps, int grp_out, int grp_in, int grp_off, void* stream) {
+// in_mode: ovg::LN_IN_F32, LN_IN_BF16 or LN_IN_F32_AS_BF16 (the last is internal: ovg_dpt_forward_f32 reads fp32 layers with it)
+static int layernorm(const void* in, int in_mode, long long ld_in, void* out, int out_is_f32, long long ld_out, int rows, int C,
+                     const float* w, const float* b, float eps, int grp_out, int grp_in, int grp_off, void* stream) {
   OVG_REQUIRE(in && out && rows > 0, "null operand");
   OVG_REQUIRE(out_is_f32 >= 0 && out_is_f32 <= 2, "output type: 0 bf16, 1 fp32, 2 fp16");
   OVG_REQUIRE((w == nullptr) == (b == nullptr), "affine needs both weight and bias");
   OVG_REQUIRE(C % 128 == 0 && C <= 2048, "C must be a multiple of 128, <= 2048");
   cudaStream_t st = reinterpret_cast<cudaStream_t>(stream);
-  ovg::LnParams p{in, in_is_bf16, ld_in, out, out_is_f32, ld_out, rows, C, w, b, eps,
+  ovg::LnParams p{in, in_mode, ld_in, out, out_is_f32, ld_out, rows, C, w, b, eps,
                   grp_out, grp_in, grp_off};
   constexpr int ln_threads = 256;     // 8 rows per block
   constexpr int ln_persist = 2;       // persistent grid: blocks per SM
@@ -401,6 +402,12 @@ int ovg_layernorm(const void* in, int in_is_bf16, long long ld_in, void* out, in
     default: return fail(OVG_E_INVALID, "ovg_layernorm: unsupported C");
   }
   return post_launch("ovg_layernorm");
+}
+
+int ovg_layernorm(const void* in, int in_is_bf16, long long ld_in, void* out, int out_is_f32, long long ld_out, int rows,
+                  int C, const float* w, const float* b, float eps, int grp_out, int grp_in, int grp_off, void* stream) {
+  return layernorm(in, in_is_bf16 ? ovg::LN_IN_BF16 : ovg::LN_IN_F32, ld_in, out, out_is_f32, ld_out, rows, C, w, b, eps, grp_out,
+                   grp_in, grp_off, stream);
 }
 
 int ovg_assemble_tokens(float* x, const float* patch, const float* cam_tok, const float* reg_tok, const float* inj0,
@@ -426,14 +433,20 @@ int ovg_peer_barrier(int* const* flag_peers, int* epoch_counter, int rank, int w
   return post_launch("ovg_peer_barrier");
 }
 
-int ovg_inject_snapshot(float* x, const float* inj, void* slot, float* cam_out, int K, int T, int C, int coff,
-                        void* stream) {
+// layer: fp32 [K*T, 2C] export of the same half (ovg_aggregator_forward_layers), or NULL
+static int inject_snapshot(float* x, const float* inj, void* slot, float* layer, float* cam_out, int K, int T, int C, int coff,
+                           void* stream) {
   OVG_REQUIRE(x && K > 0 && T > 0 && C % 4 == 0, "bad arguments");
   OVG_REQUIRE(coff == 0 || coff == C, "coff must be 0 or C");
-  ovg::InjectParams p{x, inj, reinterpret_cast<__nv_bfloat16*>(slot), cam_out, K, T, C, coff};
+  ovg::InjectParams p{x, inj, reinterpret_cast<__nv_bfloat16*>(slot), cam_out, K, T, C, coff, layer};
   const int threads = C / 4 < 256 ? ((C / 4 + 31) / 32) * 32 : 256;
-  ovg::inject_snapshot_kernel<<<slot ? K * T : K, threads, 0, reinterpret_cast<cudaStream_t>(stream)>>>(p);
+  ovg::inject_snapshot_kernel<<<(slot || layer) ? K * T : K, threads, 0, reinterpret_cast<cudaStream_t>(stream)>>>(p);
   return post_launch("ovg_inject_snapshot");
+}
+
+int ovg_inject_snapshot(float* x, const float* inj, void* slot, float* cam_out, int K, int T, int C, int coff,
+                        void* stream) {
+  return inject_snapshot(x, inj, slot, nullptr, cam_out, K, T, C, coff, stream);
 }
 
 int ovg_depth_im2col(const float* depth, const float* mask, const int* idx_stats, int n_stats, const int* idx_cols, int n_cols,

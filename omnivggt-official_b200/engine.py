@@ -325,9 +325,12 @@ class Engine:
     # ------------------------------------------------------------------------------------------ aggregator
     def aggregate(self, patch_tokens: torch.Tensor, inj: torch.Tensor, depth: Optional[torch.Tensor],
                   mask: Optional[torch.Tensor], depth_idx: List[int], B: int, S: int, H: int, W: int,
-                  keep: Sequence[int], cp=None, views_total: int = 0):
+                  keep: Sequence[int], cp=None, views_total: int = 0, slots: bool = True,
+                  layers: Optional[Sequence[Optional[torch.Tensor]]] = None):
         """patch_tokens fp32 [K,P,C]; inj fp32 [depth+1,K,C].  Returns ({layer: bf16 slot [K,T,2C]}, cam fp32 [K,2C]).
-        ``cp`` (a ContextParallel): B = 1, S = this rank's views of a scene with ``views_total`` views."""
+        ``cp`` (a ContextParallel): B = 1, S = this rank's views of a scene with ``views_total`` views.
+        ``slots=False``: no DPT head reads the kept layers; the four slots are neither allocated nor written (returns {}).
+        ``layers``: ``depth`` fp32 [K,T,2C] tensors (or None) to export every layer into (ovg_aggregator_forward_layers)."""
         lib = L.lib()
         Cc, R = self.C, self.R
         K = B * S
@@ -354,11 +357,19 @@ class Engine:
                 if n_loc:
                     idx_loc = self.cached(("depth_idx", tuple(loc)), lambda: torch.tensor(loc, dtype=torch.int32))
         wsb = self._workspace("agg_ws", lib.ovg_aggregator_workspace_bytes(self.h_agg, B, S, H, W, Sd))
-        slot_t = [self.ws.get(f"slot{i}", (K, T, 2 * Cc)) for i in self.keep]
+        slot_t = [self.ws.get(f"slot{i}", (K, T, 2 * Cc)) for i in self.keep] if slots else []
         slot_p = (C.c_void_p * 4)(*[t.data_ptr() for t in slot_t])
         cam_out = self.ws.get("cam_out", (K, 2 * Cc), F32)
         pt, ij = patch_tokens.contiguous(), inj.contiguous()
-        if cp is not None:
+        if layers is not None:
+            assert cp is None and len(layers) == self.depth
+            for t in layers:
+                assert t is None or (t.dtype == F32 and t.is_contiguous() and t.numel() == K * T * 2 * Cc)
+            layer_p = (C.c_void_p * self.depth)(*[L.ptr(t) for t in layers])
+            L.check(lib.ovg_aggregator_forward_layers(self.h_agg, pt.data_ptr(), ij.data_ptr(), L.ptr(d32), L.ptr(m32), L.ptr(idx), Sd,
+                                                      cos.data_ptr(), sin.data_ptr(), cos.shape[0], B, S, H, W, wsb.data_ptr(),
+                                                      wsb.numel(), slot_p, cam_out.data_ptr(), layer_p, L.stream()))
+        elif cp is not None:
             assert B == 1, "context parallelism shards the views of one scene"
             cd = cp.desc(self.heads, views_total * T, views_total)
             L.check(lib.ovg_aggregator_forward_cp(self.h_agg, C.byref(cd), pt.data_ptr(), ij.data_ptr(), L.ptr(d32), L.ptr(m32),
@@ -389,13 +400,18 @@ class Engine:
                 torch.empty(K, H, W, device=self.device, dtype=F32))
 
     def dpt(self, name: str, slots: Dict[int, torch.Tensor], layers: Sequence[int], K: int, H: int, W: int,
-            head_act: int, chunk: int = 8, out=None):
+            head_act: int, chunk: int = 8, out=None, nspecial: Optional[int] = None):
         """One DPT head over all K frames in chunks of 8 (reference heads/dpt_head.py:153-183: results are chunk independent).
-        Every head has its own workspace, so the two heads may run concurrently on different streams."""
+        Every head has its own workspace, so the two heads may run concurrently on different streams.
+        ``slots``: bf16 snapshots [K,T,2C] (ovg_dpt_forward) or fp32 layers (ovg_dpt_forward_f32, bit-identical on their bf16
+        rounding), indexed by layer; ``nspecial``: tokens in front of the patch tokens (default: camera + registers)."""
         lib, pk = L.lib(), self.dpt_packs[name]
         preds, conf = out if out is not None else self.dpt_alloc(name, K, H, W)
         hp, wp = H // self.patch, W // self.patch
-        T = hp * wp + self.R + 1
+        nspecial = self.R + 1 if nspecial is None else nspecial
+        T = hp * wp + nspecial
+        f32 = slots[layers[0]].dtype == F32
+        forward = lib.ovg_dpt_forward_f32 if f32 else lib.ovg_dpt_forward
         slot_p = (C.c_void_p * 4)(*[slots[i].data_ptr() for i in layers])
         tabs = [self.table(oc, hp, wp, W / H) for oc in pk.oc]
         tab_p = (C.c_void_p * 4)(*[t.data_ptr() for t in tabs])
@@ -403,7 +419,6 @@ class Engine:
         fc_max = min(chunk, K)
         wsb = self._workspace(name + ".ws", lib.ovg_dpt_workspace_bytes(self.h_dpt[name], fc_max, H, W))
         for f0 in range(0, K, chunk):
-            L.check(lib.ovg_dpt_forward(self.h_dpt[name], slot_p, T, self.R + 1, f0, min(chunk, K - f0), H, W, tab_p,
-                                        tx.data_ptr(), ty.data_ptr(), head_act, preds.data_ptr(), conf.data_ptr(),
-                                        wsb.data_ptr(), wsb.numel(), L.stream()))
+            L.check(forward(self.h_dpt[name], slot_p, T, nspecial, f0, min(chunk, K - f0), H, W, tab_p, tx.data_ptr(), ty.data_ptr(),
+                            head_act, preds.data_ptr(), conf.data_ptr(), wsb.data_ptr(), wsb.numel(), L.stream()))
         return preds, conf

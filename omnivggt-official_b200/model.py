@@ -13,7 +13,8 @@ from __future__ import annotations
 
 import os
 import warnings
-from typing import Dict, List, Optional, Sequence
+import weakref
+from typing import Dict, List, Optional, Sequence, Tuple
 
 import torch
 import torch.nn as nn
@@ -25,10 +26,12 @@ except Exception:  # pragma: no cover
         pass
 
 from . import torch_parts as TP
-from .params import AggregatorParams, CameraHeadParams, DPTParams, init_parameters
+from .params import AggregatorParams, CameraHeadParams, Component, DPTParams, init_parameters
 
 _RESNET_MEAN = (0.485, 0.456, 0.406)   # reference models/aggregator.py:22-23
 _RESNET_STD = (0.229, 0.224, 0.225)
+_HEADS = ("camera_head", "depth_head", "point_head")
+_DPT_HEADS = (("depth_head", 0), ("point_head", 1))          # name, head_act (exp / inverse-log)
 
 
 class OmniVGGT(nn.Module, PyTorchModelHubMixin):
@@ -96,6 +99,25 @@ class OmniVGGT(nn.Module, PyTorchModelHubMixin):
         self._invalidate()
         return super()._apply(fn, *a, **k)
 
+    def __setattr__(self, name, value):
+        # the submodules are callable (params.Component): each holds a weak reference to the model that owns it, kept out of
+        # parameters() / state_dict() / _modules.  A head set to None is skipped (omnivggt.py:46,:51,:58); the packed weights and
+        # the captured graphs of the old set of heads go.
+        if isinstance(value, Component):
+            object.__setattr__(value, "_owner", weakref.ref(self))
+        super().__setattr__(name, value)
+        if name in _HEADS and "_engine" in self.__dict__:
+            self._invalidate()
+
+    def __setstate__(self, state):        # copy.deepcopy / pickle: the copies' components point at the copy
+        super().__setstate__(state)
+        for m in self.children():
+            if isinstance(m, Component):
+                object.__setattr__(m, "_owner", weakref.ref(self))
+
+    def _dpt_heads(self):
+        return [(name, act) for name, act in _DPT_HEADS if getattr(self, name) is not None]
+
     def _dino_module(self):
         """The frozen patchifier in ``dino_dtype``: a cached cast of the fp32 master weights (no per-call casts)."""
         pe = self.aggregator.patch_embed
@@ -121,6 +143,16 @@ class OmniVGGT(nn.Module, PyTorchModelHubMixin):
     def forward(self, images: torch.Tensor, extrinsics: torch.Tensor = None, intrinsics: torch.Tensor = None,
                 depth: torch.Tensor = None, mask: torch.Tensor = None, depth_gt_index: list = None,
                 camera_gt_index: list = None) -> Dict[str, object]:
+        images, depth_idx, cam_idx = self._check_inputs(images, extrinsics, intrinsics, depth, mask, depth_gt_index,
+                                                        camera_gt_index)
+        eng = self.engine()
+        args = (images, extrinsics, intrinsics, depth, mask, depth_idx, cam_idx)
+        impl = self._forward_cp if self._cp is not None else self._forward_impl
+        if self.use_cuda_graph and images.is_cuda and not torch.cuda.is_current_stream_capturing():
+            return self._forward_graphed(eng, impl, *args)
+        return impl(eng, *args)
+
+    def _check_inputs(self, images, extrinsics, intrinsics, depth, mask, depth_gt_index, camera_gt_index):
         if images.dim() == 4:
             images = images.unsqueeze(0)
         B, S, Cin, H, W = images.shape
@@ -135,12 +167,7 @@ class OmniVGGT(nn.Module, PyTorchModelHubMixin):
             assert tuple(depth.shape[:4]) == tuple(mask.shape), "mask and depth must have the same first four dimensions"
         if len(cam_idx):
             assert extrinsics is not None and intrinsics is not None, "camera_gt_index given without cameras"
-        eng = self.engine()
-        args = (images, extrinsics, intrinsics, depth, mask, depth_idx, cam_idx)
-        impl = self._forward_cp if self._cp is not None else self._forward_impl
-        if self.use_cuda_graph and images.is_cuda and not torch.cuda.is_current_stream_capturing():
-            return self._forward_graphed(eng, impl, *args)
-        return impl(eng, *args)
+        return images, depth_idx, cam_idx
 
     # ---------------------------------------------------------------------------------------------- context parallelism
     def enable_context_parallel(self, group=None) -> "OmniVGGT":
@@ -173,14 +200,85 @@ class OmniVGGT(nn.Module, PyTorchModelHubMixin):
             pose = TP.aux_pose_encoding(extrinsics.index_select(1, ci), intrinsics.index_select(1, ci), H, W)
         inj = TP.injection_vectors(eng.inj_pack, pose, cam_idx, 1, S, rows)[:, sl].contiguous()
         # depth aux: full tensors + scene indices (the masked-mean normalisation is over all selected views of the scene)
-        slots, cam_loc = eng.aggregate(patch, inj, depth, mask, depth_idx, 1, n, H, W, set(self.dpt_layers), cp=cp, views_total=S)
-        pose_list = self._camera(eng, cp.cam_all, 1, S)            # [S, 2C] gathered by peer stores: the camera head attends across all views
+        heads = self._dpt_heads()
+        slots, cam_loc = eng.aggregate(patch, inj, depth, mask, depth_idx, 1, n, H, W, set(self.dpt_layers), cp=cp, views_total=S,
+                                       slots=bool(heads))
+        out: Dict[str, object] = {}
+        if self.camera_head is not None:   # [S, 2C] gathered by peer stores: the camera head attends across all views
+            pose_list = self._camera(eng, cp.cam_all, 1, S)
+            out["pose_enc"], out["pose_enc_list"] = pose_list[-1], pose_list
         eng.warm_tables(H, W)
-        d_out = eng.dpt("depth_head", slots, self.dpt_layers, n, H, W, head_act=0)
-        p_out = eng.dpt("point_head", slots, self.dpt_layers, n, H, W, head_act=1)
-        return {"pose_enc": pose_list[-1], "pose_enc_list": pose_list, "depth": d_out[0].view(1, n, H, W, 1),
-                "depth_conf": d_out[1].view(1, n, H, W), "world_points": p_out[0].view(1, n, H, W, 3),
-                "world_points_conf": p_out[1].view(1, n, H, W), "images": images[:, sl], "view_range": (v0, v0 + n)}
+        for name, act in heads:
+            preds, conf = eng.dpt(name, slots, self.dpt_layers, n, H, W, head_act=act)
+            self._put_dpt(out, name, preds, conf, 1, n, H, W)
+        out["images"], out["view_range"] = images[:, sl], (v0, v0 + n)
+        return out
+
+    @staticmethod
+    def _put_dpt(out, name, preds, conf, B, S, H, W):
+        key = "depth" if name == "depth_head" else "world_points"
+        out[key] = preds.view(B, S, H, W, preds.shape[-1])
+        out[key + "_conf"] = conf.view(B, S, H, W)
+
+    # ---------------------------------------------------------------------------------------------- components
+    # model.aggregator(...), model.camera_head(...), model.depth_head(...) and model.point_head(...) take the reference's
+    # arguments (params.Component) and land here.  They run eagerly (no CUDA graph) on one GPU.
+    def _component_engine(self):
+        if self._cp is not None:
+            raise RuntimeError("the component calls (aggregator / camera_head / depth_head / point_head) run on one GPU; "
+                               "under enable_context_parallel() call the model itself")
+        return self.engine()
+
+    @torch.no_grad()
+    def _call_aggregator(self, images, extrinsics, intrinsics, depth, mask, depth_gt_index, camera_gt_index
+                         ) -> Tuple[List[torch.Tensor], int]:
+        """All ``depth`` layers in fp32 [B, S, T, 2C] (frame half | global half) and patch_start_idx = 1 + registers, as
+        ZeroAggregator.forward returns them (omnivggt_aggregator.py:248-256).  Same patchifier, injection and kernels as
+        forward(); the layers are written by the snapshot pass of the aggregator (ovg_aggregator_forward_layers)."""
+        images, depth_idx, cam_idx = self._check_inputs(images, extrinsics, intrinsics, depth, mask, depth_gt_index,
+                                                        camera_gt_index)
+        eng = self._component_engine()
+        B, S, _, H, W = images.shape
+        T = (H // self.patch_size) * (W // self.patch_size) + eng.R + 1
+        layers = [torch.empty(B, S, T, 2 * eng.C, device=eng.device, dtype=torch.float32) for _ in range(eng.depth)]
+        self._aggregate(eng, images, extrinsics, intrinsics, depth, mask, depth_idx, cam_idx, slots=False, layers=layers)
+        return layers, 1 + eng.R
+
+    @torch.no_grad()
+    def _call_dpt(self, head, tokens, images, patch_start_idx, frames_chunk_size=8):
+        """DPTHead.forward (dpt_head.py:128-183) on the layers ``dpt_layers`` of any fp32 token list [B, S, T, 2C] with
+        T = patches + patch_start_idx; ``images`` gives H and W only.  The first LayerNorm reads the fp32 tokens and rounds them
+        to bf16 as the aggregator's own snapshot does, so the output equals forward()'s bit for bit on this aggregator's tokens.
+        Frames are chunked over B * S (the reference chunks each scene's S; every frame's result is chunk independent)."""
+        eng = self._component_engine()
+        name, act = next((n, a) for n, a in _DPT_HEADS if self._modules.get(n) is head)
+        B, S, _, H, W = images.shape
+        K = B * S
+        T = (H // self.patch_size) * (W // self.patch_size) + patch_start_idx
+        want = (B, S, T, 2 * eng.C)
+        layers = {}
+        for i in self.dpt_layers:
+            t = tokens[i]
+            if tuple(t.shape) != want:
+                raise ValueError(f"{name}: layer {i} has shape {tuple(t.shape)}, expected {want} for {H}x{W} images")
+            layers[i] = t.to(device=eng.device, dtype=torch.float32).contiguous().view(K, T, 2 * eng.C)
+        chunk = K if frames_chunk_size is None else int(frames_chunk_size)
+        if chunk <= 0:
+            raise ValueError("frames_chunk_size must be positive")
+        eng.warm_tables(H, W)
+        preds, conf = eng.dpt(name, layers, self.dpt_layers, K, H, W, head_act=act, chunk=chunk, nspecial=patch_start_idx)
+        return preds.view(B, S, H, W, preds.shape[-1]), conf.view(B, S, H, W)
+
+    @torch.no_grad()
+    def _call_camera(self, tokens, num_iterations=4) -> List[torch.Tensor]:
+        """CameraHead.forward (camera_head.py:83-103): the camera tokens tokens[-1][:, :, 0]."""
+        eng = self._component_engine()
+        last = tokens[-1]
+        B, S = last.shape[:2]
+        cam = last[:, :, 0].to(device=eng.device, dtype=torch.float32).contiguous()
+        if eng.h_cam is not None:
+            return eng.camera_head(cam.view(B * S, -1), B, S, iters=num_iterations)
+        return TP.camera_head(self.camera_head, cam, iters=num_iterations, dtype=self.camera_dtype)
 
     # ---------------------------------------------------------------------------------------------- post-processing
     @torch.no_grad()
@@ -296,8 +394,9 @@ class OmniVGGT(nn.Module, PyTorchModelHubMixin):
         need_c, need_d = len(cam_idx) > 0, len(depth_idx) > 0
         def sig(t):
             return None if t is None else (tuple(t.shape), t.dtype)
+        heads = tuple(getattr(self, n) is not None for n in _HEADS)
         key = (impl.__name__, sig(images), tuple(depth_idx), tuple(cam_idx), sig(extrinsics) if need_c else None,
-               sig(intrinsics) if need_c else None, sig(depth) if need_d else None, sig(mask) if need_d else None)
+               sig(intrinsics) if need_c else None, sig(depth) if need_d else None, sig(mask) if need_d else None, heads)
         ent = self._graphs.pop(key, None)
         if ent is None:
             ent = {"calls": 0, "graph": None}
@@ -336,8 +435,9 @@ class OmniVGGT(nn.Module, PyTorchModelHubMixin):
         ent["graph"].replay()
         out = ent["out"]
         res = {k: (v.clone() if torch.is_tensor(v) else v) for k, v in out.items() if k not in ("images", "pose_enc_list")}
-        res["pose_enc_list"] = [t.clone() for t in out["pose_enc_list"]]
-        res["pose_enc"] = res["pose_enc_list"][-1]
+        if "pose_enc_list" in out:
+            res["pose_enc_list"] = [t.clone() for t in out["pose_enc_list"]]
+            res["pose_enc"] = res["pose_enc_list"][-1]
         res["images"] = images if "view_range" not in out else images[:, out["view_range"][0]:out["view_range"][1]]
         return res
 
@@ -346,7 +446,8 @@ class OmniVGGT(nn.Module, PyTorchModelHubMixin):
             return eng.camera_head(cam_tokens, B, S)
         return TP.camera_head(self.camera_head, cam_tokens.view(B, S, -1), dtype=self.camera_dtype)
 
-    def _forward_impl(self, eng, images, extrinsics, intrinsics, depth, mask, depth_idx, cam_idx):
+    def _aggregate(self, eng, images, extrinsics, intrinsics, depth, mask, depth_idx, cam_idx, slots=True, layers=None):
+        """Patchifier, camera / depth injection and the aggregator: (bf16 slots of the kept layers, fp32 camera tokens [K, 2C])."""
         B, S, Cin, H, W = images.shape
         ag = self.aggregator
         K = B * S
@@ -377,40 +478,58 @@ class OmniVGGT(nn.Module, PyTorchModelHubMixin):
 
         # ---- hot path: aggregator on libovg
         keep = set(self.dpt_layers)
-        slots, cam_tokens = eng.aggregate(patch, inj, depth, mask, depth_idx, B, S, H, W, keep)
+        return eng.aggregate(patch, inj, depth, mask, depth_idx, B, S, H, W, keep, slots=slots, layers=layers)
+
+    def _forward_impl(self, eng, images, extrinsics, intrinsics, depth, mask, depth_idx, cam_idx):
+        B, S, Cin, H, W = images.shape
+        K = B * S
+        heads = self._dpt_heads()                 # the heads set to None are skipped, as the reference does (omnivggt.py:46-62)
+        cam_on = self.camera_head is not None
+        slots, cam_tokens = self._aggregate(eng, images, extrinsics, intrinsics, depth, mask, depth_idx, cam_idx, slots=bool(heads))
 
         # ---- heads.  The camera head and the two DPT heads only read the aggregator outputs: they run on three streams
         # (forked / joined with events, also inside a captured CUDA graph) so that their many small kernels -- 19^2 / 37^2
         # feature maps, M = 8 GEMVs -- share the 132 SMs instead of running one after the other.
         predictions: Dict[str, object] = {}
         eng.warm_tables(H, W)
-        d_out = eng.dpt_alloc("depth_head", K, H, W)
-        p_out = eng.dpt_alloc("point_head", K, H, W)
+        outs = {name: eng.dpt_alloc(name, K, H, W) for name, _ in heads}
+        pose_list = None
+
+        def dpt(name, act):
+            eng.dpt(name, slots, self.dpt_layers, K, H, W, head_act=act, out=outs[name])
+
         main = torch.cuda.current_stream() if images.is_cuda else None
-        if main is not None and self.head_streams:
+        if main is not None and self.head_streams and cam_on + len(heads) > 1:
             if self._streams is None:
                 self._streams = (torch.cuda.Stream(), torch.cuda.Stream())
-            s_cam, s_pt = self._streams
+            side = list(self._streams)
             fork = torch.cuda.Event()
             fork.record(main)
-            s_cam.wait_event(fork)
-            s_pt.wait_event(fork)
-            with torch.cuda.stream(s_cam):
+            work = ([("camera", None)] if cam_on else []) + heads[::-1]
+            for name, act in work[:-1]:                  # the camera head and the point head on side streams
+                s = side.pop(0)
+                s.wait_event(fork)
+                with torch.cuda.stream(s):
+                    if name == "camera":
+                        pose_list = self._camera(eng, cam_tokens, B, S)
+                    else:
+                        dpt(name, act)
+            name, act = work[-1]                         # the depth head (or the last head present) on the main stream
+            if name == "camera":
                 pose_list = self._camera(eng, cam_tokens, B, S)
-            with torch.cuda.stream(s_pt):
-                eng.dpt("point_head", slots, self.dpt_layers, K, H, W, head_act=1, out=p_out)
-            eng.dpt("depth_head", slots, self.dpt_layers, K, H, W, head_act=0, out=d_out)
-            main.wait_stream(s_cam)
-            main.wait_stream(s_pt)
+            else:
+                dpt(name, act)
+            for s in self._streams[:len(work) - 1]:
+                main.wait_stream(s)
         else:
-            pose_list = self._camera(eng, cam_tokens, B, S)
-            eng.dpt("depth_head", slots, self.dpt_layers, K, H, W, head_act=0, out=d_out)
-            eng.dpt("point_head", slots, self.dpt_layers, K, H, W, head_act=1, out=p_out)
-        predictions["pose_enc"] = pose_list[-1]
-        predictions["pose_enc_list"] = pose_list
-        predictions["depth"] = d_out[0].view(B, S, H, W, 1)
-        predictions["depth_conf"] = d_out[1].view(B, S, H, W)
-        predictions["world_points"] = p_out[0].view(B, S, H, W, 3)
-        predictions["world_points_conf"] = p_out[1].view(B, S, H, W)
+            if cam_on:
+                pose_list = self._camera(eng, cam_tokens, B, S)
+            for name, act in heads:
+                dpt(name, act)
+        if cam_on:
+            predictions["pose_enc"] = pose_list[-1]
+            predictions["pose_enc_list"] = pose_list
+        for name, _ in heads:
+            self._put_dpt(predictions, name, *outs[name], B, S, H, W)
         predictions["images"] = images
         return predictions

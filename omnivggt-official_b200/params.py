@@ -1,7 +1,8 @@
 """Parameter containers that reproduce the reference checkpoint schema (1 505 keys for the full model,
 SURVEY.md section 8b) so ``load_state_dict(strict=True)`` of a reference checkpoint works unchanged
-(reference inference.py:323-324).  These modules only *own* tensors; they have no forward().  Shapes follow the
-reference constructors cited per class."""
+(reference inference.py:323-324).  These modules own tensors; the four the reference calls on their own (aggregator,
+camera_head, depth_head, point_head: ``Component``) have a forward() that runs on the engine of the OmniVGGT owning them.
+Shapes follow the reference constructors cited per class."""
 from __future__ import annotations
 
 from typing import List, Sequence
@@ -88,7 +89,25 @@ class DinoParams(nn.Module):
         self.heads = heads
 
 
-class AggregatorParams(nn.Module):
+class Component(nn.Module):
+    """A submodule with the reference's call signature.  Its forward delegates to the OmniVGGT that owns it, held as a weak
+    reference in ``_owner`` (set by OmniVGGT.__setattr__ with object.__setattr__: not a parameter, buffer or child module, so
+    parameters(), state_dict() and _modules are those of a plain container)."""
+
+    def owner(self):
+        ref = self.__dict__.get("_owner")
+        m = ref() if ref is not None else None
+        if m is None or not any(m._modules.get(n) is self for n in ("aggregator", "camera_head", "depth_head", "point_head")):
+            raise RuntimeError(f"{type(self).__name__} is called through the OmniVGGT it belongs to; this one is not attached to one")
+        return m
+
+    def __getstate__(self):            # weak references do not pickle; OmniVGGT.__setstate__ sets the copy's
+        state = dict(super().__getstate__())
+        state.pop("_owner", None)
+        return state
+
+
+class AggregatorParams(Component):
     """models/aggregator.py:52-148 + models/omnivggt_aggregator.py:19-80."""
 
     def __init__(self, img_size, patch, dim, depth, head_dim, num_register_tokens, patch_embed, dino_depth, dino_heads):
@@ -106,6 +125,10 @@ class AggregatorParams(nn.Module):
         self.pose_embeddings = nn.ModuleList([WB((dim, 9)) for _ in range(depth + 1)])
         self.camera_adapters = nn.ModuleList([WB((dim, dim)) for _ in range(depth + 1)])
         self.depth_patch_embed = PatchEmbedParams(2, dim, patch)
+
+    def forward(self, images, extrinsics=None, intrinsics=None, depth=None, mask=None, depth_gt_index=None, camera_gt_index=None):
+        """ZeroAggregator.forward (omnivggt_aggregator.py:130-256) -> (list of depth fp32 [B, S, T, 2C], patch_start_idx)."""
+        return self.owner()._call_aggregator(images, extrinsics, intrinsics, depth, mask, depth_gt_index, camera_gt_index)
 
 
 class RCUParams(nn.Module):
@@ -143,7 +166,7 @@ class ScratchParams(nn.Module):
         self.output_conv2 = nn.ModuleDict({"0": WB((32, f // 2, 3, 3)), "2": WB((output_dim, 32, 1, 1))})
 
 
-class DPTParams(nn.Module):
+class DPTParams(Component):
     """heads/dpt_head.py:43-126."""
 
     def __init__(self, dim_in, output_dim, features, out_channels):
@@ -159,8 +182,12 @@ class DPTParams(nn.Module):
         self.scratch = ScratchParams(oc, features, output_dim)
         self.output_dim = output_dim
 
+    def forward(self, aggregated_tokens_list, images, patch_start_idx, frames_chunk_size=8):
+        """DPTHead.forward (dpt_head.py:128-183) -> (preds [B, S, H, W, output_dim - 1], conf [B, S, H, W])."""
+        return self.owner()._call_dpt(self, aggregated_tokens_list, images, patch_start_idx, frames_chunk_size)
 
-class CameraHeadParams(nn.Module):
+
+class CameraHeadParams(Component):
     """heads/camera_head.py:26-81."""
 
     def __init__(self, dim_in, trunk_depth, heads):
@@ -173,6 +200,10 @@ class CameraHeadParams(nn.Module):
         self.poseLN_modulation = nn.ModuleDict({"1": WB((3 * dim_in, dim_in))})
         self.pose_branch = MlpParams(dim_in, dim_in // 2, out=9)
         self.heads = heads
+
+    def forward(self, aggregated_tokens_list, num_iterations=4):
+        """CameraHead.forward (camera_head.py:83-103) -> list of num_iterations pose encodings [B, S, 9]."""
+        return self.owner()._call_camera(aggregated_tokens_list, num_iterations)
 
 
 @torch.no_grad()
