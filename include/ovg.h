@@ -166,6 +166,13 @@ int ovg_dpt_tail(const void* src, const float* tx, const float* ty, const void* 
 int ovg_preprocess_image(const unsigned char* src, int h, int w, int nw, int nh, int crop, int fh, const int* hmin, const int* hcnt,
                          const int* hk, int hksize, const int* vmin, const int* vcnt, const int* vk, int vksize,
                          unsigned char* tmp, float* out, void* stream);
+/* ovg_preprocess_image_canvas: the same resize, crop and ToTensor, written into the frame fp32 [3, out_h, out_w]: the [fh, nw]
+ * image at rows [off_y, off_y + fh) and columns [off_x, off_x + nw), every other pixel = fill.  One launch writes every output
+ * float once.  ovg_preprocess_image is this call with the frame (fh, nw) at offset 0.   omnivggt/utils/load_fn.py:85-136 */
+int ovg_preprocess_image_canvas(const unsigned char* src, int h, int w, int nw, int nh, int crop, int fh, const int* hmin,
+                                const int* hcnt, const int* hk, int hksize, const int* vmin, const int* vcnt, const int* vk,
+                                int vksize, unsigned char* tmp, float* out, int out_h, int out_w, int off_y, int off_x, float fill,
+                                void* stream);
 /* ovg_preprocess_depth: validity filter (non-finite, > max_depth, < 1e-5 -> 0) + nearest-neighbour resize through the index tables
  * sy[nh], sx[nw] + crop -> depth fp32 [fh, nw], mask fp32 [fh, nw] (depth > 1e-5).  src element (r, c) at
  * src[r * row_stride + c * col_stride] (the reference transposes PNG depth maps: swap the strides).   visual_util.py:768-791 */

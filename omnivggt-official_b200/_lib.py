@@ -113,6 +113,8 @@ EXPORTS = {
     "ovg_dpt_tail": (C.c_int, [_vp, _vp, _vp, _vp, _vp, _vp, _vp, _i, _i, _vp, _vp, _i, _i, _i, _i, _i, _i, _vp, _vp]),
     "ovg_upsample_bilinear": (C.c_int, [_vp, _vp, _vp, _vp, _i, _i, _i, _i, _i, _i, _i, _vp]),
     "ovg_preprocess_image": (C.c_int, [_vp, _i, _i, _i, _i, _i, _i, _vp, _vp, _vp, _i, _vp, _vp, _vp, _i, _vp, _vp, _vp]),
+    "ovg_preprocess_image_canvas": (C.c_int, [_vp, _i, _i, _i, _i, _i, _i, _vp, _vp, _vp, _i, _vp, _vp, _vp, _i, _vp, _vp, _i, _i,
+                                              _i, _i, _f, _vp]),
     "ovg_preprocess_depth": (C.c_int, [_vp, _ll, _ll, _vp, _vp, _i, _i, _i, _f, _vp, _vp, _vp]),
     "ovg_prepare_cameras": (C.c_int, [_vp, _vp, _vp, _vp, _vp, _vp, _i, _vp]),
     "ovg_pose_decode": (C.c_int, [_vp, _vp, _vp, _vp, _i, _i, _i, _vp]),

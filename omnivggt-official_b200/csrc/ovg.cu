@@ -577,13 +577,15 @@ int ovg_dpt_tail(const void* src, const float* tx, const float* ty, const void* 
   return post_launch("ovg_dpt_tail");
 }
 
-int ovg_preprocess_image(const unsigned char* src, int h, int w, int nw, int nh, int crop, int fh, const int* hmin, const int* hcnt,
-                         const int* hk, int hksize, const int* vmin, const int* vcnt, const int* vk, int vksize,
-                         unsigned char* tmp, float* out, void* stream) {
+int ovg_preprocess_image_canvas(const unsigned char* src, int h, int w, int nw, int nh, int crop, int fh, const int* hmin,
+                                const int* hcnt, const int* hk, int hksize, const int* vmin, const int* vcnt, const int* vk,
+                                int vksize, unsigned char* tmp, float* out, int out_h, int out_w, int off_y, int off_x, float fill,
+                                void* stream) {
   OVG_REQUIRE(src && out && h > 0 && w > 0 && nw > 0 && nh > 0 && crop >= 0 && fh > 0 && crop + fh <= nh, "bad geometry");
   OVG_REQUIRE(w == nw || (hmin && hcnt && hk && hksize > 0 && tmp), "horizontal pass needs its tap table and a temporary");
   OVG_REQUIRE(h == nh || (vmin && vcnt && vk && vksize > 0), "vertical pass needs its tap table");
-  OVG_REQUIRE(h <= 65535 && fh <= 65535, "image too tall");
+  OVG_REQUIRE(off_y >= 0 && off_x >= 0 && off_y + fh <= out_h && off_x + nw <= out_w, "image does not fit its output frame");
+  OVG_REQUIRE(h <= 65535 && out_h <= 65535, "image too tall");
   cudaStream_t st = reinterpret_cast<cudaStream_t>(stream);
   const unsigned char* mid = src;
   if (w != nw) {
@@ -593,9 +595,17 @@ int ovg_preprocess_image(const unsigned char* src, int h, int w, int nw, int nh,
     if (rc) return rc;
     mid = tmp;
   }
-  ovg::ResizeParams pv{mid, nullptr, out, vmin, vcnt, vk, vksize, h, w, nw, crop, fh, h == nh ? 1 : 0};
-  ovg::resize_v_u8_f32_kernel<<<dim3((nw + 127) / 128, fh), 128, 0, st>>>(pv);
+  ovg::ResizeParams pv{mid, nullptr, out, vmin, vcnt, vk, vksize, h, w, nw, crop, fh, h == nh ? 1 : 0,
+                       out_h, out_w, off_y, off_x, fill};
+  ovg::resize_v_u8_f32_kernel<<<dim3((out_w + 127) / 128, out_h), 128, 0, st>>>(pv);
   return post_launch("ovg_preprocess_image");
+}
+
+int ovg_preprocess_image(const unsigned char* src, int h, int w, int nw, int nh, int crop, int fh, const int* hmin, const int* hcnt,
+                         const int* hk, int hksize, const int* vmin, const int* vcnt, const int* vk, int vksize,
+                         unsigned char* tmp, float* out, void* stream) {
+  return ovg_preprocess_image_canvas(src, h, w, nw, nh, crop, fh, hmin, hcnt, hk, hksize, vmin, vcnt, vk, vksize, tmp, out, fh, nw,
+                                     0, 0, 0.f, stream);
 }
 
 int ovg_preprocess_depth(const float* src, long long row_stride, long long col_stride, const int* sy, const int* sx, int crop,

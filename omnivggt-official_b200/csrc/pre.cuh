@@ -3,6 +3,8 @@
 //   resize_h_u8 / resize_v_u8_f32   Image.resize(..., BICUBIC) -- Pillow's two-pass fixed-point convolution (Resample.c:
 //                                   22-bit taps, rounding and clip to uint8 after EACH pass), bit-exact -- then the centre crop
 //                                   and ToTensor (uint8 / 255, CHW fp32)                             visual_util.py:731-751
+//                                   placed in a larger frame padded with a constant, for utils/load_fn.py's pad mode and
+//                                   mixed-size lists (white padding)                                 load_fn.py:85-136
 //   depth_nearest                   validity filter + cv2.resize(..., INTER_NEAREST) + crop + mask   visual_util.py:768-791
 //   camera_prepare                  intrinsics rescale / crop shift, camera-to-world -> world-to-camera   :807-820
 // The per-axis tap tables and nearest-neighbour index tables are a few KB, computed once per image size on the host
@@ -29,6 +31,9 @@ struct ResizeParams {
   int ksize;
   int h, w, nw, crop, fh;
   int identity;         // this axis keeps its size: Pillow skips the pass
+  int out_h, out_w;     // vertical: the output frame [3, out_h, out_w] ...
+  int off_y, off_x;     // ... holds the [fh, nw] image at (off_y, off_x) ...
+  float fill;           // ... and this value everywhere else (load_fn.py's white padding)
 };
 
 __global__ void __launch_bounds__(128) resize_h_u8_kernel(const ResizeParams p) {
@@ -51,33 +56,41 @@ __global__ void __launch_bounds__(128) resize_h_u8_kernel(const ResizeParams p) 
   o[2] = static_cast<uint8_t>(pre_clip8(s2));
 }
 
-// vertical pass over the (already horizontally resized) rows, only for the rows that survive the centre crop
+// vertical pass over the (already horizontally resized) rows, only for the rows that survive the centre crop; one thread per
+// pixel of the output frame, so every output float is written exactly once (image pixels and padding alike)
 __global__ void __launch_bounds__(128) resize_v_u8_f32_kernel(const ResizeParams p) {
-  const int x = blockIdx.x * blockDim.x + threadIdx.x, yo = blockIdx.y;
-  if (x >= p.nw) return;
-  const int y = yo + p.crop;
-  int v0, v1, v2;
-  if (p.identity) {
-    const uint8_t* px = p.src + (static_cast<long long>(y) * p.nw + x) * 3;
-    v0 = px[0]; v1 = px[1]; v2 = px[2];
-  } else {
-    const int y0 = p.kmin[y], n = p.kcnt[y];
-    const int* k = p.kk + static_cast<long long>(y) * p.ksize;
-    int s0 = 1 << (PRE_PRECISION_BITS - 1), s1 = s0, s2 = s0;
-    for (int t = 0; t < n; ++t) {
-      const int kv = k[t];
-      const uint8_t* px = p.src + (static_cast<long long>(y0 + t) * p.nw + x) * 3;
-      s0 += px[0] * kv;
-      s1 += px[1] * kv;
-      s2 += px[2] * kv;
+  const int xo = blockIdx.x * blockDim.x + threadIdx.x, yo = blockIdx.y;
+  if (xo >= p.out_w) return;
+  const int x = xo - p.off_x, yi = yo - p.off_y;
+  float f0 = p.fill, f1 = p.fill, f2 = p.fill;
+  if (x >= 0 && x < p.nw && yi >= 0 && yi < p.fh) {
+    const int y = yi + p.crop;
+    int v0, v1, v2;
+    if (p.identity) {
+      const uint8_t* px = p.src + (static_cast<long long>(y) * p.nw + x) * 3;
+      v0 = px[0]; v1 = px[1]; v2 = px[2];
+    } else {
+      const int y0 = p.kmin[y], n = p.kcnt[y];
+      const int* k = p.kk + static_cast<long long>(y) * p.ksize;
+      int s0 = 1 << (PRE_PRECISION_BITS - 1), s1 = s0, s2 = s0;
+      for (int t = 0; t < n; ++t) {
+        const int kv = k[t];
+        const uint8_t* px = p.src + (static_cast<long long>(y0 + t) * p.nw + x) * 3;
+        s0 += px[0] * kv;
+        s1 += px[1] * kv;
+        s2 += px[2] * kv;
+      }
+      v0 = pre_clip8(s0); v1 = pre_clip8(s1); v2 = pre_clip8(s2);
     }
-    v0 = pre_clip8(s0); v1 = pre_clip8(s1); v2 = pre_clip8(s2);
+    f0 = static_cast<float>(v0) / 255.0f;               // ToTensor: uint8 -> float32, div(255)
+    f1 = static_cast<float>(v1) / 255.0f;
+    f2 = static_cast<float>(v2) / 255.0f;
   }
-  const long long plane = static_cast<long long>(p.fh) * p.nw;
-  float* o = p.dst_f32 + static_cast<long long>(yo) * p.nw + x;
-  o[0] = static_cast<float>(v0) / 255.0f;               // ToTensor: uint8 -> float32, div(255)
-  o[plane] = static_cast<float>(v1) / 255.0f;
-  o[2 * plane] = static_cast<float>(v2) / 255.0f;
+  const long long plane = static_cast<long long>(p.out_h) * p.out_w;
+  float* o = p.dst_f32 + static_cast<long long>(yo) * p.out_w + xo;
+  o[0] = f0;
+  o[plane] = f1;
+  o[2 * plane] = f2;
 }
 
 struct DepthNearestParams {

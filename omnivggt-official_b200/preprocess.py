@@ -5,7 +5,11 @@ then does per view with Pillow / OpenCV / numpy -- bicubic resize to width 518, 
 depth validity filter + nearest resize + crop + mask, intrinsics rescale, camera-to-world -> world-to-camera -- runs in libovg
 kernels on the device and returns the model's input tuple as CUDA tensors.  The small per-size tap / index tables are computed on
 the host with the arithmetic the two libraries publish (Pillow Resample.c, OpenCV resizeNN) and cached on the device, so the image
-tensor equals the reference's bit for bit (tests/test_preprocess.py compares against Pillow / OpenCV and the reference loader)."""
+tensor equals the reference's bit for bit (tests/test_preprocess.py compares against Pillow / OpenCV and the reference loader).
+
+``load_and_preprocess_images`` / ``preprocess_images`` are the same for the reference's quick-start loader
+(omnivggt/utils/load_fn.py:12-146): crop or pad mode, and lists of mixed image sizes padded with white to the largest shape,
+written straight into the output frame by the resize kernel (tests/test_load_fn.py)."""
 from __future__ import annotations
 
 import glob
@@ -77,6 +81,34 @@ def nearest_index(src: int, dst: int, device) -> torch.Tensor:
     return _tables[key][0]
 
 
+def decode_rgb(path: str) -> np.ndarray:
+    """uint8 RGB [h, w, 3] of an image file; RGBA is composited on white first (visual_util.py:722-726, load_fn.py:59-66)."""
+    from PIL import Image
+    img = Image.open(path)
+    if img.mode == "RGBA":
+        img = Image.alpha_composite(Image.new("RGBA", img.size, (255, 255, 255, 255)), img)
+    return np.asarray(img.convert("RGB"))
+
+
+def _resize_view(lib, st, im, nw: int, nh: int, crop: int, fh: int, out: torch.Tensor, dev, frame=None, fill: float = 1.0) -> list:
+    """Upload one uint8 RGB view [h, w, 3] and launch its bicubic resize to [nh, nw], rows [crop, crop + fh) and ToTensor into
+    out [3, fh, nw]; with frame = (out_h, out_w, off_y, off_x), into the frame out [3, out_h, out_w] at that offset, the rest
+    set to fill.  Returns the staging tensors, which must stay alive until the launches have run."""
+    h, w = int(im.shape[0]), int(im.shape[1])
+    src = torch.as_tensor(np.array(im, dtype=np.uint8, copy=True) if isinstance(im, np.ndarray) else im, dtype=torch.uint8).to(dev).contiguous()
+    assert src.shape == (h, w, 3), "images are uint8 RGB [h, w, 3]"
+    hk = bicubic_taps(w, nw, dev) if w != nw else (None, None, None, 0)
+    vk = bicubic_taps(h, nh, dev) if h != nh else (None, None, None, 0)
+    tmp = torch.empty(h, nw, 3, device=dev, dtype=torch.uint8) if w != nw else None
+    args = (src.data_ptr(), h, w, nw, nh, crop, fh, L.ptr(hk[0]), L.ptr(hk[1]), L.ptr(hk[2]), hk[3], L.ptr(vk[0]), L.ptr(vk[1]),
+            L.ptr(vk[2]), vk[3], L.ptr(tmp), out.data_ptr())
+    if frame is None:
+        L.check(lib.ovg_preprocess_image(*args, st))
+    else:
+        L.check(lib.ovg_preprocess_image_canvas(*args, *frame, float(fill), st))
+    return [src, tmp]
+
+
 @torch.no_grad()
 def preprocess_views(images: Sequence, cameras: Optional[Sequence] = None, depths: Optional[Sequence] = None,
                      target_size: int = 518, max_depth: float = 100.0, device="cuda", depth_transposed: Optional[Sequence[bool]] = None):
@@ -107,14 +139,7 @@ def preprocess_views(images: Sequence, cameras: Optional[Sequence] = None, depth
     st = L.stream()
     keep = []
     for i, (im, (h, w, _, nh, crop, _)) in enumerate(zip(images, geoms)):
-        src = torch.as_tensor(np.array(im, dtype=np.uint8, copy=True) if isinstance(im, np.ndarray) else im, dtype=torch.uint8).to(dev).contiguous()
-        assert src.shape == (h, w, 3), "images are uint8 RGB [h, w, 3]"
-        hk = bicubic_taps(w, nw, dev) if w != nw else (None, None, None, 0)
-        vk = bicubic_taps(h, nh, dev) if h != nh else (None, None, None, 0)
-        tmp = torch.empty(h, nw, 3, device=dev, dtype=torch.uint8) if w != nw else None
-        L.check(lib.ovg_preprocess_image(src.data_ptr(), h, w, nw, nh, crop, fh, L.ptr(hk[0]), L.ptr(hk[1]), L.ptr(hk[2]), hk[3],
-                                         L.ptr(vk[0]), L.ptr(vk[1]), L.ptr(vk[2]), vk[3], L.ptr(tmp), out[i].data_ptr(), st))
-        keep += [src, tmp]
+        keep += _resize_view(lib, st, im, nw, nh, crop, fh, out[i], dev)
         dep = depths[i]
         if dep is not None:
             d = torch.as_tensor(np.ascontiguousarray(dep, dtype=np.float32) if isinstance(dep, np.ndarray) else dep).float().to(dev).contiguous()
@@ -170,10 +195,7 @@ def load_images_and_cameras(image_folder: str, camera_folder: Optional[str] = No
     images, cams, deps, transposed = [], [], [], []
     for p in paths:
         stem = Path(p).stem
-        img = Image.open(p)
-        if img.mode == "RGBA":                                   # white background (visual_util.py:722-726)
-            img = Image.alpha_composite(Image.new("RGBA", img.size, (255, 255, 255, 255)), img)
-        images.append(np.asarray(img.convert("RGB")))
+        images.append(decode_rgb(p))
         dep, tr = None, False
         if depth_folder is not None:
             for cand in (os.path.join(depth_folder, stem + ".npy"), os.path.join(depth_folder, stem + ".png")):
@@ -189,3 +211,67 @@ def load_images_and_cameras(image_folder: str, camera_folder: Optional[str] = No
             cam = read_camera_txt(os.path.join(camera_folder, stem + ".txt"))
         cams.append(cam)
     return preprocess_views(images, cams, deps, target_size, max_depth, device, transposed)
+
+
+LOAD_FN_SIZE = 518           # load_fn.py:50; fixed in the reference
+
+
+def _check_load_fn_args(n: int, mode: str) -> None:
+    if n == 0:
+        raise ValueError("At least 1 image is required")
+    if mode not in ("crop", "pad"):
+        raise ValueError("Mode must be either 'crop' or 'pad'")
+
+
+def load_fn_layout(sizes: Sequence[Tuple[int, int]], mode: str = "crop"):
+    """Geometry of reference load_and_preprocess_images (load_fn.py:68-136) for images of sizes [(h, w)].
+    Returns (views, (H, W), shapes): per image (new_width, new_height, crop_start_y, kept_height, off_y, off_x), where
+    off_* is where its [kept_height, new_width] pixels sit in the output frame [H, W]; and the set of shapes before the
+    mixed-size padding, in the reference's insertion order (it prints that set).  Raises ValueError before any device work."""
+    _check_load_fn_args(len(sizes), mode)
+    T = LOAD_FN_SIZE
+    first, shapes = [], set()
+    for h, w in sizes:
+        if mode == "pad" and h > w:                 # :75-77 the height is the longer side: it becomes 518
+            nw, nh = round(w * (T / h) / 14) * 14, T
+            crop, fh = 0, nh
+        else:                                       # :72-74, :78-82 the width becomes 518; crop mode keeps 518 rows (:89-91)
+            nw, nh, crop, fh = target_geometry(w, h, T)
+        if nw <= 0 or nh <= 0:
+            raise ValueError(f"a {w}x{h} image resizes to {nw}x{nh}: height and width must be > 0")
+        if mode == "pad":                           # :94-107 centred in 518 x 518
+            top, left, shape = (T - fh) // 2, (T - nw) // 2, (T, T)
+        else:
+            top, left, shape = 0, 0, (fh, nw)
+        first.append((nw, nh, crop, fh, top, left, shape))
+        shapes.add(shape)
+    H, W = max(s[0] for s in shapes), max(s[1] for s in shapes)
+    # :114-136 a second centring pad to the largest shape; the offset is the sum of both pads, each rounded down on its own
+    views = [(nw, nh, crop, fh, top + (H - s[0]) // 2, left + (W - s[1]) // 2) for nw, nh, crop, fh, top, left, s in first]
+    return views, (H, W), shapes
+
+
+@torch.no_grad()
+def preprocess_images(images: Sequence, mode: str = "crop", device="cuda") -> torch.Tensor:
+    """Reference load_and_preprocess_images (load_fn.py:12-146) on decoded images: uint8 RGB arrays / tensors [h, w, 3], in
+    the given order.  Returns CUDA fp32 [N, 3, H, W], bit-identical to the reference: Pillow-exact bicubic resize, crop or
+    white (1.0) padding to 518 x 518, then white padding of mixed sizes to the largest shape, each view in one libovg call."""
+    views, (H, W), shapes = load_fn_layout([(int(im.shape[0]), int(im.shape[1])) for im in images], mode)
+    if len(shapes) > 1:
+        print(f"Warning: Found images with different shapes: {shapes}")
+    lib = L.lib()
+    dev = torch.device(device)
+    out = torch.empty(len(views), 3, H, W, device=dev, dtype=torch.float32)
+    st = L.stream()
+    keep = []
+    for i, (im, (nw, nh, crop, fh, off_y, off_x)) in enumerate(zip(images, views)):
+        keep += _resize_view(lib, st, im, nw, nh, crop, fh, out[i], dev, frame=(H, W, off_y, off_x), fill=1.0)
+    torch.cuda.current_stream().synchronize()     # the staging tensors in `keep` are released after the kernels ran
+    return out
+
+
+def load_and_preprocess_images(image_path_list: Sequence[str], mode: str = "crop", device="cuda") -> torch.Tensor:
+    """Same signature (plus device) and result as reference omnivggt.utils.load_fn.load_and_preprocess_images: the paths are
+    sorted and decoded on the host (Pillow; RGBA on white), the rest runs on the GPU (preprocess_images)."""
+    _check_load_fn_args(len(image_path_list), mode)
+    return preprocess_images([decode_rgb(p) for p in sorted(image_path_list)], mode, device)
