@@ -231,6 +231,51 @@ int ovg_point_cloud_center(const float* points, long long n, void* workspace, lo
 int ovg_point_cloud_scale(const float* xyz, long long n_kept, long long ld, void* workspace, long long workspace_bytes,
                           float* scale_out, void* stream);
 
+/* Baseline JPEG decoding on the device, bit-identical to Pillow (libjpeg-turbo's default islow IDCT, fancy upsampling and
+ * YCbCr -> RGB tables).  The plan is host code (no CUDA call): it parses every file, routes it to the device or to the host
+ * (OVG_JPEG_* below: anything the device cannot decode exactly goes to the host), and builds the staging stream (tables plus the
+ * entropy data with stuffed bytes and RST markers removed, one segment per restart interval).
+ * ovg_jpeg_plan_create: files[i] / nbytes[i] the n encoded files (the plan copies what it needs); subseq_bits: bits per
+ * subsequence of the parallel Huffman decoder, 0 = the default (512), else OVG_JPEG_MIN_SUBSEQ_BITS .. 65536. */
+#define OVG_JPEG_DEVICE 0
+#define OVG_JPEG_NOT_JPEG 1
+#define OVG_JPEG_TRUNCATED 2    /* no EOI, or the file ends inside a segment */
+#define OVG_JPEG_PROCESS 3      /* not SOF0 / SOF1: progressive, lossless, arithmetic coding */
+#define OVG_JPEG_PRECISION 4    /* not 8-bit */
+#define OVG_JPEG_COLOR 5        /* not 1 or 3 components, or 3 that libjpeg would not treat as YCbCr */
+#define OVG_JPEG_SAMPLING 6     /* luma other than 1x1 / 2x1 / 2x2, chroma other than 1x1 */
+#define OVG_JPEG_SCANS 7        /* several scans, a partial scan, DNL */
+#define OVG_JPEG_TABLES 8       /* a missing or invalid quantisation / Huffman table */
+#define OVG_JPEG_MARKER 9       /* an unexpected marker */
+#define OVG_JPEG_RESTART 10     /* RST markers out of sequence or not matching the restart interval */
+#define OVG_JPEG_SIZE 11        /* zero width or height */
+#define OVG_JPEG_MIN_SUBSEQ_BITS 32
+typedef struct ovg_jpeg_plan ovg_jpeg_plan;
+int ovg_jpeg_plan_create(const unsigned char* const* files, const long long* nbytes, int n, int subseq_bits,
+                         ovg_jpeg_plan** plan);
+void ovg_jpeg_plan_destroy(ovg_jpeg_plan* plan);
+/* file i: routing reason (OVG_JPEG_*), and for device-routed files the output size [height, width, 3] and component count */
+int ovg_jpeg_plan_file(const ovg_jpeg_plan* plan, int i, int* route, int* width, int* height, int* ncomp);
+long long ovg_jpeg_plan_stream_bytes(const ovg_jpeg_plan* plan);
+long long ovg_jpeg_plan_workspace_bytes(const ovg_jpeg_plan* plan);
+long long ovg_jpeg_plan_subsequences(const ovg_jpeg_plan* plan);
+long long ovg_jpeg_plan_segments(const ovg_jpeg_plan* plan);
+/* segment k: file index, byte offset of its unstuffed data in the staging stream, its length, first MCU and MCU count */
+int ovg_jpeg_plan_segment(const ovg_jpeg_plan* plan, long long k, int* file, long long* offset, long long* nbytes, int* first_mcu,
+                          int* n_mcu);
+/* writes the ovg_jpeg_plan_stream_bytes() staging stream to dst (host memory; pinned for an asynchronous upload) */
+int ovg_jpeg_plan_fill_stream(const ovg_jpeg_plan* plan, void* dst);
+/* sync rounds the last ovg_jpeg_decode with this plan needed (>= 1) */
+int ovg_jpeg_plan_rounds(const ovg_jpeg_plan* plan);
+/* ovg_jpeg_decode: decodes every device-routed file.  d_stream: the staging stream on the device (256-byte aligned);
+ * d_out[i]: uint8 RGB [height, width, 3] for device-routed files (ignored otherwise); d_status[n]: zeroed here, then non-zero for
+ * a file whose entropy data is inconsistent (code not in its table, coefficient past z = 63, wrong block count, data ending early)
+ * or that has a block outside the range where libjpeg-turbo's C and SIMD IDCTs agree (dequantised coefficients or pass-1 outputs
+ * beyond +-16383, samples before the range limit outside [-512, 511]): decode that file on the host.  workspace: ovg_jpeg_plan_workspace_bytes() bytes, 256-byte aligned.  The sync rounds of the
+ * Huffman decoder read a flag back after each round (stream synchronisations); everything else is enqueued on `stream`. */
+int ovg_jpeg_decode(ovg_jpeg_plan* plan, const void* d_stream, unsigned char* const* d_out, unsigned* d_status, void* workspace,
+                    long long workspace_bytes, void* stream);
+
 /* ======================================================================================================================
  * Runtime: the launch SEQUENCES of the hot path behind handles, so that a host in any language runs the path with three
  * calls and raw device pointers (SURVEY.md section 8b).  Weight pointers refer to device memory in kernel layout (bf16

@@ -125,6 +125,17 @@ EXPORTS = {
     "ovg_point_cloud_gather": (C.c_int, [_vp, _vp, _vp, _i, _i, _i, _i, _i, _i, _vp, _ll, _vp, _vp, _vp, _vp, _ll, _vp]),
     "ovg_point_cloud_center": (C.c_int, [_vp, _ll, _vp, _ll, _vp, _vp]),
     "ovg_point_cloud_scale": (C.c_int, [_vp, _ll, _ll, _vp, _ll, _vp, _vp]),
+    "ovg_jpeg_plan_create": (C.c_int, [_pp, C.POINTER(_ll), _i, _i, _pp]),
+    "ovg_jpeg_plan_destroy": (None, [_vp]),
+    "ovg_jpeg_plan_file": (C.c_int, [_vp, _i, C.POINTER(_i), C.POINTER(_i), C.POINTER(_i), C.POINTER(_i)]),
+    "ovg_jpeg_plan_stream_bytes": (_ll, [_vp]),
+    "ovg_jpeg_plan_workspace_bytes": (_ll, [_vp]),
+    "ovg_jpeg_plan_subsequences": (_ll, [_vp]),
+    "ovg_jpeg_plan_segments": (_ll, [_vp]),
+    "ovg_jpeg_plan_segment": (C.c_int, [_vp, _ll, C.POINTER(_i), C.POINTER(_ll), C.POINTER(_ll), C.POINTER(_i), C.POINTER(_i)]),
+    "ovg_jpeg_plan_fill_stream": (C.c_int, [_vp, _vp]),
+    "ovg_jpeg_plan_rounds": (C.c_int, [_vp]),
+    "ovg_jpeg_decode": (C.c_int, [_vp, _vp, _pp, _vp, _vp, _ll, _vp]),
     # ---- runtime (handle-level sequences)
     "ovg_aggregator_create": (C.c_int, [C.POINTER(AggregatorDesc), _pp]),
     "ovg_aggregator_destroy": (None, [_vp]),
@@ -155,6 +166,53 @@ PERCENTILE_WORKSPACE_BYTES = 6 * 8 + 512 * 4 + 4 * 4
 def DEPTH_SCRATCH_DOUBLES(B: int) -> int:
     """Mirror of OVG_DEPTH_SCRATCH_DOUBLES (include/ovg.h)."""
     return B * (2 * 1024 + 1)
+
+JPEG_DEVICE = 0                 # OVG_JPEG_DEVICE; the other OVG_JPEG_* values are host-routing reasons
+JPEG_MIN_SUBSEQ_BITS = 32       # OVG_JPEG_MIN_SUBSEQ_BITS
+
+
+class JpegPlan:
+    """Owner of an ``ovg_jpeg_plan`` (host code, no GPU needed): routing, sizes and the staging stream of a list of files."""
+
+    def __init__(self, files, subseq_bits: int = 0):
+        l = load()
+        self._lib = l
+        self.n = len(files)
+        files = [bytes(f) for f in files]                  # no copy for bytes; the plan copies what it keeps
+        ptrs = (_vp * max(self.n, 1))(*[C.cast(C.c_char_p(f), _vp) for f in files])
+        sizes = (_ll * max(self.n, 1))(*[len(f) for f in files])
+        h = _vp()
+        check(l.ovg_jpeg_plan_create(ptrs, sizes, self.n, int(subseq_bits), C.byref(h)))
+        self.handle = h
+        self.files = []
+        for i in range(self.n):
+            r, w, hh, c = _i(), _i(), _i(), _i()
+            check(l.ovg_jpeg_plan_file(h, i, C.byref(r), C.byref(w), C.byref(hh), C.byref(c)))
+            self.files.append((r.value, hh.value, w.value, c.value))       # (route, height, width, components)
+        self.stream_bytes = l.ovg_jpeg_plan_stream_bytes(h)
+        self.workspace_bytes = l.ovg_jpeg_plan_workspace_bytes(h)
+        self.subsequences = l.ovg_jpeg_plan_subsequences(h)
+
+    def segments(self):
+        """[(file, stream byte offset, bytes, first MCU, MCUs)] in stream order."""
+        out = []
+        for k in range(self._lib.ovg_jpeg_plan_segments(self.handle)):
+            f, o, nb, m, nm = _i(), _ll(), _ll(), _i(), _i()
+            check(self._lib.ovg_jpeg_plan_segment(self.handle, k, C.byref(f), C.byref(o), C.byref(nb), C.byref(m), C.byref(nm)))
+            out.append((f.value, o.value, nb.value, m.value, nm.value))
+        return out
+
+    def fill_stream(self, dst_ptr: int) -> None:
+        check(self._lib.ovg_jpeg_plan_fill_stream(self.handle, dst_ptr))
+
+    def rounds(self) -> int:
+        return self._lib.ovg_jpeg_plan_rounds(self.handle)
+
+    def __del__(self):
+        if getattr(self, "handle", None):
+            self._lib.ovg_jpeg_plan_destroy(self.handle)
+            self.handle = None
+
 
 _lib: Optional[C.CDLL] = None
 _device_ok = False

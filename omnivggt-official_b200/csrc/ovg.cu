@@ -16,6 +16,7 @@
 #include "post.cuh"
 #include "tail.cuh"
 #include "pre.cuh"
+#include "jpeg.cuh"
 
 namespace {
 
@@ -828,6 +829,130 @@ int ovg_point_cloud_scale(const float* xyz, long long n_kept, long long ld, void
     }
   ovg::cloud_scale_kernel<<<1, 32, 0, st>>>(w.sel, scale_out);
   return post_launch("ovg_point_cloud_scale");
+}
+
+}  // extern "C"
+
+// ------------------------------------------------------------------------------------------------------------- JPEG decode
+struct ovg_jpeg_plan : ovg::jpg::Plan {};
+
+extern "C" {
+
+int ovg_jpeg_plan_create(const unsigned char* const* files, const long long* nbytes, int n, int subseq_bits,
+                         ovg_jpeg_plan** plan) {
+  OVG_REQUIRE(plan && n >= 0 && (n == 0 || (files && nbytes)), "bad arguments");
+  OVG_REQUIRE(subseq_bits == 0 || (subseq_bits >= ovg::jpg::MIN_SUBSEQ_BITS && subseq_bits <= ovg::jpg::MAX_SUBSEQ_BITS),
+              "subseq_bits must be 0 or in [OVG_JPEG_MIN_SUBSEQ_BITS, 65536]");
+  ovg_jpeg_plan* out = nullptr;
+  try {
+    out = new ovg_jpeg_plan;
+    ovg::jpg::plan_build(out, files, nbytes, n, subseq_bits);
+  } catch (const std::exception& e) {
+    delete out;
+    return fail(OVG_E_INVALID, std::string("ovg_jpeg_plan_create: ") + e.what());
+  }
+  *plan = out;
+  return OVG_OK;
+}
+
+void ovg_jpeg_plan_destroy(ovg_jpeg_plan* plan) { delete plan; }
+
+int ovg_jpeg_plan_file(const ovg_jpeg_plan* plan, int i, int* route, int* width, int* height, int* ncomp) {
+  OVG_REQUIRE(plan && i >= 0 && i < static_cast<int>(plan->route.size()), "bad file index");
+  if (route) *route = plan->route[i];
+  if (width) *width = plan->width[i];
+  if (height) *height = plan->height[i];
+  if (ncomp) *ncomp = plan->ncomp[i];
+  return OVG_OK;
+}
+
+long long ovg_jpeg_plan_stream_bytes(const ovg_jpeg_plan* plan) { return plan ? plan->stream_bytes : -1; }
+long long ovg_jpeg_plan_subsequences(const ovg_jpeg_plan* plan) { return plan ? plan->nsub : -1; }
+long long ovg_jpeg_plan_segments(const ovg_jpeg_plan* plan) { return plan ? static_cast<long long>(plan->segs.size()) : -1; }
+int ovg_jpeg_plan_rounds(const ovg_jpeg_plan* plan) { return plan ? plan->rounds : -1; }
+
+long long ovg_jpeg_plan_workspace_bytes(const ovg_jpeg_plan* plan) {
+  return plan ? ovg::jpg::plan_workspace(plan, static_cast<int>(plan->route.size()), nullptr).bytes : -1;
+}
+
+int ovg_jpeg_plan_segment(const ovg_jpeg_plan* plan, long long k, int* file, long long* offset, long long* nbytes, int* first_mcu,
+                          int* n_mcu) {
+  OVG_REQUIRE(plan && k >= 0 && k < static_cast<long long>(plan->segs.size()), "bad segment index");
+  const ovg::jpg::HostSeg& s = plan->segs[k];
+  if (file) *file = plan->files[s.file].out_index;
+  if (offset) *offset = plan->data_off + s.byte_off;
+  if (nbytes) *nbytes = s.nbytes;
+  if (first_mcu) *first_mcu = s.first_mcu;
+  if (n_mcu) *n_mcu = s.n_mcu;
+  return OVG_OK;
+}
+
+int ovg_jpeg_plan_fill_stream(const ovg_jpeg_plan* plan, void* dst) {
+  OVG_REQUIRE(plan && (dst || plan->stream_bytes == 0), "bad arguments");
+  ovg::jpg::plan_fill(plan, static_cast<uint8_t*>(dst));
+  return OVG_OK;
+}
+
+int ovg_jpeg_decode(ovg_jpeg_plan* plan, const void* d_stream, unsigned char* const* d_out, unsigned* d_status, void* workspace,
+                    long long workspace_bytes, void* stream) {
+  using namespace ovg::jpg;
+  OVG_REQUIRE(plan && d_status, "bad arguments");
+  const int n = static_cast<int>(plan->route.size());
+  cudaStream_t st = reinterpret_cast<cudaStream_t>(stream);
+  if (n) OVG_CUDA(cudaMemsetAsync(d_status, 0, sizeof(unsigned) * n, st));
+  plan->rounds = 0;
+  if (plan->files.empty()) return OVG_OK;
+  OVG_REQUIRE(d_stream && d_out && workspace && (reinterpret_cast<uintptr_t>(d_stream) & 255) == 0 &&
+              (reinterpret_cast<uintptr_t>(workspace) & 255) == 0, "stream and workspace must be 256-byte aligned");
+  const Workspace w = plan_workspace(plan, n, workspace);
+  OVG_REQUIRE(workspace_bytes >= w.bytes, "workspace smaller than ovg_jpeg_plan_workspace_bytes()");
+  for (const FileDev& f : plan->files) OVG_REQUIRE(d_out[f.out_index], "null output for a device-routed file");
+  const uint8_t* base = static_cast<const uint8_t*>(d_stream);
+  Params p;
+  p.files = reinterpret_cast<const FileDev*>(base + plan->files_off);
+  p.segs = reinterpret_cast<const SegDev*>(base + plan->segs_off);
+  p.huffs = reinterpret_cast<const Huff*>(base + plan->huffs_off);
+  p.data = base + plan->data_off;
+  p.nfiles = static_cast<int>(plan->files.size());
+  p.nsegs = static_cast<int>(plan->segs.size());
+  p.nsub = plan->nsub; p.nblocks = plan->nblocks; p.npix = plan->npix;
+  p.subseq_bits = plan->subseq_bits;
+  p.exits = w.exits; p.counts = w.counts; p.pre = w.pre; p.chunk = w.chunk; p.coef = w.coef;
+  p.dc_agg = w.dc_agg; p.dc_aggf = w.dc_aggf; p.dc_head = w.dc_head; p.planes = w.planes; p.out = w.out;
+  p.status = d_status; p.changed = w.changed;
+  OVG_CUDA(cudaMemcpyAsync(w.out, d_out, sizeof(void*) * n, cudaMemcpyHostToDevice, st));
+  OVG_CUDA(cudaMemsetAsync(w.exits, 0, 4 * plan->nsub, st));
+  // sync rounds: each round fixes at least one more subsequence, so at most nsub + 1 rounds
+  const unsigned sub_grid = static_cast<unsigned>((plan->nsub + 255) / 256);
+  for (long long r = 0; r <= plan->nsub; ++r) {
+    OVG_CUDA(cudaMemsetAsync(w.changed, 0, 4, st));
+    jpeg_sync_kernel<<<sub_grid, 256, 0, st>>>(p);
+    int rc = post_launch("ovg_jpeg_decode(sync)");
+    if (rc) return rc;
+    int changed = 0;
+    OVG_CUDA(cudaMemcpyAsync(&changed, w.changed, 4, cudaMemcpyDeviceToHost, st));
+    OVG_CUDA(cudaStreamSynchronize(st));
+    plan->rounds = static_cast<int>(r + 1);
+    if (!changed) break;
+  }
+  const long long nsub_chunks = (plan->nsub + SCAN_CHUNK - 1) / SCAN_CHUNK;
+  jpeg_count_scan_local_kernel<<<static_cast<unsigned>(nsub_chunks), SCAN_CHUNK, 0, st>>>(p);
+  int rc = post_launch("ovg_jpeg_decode(count scan)");
+  if (rc) return rc;
+  jpeg_count_scan_chunks_kernel<<<1, SCAN_CHUNK, 0, st>>>(w.chunk, nsub_chunks);
+  if ((rc = post_launch("ovg_jpeg_decode(count scan chunks)"))) return rc;
+  OVG_CUDA(cudaMemsetAsync(w.coef, 0, 128 * plan->nblocks, st));
+  jpeg_write_kernel<<<sub_grid, 256, 0, st>>>(p);
+  if ((rc = post_launch("ovg_jpeg_decode(write)"))) return rc;
+  const long long nblk_chunks = (plan->nblocks + SCAN_CHUNK - 1) / SCAN_CHUNK;
+  jpeg_dc_local_kernel<<<static_cast<unsigned>(nblk_chunks), SCAN_CHUNK, 0, st>>>(p);
+  if ((rc = post_launch("ovg_jpeg_decode(dc scan)"))) return rc;
+  jpeg_dc_chunks_kernel<<<1, SCAN_CHUNK, 0, st>>>(w.dc_agg, w.dc_aggf, nblk_chunks);
+  if ((rc = post_launch("ovg_jpeg_decode(dc scan chunks)"))) return rc;
+  jpeg_idct_kernel<<<static_cast<unsigned>((plan->nblocks + 127) / 128), 128, 0, st>>>(p);
+  if ((rc = post_launch("ovg_jpeg_decode(idct)"))) return rc;
+  jpeg_color_kernel<<<static_cast<unsigned>((plan->npix + 255) / 256), 256, 0, st>>>(p);
+  return post_launch("ovg_jpeg_decode(color)");
 }
 
 }  // extern "C"

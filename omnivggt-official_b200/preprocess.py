@@ -1,6 +1,8 @@
 """GPU input pipeline: drop-in for reference ``visual_util.load_images_and_cameras`` (visual_util.py:679-841).
 
-Decoding (PNG / JPEG / .npy / camera .txt parsing, RGBA -> RGB on white) stays on the host, as file I/O; everything the reference
+Baseline JPEGs (what cameras and phones write) are decoded on the device, bit-identical to Pillow (``decode_images``,
+csrc/jpeg.cuh); every other file (PNG, progressive JPEG, CMYK, ...) and .npy / camera .txt parsing stays on the host, and
+RGBA is composited on white there.  Everything the reference
 then does per view with Pillow / OpenCV / numpy -- bicubic resize to width 518, height to a multiple of 14, centre crop, ToTensor,
 depth validity filter + nearest resize + crop + mask, intrinsics rescale, camera-to-world -> world-to-camera -- runs in libovg
 kernels on the device and returns the model's input tuple as CUDA tensors.  The small per-size tap / index tables are computed on
@@ -12,6 +14,7 @@ tensor equals the reference's bit for bit (tests/test_preprocess.py compares aga
 written straight into the output frame by the resize kernel (tests/test_load_fn.py)."""
 from __future__ import annotations
 
+import ctypes
 import glob
 import math
 import os
@@ -88,6 +91,44 @@ def decode_rgb(path: str) -> np.ndarray:
     if img.mode == "RGBA":
         img = Image.alpha_composite(Image.new("RGBA", img.size, (255, 255, 255, 255)), img)
     return np.asarray(img.convert("RGB"))
+
+
+@torch.no_grad()
+def decode_images(paths: Sequence[str], device="cuda", subseq_bits: int = 0) -> List[torch.Tensor]:
+    """uint8 RGB [h, w, 3] tensors on `device`, in the given order, equal to ``decode_rgb`` bit for bit.  One plan for the list,
+    one pinned host-to-device copy of its staging stream and one ``ovg_jpeg_decode`` for every baseline JPEG; ``decode_rgb``
+    (Pillow) and an upload for the other files and for any file the device flags (inconsistent entropy data, or a block
+    outside the range where libjpeg-turbo's C and SIMD IDCTs agree).  subseq_bits: bits per
+    subsequence of the parallel Huffman decoder (0: the default, 512)."""
+    paths = list(paths)
+    dev = torch.device(device)
+    data = [Path(p).read_bytes() for p in paths]
+    plan = L.JpegPlan(data, subseq_bits)
+    out: List[Optional[torch.Tensor]] = [None] * len(paths)
+    on_device = [i for i, f in enumerate(plan.files) if f[0] == L.JPEG_DEVICE]
+    if on_device:
+        lib = L.lib()
+        staging = torch.empty(plan.stream_bytes, dtype=torch.uint8, pin_memory=dev.type == "cuda")
+        plan.fill_stream(staging.data_ptr())
+        stream = staging.to(dev, non_blocking=True)
+        ws = torch.empty(plan.workspace_bytes, dtype=torch.uint8, device=dev)
+        st = torch.zeros(len(paths), dtype=torch.int32, device=dev)
+        ptrs = (ctypes.c_void_p * len(paths))()
+        for i in on_device:
+            _, h, w, _ = plan.files[i]
+            out[i] = torch.empty(h, w, 3, dtype=torch.uint8, device=dev)
+            ptrs[i] = out[i].data_ptr()
+        L.check(lib.ovg_jpeg_decode(plan.handle, stream.data_ptr(), ptrs, st.data_ptr(), ws.data_ptr(), plan.workspace_bytes,
+                                    L.stream()))
+    for i, p in enumerate(paths):                  # overlaps the scan, IDCT and colour kernels (not the sync rounds)
+        if out[i] is None:
+            out[i] = torch.from_numpy(np.array(decode_rgb(p))).to(dev)
+    if on_device:
+        status = st.cpu()                          # synchronises: the staging buffers are free after this
+        for i in on_device:
+            if int(status[i]):
+                out[i] = torch.from_numpy(np.array(decode_rgb(paths[i]))).to(dev)
+    return out
 
 
 def _resize_view(lib, st, im, nw: int, nh: int, crop: int, fh: int, out: torch.Tensor, dev, frame=None, fill: float = 1.0) -> list:
@@ -188,14 +229,15 @@ def read_camera_txt(path: str):
 def load_images_and_cameras(image_folder: str, camera_folder: Optional[str] = None, depth_folder: Optional[str] = None,
                             target_size: int = 518, max_depth: float = 100, device="cuda"):
     """Same signature, file layout and return tuple as reference visual_util.load_images_and_cameras (visual_util.py:679-841);
-    files are decoded on the host (Pillow / numpy), the rest runs on the GPU."""
+    images are decoded by ``decode_images`` (baseline JPEGs on the device), depth maps and cameras on the host, the rest runs
+    on the GPU."""
     from PIL import Image
     paths = sorted(glob.glob(os.path.join(image_folder, "*")))
     paths = [p for p in paths if p.lower().endswith((".png", ".jpg", ".jpeg"))]
-    images, cams, deps, transposed = [], [], [], []
+    images = decode_images(paths, device)
+    cams, deps, transposed = [], [], []
     for p in paths:
         stem = Path(p).stem
-        images.append(decode_rgb(p))
         dep, tr = None, False
         if depth_folder is not None:
             for cand in (os.path.join(depth_folder, stem + ".npy"), os.path.join(depth_folder, stem + ".png")):
@@ -272,6 +314,7 @@ def preprocess_images(images: Sequence, mode: str = "crop", device="cuda") -> to
 
 def load_and_preprocess_images(image_path_list: Sequence[str], mode: str = "crop", device="cuda") -> torch.Tensor:
     """Same signature (plus device) and result as reference omnivggt.utils.load_fn.load_and_preprocess_images: the paths are
-    sorted and decoded on the host (Pillow; RGBA on white), the rest runs on the GPU (preprocess_images)."""
+    sorted and decoded by ``decode_images`` (baseline JPEGs on the device, other files with Pillow, RGBA on white), the rest
+    runs on the GPU (preprocess_images)."""
     _check_load_fn_args(len(image_path_list), mode)
-    return preprocess_images([decode_rgb(p) for p in sorted(image_path_list)], mode, device)
+    return preprocess_images(decode_images(sorted(image_path_list), device), mode, device)
