@@ -231,6 +231,35 @@ int ovg_point_cloud_center(const float* points, long long n, void* workspace, lo
 int ovg_point_cloud_scale(const float* xyz, long long n_kept, long long ld, void* workspace, long long workspace_bytes,
                           float* scale_out, void* stream);
 
+/* Reciprocal nearest-neighbour matches between views: utils/geometry.py:435-451 (find_reciprocal_matches, two cKDTree builds and
+ * queries per pair) for every requested pair of a scene.  points fp32 [V, cap, 3]; the point set of view v is its kept rows
+ * (keep uint8 [V, cap], NULL = all cap rows) in row order, so a point's index is its rank among the kept rows of its view.
+ * Nearest neighbour: fp64 d2 = ((dx*dx) + (dy*dy)) + dz*dz, dx = double(q.x) - double(p.x), no contraction, as cKDTree computes
+ * it; among points at the same d2 the lowest index wins.  reciprocal_in_P2[j] = nn1_in_P2[nn2_in_P1[j]] == j for P1 = view i,
+ * P2 = view j of a pair (i, j) (geometry.py:448-449).  An empty view has no matches.  Results are deterministic.
+ * One workspace of ovg_match_workspace_bytes(V, cap, P) bytes (256-byte aligned) serves the calls below; run them in order on
+ * one stream with the same V, cap, P.  The number of kernel launches of a call does not depend on P.
+ * ovg_match_index: compacts every view's kept points and builds its exact 3-D nearest-neighbour index (a uniform grid, stable
+ *     radix sort by cell), all views in one pass.  points and cap: cap < 2^30. */
+long long ovg_match_workspace_bytes(int V, long long cap, int P);
+int ovg_match_index(const float* points, const unsigned char* keep, int V, long long cap, int P, void* workspace,
+                    long long workspace_bytes, void* stream);
+/* ovg_match_query: pairs device int32 [P, 2] = (i, j); the nearest neighbour of every point of i among the points of j and the
+ * reverse, the reciprocity of every pair, and counts_out device int64 [P + 1]: the matches of each pair, then 1 if a kept point
+ * is not finite (0 otherwise; cKDTree refuses such input).  Reading counts_out back to size the outputs is the one host
+ * synchronisation of a call. */
+int ovg_match_query(const int* pairs, int P, int V, long long cap, void* workspace, long long workspace_bytes, long long* counts_out,
+                    void* stream);
+/* ovg_match_gather: the matches of all pairs, pairs in order, each pair's in ascending index in view j: xy_j int64 [total, 2] =
+ * (x, y) of the matched pixel of view j and xy_i the pixel of its neighbour in view i, with the row index r of a kept point
+ * mapped to (r % W, r / W) (geometry.py:15-37, xy_grid). */
+int ovg_match_gather(const int* pairs, int P, int V, long long cap, int W, const void* workspace, long long workspace_bytes,
+                     long long* xy_i, long long* xy_j, void* stream);
+/* ovg_match_pair: the per-point outputs of find_reciprocal_matches for pair `pair`: reciprocal uint8 [n_j] (reciprocal_in_P2)
+ * and nn int64 [n_j] (nn2_in_P1), n_j the points of view j. */
+int ovg_match_pair(const int* pairs, int P, int V, long long cap, int pair, const void* workspace, long long workspace_bytes,
+                   unsigned char* reciprocal, long long* nn, void* stream);
+
 /* Baseline JPEG decoding on the device, bit-identical to Pillow (libjpeg-turbo's default islow IDCT, fancy upsampling and
  * YCbCr -> RGB tables).  The plan is host code (no CUDA call): it parses every file, routes it to the device or to the host
  * (OVG_JPEG_* below: anything the device cannot decode exactly goes to the host), and builds the staging stream (tables plus the

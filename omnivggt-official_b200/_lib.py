@@ -125,6 +125,11 @@ EXPORTS = {
     "ovg_point_cloud_gather": (C.c_int, [_vp, _vp, _vp, _i, _i, _i, _i, _i, _i, _vp, _ll, _vp, _vp, _vp, _vp, _ll, _vp]),
     "ovg_point_cloud_center": (C.c_int, [_vp, _ll, _vp, _ll, _vp, _vp]),
     "ovg_point_cloud_scale": (C.c_int, [_vp, _ll, _ll, _vp, _ll, _vp, _vp]),
+    "ovg_match_workspace_bytes": (_ll, [_i, _ll, _i]),
+    "ovg_match_index": (C.c_int, [_vp, _vp, _i, _ll, _i, _vp, _ll, _vp]),
+    "ovg_match_query": (C.c_int, [_vp, _i, _i, _ll, _vp, _ll, _vp, _vp]),
+    "ovg_match_gather": (C.c_int, [_vp, _i, _i, _ll, _i, _vp, _ll, _vp, _vp, _vp]),
+    "ovg_match_pair": (C.c_int, [_vp, _i, _i, _ll, _i, _vp, _ll, _vp, _vp, _vp]),
     "ovg_jpeg_plan_create": (C.c_int, [_pp, C.POINTER(_ll), _i, _i, _pp]),
     "ovg_jpeg_plan_destroy": (None, [_vp]),
     "ovg_jpeg_plan_file": (C.c_int, [_vp, _i, C.POINTER(_i), C.POINTER(_i), C.POINTER(_i), C.POINTER(_i)]),

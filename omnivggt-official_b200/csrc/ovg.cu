@@ -14,6 +14,7 @@
 #include "elem.cuh"
 #include "gemm.cuh"
 #include "post.cuh"
+#include "match.cuh"
 #include "tail.cuh"
 #include "pre.cuh"
 #include "jpeg.cuh"
@@ -829,6 +830,179 @@ int ovg_point_cloud_scale(const float* xyz, long long n_kept, long long ld, void
     }
   ovg::cloud_scale_kernel<<<1, 32, 0, st>>>(w.sel, scale_out);
   return post_launch("ovg_point_cloud_scale");
+}
+
+}  // extern "C"
+
+// ------------------------------------------------------------------------------------------------------- reciprocal matches
+namespace {
+
+// Match workspace, carved the same way by the size query and by every entry point.
+struct MatchWorkspace {
+  ovg::MatchParams p;
+  int passes;          // 8-bit radix-sort passes over the cell ids
+  long long bytes;
+};
+
+MatchWorkspace match_workspace(void* base, int V, long long cap, int P) {
+  char* b = static_cast<char*>(base);
+  long long off = 0;
+  auto carve = [&](long long bytes) {
+    char* r = b ? b + off : nullptr;
+    off += (bytes + 255) / 256 * 256;
+    return r;
+  };
+  MatchWorkspace w;
+  ovg::MatchParams& p = w.p;
+  p = ovg::MatchParams{};
+  p.V = V; p.cap = cap; p.P = P;
+  p.tiles = static_cast<int>(ovg::match_tiles(cap));
+  p.ptiles = p.tiles;
+  p.cells_cap = ovg::match_cells_cap(cap);
+  p.flag = reinterpret_cast<unsigned int*>(carve(4));
+  p.hist = reinterpret_cast<unsigned int*>(carve(4LL * V * 3 * ovg::MATCH_BINS));
+  p.grid = reinterpret_cast<ovg::MatchGrid*>(carve(static_cast<long long>(sizeof(ovg::MatchGrid)) * V));
+  p.range0 = reinterpret_cast<float*>(carve(4LL * V * 6));
+  p.view_tile_count = reinterpret_cast<unsigned int*>(carve(4LL * V * p.tiles));
+  p.view_tile_offset = reinterpret_cast<unsigned int*>(carve(4LL * V * p.tiles));
+  p.pts = reinterpret_cast<float4*>(carve(16LL * V * cap));
+  p.rtiles = static_cast<int>((cap + ovg::MATCH_RADIX_TILE - 1) / ovg::MATCH_RADIX_TILE);
+  for (int b = 0; b < 2; ++b) {
+    p.keys[b] = reinterpret_cast<int*>(carve(4LL * V * cap));
+    p.vals[b] = reinterpret_cast<float4*>(carve(16LL * V * cap));
+  }
+  p.radix_off = reinterpret_cast<unsigned int*>(carve(4LL * V * 256 * p.rtiles));
+  int bits = 0;
+  while ((1LL << bits) < p.cells_cap) ++bits;
+  w.passes = (bits + 7) / 8;
+  p.sorted = p.vals[w.passes & 1];
+  p.cell_count = reinterpret_cast<int*>(carve(4LL * V * p.cells_cap));
+  p.cell_start = reinterpret_cast<int*>(carve(4LL * V * (p.cells_cap + 1)));
+  p.nn = reinterpret_cast<int*>(carve(4LL * 2 * P * cap));
+  p.pair_tile_count = reinterpret_cast<unsigned int*>(carve(4LL * P * p.ptiles));
+  p.pair_tile_offset = reinterpret_cast<unsigned long long*>(carve(8LL * P * p.ptiles));
+  p.total = reinterpret_cast<unsigned long long*>(carve(8));
+  w.bytes = off;
+  return w;
+}
+
+int match_check(int V, long long cap, int P, const void* workspace, long long workspace_bytes, ovg::MatchParams* p,
+                int* passes = nullptr) {
+  // cap < 2^30 keeps the cell ids (cells_cap = 2 cap + 64) and the slots inside a view in int range
+  OVG_REQUIRE(V > 0 && V <= 65535 && cap > 0 && cap < (1LL << 30) && P > 0 && 2LL * P <= 65535, "bad sizes");
+  OVG_REQUIRE(static_cast<long long>(V) * cap < (1LL << 40), "too many points");
+  const MatchWorkspace w = match_workspace(const_cast<void*>(workspace), V, cap, P);
+  OVG_REQUIRE(workspace && (reinterpret_cast<uintptr_t>(workspace) & 255) == 0 && workspace_bytes >= w.bytes,
+              "workspace must be 256-byte aligned and ovg_match_workspace_bytes(V, cap, P) long");
+  *p = w.p;
+  if (passes) *passes = w.passes;
+  return OVG_OK;
+}
+
+// grid-stride blocks over one view's points, per view
+int match_blocks(long long cap) {
+  const long long b = (cap + 255) / 256;
+  return static_cast<int>(b < 64 ? (b < 1 ? 1 : b) : 64);
+}
+
+}  // namespace
+
+extern "C" {
+
+long long ovg_match_workspace_bytes(int V, long long cap, int P) {
+  return (V > 0 && cap > 0 && P > 0) ? match_workspace(nullptr, V, cap, P).bytes : -1;
+}
+
+int ovg_match_index(const float* points, const unsigned char* keep, int V, long long cap, int P, void* workspace,
+                    long long workspace_bytes, void* stream) {
+  ovg::MatchParams p;
+  int passes = 0;
+  int rc = match_check(V, cap, P, workspace, workspace_bytes, &p, &passes);
+  if (rc) return rc;
+  OVG_REQUIRE(points, "null points");
+  p.points = points;
+  p.keep = keep;
+  cudaStream_t st = reinterpret_cast<cudaStream_t>(stream);
+  OVG_CUDA(cudaMemsetAsync(p.flag, 0, 4, st));
+  OVG_CUDA(cudaMemsetAsync(p.hist, 0, 4LL * V * 3 * ovg::MATCH_BINS, st));
+  OVG_CUDA(cudaMemsetAsync(p.cell_count, 0, 4LL * V * p.cells_cap, st));
+  ovg::match_keep_count_kernel<<<dim3(p.tiles, V), ovg::MATCH_THREADS, 0, st>>>(p);
+  if ((rc = post_launch("ovg_match_index(keep count)"))) return rc;
+  ovg::match_keep_scan_kernel<<<V, 32, 0, st>>>(p);
+  if ((rc = post_launch("ovg_match_index(keep scan)"))) return rc;
+  ovg::match_keep_gather_kernel<<<dim3(p.tiles, V), ovg::MATCH_THREADS, 0, st>>>(p);
+  if ((rc = post_launch("ovg_match_index(keep gather)"))) return rc;
+  const dim3 grid(match_blocks(cap), V);
+  for (int pass = 0; pass < 2; ++pass) {
+    ovg::match_hist_kernel<<<grid, 256, 0, st>>>(p, pass);
+    if ((rc = post_launch("ovg_match_index(histogram)"))) return rc;
+    ovg::match_range_kernel<<<V, 32, 0, st>>>(p, pass);
+    if ((rc = post_launch("ovg_match_index(range)"))) return rc;
+  }
+  ovg::match_cell_count_kernel<<<grid, 256, 0, st>>>(p);
+  if ((rc = post_launch("ovg_match_index(cell count)"))) return rc;
+  ovg::match_cell_scan_kernel<<<V, 1024, 0, st>>>(p);
+  if ((rc = post_launch("ovg_match_index(cell scan)"))) return rc;
+  const dim3 rgrid(p.rtiles, V);
+  for (int pass = 0; pass < passes; ++pass) {
+    ovg::match_radix_count_kernel<<<rgrid, ovg::MATCH_RADIX_TILE, 0, st>>>(p, 8 * pass, pass & 1);
+    if ((rc = post_launch("ovg_match_index(radix count)"))) return rc;
+    ovg::match_radix_scan_kernel<<<V, 1024, 0, st>>>(p);
+    if ((rc = post_launch("ovg_match_index(radix scan)"))) return rc;
+    ovg::match_radix_scatter_kernel<<<rgrid, ovg::MATCH_RADIX_TILE, 0, st>>>(p, 8 * pass, pass & 1);
+    if ((rc = post_launch("ovg_match_index(radix scatter)"))) return rc;
+  }
+  return OVG_OK;
+}
+
+int ovg_match_query(const int* pairs, int P, int V, long long cap, void* workspace, long long workspace_bytes, long long* counts_out,
+                    void* stream) {
+  ovg::MatchParams p;
+  int rc = match_check(V, cap, P, workspace, workspace_bytes, &p);
+  if (rc) return rc;
+  OVG_REQUIRE(pairs && counts_out, "null pairs / counts_out");
+  OVG_REQUIRE(static_cast<long long>(P) * p.ptiles < (1LL << 31), "too many pairs");
+  p.pairs = pairs;
+  p.counts = counts_out;
+  cudaStream_t st = reinterpret_cast<cudaStream_t>(stream);
+  ovg::match_query_kernel<<<dim3(static_cast<unsigned>((cap + ovg::MATCH_QUERY_THREADS - 1) / ovg::MATCH_QUERY_THREADS), 2 * P),
+                            ovg::MATCH_QUERY_THREADS, 0, st>>>(p);
+  if ((rc = post_launch("ovg_match_query"))) return rc;
+  ovg::match_recip_count_kernel<<<dim3(p.ptiles, P), ovg::MATCH_THREADS, 0, st>>>(p);
+  if ((rc = post_launch("ovg_match_query(reciprocal count)"))) return rc;
+  ovg::CloudParams sp{};
+  sp.tile_count = p.pair_tile_count;
+  sp.tile_offset = p.pair_tile_offset;
+  sp.total = p.total;
+  sp.tiles = P * p.ptiles;
+  ovg::cloud_scan_kernel<<<1, 1024, 0, st>>>(sp);
+  if ((rc = post_launch("ovg_match_query(scan)"))) return rc;
+  ovg::match_counts_kernel<<<(P + 1 + 255) / 256, 256, 0, st>>>(p);
+  return post_launch("ovg_match_query(counts)");
+}
+
+int ovg_match_gather(const int* pairs, int P, int V, long long cap, int W, const void* workspace, long long workspace_bytes,
+                     long long* xy_i, long long* xy_j, void* stream) {
+  ovg::MatchParams p;
+  int rc = match_check(V, cap, P, workspace, workspace_bytes, &p);
+  if (rc) return rc;
+  OVG_REQUIRE(pairs && xy_i && xy_j && W > 0, "bad arguments");
+  p.pairs = pairs;
+  ovg::MatchOut o{W, xy_i, xy_j, -1, nullptr, nullptr};
+  ovg::match_gather_kernel<<<dim3(p.ptiles, P), ovg::MATCH_THREADS, 0, reinterpret_cast<cudaStream_t>(stream)>>>(p, o);
+  return post_launch("ovg_match_gather");
+}
+
+int ovg_match_pair(const int* pairs, int P, int V, long long cap, int pair, const void* workspace, long long workspace_bytes,
+                   unsigned char* reciprocal, long long* nn, void* stream) {
+  ovg::MatchParams p;
+  int rc = match_check(V, cap, P, workspace, workspace_bytes, &p);
+  if (rc) return rc;
+  OVG_REQUIRE(pairs && reciprocal && nn && pair >= 0 && pair < P, "bad arguments");
+  p.pairs = pairs;
+  ovg::MatchOut o{1, nullptr, nullptr, pair, reciprocal, nn};
+  ovg::match_pair_kernel<<<static_cast<unsigned>((cap + 255) / 256), 256, 0, reinterpret_cast<cudaStream_t>(stream)>>>(p, o);
+  return post_launch("ovg_match_pair");
 }
 
 }  // extern "C"

@@ -305,31 +305,20 @@ class OmniVGGT(nn.Module, PyTorchModelHubMixin):
         return predictions
 
     @staticmethod
-    @torch.no_grad()
-    def point_cloud(predictions: Dict[str, object], *, source: str = "depth", conf_percent: float = 50.0,
-                    conf_floor: float = 1e-5, frame: Optional[int] = None, mask_black_bg: bool = False,
-                    mask_white_bg: bool = False, scene: int = 0) -> Dict[str, torch.Tensor]:
-        """The filtered, coloured point cloud of one scene, built on the device (libovg kernels).
-
-        Replaces the host numpy of the reference's GLB export (visual_util.py:190-236,:320-358 predictions_to_glb) and
-        viewer (inference.py:96-151).  ``source="depth"``: ``world_points_from_depth`` (computed here when ``postprocess``
-        has not run) with ``depth_conf``, as ``--save_glb`` uses it; ``"pointmap"``: ``world_points`` with
-        ``world_points_conf``.  ``frame``: keep only that view, selected before the percentile (visual_util.py:190-194).
-        Kept: conf >= percentile(conf, conf_percent) (0 for conf_percent == 0, visual_util.py:206-207) and conf > conf_floor,
-        minus black / white background pixels when asked.  ``conf_floor=0.1`` reproduces the viewer's initial mask
-        (inference.py:132-133); its frame dropdown is ``cloud["frame"] == i`` on the ``frame=None`` cloud.
-
-        Returns ``points`` fp32 [n,3], ``colors`` uint8 [n,3], ``frame`` int32 [n] (numpy boolean-indexing order),
-        ``conf_threshold`` (0-d), ``center`` fp32 [3] (mean of all points of the selected views, inference.py:111),
-        ``scale`` (0-d, ||p95 - p5||, 1.0 when nothing is kept) and ``align`` fp64 [4,4] = inv(E0) diag(1,-1,-1,1) R_y(180)
-        with E0 the first selected camera (visual_util.py:320-341).  The kept count and E0 are the only device-to-host reads."""
-        from . import ops
+    def _check_source(source: str, conf_percent: float, conf_floor: float) -> None:
         if source not in ("depth", "pointmap"):
             raise ValueError(f"source must be 'depth' or 'pointmap', got {source!r}")
         if not 0.0 <= conf_percent <= 100.0:
             raise ValueError("conf_percent must be in [0, 100]")
         if conf_floor < 0.0:
             raise ValueError("conf_floor must be >= 0")        # the reference's floors are 1e-5 and 0.1
+
+    @staticmethod
+    def _scene_source(predictions: Dict[str, object], source: str, scene: int):
+        """(images fp32 [S,3,H,W], extrinsic [S,3,4], points [S,H,W,3], conf [S,H,W]) of one scene.  ``source="depth"``:
+        ``world_points_from_depth`` (unprojected here when ``postprocess`` has not run) with ``depth_conf``; ``"pointmap"``:
+        ``world_points`` with ``world_points_conf``."""
+        from . import ops
 
         def scene_of(t, trailing):                             # [B, S, ...] or [S, ...] -> [S, ...] of the scene
             return t[scene] if t.dim() == trailing + 2 else t
@@ -353,6 +342,63 @@ class OmniVGGT(nn.Module, PyTorchModelHubMixin):
                 depth = scene_of(predictions["depth"], 3).float().reshape(S, H, W)
                 points = ops.unproject_depth(depth, intr, c2w, H, W)
             conf = scene_of(predictions["depth_conf"], 2)
+        return images, ext, points, conf
+
+    @staticmethod
+    @torch.no_grad()
+    def matches(predictions: Dict[str, object], pairs=None, *, source: str = "depth", conf_percent: float = 50.0,
+                conf_floor: float = 1e-5, scene: int = 0) -> List[Dict[str, object]]:
+        """Dense cross-view correspondences of one scene by reciprocal nearest neighbours of the predicted points (the
+        DUSt3R-family recipe on utils/geometry.py:435-451 find_reciprocal_matches and :15-37 xy_grid), on the device.
+
+        ``source`` and the keep mask are ``point_cloud``'s: conf >= percentile(conf over the scene's S views, conf_percent) and
+        conf > conf_floor.  For each pair (i, j) (default: every i < j), P1 and P2 are the kept points of views i and j in
+        row-major order, and the result is ``{"xy_i", "xy_j", "count"}`` with ``xy_j = grid_j[kept_j][reciprocal_in_P2]`` and
+        ``xy_i = grid_i[kept_i][nn2_in_P1][reciprocal_in_P2]``: int64 [count, 2] (x, y) pixel coordinates on the device.
+        Every view's index is built once; all pairs are queried in one pass; the match counts are the one host read.  Kept
+        points that are not finite raise ValueError; a view with no kept point has no matches."""
+        from . import geometry, ops
+        OmniVGGT._check_source(source, conf_percent, conf_floor)
+        images = predictions["images"]
+        S = (images[scene] if images.dim() == 5 else images).shape[0]
+        pair_arr = geometry.check_pairs(pairs, S)
+        if len(pair_arr) == 0:
+            return []
+        images, _, points, conf = OmniVGGT._scene_source(predictions, source, scene)
+        _, _, H, W = images.shape
+        dev = images.device
+        mask, _, _ = ops.conf_percentile_mask(conf.float().contiguous(), conf_percent, conf_floor)
+        mt = ops.Matcher(points.float().contiguous().view(S, H * W, 3), mask.view(S, H * W),
+                         torch.from_numpy(pair_arr).to(dev))
+        counts, nonfinite = mt.counts()
+        if nonfinite:
+            raise ValueError("kept points must be finite (cKDTree: data must be finite, check for nan or inf values)")
+        xy_i, xy_j = mt.gather(sum(counts), W)
+        return [{"xy_i": a, "xy_j": b, "count": c} for a, b, c in zip(xy_i.split(counts), xy_j.split(counts), counts)]
+
+    @staticmethod
+    @torch.no_grad()
+    def point_cloud(predictions: Dict[str, object], *, source: str = "depth", conf_percent: float = 50.0,
+                    conf_floor: float = 1e-5, frame: Optional[int] = None, mask_black_bg: bool = False,
+                    mask_white_bg: bool = False, scene: int = 0) -> Dict[str, torch.Tensor]:
+        """The filtered, coloured point cloud of one scene, built on the device (libovg kernels).
+
+        Replaces the host numpy of the reference's GLB export (visual_util.py:190-236,:320-358 predictions_to_glb) and
+        viewer (inference.py:96-151).  ``source="depth"``: ``world_points_from_depth`` (computed here when ``postprocess``
+        has not run) with ``depth_conf``, as ``--save_glb`` uses it; ``"pointmap"``: ``world_points`` with
+        ``world_points_conf``.  ``frame``: keep only that view, selected before the percentile (visual_util.py:190-194).
+        Kept: conf >= percentile(conf, conf_percent) (0 for conf_percent == 0, visual_util.py:206-207) and conf > conf_floor,
+        minus black / white background pixels when asked.  ``conf_floor=0.1`` reproduces the viewer's initial mask
+        (inference.py:132-133); its frame dropdown is ``cloud["frame"] == i`` on the ``frame=None`` cloud.
+
+        Returns ``points`` fp32 [n,3], ``colors`` uint8 [n,3], ``frame`` int32 [n] (numpy boolean-indexing order),
+        ``conf_threshold`` (0-d), ``center`` fp32 [3] (mean of all points of the selected views, inference.py:111),
+        ``scale`` (0-d, ||p95 - p5||, 1.0 when nothing is kept) and ``align`` fp64 [4,4] = inv(E0) diag(1,-1,-1,1) R_y(180)
+        with E0 the first selected camera (visual_util.py:320-341).  The kept count and E0 are the only device-to-host reads."""
+        from . import ops
+        OmniVGGT._check_source(source, conf_percent, conf_floor)
+        images, ext, points, conf = OmniVGGT._scene_source(predictions, source, scene)
+        S, _, H, W = images.shape
         f0 = 0
         if frame is not None:
             if not 0 <= frame < S:

@@ -258,3 +258,55 @@ def point_cloud_scale(xyz, n_kept: int, ws):
     L.check(L.lib().ovg_point_cloud_scale(xyz.data_ptr(), n_kept, xyz.shape[1], ws.data_ptr(), ws.numel(), scale.data_ptr(),
                                           L.stream()))
     return scale
+
+
+def host_read(t: torch.Tensor) -> torch.Tensor:
+    """The device-to-host read of a matching call (its one synchronisation)."""
+    return t.cpu()
+
+
+class Matcher:
+    """Reciprocal nearest-neighbour matches (ovg_match_*) between the kept points of V views: points fp32 [V, cap, 3] and keep
+    uint8 [V, cap] (or None: all rows), pairs int32 [P, 2] on the device.  Builds every view's index once (ovg_match_index), then
+    queries all pairs in both directions (ovg_match_query); ``counts()`` is the one host read."""
+
+    def __init__(self, points: torch.Tensor, keep: Optional[torch.Tensor], pairs: torch.Tensor):
+        _chk(points, F32, "points")
+        _chk(pairs, torch.int32, "pairs")
+        assert points.dim() == 3 and points.shape[2] == 3 and points.is_contiguous() and pairs.is_contiguous()
+        self.V, self.cap = points.shape[0], points.shape[1]
+        self.P = pairs.shape[0]
+        if keep is not None:
+            _chk(keep, torch.uint8, "keep")
+            assert keep.is_contiguous() and keep.numel() == self.V * self.cap
+        self.pairs = pairs
+        lib = L.lib()
+        self.ws = torch.empty(lib.ovg_match_workspace_bytes(self.V, self.cap, self.P), device=points.device, dtype=torch.uint8)
+        self._counts = torch.zeros(self.P + 1, device=points.device, dtype=torch.int64)
+        L.check(lib.ovg_match_index(points.data_ptr(), L.ptr(keep), self.V, self.cap, self.P, self.ws.data_ptr(), self.ws.numel(),
+                                    L.stream()))
+        L.check(lib.ovg_match_query(pairs.data_ptr(), self.P, self.V, self.cap, self.ws.data_ptr(), self.ws.numel(),
+                                    self._counts.data_ptr(), L.stream()))
+
+    def counts(self):
+        """(matches per pair as a list of ints, whether a kept point is not finite): the one host read."""
+        c = host_read(self._counts).tolist()
+        return c[:self.P], bool(c[self.P])
+
+    def gather(self, total: int, W: int):
+        """xy_i, xy_j int64 [total, 2]: the matches of all pairs in order (pixel (x, y) = (row % W, row // W))."""
+        xy_i = torch.empty(total, 2, device=self.ws.device, dtype=torch.int64)
+        xy_j = torch.empty(total, 2, device=self.ws.device, dtype=torch.int64)
+        if total:
+            L.check(L.lib().ovg_match_gather(self.pairs.data_ptr(), self.P, self.V, self.cap, W, self.ws.data_ptr(), self.ws.numel(),
+                                             xy_i.data_ptr(), xy_j.data_ptr(), L.stream()))
+        return xy_i, xy_j
+
+    def pair(self, k: int, n_j: int):
+        """(reciprocal_in_P2 bool [n_j], nn2_in_P1 int64 [n_j]) of pair k."""
+        rec = torch.empty(n_j, device=self.ws.device, dtype=torch.uint8)
+        nn = torch.empty(n_j, device=self.ws.device, dtype=torch.int64)
+        if n_j:
+            L.check(L.lib().ovg_match_pair(self.pairs.data_ptr(), self.P, self.V, self.cap, k, self.ws.data_ptr(), self.ws.numel(),
+                                           rec.data_ptr(), nn.data_ptr(), L.stream()))
+        return rec.bool(), nn
