@@ -260,6 +260,33 @@ int ovg_match_gather(const int* pairs, int P, int V, long long cap, int W, const
 int ovg_match_pair(const int* pairs, int P, int V, long long cap, int pair, const void* workspace, long long workspace_bytes,
                    unsigned char* reciprocal, long long* nn, void* stream);
 
+/* Triangle mesh of point maps: viz.py:40-89 (pts3d_to_trimesh per view, cat_meshes across views) for F views at once.
+ * Pixels are numbered i = (f H + y) W + x.  The quad at (y, x), y < H-1, x < W-1, gives the TL triangle (tl, tr, bl) and the BR
+ * triangle (tr, bl, br); a triangle is kept when its three vertices are.  Reference layout: per view, the kept TL triangles,
+ * the same reversed (bl, tr, tl), the kept BR triangles, the same reversed (br, bl, tr), each class in row-major quad order,
+ * indices i (already offset by f H W); face colours: tl's pixel for the TL classes, br's for the BR classes.  GLB layout: the
+ * used vertices (corners of a kept triangle) in index order, and the forward triangles (TL then BR per view) as int32 ranks
+ * among them.  No atomic decides a position: results are deterministic.  The number of launches does not depend on F.
+ * One workspace of ovg_mesh_workspace_bytes(F, H, W) bytes (256-byte aligned) serves the calls of one mesh; run them in order
+ * on one stream with the same sizes.  F <= 65535 and F H W < 2^31.
+ * ovg_mesh_count: keep[i] = the point cloud's keep bit (ovg_point_cloud_count: conf_mask and the background tests on the
+ *     colours of images fp32 [F,3,H,W]); images may be NULL without background tests, keep[i] = conf_mask[i] then.
+ *     counts_out: device int64 [3] = reference faces, used vertices, forward faces.  Reading it back to size the outputs is the
+ *     one host synchronisation of a mesh.  viz.py:40-77. */
+long long ovg_mesh_workspace_bytes(int F, int H, int W);
+int ovg_mesh_count(const unsigned char* conf_mask, const float* images, int F, int H, int W, int mask_black_bg,
+                   int mask_white_bg, void* workspace, long long workspace_bytes, long long* counts_out, void* stream);
+/* ovg_mesh_faces: the reference layout, viz.py:47-74,:80-89: faces int64 [reference faces, 3] and face_colors [reference
+ * faces, 3], uint8(trunc(x * 255)) of images when images is not NULL, else copied from colors [F H W, 3] (elements of
+ * color_bytes = 1, 2, 4 or 8, any dtype of that size) into elements of the same size. */
+int ovg_mesh_faces(const float* images, const void* colors, int color_bytes, int F, int H, int W, const void* workspace,
+                   long long workspace_bytes, long long* faces, void* face_colors, void* stream);
+/* ovg_mesh_compact: the GLB layout of the same mesh, viz.py:40-89 with the reversed copies left out: positions fp32 [used, 3]
+ * from points fp32 [F H W, 3] and colors uint8 [used, 3] (each vertex its own pixel's colour from images) of the used
+ * vertices in index order, and indices int32 [forward faces, 3]. */
+int ovg_mesh_compact(const float* points, const float* images, int F, int H, int W, const void* workspace,
+                     long long workspace_bytes, float* positions, unsigned char* colors, int* indices, void* stream);
+
 /* Baseline JPEG decoding on the device, bit-identical to Pillow (libjpeg-turbo's default islow IDCT, fancy upsampling and
  * YCbCr -> RGB tables).  The plan is host code (no CUDA call): it parses every file, routes it to the device or to the host
  * (OVG_JPEG_* below: anything the device cannot decode exactly goes to the host), and builds the staging stream (tables plus the

@@ -130,6 +130,10 @@ EXPORTS = {
     "ovg_match_query": (C.c_int, [_vp, _i, _i, _ll, _vp, _ll, _vp, _vp]),
     "ovg_match_gather": (C.c_int, [_vp, _i, _i, _ll, _i, _vp, _ll, _vp, _vp, _vp]),
     "ovg_match_pair": (C.c_int, [_vp, _i, _i, _ll, _i, _vp, _ll, _vp, _vp, _vp]),
+    "ovg_mesh_workspace_bytes": (_ll, [_i, _i, _i]),
+    "ovg_mesh_count": (C.c_int, [_vp, _vp, _i, _i, _i, _i, _i, _vp, _ll, _vp, _vp]),
+    "ovg_mesh_faces": (C.c_int, [_vp, _vp, _i, _i, _i, _i, _vp, _ll, _vp, _vp, _vp]),
+    "ovg_mesh_compact": (C.c_int, [_vp, _vp, _i, _i, _i, _vp, _ll, _vp, _vp, _vp, _vp]),
     "ovg_jpeg_plan_create": (C.c_int, [_pp, C.POINTER(_ll), _i, _i, _pp]),
     "ovg_jpeg_plan_destroy": (None, [_vp]),
     "ovg_jpeg_plan_file": (C.c_int, [_vp, _i, C.POINTER(_i), C.POINTER(_i), C.POINTER(_i), C.POINTER(_i)]),

@@ -15,6 +15,7 @@
 #include "gemm.cuh"
 #include "post.cuh"
 #include "match.cuh"
+#include "mesh.cuh"
 #include "tail.cuh"
 #include "pre.cuh"
 #include "jpeg.cuh"
@@ -1003,6 +1004,110 @@ int ovg_match_pair(const int* pairs, int P, int V, long long cap, int pair, cons
   ovg::MatchOut o{1, nullptr, nullptr, pair, reciprocal, nn};
   ovg::match_pair_kernel<<<static_cast<unsigned>((cap + 255) / 256), 256, 0, reinterpret_cast<cudaStream_t>(stream)>>>(p, o);
   return post_launch("ovg_match_pair");
+}
+
+}  // extern "C"
+
+// -------------------------------------------------------------------------------------------------------------- triangle mesh
+namespace {
+
+// Mesh workspace, carved the same way by the size query and by every entry point.
+ovg::MeshParams mesh_workspace(void* base, int F, int H, int W, long long* bytes) {
+  char* b = static_cast<char*>(base);
+  long long off = 0;
+  auto carve = [&](long long n) {
+    char* r = b ? b + off : nullptr;
+    off += (n + 255) / 256 * 256;
+    return r;
+  };
+  ovg::MeshParams p{};
+  p.H = H; p.W = W;
+  p.hw = static_cast<long long>(H) * W;
+  p.n = F * p.hw;
+  p.tpv = static_cast<int>((p.hw + ovg::MESH_TILE - 1) / ovg::MESH_TILE);
+  p.T = F * p.tpv;
+  p.keep = reinterpret_cast<unsigned char*>(carve(p.n));
+  p.remap = reinterpret_cast<int*>(carve(4 * p.n));
+  p.tile_count = reinterpret_cast<unsigned int*>(carve(4LL * ovg::MESH_STREAMS * p.T));
+  p.tile_offset = reinterpret_cast<unsigned long long*>(carve(8LL * (ovg::MESH_STREAMS * p.T + 1)));
+  *bytes = off;
+  return p;
+}
+
+int mesh_check(int F, int H, int W, const void* workspace, long long workspace_bytes, ovg::MeshParams* p) {
+  OVG_REQUIRE(F > 0 && F <= 65535 && H > 0 && W > 0, "bad sizes");
+  OVG_REQUIRE(static_cast<long long>(F) * H * W < (1LL << 31), "F*H*W must be below 2^31");
+  long long bytes = 0;
+  *p = mesh_workspace(const_cast<void*>(workspace), F, H, W, &bytes);
+  OVG_REQUIRE(workspace && (reinterpret_cast<uintptr_t>(workspace) & 255) == 0 && workspace_bytes >= bytes,
+              "workspace must be 256-byte aligned and ovg_mesh_workspace_bytes(F, H, W) long");
+  return OVG_OK;
+}
+
+}  // namespace
+
+extern "C" {
+
+long long ovg_mesh_workspace_bytes(int F, int H, int W) {
+  if (F <= 0 || H <= 0 || W <= 0) return -1;
+  long long bytes = 0;
+  mesh_workspace(nullptr, F, H, W, &bytes);
+  return bytes;
+}
+
+int ovg_mesh_count(const unsigned char* conf_mask, const float* images, int F, int H, int W, int mask_black_bg,
+                   int mask_white_bg, void* workspace, long long workspace_bytes, long long* counts_out, void* stream) {
+  ovg::MeshParams p;
+  int rc = mesh_check(F, H, W, workspace, workspace_bytes, &p);
+  if (rc) return rc;
+  OVG_REQUIRE(conf_mask && counts_out, "null conf_mask / counts_out");
+  OVG_REQUIRE(images || !(mask_black_bg || mask_white_bg), "the background masks need images");
+  p.conf_mask = conf_mask; p.images = images;
+  p.black_bg = mask_black_bg ? 1 : 0; p.white_bg = mask_white_bg ? 1 : 0;
+  p.totals = counts_out;
+  cudaStream_t st = reinterpret_cast<cudaStream_t>(stream);
+  ovg::mesh_keep_kernel<<<static_cast<unsigned>((p.n + 255) / 256), 256, 0, st>>>(p);
+  if ((rc = post_launch("ovg_mesh_count(keep)"))) return rc;
+  ovg::mesh_count_kernel<<<dim3(p.tpv, F), ovg::MESH_THREADS, 0, st>>>(p);
+  if ((rc = post_launch("ovg_mesh_count"))) return rc;
+  ovg::CloudParams sp{};
+  sp.tile_count = p.tile_count;
+  sp.tile_offset = p.tile_offset;
+  sp.total = p.tile_offset + ovg::MESH_STREAMS * p.T;
+  sp.tiles = ovg::MESH_STREAMS * p.T;
+  ovg::cloud_scan_kernel<<<1, 1024, 0, st>>>(sp);
+  if ((rc = post_launch("ovg_mesh_count(scan)"))) return rc;
+  ovg::mesh_totals_kernel<<<1, 32, 0, st>>>(p);
+  return post_launch("ovg_mesh_count(totals)");
+}
+
+int ovg_mesh_faces(const float* images, const void* colors, int color_bytes, int F, int H, int W, const void* workspace,
+                   long long workspace_bytes, long long* faces, void* face_colors, void* stream) {
+  ovg::MeshParams p;
+  int rc = mesh_check(F, H, W, workspace, workspace_bytes, &p);
+  if (rc) return rc;
+  OVG_REQUIRE(faces && face_colors, "null faces / face_colors");
+  OVG_REQUIRE(images || (colors && (color_bytes == 1 || color_bytes == 2 || color_bytes == 4 || color_bytes == 8)),
+              "face colours need images, or colors with color_bytes 1, 2, 4 or 8");
+  p.images = images; p.colors = colors; p.color_bytes = color_bytes;
+  p.faces = faces; p.face_colors = face_colors;
+  ovg::mesh_faces_kernel<<<dim3(p.tpv, F), ovg::MESH_THREADS, 0, reinterpret_cast<cudaStream_t>(stream)>>>(p);
+  return post_launch("ovg_mesh_faces");
+}
+
+int ovg_mesh_compact(const float* points, const float* images, int F, int H, int W, const void* workspace,
+                     long long workspace_bytes, float* positions, unsigned char* colors, int* indices, void* stream) {
+  ovg::MeshParams p;
+  int rc = mesh_check(F, H, W, workspace, workspace_bytes, &p);
+  if (rc) return rc;
+  OVG_REQUIRE(points && images && positions && colors && indices, "null operand");
+  p.points = points; p.images = images;
+  p.positions = positions; p.vertex_colors = colors; p.indices = indices;
+  cudaStream_t st = reinterpret_cast<cudaStream_t>(stream);
+  ovg::mesh_vertices_kernel<<<dim3(p.tpv, F), ovg::MESH_THREADS, 0, st>>>(p);
+  if ((rc = post_launch("ovg_mesh_compact(vertices)"))) return rc;
+  ovg::mesh_indices_kernel<<<dim3(p.tpv, F), ovg::MESH_THREADS, 0, st>>>(p);
+  return post_launch("ovg_mesh_compact(indices)");
 }
 
 }  // extern "C"

@@ -299,17 +299,30 @@ struct CloudParams {
 };
 
 // colours as visual_util.py:202 computes them, (x * 255).astype(uint8): fp32 product, truncation (mod 256 like the x86
-// conversion numpy uses for values outside [0, 256)); background tests of :213-221 on those bytes.
-__device__ __forceinline__ bool cloud_keep(const CloudParams& p, long long i, int& f, uchar3& rgb) {
-  f = static_cast<int>(i / p.hw);
-  const float* img = p.images + f * 2 * p.hw + i;         // = images + (3 f) hw + (i - f hw)
+// conversion numpy uses for values outside [0, 256)), of pixel i of frame f in images fp32 [F, 3, H, W].
+__device__ __forceinline__ uchar3 pixel_rgb(const float* images, long long hw, long long i, int f) {
+  const float* img = images + f * 2 * hw + i;             // = images + (3 f) hw + (i - f hw)
+  uchar3 rgb;
   rgb.x = static_cast<unsigned char>(__float2int_rz(__fmul_rn(img[0], 255.0f)));
-  rgb.y = static_cast<unsigned char>(__float2int_rz(__fmul_rn(img[p.hw], 255.0f)));
-  rgb.z = static_cast<unsigned char>(__float2int_rz(__fmul_rn(img[2 * p.hw], 255.0f)));
-  bool keep = p.conf_mask[i] != 0;
-  if (p.black_bg) keep = keep && static_cast<int>(rgb.x) + rgb.y + rgb.z >= 16;
-  if (p.white_bg) keep = keep && !(rgb.x > 240 && rgb.y > 240 && rgb.z > 240);
+  rgb.y = static_cast<unsigned char>(__float2int_rz(__fmul_rn(img[hw], 255.0f)));
+  rgb.z = static_cast<unsigned char>(__float2int_rz(__fmul_rn(img[2 * hw], 255.0f)));
+  return rgb;
+}
+
+// The keep bit of pixel i shared by the point cloud and the mesh: the confidence mask, then the background tests of
+// visual_util.py:213-221 on the pixel's colour bytes.
+__device__ __forceinline__ bool pixel_keep(const unsigned char* conf_mask, const float* images, long long hw, int black_bg,
+                                           int white_bg, long long i, int& f, uchar3& rgb) {
+  f = static_cast<int>(i / hw);
+  rgb = pixel_rgb(images, hw, i, f);
+  bool keep = conf_mask[i] != 0;
+  if (black_bg) keep = keep && static_cast<int>(rgb.x) + rgb.y + rgb.z >= 16;
+  if (white_bg) keep = keep && !(rgb.x > 240 && rgb.y > 240 && rgb.z > 240);
   return keep;
+}
+
+__device__ __forceinline__ bool cloud_keep(const CloudParams& p, long long i, int& f, uchar3& rgb) {
+  return pixel_keep(p.conf_mask, p.images, p.hw, p.black_bg, p.white_bg, i, f, rgb);
 }
 
 __global__ void __launch_bounds__(CLOUD_THREADS) cloud_count_kernel(const CloudParams p) {

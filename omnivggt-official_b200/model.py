@@ -418,11 +418,7 @@ class OmniVGGT(nn.Module, PyTorchModelHubMixin):
         cnt = ops.point_cloud_count(mask, images, ws, mask_black_bg, mask_white_bg)
         center = ops.point_cloud_center(points, ws)
         n = int(cnt.item())
-        e0 = torch.eye(4, dtype=torch.float64)
-        e0[:3, :4] = ext[f0].double().cpu()
-        gl = torch.diag(torch.tensor([1.0, -1.0, -1.0, 1.0], dtype=torch.float64))
-        rot_y = torch.diag(torch.tensor([-1.0, 1.0, -1.0, 1.0], dtype=torch.float64))
-        align = (torch.linalg.inv(e0) @ gl @ rot_y).to(dev)
+        align = OmniVGGT._align(ext[f0].double().cpu()).to(dev)
         if n == 0:
             return {"points": torch.empty(0, 3, device=dev), "colors": torch.empty(0, 3, device=dev, dtype=torch.uint8),
                     "frame": torch.empty(0, device=dev, dtype=torch.int32), "conf_threshold": thr, "center": center,
@@ -430,6 +426,69 @@ class OmniVGGT(nn.Module, PyTorchModelHubMixin):
         pts, cols, fr, xyz = ops.point_cloud_gather(points, mask, images, ws, n, mask_black_bg, mask_white_bg, f0)
         scale = ops.point_cloud_scale(xyz, n, ws)
         return {"points": pts, "colors": cols, "frame": fr, "conf_threshold": thr, "center": center, "scale": scale,
+                "align": align}
+
+    @staticmethod
+    def _align(e0: torch.Tensor) -> torch.Tensor:
+        """inv(E0) diag(1,-1,-1,1) R_y(180), fp64 [4,4] on the host, from the host camera E0 [3,4] (visual_util.py:320-341)."""
+        e = torch.eye(4, dtype=torch.float64)
+        e[:3, :4] = e0
+        gl = torch.diag(torch.tensor([1.0, -1.0, -1.0, 1.0], dtype=torch.float64))
+        rot_y = torch.diag(torch.tensor([-1.0, 1.0, -1.0, 1.0], dtype=torch.float64))
+        return torch.linalg.inv(e) @ gl @ rot_y
+
+    @staticmethod
+    @torch.no_grad()
+    def mesh(predictions: Dict[str, object], *, source: str = "depth", conf_percent: float = 50.0, conf_floor: float = 1e-5,
+             frame: Optional[int] = None, mask_black_bg: bool = False, mask_white_bg: bool = False, scene: int = 0,
+             layout: str = "reference") -> Dict[str, torch.Tensor]:
+        """The coloured triangle mesh of one scene's point maps, built on the device (libovg kernels): the DUSt3R-family
+        recipe of viz.py:40-89, ``cat_meshes([pts3d_to_trimesh(colors[f], points[f], keep[f]) for f in views])``.
+
+        ``source``, ``conf_percent``, ``conf_floor``, ``frame``, the background masks and ``scene`` select the views and the
+        kept pixels exactly as in ``point_cloud``; colours are (images * 255).astype(uint8).  Every pixel quad gives two
+        triangles, (tl, tr, bl) and (tr, bl, br); a triangle is kept when its three pixels are.
+
+        ``layout="reference"``: ``vertices`` fp32 [F*H*W, 3] (every point of the selected views), ``face_colors`` uint8 [n, 3]
+        and ``faces`` int64 [n, 3], as viz.py returns them: per view the kept (tl, tr, bl) triangles, the same reversed, the kept
+        (tr, bl, br) triangles, the same reversed, each in row-major order; colours from tl and br.
+        ``layout="glb"``: ``positions`` fp32 [m, 3] and ``colors`` uint8 [m, 3] of the vertices the forward triangles use, in
+        index order, each with its own pixel's colour, and ``indices`` int32 [k, 3] of the forward triangles only, for
+        ``glb.write_mesh_glb`` (whose material is double-sided in place of the reversed copies).
+        Both add ``conf_threshold`` and ``align``, as ``point_cloud`` returns them.  The three totals and the first camera are
+        read back together: the one host synchronisation."""
+        from . import ops
+        OmniVGGT._check_source(source, conf_percent, conf_floor)
+        if layout not in ("reference", "glb"):
+            raise ValueError(f"layout must be 'reference' or 'glb', got {layout!r}")
+        images = predictions["images"]
+        S = (images[scene] if images.dim() == 5 else images).shape[0]
+        if frame is not None and not 0 <= frame < S:
+            raise IndexError(f"frame {frame} out of range for {S} views")
+        images, ext, points, conf = OmniVGGT._scene_source(predictions, source, scene)
+        _, _, H, W = images.shape
+        f0 = 0
+        if frame is not None:
+            f0 = frame
+            images, points, conf = images[frame:frame + 1], points[frame:frame + 1], conf[frame:frame + 1]
+        images = images.contiguous()
+        points = points.float().contiguous()
+        conf = conf.float().contiguous()
+        F = images.shape[0]
+        dev = images.device
+
+        mask, thr, _ = ops.conf_percentile_mask(conf, conf_percent, conf_floor)
+        if conf_percent == 0.0:
+            thr = torch.zeros((), device=dev, dtype=torch.float32)   # same mask: conf > conf_floor >= 0 implies conf >= 0
+        mesher = ops.Mesher(mask.view(-1), images, F, H, W, mask_black_bg, mask_white_bg)
+        host = ops.host_read(torch.cat([mesher.totals.double(), ext[f0].double().reshape(-1)]))   # totals < 2^33: exact
+        n_ref, n_used, n_fwd = (int(v) for v in host[:3].tolist())
+        align = OmniVGGT._align(host[3:].view(3, 4)).to(dev)
+        if layout == "glb":
+            pos, cols, idx = mesher.compact(points.view(-1, 3), n_used, n_fwd)
+            return {"positions": pos, "colors": cols, "indices": idx, "conf_threshold": thr, "align": align}
+        faces, face_colors = mesher.faces(n_ref)
+        return {"vertices": points.view(-1, 3).clone(), "face_colors": face_colors, "faces": faces, "conf_threshold": thr,
                 "align": align}
 
     # ---------------------------------------------------------------------------------------------- CUDA graph replay

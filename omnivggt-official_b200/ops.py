@@ -261,8 +261,56 @@ def point_cloud_scale(xyz, n_kept: int, ws):
 
 
 def host_read(t: torch.Tensor) -> torch.Tensor:
-    """The device-to-host read of a matching call (its one synchronisation)."""
+    """The device-to-host read of a matching or mesh call (its one synchronisation)."""
     return t.cpu()
+
+
+class Mesher:
+    """Triangle mesh (ovg_mesh_*) of F point maps of H x W pixels: ``keep`` uint8 [F*H*W] is the confidence mask (or a caller's
+    valid mask); ``images`` fp32 [F,3,H,W] give the colours and the background tests, or None (keep = the mask alone).
+    ovg_mesh_count runs here; ``totals`` int64 [3] (reference faces, used vertices, forward faces) is read by the caller, once."""
+
+    def __init__(self, keep: torch.Tensor, images: Optional[torch.Tensor], F: int, H: int, W: int,
+                 mask_black_bg: bool = False, mask_white_bg: bool = False):
+        _chk(keep, torch.uint8, "keep")
+        assert keep.is_contiguous() and keep.numel() == F * H * W
+        if images is not None:
+            _chk(images, F32, "images")
+            assert images.is_contiguous() and tuple(images.shape) == (F, 3, H, W)
+        self.F, self.H, self.W, self.images = F, H, W, images
+        lib = L.lib()
+        dev = keep.device
+        self.ws = torch.empty(max(lib.ovg_mesh_workspace_bytes(F, H, W), 0), device=dev, dtype=torch.uint8)
+        self.totals = torch.zeros(3, device=dev, dtype=torch.int64)
+        L.check(lib.ovg_mesh_count(keep.data_ptr(), L.ptr(images), F, H, W, int(mask_black_bg), int(mask_white_bg),
+                                   self.ws.data_ptr(), self.ws.numel(), self.totals.data_ptr(), L.stream()))
+
+    def faces(self, n: int, colors: Optional[torch.Tensor] = None):
+        """The reference layout: (faces int64 [n, 3], face_colors [n, 3]).  Colours: uint8 of ``images``, or gathered from
+        ``colors`` [F*H*W, 3] (any dtype of 1, 2, 4 or 8 bytes) into its dtype."""
+        dev = self.ws.device
+        if colors is None:
+            dtype, cptr, cbytes = torch.uint8, None, 1
+        else:
+            assert colors.is_contiguous() and colors.numel() == self.F * self.H * self.W * 3
+            dtype, cptr, cbytes = colors.dtype, colors.data_ptr(), colors.element_size()
+        faces = torch.empty(max(n, 1), 3, device=dev, dtype=torch.int64)       # >= 1 row: the library wants real pointers
+        cols = torch.empty(max(n, 1), 3, device=dev, dtype=dtype)
+        L.check(L.lib().ovg_mesh_faces(L.ptr(self.images), cptr, cbytes, self.F, self.H, self.W, self.ws.data_ptr(),
+                                       self.ws.numel(), faces.data_ptr(), cols.data_ptr(), L.stream()))
+        return faces[:n], cols[:n]
+
+    def compact(self, points: torch.Tensor, n_used: int, n_fwd: int):
+        """The GLB layout: (positions fp32 [n_used, 3], colors uint8 [n_used, 3], indices int32 [n_fwd, 3])."""
+        _chk(points, F32, "points")
+        assert points.is_contiguous() and points.numel() == self.F * self.H * self.W * 3 and self.images is not None
+        dev = self.ws.device
+        pos = torch.empty(max(n_used, 1), 3, device=dev, dtype=F32)
+        cols = torch.empty(max(n_used, 1), 3, device=dev, dtype=torch.uint8)
+        idx = torch.empty(max(n_fwd, 1), 3, device=dev, dtype=torch.int32)
+        L.check(L.lib().ovg_mesh_compact(points.data_ptr(), self.images.data_ptr(), self.F, self.H, self.W, self.ws.data_ptr(),
+                                         self.ws.numel(), pos.data_ptr(), cols.data_ptr(), idx.data_ptr(), L.stream()))
+        return pos[:n_used], cols[:n_used], idx[:n_fwd]
 
 
 class Matcher:
