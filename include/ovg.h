@@ -287,6 +287,24 @@ int ovg_mesh_faces(const float* images, const void* colors, int color_bytes, int
 int ovg_mesh_compact(const float* points, const float* images, int F, int H, int W, const void* workspace,
                      long long workspace_bytes, float* positions, unsigned char* colors, int* indices, void* stream);
 
+/* Model-free sky segmentation: viz.py:357-393 (segment_sky) on F views of H x W at once, and the --mask_sky confidence of
+ * visual_util.py:184-188.  Per view: u8 = the image (uint8), or uint8(trunc(255 * clamp(x, 0, 1))) in fp32; OpenCV's integer
+ * BGR2HSV of u8 with channel 0 read as B; the colour test (H <= 30 && V >= 100) | (S < 10 && V > 150) | (S < 30 && V > 180) |
+ * (S < 50 && V > 220); a 5 x 5 binary opening with outside the image false; then the 8-connected components of the opened mask
+ * whose area satisfies 2 area > the view's largest area are the sky.  Labelling is a union-find whose only atomics are integer
+ * atomicMin (the root of a component is its smallest pixel index, whatever the order of the unions) and integer atomicAdd /
+ * atomicMax of the areas: results are bit-identical from run to run.  No host synchronisation; the number of launches depends
+ * neither on F nor on the image content.  F <= 65535 and F H W < 2^31.
+ * ovg_segment_sky: image element (f, y, x, c) at f view_stride + (y W + x) pixel_stride + c channel_stride (elements of uint8
+ *     when image_u8, else fp32); sky_out uint8 [F, H, W] (1 = sky); conf fp32 [F, H, W] or NULL, and then conf_out fp32
+ *     [F, H, W] = conf * (sky ? 0.f : 1.f).  workspace: ovg_sky_workspace_bytes(F, H, W) bytes, 256-byte aligned. */
+long long ovg_sky_workspace_bytes(int F, int H, int W);
+int ovg_segment_sky(const void* image, int image_u8, long long view_stride, long long pixel_stride, long long channel_stride,
+                    int F, int H, int W, const float* conf, void* workspace, long long workspace_bytes, unsigned char* sky_out,
+                    float* conf_out, void* stream);
+/* ovg_sky_mask_conf: conf_out[i] = conf[i] * (sky[i] ? 0.f : 1.f) over n elements, for a sky mask made elsewhere. */
+int ovg_sky_mask_conf(const float* conf, const unsigned char* sky, long long n, float* conf_out, void* stream);
+
 /* Baseline JPEG decoding on the device, bit-identical to Pillow (libjpeg-turbo's default islow IDCT, fancy upsampling and
  * YCbCr -> RGB tables).  The plan is host code (no CUDA call): it parses every file, routes it to the device or to the host
  * (OVG_JPEG_* below: anything the device cannot decode exactly goes to the host), and builds the staging stream (tables plus the

@@ -134,6 +134,9 @@ EXPORTS = {
     "ovg_mesh_count": (C.c_int, [_vp, _vp, _i, _i, _i, _i, _i, _vp, _ll, _vp, _vp]),
     "ovg_mesh_faces": (C.c_int, [_vp, _vp, _i, _i, _i, _i, _vp, _ll, _vp, _vp, _vp]),
     "ovg_mesh_compact": (C.c_int, [_vp, _vp, _i, _i, _i, _vp, _ll, _vp, _vp, _vp, _vp]),
+    "ovg_sky_workspace_bytes": (_ll, [_i, _i, _i]),
+    "ovg_segment_sky": (C.c_int, [_vp, _i, _ll, _ll, _ll, _i, _i, _i, _vp, _vp, _ll, _vp, _vp, _vp]),
+    "ovg_sky_mask_conf": (C.c_int, [_vp, _vp, _ll, _vp, _vp]),
     "ovg_jpeg_plan_create": (C.c_int, [_pp, C.POINTER(_ll), _i, _i, _pp]),
     "ovg_jpeg_plan_destroy": (None, [_vp]),
     "ovg_jpeg_plan_file": (C.c_int, [_vp, _i, C.POINTER(_i), C.POINTER(_i), C.POINTER(_i), C.POINTER(_i)]),

@@ -16,6 +16,7 @@
 #include "post.cuh"
 #include "match.cuh"
 #include "mesh.cuh"
+#include "sky.cuh"
 #include "tail.cuh"
 #include "pre.cuh"
 #include "jpeg.cuh"
@@ -1108,6 +1109,79 @@ int ovg_mesh_compact(const float* points, const float* images, int F, int H, int
   if ((rc = post_launch("ovg_mesh_compact(vertices)"))) return rc;
   ovg::mesh_indices_kernel<<<dim3(p.tpv, F), ovg::MESH_THREADS, 0, st>>>(p);
   return post_launch("ovg_mesh_compact(indices)");
+}
+
+}  // extern "C"
+
+// ------------------------------------------------------------------------------------------------------- sky segmentation
+namespace {
+
+// Sky workspace, carved the same way by the size query and by the entry point.
+ovg::SkyParams sky_workspace(void* base, int F, int H, int W, long long* bytes) {
+  char* b = static_cast<char*>(base);
+  long long off = 0;
+  auto carve = [&](long long n) {
+    char* r = b ? b + off : nullptr;
+    off += (n + 255) / 256 * 256;
+    return r;
+  };
+  ovg::SkyParams p{};
+  p.F = F; p.H = H; p.W = W;
+  p.hw = static_cast<long long>(H) * W;
+  p.n = F * p.hw;
+  p.tiles_x = (W + ovg::SKY_TILE - 1) / ovg::SKY_TILE;
+  p.label = reinterpret_cast<int*>(carve(4 * p.n));
+  p.area = reinterpret_cast<int*>(carve(4 * p.n));
+  p.view_max = reinterpret_cast<int*>(carve(4LL * F));
+  *bytes = off;
+  return p;
+}
+
+}  // namespace
+
+extern "C" {
+
+long long ovg_sky_workspace_bytes(int F, int H, int W) {
+  if (F <= 0 || H <= 0 || W <= 0) return -1;
+  long long bytes = 0;
+  sky_workspace(nullptr, F, H, W, &bytes);
+  return bytes;
+}
+
+int ovg_segment_sky(const void* image, int image_u8, long long view_stride, long long pixel_stride, long long channel_stride,
+                    int F, int H, int W, const float* conf, void* workspace, long long workspace_bytes, unsigned char* sky_out,
+                    float* conf_out, void* stream) {
+  OVG_REQUIRE(F > 0 && F <= 65535 && H > 0 && W > 0, "bad sizes");
+  OVG_REQUIRE(static_cast<long long>(F) * H * W < (1LL << 31), "F*H*W must be below 2^31");
+  OVG_REQUIRE(image && sky_out && (conf == nullptr) == (conf_out == nullptr), "null image / sky_out, or conf without conf_out");
+  long long bytes = 0;
+  ovg::SkyParams p = sky_workspace(workspace, F, H, W, &bytes);
+  OVG_REQUIRE(workspace && (reinterpret_cast<uintptr_t>(workspace) & 255) == 0 && workspace_bytes >= bytes,
+              "workspace must be 256-byte aligned and ovg_sky_workspace_bytes(F, H, W) long");
+  p.image = image; p.u8 = image_u8 ? 1 : 0;
+  p.view_stride = view_stride; p.pixel_stride = pixel_stride; p.channel_stride = channel_stride;
+  p.conf = conf; p.conf_out = conf_out; p.sky = sky_out;
+  cudaStream_t st = reinterpret_cast<cudaStream_t>(stream);
+  const int tiles = p.tiles_x * ((H + ovg::SKY_TILE - 1) / ovg::SKY_TILE);
+  ovg::sky_open_kernel<<<dim3(tiles, F), ovg::SKY_THREADS, 0, st>>>(p);
+  int rc = post_launch("ovg_segment_sky(colour test, opening)");
+  if (rc) return rc;
+  const unsigned blocks = static_cast<unsigned>((p.n + 255) / 256);
+  ovg::sky_merge_kernel<<<blocks, 256, 0, st>>>(p);
+  if ((rc = post_launch("ovg_segment_sky(merge)"))) return rc;
+  ovg::sky_area_kernel<<<blocks, 256, 0, st>>>(p);
+  if ((rc = post_launch("ovg_segment_sky(area)"))) return rc;
+  ovg::sky_max_kernel<<<blocks, 256, 0, st>>>(p);
+  if ((rc = post_launch("ovg_segment_sky(max area)"))) return rc;
+  ovg::sky_select_kernel<<<blocks, 256, 0, st>>>(p);
+  return post_launch("ovg_segment_sky(select)");
+}
+
+int ovg_sky_mask_conf(const float* conf, const unsigned char* sky, long long n, float* conf_out, void* stream) {
+  OVG_REQUIRE(conf && sky && conf_out && n > 0 && n < (1LL << 40), "bad arguments");
+  ovg::sky_mask_conf_kernel<<<static_cast<unsigned>((n + 255) / 256), 256, 0, reinterpret_cast<cudaStream_t>(stream)>>>(
+      conf, sky, n, conf_out);
+  return post_launch("ovg_sky_mask_conf");
 }
 
 }  // extern "C"

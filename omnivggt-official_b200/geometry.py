@@ -1,6 +1,7 @@
 """Geometry of point maps on the device: dense correspondence (libovg ovg_match_*, the reference's
-omnivggt/utils/geometry.py:435-451 find_reciprocal_matches) and triangle meshes (libovg ovg_mesh_*, the reference's
-omnivggt/viz.py:40-89 pts3d_to_trimesh and cat_meshes)."""
+omnivggt/utils/geometry.py:435-451 find_reciprocal_matches), triangle meshes (libovg ovg_mesh_*, the reference's
+omnivggt/viz.py:40-89 pts3d_to_trimesh and cat_meshes) and model-free sky segmentation (libovg ovg_segment_sky, the
+reference's omnivggt/viz.py:357-393 segment_sky)."""
 from __future__ import annotations
 
 import numpy as np
@@ -97,6 +98,30 @@ def pts3d_to_trimesh(img, pts3d, valid=None):
     n = int(ops.host_read(mesher.totals)[0])
     faces, face_colors = mesher.faces(n, colors.view(H * W, 3))
     return {"vertices": pts.reshape(-1, 3), "face_colors": face_colors, "faces": faces}
+
+
+def segment_sky(image):
+    """Drop-in for viz.py:357-393: the sky of one image.  image [H, W, 3] of dtype uint8, float32 or float64: a CUDA or CPU
+    tensor, or an array (moved to the current CUDA device).  Floating images become uint8(255 * clip(x, 0, 1)) in their own
+    dtype, truncated (float64 by torch on the device, float32 inside the kernel); channel 0 is read as B, as the reference's
+    cv2.cvtColor(..., COLOR_BGR2HSV) does.  Returns bool [H, W] on the device, True = sky."""
+    shape = tuple(image.shape) if hasattr(image, "shape") else np.shape(image)
+    if len(shape) != 3 or shape[2] != 3:
+        raise ValueError(f"image must have shape [H, W, 3], got {shape}")
+    dtype = image.dtype if torch.is_tensor(image) else np.asarray(image).dtype
+    ok = (dtype in (torch.uint8, torch.float32, torch.float64) if torch.is_tensor(image)
+          else dtype in (np.uint8, np.float32, np.float64))
+    if not ok:
+        raise ValueError(f"image dtype must be uint8, float32 or float64, got {dtype}")
+    H, W = shape[:2]
+    if H == 0 or W == 0:
+        return torch.zeros(H, W, device=_device_of(image), dtype=torch.bool)
+    img = _to(image, _device_of(image))
+    if img.dtype == torch.float64:
+        img = (255 * img.clamp(0, 1)).to(torch.uint8)
+    img = img.contiguous()
+    sky, _ = ops.segment_sky(img, 1, H, W, H * W * 3, 3, 1)
+    return sky.view(H, W).bool()
 
 
 def cat_meshes(meshes):

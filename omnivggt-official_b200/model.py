@@ -16,6 +16,7 @@ import warnings
 import weakref
 from typing import Dict, List, Optional, Sequence, Tuple
 
+import numpy as np
 import torch
 import torch.nn as nn
 
@@ -345,9 +346,61 @@ class OmniVGGT(nn.Module, PyTorchModelHubMixin):
         return images, ext, points, conf
 
     @staticmethod
+    def _segment_views(images: torch.Tensor, conf: Optional[torch.Tensor] = None):
+        """ops.segment_sky over the views of images fp32 [S,3,H,W], read in place when each channel plane is contiguous."""
+        from . import ops
+        S, _, H, W = images.shape
+        if images.stride(3) != 1 or images.stride(2) != W:
+            images = images.contiguous()
+        return ops.segment_sky(images, S, H, W, images.stride(0), 1, images.stride(1), conf)
+
+    @staticmethod
+    @torch.no_grad()
+    def sky_mask(predictions: Dict[str, object], *, scene: int = 0) -> torch.Tensor:
+        """The sky of every view of one scene: the reference's model-free segment_sky (viz.py:357-393) on the images the model
+        saw, ``predictions["images"]`` fp32 [S,3,H,W] (or [B,S,3,H,W]), all views in one call with no host read.  Returns bool
+        [S, H, W] on the device, True = sky; ``point_cloud``, ``mesh`` and ``matches`` take it as ``mask_sky``."""
+        images = predictions["images"]
+        images = (images[scene] if images.dim() == 5 else images).float()
+        sky, _ = OmniVGGT._segment_views(images)
+        return sky.bool()
+
+    @staticmethod
+    def _check_mask_sky(mask_sky, predictions: Dict[str, object], scene: int) -> None:
+        """mask_sky is a bool, or a bool tensor [S, H, W] / [B, S, H, W] (True = sky) on the images' device."""
+        if isinstance(mask_sky, (bool, np.bool_)):
+            return
+        if not torch.is_tensor(mask_sky) or mask_sky.dtype != torch.bool:
+            raise ValueError(f"mask_sky must be a bool or a bool tensor, got {getattr(mask_sky, 'dtype', type(mask_sky))}")
+        images = predictions["images"]
+        want = (tuple(images.shape[:2]) if images.dim() == 5 else (images.shape[0],)) + tuple(images.shape[-2:])
+        if mask_sky.dim() == 4 and images.dim() == 5:
+            ok = tuple(mask_sky.shape) == want
+        else:
+            ok = tuple(mask_sky.shape) == want[-3:]
+        if not ok:
+            raise ValueError(f"mask_sky must have shape [S, H, W] = {list(want[-3:])}"
+                             + (f" or [B, S, H, W] = {list(want)}" if images.dim() == 5 else "") + f", got {list(mask_sky.shape)}")
+        if mask_sky.device != images.device:
+            raise ValueError(f"mask_sky is on {mask_sky.device}, the images on {images.device}")
+
+    @staticmethod
+    def _sky_conf(mask_sky, images: torch.Tensor, conf: torch.Tensor, scene: int) -> torch.Tensor:
+        """conf [S,H,W] of the scene times non-sky, over all S views, as visual_util.py:186-188 does before the frame selection
+        and the percentile.  mask_sky False: conf unchanged, no launch."""
+        from . import ops
+        if isinstance(mask_sky, (bool, np.bool_)):
+            if not mask_sky:
+                return conf
+            _, out = OmniVGGT._segment_views(images, conf.float().contiguous())
+            return out
+        sky = mask_sky[scene] if mask_sky.dim() == 4 else mask_sky
+        return ops.sky_mask_conf(conf.float().contiguous(), sky.contiguous().view(torch.uint8))
+
+    @staticmethod
     @torch.no_grad()
     def matches(predictions: Dict[str, object], pairs=None, *, source: str = "depth", conf_percent: float = 50.0,
-                conf_floor: float = 1e-5, scene: int = 0) -> List[Dict[str, object]]:
+                conf_floor: float = 1e-5, scene: int = 0, mask_sky=False) -> List[Dict[str, object]]:
         """Dense cross-view correspondences of one scene by reciprocal nearest neighbours of the predicted points (the
         DUSt3R-family recipe on utils/geometry.py:435-451 find_reciprocal_matches and :15-37 xy_grid), on the device.
 
@@ -356,9 +409,11 @@ class OmniVGGT(nn.Module, PyTorchModelHubMixin):
         row-major order, and the result is ``{"xy_i", "xy_j", "count"}`` with ``xy_j = grid_j[kept_j][reciprocal_in_P2]`` and
         ``xy_i = grid_i[kept_i][nn2_in_P1][reciprocal_in_P2]``: int64 [count, 2] (x, y) pixel coordinates on the device.
         Every view's index is built once; all pairs are queried in one pass; the match counts are the one host read.  Kept
-        points that are not finite raise ValueError; a view with no kept point has no matches."""
+        points that are not finite raise ValueError; a view with no kept point has no matches.  ``mask_sky``: as in
+        ``point_cloud``."""
         from . import geometry, ops
         OmniVGGT._check_source(source, conf_percent, conf_floor)
+        OmniVGGT._check_mask_sky(mask_sky, predictions, scene)
         images = predictions["images"]
         S = (images[scene] if images.dim() == 5 else images).shape[0]
         pair_arr = geometry.check_pairs(pairs, S)
@@ -367,6 +422,7 @@ class OmniVGGT(nn.Module, PyTorchModelHubMixin):
         images, _, points, conf = OmniVGGT._scene_source(predictions, source, scene)
         _, _, H, W = images.shape
         dev = images.device
+        conf = OmniVGGT._sky_conf(mask_sky, images, conf, scene)
         mask, _, _ = ops.conf_percentile_mask(conf.float().contiguous(), conf_percent, conf_floor)
         mt = ops.Matcher(points.float().contiguous().view(S, H * W, 3), mask.view(S, H * W),
                          torch.from_numpy(pair_arr).to(dev))
@@ -380,7 +436,7 @@ class OmniVGGT(nn.Module, PyTorchModelHubMixin):
     @torch.no_grad()
     def point_cloud(predictions: Dict[str, object], *, source: str = "depth", conf_percent: float = 50.0,
                     conf_floor: float = 1e-5, frame: Optional[int] = None, mask_black_bg: bool = False,
-                    mask_white_bg: bool = False, scene: int = 0) -> Dict[str, torch.Tensor]:
+                    mask_white_bg: bool = False, scene: int = 0, mask_sky=False) -> Dict[str, torch.Tensor]:
         """The filtered, coloured point cloud of one scene, built on the device (libovg kernels).
 
         Replaces the host numpy of the reference's GLB export (visual_util.py:190-236,:320-358 predictions_to_glb) and
@@ -394,10 +450,17 @@ class OmniVGGT(nn.Module, PyTorchModelHubMixin):
         Returns ``points`` fp32 [n,3], ``colors`` uint8 [n,3], ``frame`` int32 [n] (numpy boolean-indexing order),
         ``conf_threshold`` (0-d), ``center`` fp32 [3] (mean of all points of the selected views, inference.py:111),
         ``scale`` (0-d, ||p95 - p5||, 1.0 when nothing is kept) and ``align`` fp64 [4,4] = inv(E0) diag(1,-1,-1,1) R_y(180)
-        with E0 the first selected camera (visual_util.py:320-341).  The kept count and E0 are the only device-to-host reads."""
+        with E0 the first selected camera (visual_util.py:320-341).  The kept count and E0 are the only device-to-host reads.
+
+        ``mask_sky`` (the reference's --mask_sky, visual_util.py:140-188): False, no sky masking; True, the sky of every view
+        by ``sky_mask``; or a bool tensor [S,H,W] / [B,S,H,W], True = sky (a reference mask file m, uint8 255 = non-sky, at
+        H x W is ``m == 0``).  The confidence of every view becomes conf * non-sky before the frame selection and the
+        percentile, as the reference orders it; no host read is added."""
         from . import ops
         OmniVGGT._check_source(source, conf_percent, conf_floor)
+        OmniVGGT._check_mask_sky(mask_sky, predictions, scene)
         images, ext, points, conf = OmniVGGT._scene_source(predictions, source, scene)
+        conf = OmniVGGT._sky_conf(mask_sky, images, conf, scene)
         S, _, H, W = images.shape
         f0 = 0
         if frame is not None:
@@ -441,7 +504,7 @@ class OmniVGGT(nn.Module, PyTorchModelHubMixin):
     @torch.no_grad()
     def mesh(predictions: Dict[str, object], *, source: str = "depth", conf_percent: float = 50.0, conf_floor: float = 1e-5,
              frame: Optional[int] = None, mask_black_bg: bool = False, mask_white_bg: bool = False, scene: int = 0,
-             layout: str = "reference") -> Dict[str, torch.Tensor]:
+             layout: str = "reference", mask_sky=False) -> Dict[str, torch.Tensor]:
         """The coloured triangle mesh of one scene's point maps, built on the device (libovg kernels): the DUSt3R-family
         recipe of viz.py:40-89, ``cat_meshes([pts3d_to_trimesh(colors[f], points[f], keep[f]) for f in views])``.
 
@@ -456,7 +519,7 @@ class OmniVGGT(nn.Module, PyTorchModelHubMixin):
         index order, each with its own pixel's colour, and ``indices`` int32 [k, 3] of the forward triangles only, for
         ``glb.write_mesh_glb`` (whose material is double-sided in place of the reversed copies).
         Both add ``conf_threshold`` and ``align``, as ``point_cloud`` returns them.  The three totals and the first camera are
-        read back together: the one host synchronisation."""
+        read back together: the one host synchronisation.  ``mask_sky``: as in ``point_cloud``."""
         from . import ops
         OmniVGGT._check_source(source, conf_percent, conf_floor)
         if layout not in ("reference", "glb"):
@@ -465,7 +528,9 @@ class OmniVGGT(nn.Module, PyTorchModelHubMixin):
         S = (images[scene] if images.dim() == 5 else images).shape[0]
         if frame is not None and not 0 <= frame < S:
             raise IndexError(f"frame {frame} out of range for {S} views")
+        OmniVGGT._check_mask_sky(mask_sky, predictions, scene)
         images, ext, points, conf = OmniVGGT._scene_source(predictions, source, scene)
+        conf = OmniVGGT._sky_conf(mask_sky, images, conf, scene)
         _, _, H, W = images.shape
         f0 = 0
         if frame is not None:

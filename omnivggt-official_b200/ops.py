@@ -260,6 +260,35 @@ def point_cloud_scale(xyz, n_kept: int, ws):
     return scale
 
 
+def segment_sky(image, F: int, H: int, W: int, view_stride: int, pixel_stride: int, channel_stride: int,
+                conf: Optional[torch.Tensor] = None):
+    """Sky of F views (ovg_segment_sky): image uint8 or fp32 on the device, element (f, y, x, c) at f view_stride +
+    (y W + x) pixel_stride + c channel_stride.  Returns (sky uint8 [F, H, W], conf fp32 [F, H, W] * non-sky or None)."""
+    if image.dtype not in (torch.uint8, F32) or not _on_device(image):
+        raise TypeError(f"image: expected cuda uint8 or float32, got {image.device} {image.dtype}")
+    dev = image.device
+    sky = torch.empty(F, H, W, device=dev, dtype=torch.uint8)
+    conf_out = None
+    if conf is not None:
+        _chk(conf, F32, "conf")
+        assert conf.is_contiguous() and conf.numel() == F * H * W
+        conf_out = torch.empty(F, H, W, device=dev, dtype=F32)
+    lib = L.lib()
+    ws = torch.empty(max(lib.ovg_sky_workspace_bytes(F, H, W), 0), device=dev, dtype=torch.uint8)
+    L.check(lib.ovg_segment_sky(image.data_ptr(), int(image.dtype == torch.uint8), view_stride, pixel_stride, channel_stride,
+                                F, H, W, L.ptr(conf), ws.data_ptr(), ws.numel(), sky.data_ptr(), L.ptr(conf_out), L.stream()))
+    return sky, conf_out
+
+
+def sky_mask_conf(conf, sky):
+    """conf fp32 [n...] * (sky ? 0 : 1) for a bool / uint8 sky mask of the same size (ovg_sky_mask_conf)."""
+    _chk(conf, F32, "conf")
+    assert conf.is_contiguous() and sky.is_contiguous() and sky.numel() == conf.numel() and sky.element_size() == 1
+    out = torch.empty_like(conf)
+    L.check(L.lib().ovg_sky_mask_conf(conf.data_ptr(), sky.data_ptr(), conf.numel(), out.data_ptr(), L.stream()))
+    return out
+
+
 def host_read(t: torch.Tensor) -> torch.Tensor:
     """The device-to-host read of a matching or mesh call (its one synchronisation)."""
     return t.cpu()
