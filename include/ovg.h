@@ -94,9 +94,10 @@ int ovg_gemm(const ovg_gemm_args* args, void* stream);
  * nq == nkv is self-attention; nq < nkv is what a context-parallel rank runs: its own queries against the keys / values of
  * all ranks.  Replaces F.scaled_dot_product_attention, layers/attention.py:61-66.
  * scratch: NULL, or ovg_attention_scratch_bytes() bytes (16-byte aligned).  With scratch, for long sequences whose 128-row query
- * tiles do not fill the last wave of resident CTAs (two per SM), the tiles of that wave are cut into 2-4 key ranges, one CTA each,
- * and a small kernel merges their (un-normalised O, softmax reference, row sum) -- e.g. 1 376 tiles on 296 slots: 4.67 instead of
- * 5 waves.  Results are deterministic (fixed merge order); scratch NULL = no split. */
+ * tiles do not fill the last wave of resident CTAs (one per SM), the tiles of that wave are cut into 2-4 key ranges, one CTA each,
+ * and a small kernel merges their (un-normalised O, softmax reference, row sum) -- e.g. on an H100 SXM (132 SMs) 1 376 tiles leave
+ * a last wave of 56 tiles, which runs as 112 half-length CTAs: 10.5 instead of 11 waves.  Results are deterministic (fixed merge
+ * order); scratch NULL = no split. */
 long long ovg_attention_scratch_bytes(void);
 int ovg_attention(const void* q, const void* k, const void* v, void* out, int batch, int heads, int nq, int nkv,
                   void* scratch, long long scratch_bytes, void* stream);
@@ -454,7 +455,7 @@ int ovg_dpt_forward_f32(ovg_dpt* h, const float* const* layers, int T, int nspec
 
 /* Camera head: iterative pose refinement on the camera tokens; reference heads/camera_head.py:83-154.  The weight-streaming
  * GEMMs run on the wgmma GEMM; AdaLN, the S-token attention (head_dim D / heads) and the 9-wide pose update are small fp32
- * kernels. */
+ * kernels.  ovg_camera_create rejects a head_dim other than 32, 64, 128 or 256. */
 typedef struct ovg_camera_desc {
   int D; int heads; int trunk_depth;                           /* 2*embed_dim (2048), 16, 4 */
   const ovg_block_weights* trunk;                              /* host array [trunk_depth]; qn_w .. kn_b NULL */

@@ -207,8 +207,10 @@ def test_attention_global_sizes_of_baseline_configs(heads, n):
 
 @pytest.mark.parametrize("batch,heads,n", [(1, 16, 4 * 1374), (2, 16, 4 * 1374), (1, 7, 9000)])
 def test_attention_split_tail_shapes(batch, heads, n):
-    """KV-split tail tiles at other tile counts (688 / 1 376 over two batch entries / 497 tiles on 296 resident CTAs), ragged last KV
-    tile, peaky rows."""
+    """Attention with scratch at other tile counts, ragged last KV tile, peaky rows.  On an H100 SXM (132 resident CTAs, one per SM)
+    688 tiles leave a last wave of 28 tiles, split in 3 parts; 1 376 tiles over two batch entries leave 56, split in 2; 497 tiles leave
+    101, which the cost rule does not split, so that case checks the unsplit path with scratch given.  test_kernel_bounds_gpu.py
+    asserts which path each of its shapes takes on the device it runs on."""
     ops = _ops()
     q = randn(batch, heads, n, 64, seed=1) * 1.5
     k = randn(batch, heads, n, 64, seed=2)
