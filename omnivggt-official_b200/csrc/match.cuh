@@ -1,12 +1,15 @@
 // Reciprocal nearest-neighbour matches between the point sets of several views (utils/geometry.py:435-451,
 // find_reciprocal_matches: two cKDTree builds and two queries per pair on the host).
-//   match_keep_* kernels     per-view ordered compaction of the kept points (tile count / scan / ballot scatter)
+//   match_keep_* kernels     per-view ordered compaction of the kept points (compact.cuh: tile count / scan / gather)
 //   match_hist_* kernels     per-view grid range: 0.1 % / 99.9 % quantiles per axis, coarse (fp32 key) then linear bins
 //   match_cell_* kernels     uniform grid per view: cell of every point, counts, per-view scan of the cell starts
 //   match_radix_* kernels    stable LSD radix sort of every view's points by cell (kept-index order inside a cell)
 //   match_query_kernel       exact nearest neighbour of every point of view a among the points of view b, both directions of
 //                            every pair in one launch
-//   match_recip_* kernels    reciprocity nn1[nn2[j]] == j, per-pair counts, ordered compaction of the matches
+//   match_recip_count_kernel reciprocity nn1[nn2[j]] == j, tile counts of every pair
+//   tile_scan_kernel         one scan over the pairs' tile counts, concatenated (compact.cuh)
+//   match_counts_kernel      matches per pair
+//   match_gather_kernel      ordered compaction of the matches
 // Distances are fp64, d2 = ((dx * dx) + (dy * dy)) + dz * dz without contraction, as cKDTree computes them for 3-D data; among
 // points at the same d2 the lowest index wins.  The grid only prunes: a cell or a whole shell of cells is skipped only when a
 // lower bound on its d2 is strictly greater than the best d2 so far, so the result is the exact (d2, index) minimum over all
@@ -16,15 +19,11 @@
 
 namespace ovg {
 
-constexpr int MATCH_THREADS = 256;
-constexpr int MATCH_ITERS = 16;
-constexpr int MATCH_TILE = MATCH_THREADS * MATCH_ITERS;   // points per compaction tile
 constexpr int MATCH_BINS = 2048;                           // histogram bins per axis
 constexpr int MATCH_MAX_DIM = 4096;                        // cells per axis
 constexpr int MATCH_QUERY_THREADS = 128;
 
 __host__ __device__ inline long long match_cells_cap(long long cap) { return 2 * cap + 64; }   // cells per view
-__host__ __device__ inline long long match_tiles(long long cap) { return (cap + MATCH_TILE - 1) / MATCH_TILE; }
 
 struct MatchGrid {        // one view's grid; cell k along an axis holds lo + k h <= x < lo + (k + 1) h (up to rounding, see pad)
   double lo[3];
@@ -39,7 +38,7 @@ struct MatchParams {
   const unsigned char* keep;      // [V, cap] or NULL (all kept)
   int V;
   long long cap;
-  int tiles;                      // compaction tiles per view (match_tiles(cap))
+  int tiles;                      // compaction tiles per view (compact_tiles(cap))
   unsigned int* flag;             // bit 0: a kept point is not finite
   unsigned int* view_tile_count;  // [V, tiles]
   unsigned int* view_tile_offset; // [V, tiles]
@@ -59,7 +58,7 @@ struct MatchParams {
   const int* pairs;               // [P, 2]
   int P;
   int* nn;                        // [2P, cap]: segment 2p = view i into view j, 2p + 1 = view j into view i
-  int ptiles;                     // reciprocity tiles per pair (match_tiles(cap))
+  int ptiles;                     // reciprocity tiles per pair (compact_tiles(cap))
   unsigned int* pair_tile_count;  // [P, ptiles]
   unsigned long long* pair_tile_offset;
   unsigned long long* total;
@@ -72,60 +71,38 @@ __device__ __forceinline__ bool match_kept(const MatchParams& p, int v, long lon
 }
 
 // grid (tiles, V): kept points per tile
-__global__ void __launch_bounds__(MATCH_THREADS) match_keep_count_kernel(const MatchParams p) {
-  __shared__ unsigned int warp_sum[MATCH_THREADS / 32];
+__global__ void __launch_bounds__(COMPACT_THREADS) match_keep_count_kernel(const MatchParams p) {
   const int v = blockIdx.y;
-  const long long base = static_cast<long long>(blockIdx.x) * MATCH_TILE;
-  unsigned int kept = 0;
-  for (int it = 0; it < MATCH_ITERS; ++it) kept += match_kept(p, v, base + it * MATCH_THREADS + threadIdx.x) ? 1u : 0u;
-#pragma unroll
-  for (int o = 16; o > 0; o >>= 1) kept += __shfl_xor_sync(0xffffffffu, kept, o);
-  if ((threadIdx.x & 31) == 0) warp_sum[threadIdx.x >> 5] = kept;
-  __syncthreads();
-  if (threadIdx.x == 0) {
-    unsigned int s = 0;
-    for (int w = 0; w < MATCH_THREADS / 32; ++w) s += warp_sum[w];
-    p.view_tile_count[v * p.tiles + blockIdx.x] = s;
-  }
+  const long long base = static_cast<long long>(blockIdx.x) * COMPACT_TILE;
+  unsigned int kept[1] = {0u};
+  for (int it = 0; it < COMPACT_ITERS; ++it) kept[0] += match_kept(p, v, base + it * COMPACT_THREADS + threadIdx.x) ? 1u : 0u;
+  const unsigned int s = tile_sum<1>(kept);
+  if (threadIdx.x == 0) p.view_tile_count[v * p.tiles + blockIdx.x] = s;
 }
 
-// grid V, one thread: exclusive scan of the view's tile counts (a view has cap / 4096 tiles), the view's kept count
-__global__ void match_keep_scan_kernel(const MatchParams p) {
-  if (threadIdx.x != 0) return;
+// grid V, 1024 threads: exclusive scan of the view's tile counts, the view's kept count
+__global__ void __launch_bounds__(1024) match_keep_scan_kernel(const MatchParams p) {
   const int v = blockIdx.x;
-  unsigned int s = 0;
-  for (int t = 0; t < p.tiles; ++t) {
-    p.view_tile_offset[v * p.tiles + t] = s;
-    s += p.view_tile_count[v * p.tiles + t];
-  }
-  p.grid[v].n = static_cast<int>(s);
+  const unsigned int n = block_exclusive_scan(p.view_tile_count + v * p.tiles, p.view_tile_offset + v * p.tiles, p.tiles);
+  if (threadIdx.x == 0) p.grid[v].n = static_cast<int>(n);
 }
 
 // grid (tiles, V): kept point k of view v -> pts[v, k] = (x, y, z, pixel index), in pixel order
-__global__ void __launch_bounds__(MATCH_THREADS) match_keep_gather_kernel(const MatchParams p) {
-  __shared__ unsigned int warp_pre[MATCH_THREADS / 32 + 1];
+__global__ void __launch_bounds__(COMPACT_THREADS) match_keep_gather_kernel(const MatchParams p) {
   const int v = blockIdx.y;
-  const int lane = threadIdx.x & 31, warp = threadIdx.x >> 5;
-  const long long base = static_cast<long long>(blockIdx.x) * MATCH_TILE;
+  const long long base = static_cast<long long>(blockIdx.x) * COMPACT_TILE;
   unsigned int out = p.view_tile_offset[v * p.tiles + blockIdx.x];
-  for (int it = 0; it < MATCH_ITERS; ++it) {
-    const long long i = base + it * MATCH_THREADS + threadIdx.x;
-    const bool keep = match_kept(p, v, i);
-    const unsigned int ballot = __ballot_sync(0xffffffffu, keep);
-    if (lane == 0) warp_pre[warp + 1] = __popc(ballot);
-    __syncthreads();
-    if (threadIdx.x == 0) {
-      warp_pre[0] = 0;
-      for (int w = 1; w <= MATCH_THREADS / 32; ++w) warp_pre[w] += warp_pre[w - 1];
-    }
-    __syncthreads();
-    if (keep) {
-      const unsigned int k = out + warp_pre[warp] + __popc(ballot & ((1u << lane) - 1u));
+  for (int it = 0; it < COMPACT_ITERS; ++it) {
+    const long long i = base + it * COMPACT_THREADS + threadIdx.x;
+    const bool keep[1] = {match_kept(p, v, i)};
+    unsigned int rank[1], sum[1];
+    chunk_ranks<1>(keep, rank, sum);
+    if (keep[0]) {
+      const unsigned int k = out + rank[0];
       const float* s = p.points + (v * p.cap + i) * 3;
       p.pts[v * p.cap + k] = make_float4(s[0], s[1], s[2], __int_as_float(static_cast<int>(i)));
     }
-    out += warp_pre[MATCH_THREADS / 32];
-    __syncthreads();
+    out += sum[0];
   }
 }
 
@@ -258,41 +235,13 @@ __global__ void __launch_bounds__(256) match_cell_count_kernel(const MatchParams
   }
 }
 
-// One block of 1024 threads: exclusive scan of cnt[0, len) into out (out may be cnt), runs per thread, Hillis-Steele over the
-// runs; returns the total to every thread.
-template <typename T>
-__device__ T match_block_scan(const T* cnt, T* out, long long len) {
-  __shared__ T run[1024];
-  const long long per = (len + 1023) / 1024;
-  const long long c0 = threadIdx.x * per, c1 = min(c0 + per, len);
-  T s = 0;
-  for (long long c = c0; c < c1; ++c) s += cnt[c];
-  run[threadIdx.x] = s;
-  __syncthreads();
-  for (int o = 1; o < 1024; o <<= 1) {
-    const T t = threadIdx.x >= o ? run[threadIdx.x - o] : T(0);
-    __syncthreads();
-    run[threadIdx.x] += t;
-    __syncthreads();
-  }
-  T off = run[threadIdx.x] - s;
-  for (long long c = c0; c < c1; ++c) {
-    const T x = cnt[c];
-    out[c] = off;
-    off += x;
-  }
-  const T total = run[1023];
-  __syncthreads();
-  return total;
-}
-
 // grid V, 1024 threads: cell_start = exclusive scan of the view's cell counts, cell_start[cells] = n
 __global__ void __launch_bounds__(1024) match_cell_scan_kernel(const MatchParams p) {
   const int v = blockIdx.x;
   const MatchGrid& g = p.grid[v];
   const long long cells = static_cast<long long>(g.dim[0]) * g.dim[1] * g.dim[2];
   int* start = p.cell_start + v * (p.cells_cap + 1);
-  const int total = match_block_scan<int>(p.cell_count + v * p.cells_cap, start, cells);
+  const int total = block_exclusive_scan(p.cell_count + v * p.cells_cap, start, cells);
   if (threadIdx.x == 0) start[cells] = total;
 }
 
@@ -317,7 +266,7 @@ __global__ void __launch_bounds__(MATCH_RADIX_TILE) match_radix_count_kernel(con
 // grid V, 1024 threads
 __global__ void __launch_bounds__(1024) match_radix_scan_kernel(const MatchParams p) {
   unsigned int* off = p.radix_off + static_cast<long long>(blockIdx.x) * 256 * p.rtiles;
-  match_block_scan<unsigned int>(off, off, 256LL * p.rtiles);
+  block_exclusive_scan(off, off, 256LL * p.rtiles);
 }
 
 // grid (rtiles, V)
@@ -470,24 +419,16 @@ __device__ __forceinline__ bool match_recip(const MatchParams& p, int pr, long l
 }
 
 // grid (ptiles, P)
-__global__ void __launch_bounds__(MATCH_THREADS) match_recip_count_kernel(const MatchParams p) {
-  __shared__ unsigned int warp_sum[MATCH_THREADS / 32];
+__global__ void __launch_bounds__(COMPACT_THREADS) match_recip_count_kernel(const MatchParams p) {
   const int pr = blockIdx.y;
-  const long long base = static_cast<long long>(blockIdx.x) * MATCH_TILE;
-  unsigned int kept = 0;
-  for (int it = 0; it < MATCH_ITERS; ++it) {
+  const long long base = static_cast<long long>(blockIdx.x) * COMPACT_TILE;
+  unsigned int kept[1] = {0u};
+  for (int it = 0; it < COMPACT_ITERS; ++it) {
     int nn_i;
-    kept += match_recip(p, pr, base + it * MATCH_THREADS + threadIdx.x, &nn_i) ? 1u : 0u;
+    kept[0] += match_recip(p, pr, base + it * COMPACT_THREADS + threadIdx.x, &nn_i) ? 1u : 0u;
   }
-#pragma unroll
-  for (int o = 16; o > 0; o >>= 1) kept += __shfl_xor_sync(0xffffffffu, kept, o);
-  if ((threadIdx.x & 31) == 0) warp_sum[threadIdx.x >> 5] = kept;
-  __syncthreads();
-  if (threadIdx.x == 0) {
-    unsigned int s = 0;
-    for (int w = 0; w < MATCH_THREADS / 32; ++w) s += warp_sum[w];
-    p.pair_tile_count[pr * p.ptiles + blockIdx.x] = s;
-  }
+  const unsigned int s = tile_sum<1>(kept);
+  if (threadIdx.x == 0) p.pair_tile_count[pr * p.ptiles + blockIdx.x] = s;
 }
 
 // one thread per pair, after the scan of the tile counts: matches of the pair; then the non-finite flag
@@ -513,35 +454,26 @@ struct MatchOut {
 };
 
 // grid (ptiles, P): the matches of every pair in ascending jj, pairs in order (offsets from the scan of the tile counts)
-__global__ void __launch_bounds__(MATCH_THREADS) match_gather_kernel(const MatchParams p, const MatchOut o) {
-  __shared__ unsigned int warp_pre[MATCH_THREADS / 32 + 1];
+__global__ void __launch_bounds__(COMPACT_THREADS) match_gather_kernel(const MatchParams p, const MatchOut o) {
   const int pr = blockIdx.y;
-  const int lane = threadIdx.x & 31, warp = threadIdx.x >> 5;
-  const long long base = static_cast<long long>(blockIdx.x) * MATCH_TILE;
+  const long long base = static_cast<long long>(blockIdx.x) * COMPACT_TILE;
   unsigned long long out = p.pair_tile_offset[static_cast<long long>(pr) * p.ptiles + blockIdx.x];
   const int vi = p.pairs[2 * pr], vj = p.pairs[2 * pr + 1];
-  for (int it = 0; it < MATCH_ITERS; ++it) {
-    const long long jj = base + it * MATCH_THREADS + threadIdx.x;
+  for (int it = 0; it < COMPACT_ITERS; ++it) {
+    const long long jj = base + it * COMPACT_THREADS + threadIdx.x;
     int nn_i = -1;
-    const bool keep = match_recip(p, pr, jj, &nn_i);
-    const unsigned int ballot = __ballot_sync(0xffffffffu, keep);
-    if (lane == 0) warp_pre[warp + 1] = __popc(ballot);
-    __syncthreads();
-    if (threadIdx.x == 0) {
-      warp_pre[0] = 0;
-      for (int w = 1; w <= MATCH_THREADS / 32; ++w) warp_pre[w] += warp_pre[w - 1];
-    }
-    __syncthreads();
-    if (keep) {
-      const unsigned long long k = out + warp_pre[warp] + __popc(ballot & ((1u << lane) - 1u));
+    const bool keep[1] = {match_recip(p, pr, jj, &nn_i)};
+    unsigned int rank[1], sum[1];
+    chunk_ranks<1>(keep, rank, sum);
+    if (keep[0]) {
+      const unsigned long long k = out + rank[0];
       const long long pj = __float_as_int(p.pts[vj * p.cap + jj].w), pi = __float_as_int(p.pts[vi * p.cap + nn_i].w);
       o.xy_j[2 * k] = pj % o.W;
       o.xy_j[2 * k + 1] = pj / o.W;
       o.xy_i[2 * k] = pi % o.W;
       o.xy_i[2 * k + 1] = pi / o.W;
     }
-    out += warp_pre[MATCH_THREADS / 32];
-    __syncthreads();
+    out += sum[0];
   }
 }
 

@@ -2,7 +2,7 @@
 // (cat_meshes), all views in one pass.
 //   mesh_keep_kernel      the per-pixel keep bit (pixel_keep of the point cloud, or a caller mask alone)
 //   mesh_count_kernel     per tile of a view: kept TL / BR triangles of the pixel quads and vertices used by a kept one
-//   cloud_scan_kernel     one scan over the three streams' tile counts, concatenated (post.cuh)
+//   tile_scan_kernel      one scan over the three streams' tile counts, concatenated (compact.cuh)
 //   mesh_totals_kernel    reference faces, used vertices, forward faces
 //   mesh_faces_kernel     the reference layout: every kept triangle and its reversed copy, int64 indices, face colours
 //   mesh_vertices_kernel  the GLB layout: used vertices in index order and the remap of their indices
@@ -10,16 +10,13 @@
 // The quad at (y, x) of a view, y < H - 1 and x < W - 1, has the corners tl (y, x), tr (y, x + 1), bl (y + 1, x) and
 // br (y + 1, x + 1); its TL triangle (tl, tr, bl) is kept when all three corners are, its BR triangle (tr, bl, br) likewise.
 // A view's faces are the kept TL triangles, the same reversed, the kept BR triangles, the same reversed, each class in
-// row-major quad order.  Outputs are placed by tile offsets plus ballot ranks, never by atomics: runs are bit-identical.
+// row-major quad order.  Every stream is compacted per view by tiles of COMPACT_TILE pixels as compact.cuh describes.
 #pragma once
 #include "post.cuh"
 
 namespace ovg {
 
-constexpr int MESH_THREADS = 256;
-constexpr int MESH_ITERS = 16;
-constexpr int MESH_TILE = MESH_THREADS * MESH_ITERS;   // pixels of one view per count / faces / compact block
-constexpr int MESH_STREAMS = 3;                        // TL triangles, BR triangles, used vertices
+constexpr int MESH_STREAMS = 3;   // TL triangles, BR triangles, used vertices
 
 struct MeshParams {
   const unsigned char* conf_mask;   // [n]
@@ -72,13 +69,12 @@ __global__ void __launch_bounds__(256) mesh_keep_kernel(const MeshParams p) {
   p.keep[i] = k ? 1 : 0;
 }
 
-// Block (t, f): pixels [t MESH_TILE, (t + 1) MESH_TILE) of view f.
-__global__ void __launch_bounds__(MESH_THREADS) mesh_count_kernel(const MeshParams p) {
-  __shared__ unsigned int warp_sum[MESH_STREAMS][MESH_THREADS / 32];
+// Block (t, f): pixels [t COMPACT_TILE, (t + 1) COMPACT_TILE) of view f.
+__global__ void __launch_bounds__(COMPACT_THREADS) mesh_count_kernel(const MeshParams p) {
   const int f = blockIdx.y;
   unsigned int c[MESH_STREAMS] = {0u, 0u, 0u};
-  for (int it = 0; it < MESH_ITERS; ++it) {
-    const long long q = static_cast<long long>(blockIdx.x) * MESH_TILE + it * MESH_THREADS + threadIdx.x;
+  for (int it = 0; it < COMPACT_ITERS; ++it) {
+    const long long q = static_cast<long long>(blockIdx.x) * COMPACT_TILE + it * COMPACT_THREADS + threadIdx.x;
     if (q < p.hw) {
       const int y = static_cast<int>(q / p.W), x = static_cast<int>(q - static_cast<long long>(y) * p.W);
       const long long i = f * p.hw + q;
@@ -87,19 +83,8 @@ __global__ void __launch_bounds__(MESH_THREADS) mesh_count_kernel(const MeshPara
       c[2] += mesh_used(p, i, y, x);
     }
   }
-#pragma unroll
-  for (int s = 0; s < MESH_STREAMS; ++s) {
-#pragma unroll
-    for (int o = 16; o > 0; o >>= 1) c[s] += __shfl_xor_sync(0xffffffffu, c[s], o);
-    if ((threadIdx.x & 31) == 0) warp_sum[s][threadIdx.x >> 5] = c[s];
-  }
-  __syncthreads();
-  if (threadIdx.x < MESH_STREAMS) {
-    unsigned int sum = 0;
-#pragma unroll
-    for (int w = 0; w < MESH_THREADS / 32; ++w) sum += warp_sum[threadIdx.x][w];
-    p.tile_count[threadIdx.x * p.T + f * p.tpv + blockIdx.x] = sum;
-  }
+  const unsigned int sum = tile_sum<MESH_STREAMS>(c);
+  if (threadIdx.x < MESH_STREAMS) p.tile_count[threadIdx.x * p.T + f * p.tpv + blockIdx.x] = sum;
 }
 
 __global__ void mesh_totals_kernel(const MeshParams p) {
@@ -110,33 +95,6 @@ __global__ void mesh_totals_kernel(const MeshParams p) {
     p.totals[1] = static_cast<long long>(o[3 * p.T] - o[2 * p.T]);
     p.totals[2] = tl + br;
   }
-}
-
-// Ranks of a chunk of MESH_THREADS pixels in S streams: rank[s] = the set flags of stream s before this thread in the chunk,
-// sum[s] = the chunk's set flags.  pre: shared [S][MESH_THREADS / 32 + 1].
-template <int S>
-__device__ __forceinline__ void mesh_chunk_ranks(const bool (&flag)[S], unsigned int (*pre)[MESH_THREADS / 32 + 1],
-                                                 unsigned int (&rank)[S], unsigned int (&sum)[S]) {
-  const int lane = threadIdx.x & 31, warp = threadIdx.x >> 5;
-  unsigned int ballot[S];
-#pragma unroll
-  for (int s = 0; s < S; ++s) {
-    ballot[s] = __ballot_sync(0xffffffffu, flag[s]);
-    if (lane == 0) pre[s][warp + 1] = __popc(ballot[s]);
-  }
-  __syncthreads();
-  if (threadIdx.x < S) {
-    pre[threadIdx.x][0] = 0;
-#pragma unroll
-    for (int w = 1; w <= MESH_THREADS / 32; ++w) pre[threadIdx.x][w] += pre[threadIdx.x][w - 1];
-  }
-  __syncthreads();
-#pragma unroll
-  for (int s = 0; s < S; ++s) {
-    rank[s] = pre[s][warp] + __popc(ballot[s] & ((1u << lane) - 1u));
-    sum[s] = pre[s][MESH_THREADS / 32];
-  }
-  __syncthreads();                                 // pre is rewritten by the next chunk
 }
 
 // Colour of pixel j (frame f) into element k of the face colours.
@@ -183,21 +141,20 @@ __device__ __forceinline__ MeshView mesh_view(const MeshParams& p, int f) {
 }
 
 // Reference layout (viz.py:53-74 per view, :80-89 across views): view f's faces start at 2 (TL + BR kept before f).
-__global__ void __launch_bounds__(MESH_THREADS) mesh_faces_kernel(const MeshParams p) {
-  __shared__ unsigned int pre[2][MESH_THREADS / 32 + 1];
+__global__ void __launch_bounds__(COMPACT_THREADS) mesh_faces_kernel(const MeshParams p) {
   const int f = blockIdx.y;
   const MeshView v = mesh_view(p, f);
   const unsigned long long base = 2 * (v.tl0 + v.br0);
   unsigned long long r_tl = p.tile_offset[f * p.tpv + blockIdx.x] - p.tile_offset[f * p.tpv];
   unsigned long long r_br = p.tile_offset[p.T + f * p.tpv + blockIdx.x] - p.tile_offset[p.T + f * p.tpv];
-  for (int it = 0; it < MESH_ITERS; ++it) {
-    const long long q = static_cast<long long>(blockIdx.x) * MESH_TILE + it * MESH_THREADS + threadIdx.x;
+  for (int it = 0; it < COMPACT_ITERS; ++it) {
+    const long long q = static_cast<long long>(blockIdx.x) * COMPACT_TILE + it * COMPACT_THREADS + threadIdx.x;
     const int y = static_cast<int>(q / p.W), x = static_cast<int>(q - static_cast<long long>(y) * p.W);
     const long long i = f * p.hw + q;
     const bool in = q < p.hw;
     const bool flag[2] = {in && mesh_tl(p, i, y, x), in && mesh_br(p, i, y, x)};
     unsigned int rank[2], sum[2];
-    mesh_chunk_ranks<2>(flag, pre, rank, sum);
+    chunk_ranks<2>(flag, rank, sum);
     const long long tr = i + 1, bl = i + p.W, br = i + p.W + 1;
     if (flag[0]) {
       const unsigned long long k = base + r_tl + rank[0];
@@ -219,17 +176,16 @@ __global__ void __launch_bounds__(MESH_THREADS) mesh_faces_kernel(const MeshPara
 }
 
 // GLB layout, part 1: the used vertices in index order with their own pixel's colour, and remap[i] = the rank of vertex i.
-__global__ void __launch_bounds__(MESH_THREADS) mesh_vertices_kernel(const MeshParams p) {
-  __shared__ unsigned int pre[1][MESH_THREADS / 32 + 1];
+__global__ void __launch_bounds__(COMPACT_THREADS) mesh_vertices_kernel(const MeshParams p) {
   const int f = blockIdx.y;
   unsigned long long r = p.tile_offset[2 * p.T + f * p.tpv + blockIdx.x] - p.tile_offset[2 * p.T];
-  for (int it = 0; it < MESH_ITERS; ++it) {
-    const long long q = static_cast<long long>(blockIdx.x) * MESH_TILE + it * MESH_THREADS + threadIdx.x;
+  for (int it = 0; it < COMPACT_ITERS; ++it) {
+    const long long q = static_cast<long long>(blockIdx.x) * COMPACT_TILE + it * COMPACT_THREADS + threadIdx.x;
     const int y = static_cast<int>(q / p.W), x = static_cast<int>(q - static_cast<long long>(y) * p.W);
     const long long i = f * p.hw + q;
     const bool flag[1] = {q < p.hw && mesh_used(p, i, y, x)};
     unsigned int rank[1], sum[1];
-    mesh_chunk_ranks<1>(flag, pre, rank, sum);
+    chunk_ranks<1>(flag, rank, sum);
     if (flag[0]) {
       const unsigned long long u = r + rank[0];
       p.remap[i] = static_cast<int>(u);
@@ -246,21 +202,20 @@ __global__ void __launch_bounds__(MESH_THREADS) mesh_vertices_kernel(const MeshP
 }
 
 // GLB layout, part 2: the forward triangles (classes 1 and 3 of the reference layout, same order) through the remap.
-__global__ void __launch_bounds__(MESH_THREADS) mesh_indices_kernel(const MeshParams p) {
-  __shared__ unsigned int pre[2][MESH_THREADS / 32 + 1];
+__global__ void __launch_bounds__(COMPACT_THREADS) mesh_indices_kernel(const MeshParams p) {
   const int f = blockIdx.y;
   const MeshView v = mesh_view(p, f);
   const unsigned long long base = v.tl0 + v.br0;
   unsigned long long r_tl = p.tile_offset[f * p.tpv + blockIdx.x] - p.tile_offset[f * p.tpv];
   unsigned long long r_br = p.tile_offset[p.T + f * p.tpv + blockIdx.x] - p.tile_offset[p.T + f * p.tpv];
-  for (int it = 0; it < MESH_ITERS; ++it) {
-    const long long q = static_cast<long long>(blockIdx.x) * MESH_TILE + it * MESH_THREADS + threadIdx.x;
+  for (int it = 0; it < COMPACT_ITERS; ++it) {
+    const long long q = static_cast<long long>(blockIdx.x) * COMPACT_TILE + it * COMPACT_THREADS + threadIdx.x;
     const int y = static_cast<int>(q / p.W), x = static_cast<int>(q - static_cast<long long>(y) * p.W);
     const long long i = f * p.hw + q;
     const bool in = q < p.hw;
     const bool flag[2] = {in && mesh_tl(p, i, y, x), in && mesh_br(p, i, y, x)};
     unsigned int rank[2], sum[2];
-    mesh_chunk_ranks<2>(flag, pre, rank, sum);
+    chunk_ranks<2>(flag, rank, sum);
     if (flag[0] || flag[1]) {
       const int tr = p.remap[i + 1], bl = p.remap[i + p.W];
       if (flag[0]) {

@@ -690,6 +690,27 @@ int radix_percentile(const float* v, long long n, float percent, void* workspace
   return OVG_OK;
 }
 
+struct Arena {
+  char* base;
+  long long cap, off = 0;
+  bool dry;        // size query: no pointers are formed
+  Arena(void* b, long long c) : base(static_cast<char*>(b)), cap(c), dry(b == nullptr) {}
+  void* take(long long bytes) {
+    const long long at = (off + 255) & ~255LL;
+    off = at + bytes;
+    return dry ? nullptr : base + at;
+  }
+  template <typename T>
+  T* get(long long n) { return static_cast<T*>(take(n * static_cast<long long>(sizeof(T)))); }
+  bool ok() const { return dry || off <= cap; }
+  long long bytes() const { return (off + 255) & ~255LL; }   // the layout's size in whole 256-byte blocks
+};
+
+// A caller's workspace for a layout of `need` bytes: non-null, `align`-byte aligned and at least `need` bytes long.
+bool workspace_ok(const void* workspace, long long workspace_bytes, long long need, uintptr_t align) {
+  return workspace && (reinterpret_cast<uintptr_t>(workspace) & (align - 1)) == 0 && workspace_bytes >= need;
+}
+
 // Point-cloud workspace, carved the same way by the size query and by every entry point.
 struct CloudWorkspace {
   void* select;                      // OVG_PERCENTILE_WORKSPACE_BYTES
@@ -701,21 +722,14 @@ struct CloudWorkspace {
 };
 
 CloudWorkspace cloud_workspace(void* base, long long n) {
-  const long long tiles = (n + ovg::CLOUD_TILE - 1) / ovg::CLOUD_TILE;
-  char* p = static_cast<char*>(base);
-  long long off = 0;
-  auto carve = [&](long long bytes) {
-    char* r = p ? p + off : nullptr;
-    off += (bytes + 255) / 256 * 256;
-    return r;
-  };
+  Arena ar(base, 0);
   CloudWorkspace w;
-  w.select = carve(OVG_PERCENTILE_WORKSPACE_BYTES);
-  w.sel = reinterpret_cast<float*>(carve(18 * sizeof(float)));
-  w.center_partial = reinterpret_cast<double*>(carve(3LL * ovg::CLOUD_CENTER_BLOCKS * sizeof(double)));
-  w.tile_count = reinterpret_cast<unsigned int*>(carve(tiles * 4));
-  w.tile_offset = reinterpret_cast<unsigned long long*>(carve(tiles * 8));
-  w.bytes = off;
+  w.select = ar.take(OVG_PERCENTILE_WORKSPACE_BYTES);
+  w.sel = ar.get<float>(18);
+  w.center_partial = ar.get<double>(3LL * ovg::CLOUD_CENTER_BLOCKS);
+  w.tile_count = ar.get<unsigned int>(ovg::compact_tiles(n));
+  w.tile_offset = ar.get<unsigned long long>(ovg::compact_tiles(n));
+  w.bytes = ar.bytes();
   return w;
 }
 
@@ -753,14 +767,14 @@ int cloud_params(const unsigned char* conf_mask, const float* images, int F, int
   OVG_REQUIRE(conf_mask && images && workspace && F > 0 && H > 0 && W > 0, "bad arguments");
   const long long n = static_cast<long long>(F) * H * W;
   const CloudWorkspace w = cloud_workspace(workspace, n);
-  OVG_REQUIRE((reinterpret_cast<uintptr_t>(workspace) & 15) == 0 && workspace_bytes >= w.bytes,
+  OVG_REQUIRE(workspace_ok(workspace, workspace_bytes, w.bytes, 16),
               "workspace must be 16-byte aligned and ovg_point_cloud_workspace_bytes(F*H*W) long");
-  OVG_REQUIRE((n + ovg::CLOUD_TILE - 1) / ovg::CLOUD_TILE < (1LL << 31), "too many pixels");
+  OVG_REQUIRE(ovg::compact_tiles(n) < (1LL << 31), "too many pixels");
   *p = ovg::CloudParams{};
   p->conf_mask = conf_mask; p->images = images; p->n = n; p->hw = static_cast<long long>(H) * W;
   p->black_bg = mask_black_bg ? 1 : 0; p->white_bg = mask_white_bg ? 1 : 0;
   p->tile_count = w.tile_count; p->tile_offset = w.tile_offset;
-  p->tiles = static_cast<int>((n + ovg::CLOUD_TILE - 1) / ovg::CLOUD_TILE);
+  p->tiles = static_cast<int>(ovg::compact_tiles(n));
   return OVG_OK;
 }
 
@@ -775,12 +789,11 @@ int ovg_point_cloud_count(const unsigned char* conf_mask, const float* images, i
   ovg::CloudParams p;
   int rc = cloud_params(conf_mask, images, F, H, W, mask_black_bg, mask_white_bg, workspace, workspace_bytes, &p);
   if (rc) return rc;
-  p.total = count_out;
   cudaStream_t st = reinterpret_cast<cudaStream_t>(stream);
-  ovg::cloud_count_kernel<<<p.tiles, ovg::CLOUD_THREADS, 0, st>>>(p);
+  ovg::cloud_count_kernel<<<p.tiles, ovg::COMPACT_THREADS, 0, st>>>(p);
   rc = post_launch("ovg_point_cloud_count");
   if (rc) return rc;
-  ovg::cloud_scan_kernel<<<1, 1024, 0, st>>>(p);
+  ovg::tile_scan_kernel<<<1, 1024, 0, st>>>(p.tile_count, p.tile_offset, count_out, p.tiles);
   return post_launch("ovg_point_cloud_count(scan)");
 }
 
@@ -797,7 +810,7 @@ int ovg_point_cloud_gather(const float* points, const unsigned char* conf_mask, 
               "xyz must be 16-byte aligned with a column stride ld % 4 == 0");
   p.points = points; p.frame0 = frame0;
   p.points_out = points_out; p.colors_out = colors_out; p.frame_out = frame_out; p.xyz = xyz; p.ld = ld;
-  ovg::cloud_gather_kernel<<<p.tiles, ovg::CLOUD_THREADS, 0, reinterpret_cast<cudaStream_t>(stream)>>>(p);
+  ovg::cloud_gather_kernel<<<p.tiles, ovg::COMPACT_THREADS, 0, reinterpret_cast<cudaStream_t>(stream)>>>(p);
   return post_launch("ovg_point_cloud_gather");
 }
 
@@ -805,7 +818,7 @@ int ovg_point_cloud_center(const float* points, long long n, void* workspace, lo
                            void* stream) {
   OVG_REQUIRE(points && workspace && center_out && n > 0, "bad arguments");
   const CloudWorkspace w = cloud_workspace(workspace, n);
-  OVG_REQUIRE((reinterpret_cast<uintptr_t>(workspace) & 15) == 0 && workspace_bytes >= w.bytes,
+  OVG_REQUIRE(workspace_ok(workspace, workspace_bytes, w.bytes, 16),
               "workspace must be 16-byte aligned and ovg_point_cloud_workspace_bytes(n) long");
   cudaStream_t st = reinterpret_cast<cudaStream_t>(stream);
   ovg::CloudCenterParams p{points, n, w.center_partial, center_out};
@@ -821,7 +834,7 @@ int ovg_point_cloud_scale(const float* xyz, long long n_kept, long long ld, void
   OVG_REQUIRE(xyz && workspace && scale_out && n_kept > 0 && ld >= n_kept && ld % 4 == 0, "bad arguments");
   OVG_REQUIRE((reinterpret_cast<uintptr_t>(xyz) & 15) == 0, "xyz must be 16-byte aligned");
   const CloudWorkspace w = cloud_workspace(workspace, 1);   // the scale uses only the fixed-size head of the workspace
-  OVG_REQUIRE((reinterpret_cast<uintptr_t>(workspace) & 15) == 0 && workspace_bytes >= w.bytes,
+  OVG_REQUIRE(workspace_ok(workspace, workspace_bytes, w.bytes, 16),
               "workspace must be 16-byte aligned and ovg_point_cloud_workspace_bytes() long");
   cudaStream_t st = reinterpret_cast<cudaStream_t>(stream);
   for (int q = 0; q < 2; ++q)
@@ -847,44 +860,38 @@ struct MatchWorkspace {
 };
 
 MatchWorkspace match_workspace(void* base, int V, long long cap, int P) {
-  char* b = static_cast<char*>(base);
-  long long off = 0;
-  auto carve = [&](long long bytes) {
-    char* r = b ? b + off : nullptr;
-    off += (bytes + 255) / 256 * 256;
-    return r;
-  };
+  Arena ar(base, 0);
   MatchWorkspace w;
   ovg::MatchParams& p = w.p;
   p = ovg::MatchParams{};
   p.V = V; p.cap = cap; p.P = P;
-  p.tiles = static_cast<int>(ovg::match_tiles(cap));
+  p.tiles = static_cast<int>(ovg::compact_tiles(cap));
   p.ptiles = p.tiles;
   p.cells_cap = ovg::match_cells_cap(cap);
-  p.flag = reinterpret_cast<unsigned int*>(carve(4));
-  p.hist = reinterpret_cast<unsigned int*>(carve(4LL * V * 3 * ovg::MATCH_BINS));
-  p.grid = reinterpret_cast<ovg::MatchGrid*>(carve(static_cast<long long>(sizeof(ovg::MatchGrid)) * V));
-  p.range0 = reinterpret_cast<float*>(carve(4LL * V * 6));
-  p.view_tile_count = reinterpret_cast<unsigned int*>(carve(4LL * V * p.tiles));
-  p.view_tile_offset = reinterpret_cast<unsigned int*>(carve(4LL * V * p.tiles));
-  p.pts = reinterpret_cast<float4*>(carve(16LL * V * cap));
+  p.flag = ar.get<unsigned int>(1);
+  p.hist = ar.get<unsigned int>(3LL * V * ovg::MATCH_BINS);
+  p.grid = ar.get<ovg::MatchGrid>(V);
+  p.range0 = ar.get<float>(6LL * V);
+  p.view_tile_count = ar.get<unsigned int>(static_cast<long long>(V) * p.tiles);
+  p.view_tile_offset = ar.get<unsigned int>(static_cast<long long>(V) * p.tiles);
+  p.pts = ar.get<float4>(V * cap);
   p.rtiles = static_cast<int>((cap + ovg::MATCH_RADIX_TILE - 1) / ovg::MATCH_RADIX_TILE);
   for (int b = 0; b < 2; ++b) {
-    p.keys[b] = reinterpret_cast<int*>(carve(4LL * V * cap));
-    p.vals[b] = reinterpret_cast<float4*>(carve(16LL * V * cap));
+    p.keys[b] = ar.get<int>(V * cap);
+    p.vals[b] = ar.get<float4>(V * cap);
   }
-  p.radix_off = reinterpret_cast<unsigned int*>(carve(4LL * V * 256 * p.rtiles));
+  p.radix_off = ar.get<unsigned int>(256LL * V * p.rtiles);
   int bits = 0;
   while ((1LL << bits) < p.cells_cap) ++bits;
   w.passes = (bits + 7) / 8;
   p.sorted = p.vals[w.passes & 1];
-  p.cell_count = reinterpret_cast<int*>(carve(4LL * V * p.cells_cap));
-  p.cell_start = reinterpret_cast<int*>(carve(4LL * V * (p.cells_cap + 1)));
-  p.nn = reinterpret_cast<int*>(carve(4LL * 2 * P * cap));
-  p.pair_tile_count = reinterpret_cast<unsigned int*>(carve(4LL * P * p.ptiles));
-  p.pair_tile_offset = reinterpret_cast<unsigned long long*>(carve(8LL * P * p.ptiles));
-  p.total = reinterpret_cast<unsigned long long*>(carve(8));
-  w.bytes = off;
+  p.cell_count = ar.get<int>(V * p.cells_cap);
+  p.cell_start = ar.get<int>(V * (p.cells_cap + 1));
+  p.nn = ar.get<int>(2LL * P * cap);
+  p.pair_tile_count = ar.get<unsigned int>(static_cast<long long>(P) * p.ptiles);
+  p.pair_tile_offset = ar.get<unsigned long long>(static_cast<long long>(P) * p.ptiles);
+  p.total = ar.get<unsigned long long>(1);
+  w.bytes = ar.bytes();
   return w;
 }
 
@@ -894,7 +901,7 @@ int match_check(int V, long long cap, int P, const void* workspace, long long wo
   OVG_REQUIRE(V > 0 && V <= 65535 && cap > 0 && cap < (1LL << 30) && P > 0 && 2LL * P <= 65535, "bad sizes");
   OVG_REQUIRE(static_cast<long long>(V) * cap < (1LL << 40), "too many points");
   const MatchWorkspace w = match_workspace(const_cast<void*>(workspace), V, cap, P);
-  OVG_REQUIRE(workspace && (reinterpret_cast<uintptr_t>(workspace) & 255) == 0 && workspace_bytes >= w.bytes,
+  OVG_REQUIRE(workspace_ok(workspace, workspace_bytes, w.bytes, 256),
               "workspace must be 256-byte aligned and ovg_match_workspace_bytes(V, cap, P) long");
   *p = w.p;
   if (passes) *passes = w.passes;
@@ -928,11 +935,11 @@ int ovg_match_index(const float* points, const unsigned char* keep, int V, long 
   OVG_CUDA(cudaMemsetAsync(p.flag, 0, 4, st));
   OVG_CUDA(cudaMemsetAsync(p.hist, 0, 4LL * V * 3 * ovg::MATCH_BINS, st));
   OVG_CUDA(cudaMemsetAsync(p.cell_count, 0, 4LL * V * p.cells_cap, st));
-  ovg::match_keep_count_kernel<<<dim3(p.tiles, V), ovg::MATCH_THREADS, 0, st>>>(p);
+  ovg::match_keep_count_kernel<<<dim3(p.tiles, V), ovg::COMPACT_THREADS, 0, st>>>(p);
   if ((rc = post_launch("ovg_match_index(keep count)"))) return rc;
-  ovg::match_keep_scan_kernel<<<V, 32, 0, st>>>(p);
+  ovg::match_keep_scan_kernel<<<V, 1024, 0, st>>>(p);
   if ((rc = post_launch("ovg_match_index(keep scan)"))) return rc;
-  ovg::match_keep_gather_kernel<<<dim3(p.tiles, V), ovg::MATCH_THREADS, 0, st>>>(p);
+  ovg::match_keep_gather_kernel<<<dim3(p.tiles, V), ovg::COMPACT_THREADS, 0, st>>>(p);
   if ((rc = post_launch("ovg_match_index(keep gather)"))) return rc;
   const dim3 grid(match_blocks(cap), V);
   for (int pass = 0; pass < 2; ++pass) {
@@ -970,14 +977,10 @@ int ovg_match_query(const int* pairs, int P, int V, long long cap, void* workspa
   ovg::match_query_kernel<<<dim3(static_cast<unsigned>((cap + ovg::MATCH_QUERY_THREADS - 1) / ovg::MATCH_QUERY_THREADS), 2 * P),
                             ovg::MATCH_QUERY_THREADS, 0, st>>>(p);
   if ((rc = post_launch("ovg_match_query"))) return rc;
-  ovg::match_recip_count_kernel<<<dim3(p.ptiles, P), ovg::MATCH_THREADS, 0, st>>>(p);
+  ovg::match_recip_count_kernel<<<dim3(p.ptiles, P), ovg::COMPACT_THREADS, 0, st>>>(p);
   if ((rc = post_launch("ovg_match_query(reciprocal count)"))) return rc;
-  ovg::CloudParams sp{};
-  sp.tile_count = p.pair_tile_count;
-  sp.tile_offset = p.pair_tile_offset;
-  sp.total = p.total;
-  sp.tiles = P * p.ptiles;
-  ovg::cloud_scan_kernel<<<1, 1024, 0, st>>>(sp);
+  ovg::tile_scan_kernel<<<1, 1024, 0, st>>>(p.pair_tile_count, p.pair_tile_offset, p.total,
+                                            static_cast<long long>(P) * p.ptiles);
   if ((rc = post_launch("ovg_match_query(scan)"))) return rc;
   ovg::match_counts_kernel<<<(P + 1 + 255) / 256, 256, 0, st>>>(p);
   return post_launch("ovg_match_query(counts)");
@@ -991,7 +994,7 @@ int ovg_match_gather(const int* pairs, int P, int V, long long cap, int W, const
   OVG_REQUIRE(pairs && xy_i && xy_j && W > 0, "bad arguments");
   p.pairs = pairs;
   ovg::MatchOut o{W, xy_i, xy_j, -1, nullptr, nullptr};
-  ovg::match_gather_kernel<<<dim3(p.ptiles, P), ovg::MATCH_THREADS, 0, reinterpret_cast<cudaStream_t>(stream)>>>(p, o);
+  ovg::match_gather_kernel<<<dim3(p.ptiles, P), ovg::COMPACT_THREADS, 0, reinterpret_cast<cudaStream_t>(stream)>>>(p, o);
   return post_launch("ovg_match_gather");
 }
 
@@ -1014,24 +1017,18 @@ namespace {
 
 // Mesh workspace, carved the same way by the size query and by every entry point.
 ovg::MeshParams mesh_workspace(void* base, int F, int H, int W, long long* bytes) {
-  char* b = static_cast<char*>(base);
-  long long off = 0;
-  auto carve = [&](long long n) {
-    char* r = b ? b + off : nullptr;
-    off += (n + 255) / 256 * 256;
-    return r;
-  };
+  Arena ar(base, 0);
   ovg::MeshParams p{};
   p.H = H; p.W = W;
   p.hw = static_cast<long long>(H) * W;
   p.n = F * p.hw;
-  p.tpv = static_cast<int>((p.hw + ovg::MESH_TILE - 1) / ovg::MESH_TILE);
+  p.tpv = static_cast<int>(ovg::compact_tiles(p.hw));
   p.T = F * p.tpv;
-  p.keep = reinterpret_cast<unsigned char*>(carve(p.n));
-  p.remap = reinterpret_cast<int*>(carve(4 * p.n));
-  p.tile_count = reinterpret_cast<unsigned int*>(carve(4LL * ovg::MESH_STREAMS * p.T));
-  p.tile_offset = reinterpret_cast<unsigned long long*>(carve(8LL * (ovg::MESH_STREAMS * p.T + 1)));
-  *bytes = off;
+  p.keep = ar.get<unsigned char>(p.n);
+  p.remap = ar.get<int>(p.n);
+  p.tile_count = ar.get<unsigned int>(static_cast<long long>(ovg::MESH_STREAMS) * p.T);
+  p.tile_offset = ar.get<unsigned long long>(static_cast<long long>(ovg::MESH_STREAMS) * p.T + 1);
+  *bytes = ar.bytes();
   return p;
 }
 
@@ -1040,7 +1037,7 @@ int mesh_check(int F, int H, int W, const void* workspace, long long workspace_b
   OVG_REQUIRE(static_cast<long long>(F) * H * W < (1LL << 31), "F*H*W must be below 2^31");
   long long bytes = 0;
   *p = mesh_workspace(const_cast<void*>(workspace), F, H, W, &bytes);
-  OVG_REQUIRE(workspace && (reinterpret_cast<uintptr_t>(workspace) & 255) == 0 && workspace_bytes >= bytes,
+  OVG_REQUIRE(workspace_ok(workspace, workspace_bytes, bytes, 256),
               "workspace must be 256-byte aligned and ovg_mesh_workspace_bytes(F, H, W) long");
   return OVG_OK;
 }
@@ -1069,14 +1066,10 @@ int ovg_mesh_count(const unsigned char* conf_mask, const float* images, int F, i
   cudaStream_t st = reinterpret_cast<cudaStream_t>(stream);
   ovg::mesh_keep_kernel<<<static_cast<unsigned>((p.n + 255) / 256), 256, 0, st>>>(p);
   if ((rc = post_launch("ovg_mesh_count(keep)"))) return rc;
-  ovg::mesh_count_kernel<<<dim3(p.tpv, F), ovg::MESH_THREADS, 0, st>>>(p);
+  ovg::mesh_count_kernel<<<dim3(p.tpv, F), ovg::COMPACT_THREADS, 0, st>>>(p);
   if ((rc = post_launch("ovg_mesh_count"))) return rc;
-  ovg::CloudParams sp{};
-  sp.tile_count = p.tile_count;
-  sp.tile_offset = p.tile_offset;
-  sp.total = p.tile_offset + ovg::MESH_STREAMS * p.T;
-  sp.tiles = ovg::MESH_STREAMS * p.T;
-  ovg::cloud_scan_kernel<<<1, 1024, 0, st>>>(sp);
+  const long long tiles = static_cast<long long>(ovg::MESH_STREAMS) * p.T;
+  ovg::tile_scan_kernel<<<1, 1024, 0, st>>>(p.tile_count, p.tile_offset, p.tile_offset + tiles, tiles);
   if ((rc = post_launch("ovg_mesh_count(scan)"))) return rc;
   ovg::mesh_totals_kernel<<<1, 32, 0, st>>>(p);
   return post_launch("ovg_mesh_count(totals)");
@@ -1092,7 +1085,7 @@ int ovg_mesh_faces(const float* images, const void* colors, int color_bytes, int
               "face colours need images, or colors with color_bytes 1, 2, 4 or 8");
   p.images = images; p.colors = colors; p.color_bytes = color_bytes;
   p.faces = faces; p.face_colors = face_colors;
-  ovg::mesh_faces_kernel<<<dim3(p.tpv, F), ovg::MESH_THREADS, 0, reinterpret_cast<cudaStream_t>(stream)>>>(p);
+  ovg::mesh_faces_kernel<<<dim3(p.tpv, F), ovg::COMPACT_THREADS, 0, reinterpret_cast<cudaStream_t>(stream)>>>(p);
   return post_launch("ovg_mesh_faces");
 }
 
@@ -1105,9 +1098,9 @@ int ovg_mesh_compact(const float* points, const float* images, int F, int H, int
   p.points = points; p.images = images;
   p.positions = positions; p.vertex_colors = colors; p.indices = indices;
   cudaStream_t st = reinterpret_cast<cudaStream_t>(stream);
-  ovg::mesh_vertices_kernel<<<dim3(p.tpv, F), ovg::MESH_THREADS, 0, st>>>(p);
+  ovg::mesh_vertices_kernel<<<dim3(p.tpv, F), ovg::COMPACT_THREADS, 0, st>>>(p);
   if ((rc = post_launch("ovg_mesh_compact(vertices)"))) return rc;
-  ovg::mesh_indices_kernel<<<dim3(p.tpv, F), ovg::MESH_THREADS, 0, st>>>(p);
+  ovg::mesh_indices_kernel<<<dim3(p.tpv, F), ovg::COMPACT_THREADS, 0, st>>>(p);
   return post_launch("ovg_mesh_compact(indices)");
 }
 
@@ -1118,22 +1111,16 @@ namespace {
 
 // Sky workspace, carved the same way by the size query and by the entry point.
 ovg::SkyParams sky_workspace(void* base, int F, int H, int W, long long* bytes) {
-  char* b = static_cast<char*>(base);
-  long long off = 0;
-  auto carve = [&](long long n) {
-    char* r = b ? b + off : nullptr;
-    off += (n + 255) / 256 * 256;
-    return r;
-  };
+  Arena ar(base, 0);
   ovg::SkyParams p{};
   p.F = F; p.H = H; p.W = W;
   p.hw = static_cast<long long>(H) * W;
   p.n = F * p.hw;
   p.tiles_x = (W + ovg::SKY_TILE - 1) / ovg::SKY_TILE;
-  p.label = reinterpret_cast<int*>(carve(4 * p.n));
-  p.area = reinterpret_cast<int*>(carve(4 * p.n));
-  p.view_max = reinterpret_cast<int*>(carve(4LL * F));
-  *bytes = off;
+  p.label = ar.get<int>(p.n);
+  p.area = ar.get<int>(p.n);
+  p.view_max = ar.get<int>(F);
+  *bytes = ar.bytes();
   return p;
 }
 
@@ -1156,7 +1143,7 @@ int ovg_segment_sky(const void* image, int image_u8, long long view_stride, long
   OVG_REQUIRE(image && sky_out && (conf == nullptr) == (conf_out == nullptr), "null image / sky_out, or conf without conf_out");
   long long bytes = 0;
   ovg::SkyParams p = sky_workspace(workspace, F, H, W, &bytes);
-  OVG_REQUIRE(workspace && (reinterpret_cast<uintptr_t>(workspace) & 255) == 0 && workspace_bytes >= bytes,
+  OVG_REQUIRE(workspace_ok(workspace, workspace_bytes, bytes, 256),
               "workspace must be 256-byte aligned and ovg_sky_workspace_bytes(F, H, W) long");
   p.image = image; p.u8 = image_u8 ? 1 : 0;
   p.view_stride = view_stride; p.pixel_stride = pixel_stride; p.channel_stride = channel_stride;

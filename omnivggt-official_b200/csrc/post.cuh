@@ -9,6 +9,7 @@
 // All HBM-bound: one coalesced pass per kernel, 16-byte accesses where the layout allows; the percentile is an exact
 // order statistic by 4 x 8-bit radix-select passes over the fp32 bit patterns (integer histograms: deterministic).
 #pragma once
+#include "compact.cuh"
 #include "ptx.cuh"
 
 namespace ovg {
@@ -271,13 +272,8 @@ __global__ void __launch_bounds__(256) conf_mask_kernel(const ConfMaskParams p) 
 
 // ---------------------------------------------------------------------------------------------------
 // Point cloud (visual_util.py:190-236 predictions_to_glb, inference.py:96-151 viewer): filter, compact, centre, scale.
-// Pixels are numbered i = (f * H + y) * W + x, the order of numpy boolean indexing.  Block b of the count / gather kernels
-// owns the tile [b * CLOUD_TILE, (b + 1) * CLOUD_TILE), walked in CLOUD_ITERS chunks of 256 consecutive pixels; the count
-// kernel stores the tile's kept count, a one-block scan turns the counts into tile offsets, and the gather kernel places
-// each kept pixel at its tile offset + its rank inside the tile (ballot / popc within a warp, a scan over the 8 warps).
-constexpr int CLOUD_THREADS = 256;
-constexpr int CLOUD_ITERS = 16;
-constexpr int CLOUD_TILE = CLOUD_THREADS * CLOUD_ITERS;
+// Pixels are numbered i = (f * H + y) * W + x, the order of numpy boolean indexing, and compacted as compact.cuh describes:
+// cloud_count_kernel, tile_scan_kernel, cloud_gather_kernel.
 constexpr int CLOUD_CENTER_BLOCKS = 256;   // fixed, so the fp64 summation order does not depend on the device
 
 struct CloudParams {
@@ -289,8 +285,7 @@ struct CloudParams {
   int black_bg, white_bg, frame0;
   unsigned int* tile_count;         // [tiles]
   unsigned long long* tile_offset;  // [tiles] exclusive prefix of tile_count
-  unsigned long long* total;        // kept points
-  int tiles;
+  int tiles;                        // compact_tiles(n)
   float* points_out;                // [n_kept, 3]
   unsigned char* colors_out;        // [n_kept, 3]
   int* frame_out;                   // [n_kept]
@@ -325,74 +320,32 @@ __device__ __forceinline__ bool cloud_keep(const CloudParams& p, long long i, in
   return pixel_keep(p.conf_mask, p.images, p.hw, p.black_bg, p.white_bg, i, f, rgb);
 }
 
-__global__ void __launch_bounds__(CLOUD_THREADS) cloud_count_kernel(const CloudParams p) {
-  __shared__ unsigned int warp_sum[CLOUD_THREADS / 32];
-  const long long base = static_cast<long long>(blockIdx.x) * CLOUD_TILE;
-  unsigned int kept = 0;
+__global__ void __launch_bounds__(COMPACT_THREADS) cloud_count_kernel(const CloudParams p) {
+  const long long base = static_cast<long long>(blockIdx.x) * COMPACT_TILE;
+  unsigned int kept[1] = {0u};
 #pragma unroll 4
-  for (int it = 0; it < CLOUD_ITERS; ++it) {
-    const long long i = base + it * CLOUD_THREADS + threadIdx.x;
+  for (int it = 0; it < COMPACT_ITERS; ++it) {
+    const long long i = base + it * COMPACT_THREADS + threadIdx.x;
     int f;
     uchar3 rgb;
-    if (i < p.n && cloud_keep(p, i, f, rgb)) ++kept;
+    if (i < p.n && cloud_keep(p, i, f, rgb)) ++kept[0];
   }
-#pragma unroll
-  for (int o = 16; o > 0; o >>= 1) kept += __shfl_xor_sync(0xffffffffu, kept, o);
-  if ((threadIdx.x & 31) == 0) warp_sum[threadIdx.x >> 5] = kept;
-  __syncthreads();
-  if (threadIdx.x == 0) {
-    unsigned int s = 0;
-#pragma unroll
-    for (int w = 0; w < CLOUD_THREADS / 32; ++w) s += warp_sum[w];
-    p.tile_count[blockIdx.x] = s;
-  }
+  const unsigned int s = tile_sum<1>(kept);
+  if (threadIdx.x == 0) p.tile_count[blockIdx.x] = s;
 }
 
-// One block of 1024 threads: thread t sums a contiguous run of tile counts, the 1024 run sums are scanned in shared memory.
-__global__ void __launch_bounds__(1024) cloud_scan_kernel(const CloudParams p) {
-  __shared__ unsigned long long run[1024];
-  const int per = (p.tiles + 1023) / 1024;
-  const int b0 = threadIdx.x * per;
-  const int b1 = min(b0 + per, p.tiles);
-  unsigned long long s = 0;
-  for (int b = b0; b < b1; ++b) s += p.tile_count[b];
-  run[threadIdx.x] = s;
-  __syncthreads();
-  for (int o = 1; o < 1024; o <<= 1) {          // Hillis-Steele inclusive scan
-    const unsigned long long v = threadIdx.x >= o ? run[threadIdx.x - o] : 0ull;
-    __syncthreads();
-    run[threadIdx.x] += v;
-    __syncthreads();
-  }
-  unsigned long long off = run[threadIdx.x] - s;
-  for (int b = b0; b < b1; ++b) {
-    p.tile_offset[b] = off;
-    off += p.tile_count[b];
-  }
-  if (threadIdx.x == 1023) *p.total = run[1023];
-}
-
-__global__ void __launch_bounds__(CLOUD_THREADS) cloud_gather_kernel(const CloudParams p) {
-  __shared__ unsigned int warp_pre[CLOUD_THREADS / 32 + 1];
-  const int lane = threadIdx.x & 31, warp = threadIdx.x >> 5;
-  const long long base = static_cast<long long>(blockIdx.x) * CLOUD_TILE;
+__global__ void __launch_bounds__(COMPACT_THREADS) cloud_gather_kernel(const CloudParams p) {
+  const long long base = static_cast<long long>(blockIdx.x) * COMPACT_TILE;
   unsigned long long out = p.tile_offset[blockIdx.x];
-  for (int it = 0; it < CLOUD_ITERS; ++it) {
-    const long long i = base + it * CLOUD_THREADS + threadIdx.x;
+  for (int it = 0; it < COMPACT_ITERS; ++it) {
+    const long long i = base + it * COMPACT_THREADS + threadIdx.x;
     int f = 0;
     uchar3 rgb = make_uchar3(0, 0, 0);
-    const bool keep = i < p.n && cloud_keep(p, i, f, rgb);
-    const unsigned int ballot = __ballot_sync(0xffffffffu, keep);
-    if (lane == 0) warp_pre[warp + 1] = __popc(ballot);
-    __syncthreads();
-    if (threadIdx.x == 0) {
-      warp_pre[0] = 0;
-#pragma unroll
-      for (int w = 1; w <= CLOUD_THREADS / 32; ++w) warp_pre[w] += warp_pre[w - 1];
-    }
-    __syncthreads();
-    if (keep) {
-      const unsigned long long k = out + warp_pre[warp] + __popc(ballot & ((1u << lane) - 1u));
+    const bool keep[1] = {i < p.n && cloud_keep(p, i, f, rgb)};
+    unsigned int rank[1], sum[1];
+    chunk_ranks<1>(keep, rank, sum);
+    if (keep[0]) {
+      const unsigned long long k = out + rank[0];
       const float x = p.points[3 * i], y = p.points[3 * i + 1], z = p.points[3 * i + 2];
       p.points_out[3 * k] = x;
       p.points_out[3 * k + 1] = y;
@@ -405,8 +358,7 @@ __global__ void __launch_bounds__(CLOUD_THREADS) cloud_gather_kernel(const Cloud
       p.xyz[p.ld + k] = y;
       p.xyz[2 * p.ld + k] = z;
     }
-    out += warp_pre[CLOUD_THREADS / 32];
-    __syncthreads();                               // warp_pre is rewritten by the next chunk
+    out += sum[0];
   }
 }
 

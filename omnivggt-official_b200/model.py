@@ -306,13 +306,39 @@ class OmniVGGT(nn.Module, PyTorchModelHubMixin):
         return predictions
 
     @staticmethod
-    def _check_source(source: str, conf_percent: float, conf_floor: float) -> None:
+    def _check_views(predictions: Dict[str, object], source: str, conf_percent: float, conf_floor: float,
+                     frame: Optional[int], scene: int, mask_sky) -> int:
+        """The argument checks of point_cloud, mesh and matches, before any library call; returns the scene's view count."""
         if source not in ("depth", "pointmap"):
             raise ValueError(f"source must be 'depth' or 'pointmap', got {source!r}")
         if not 0.0 <= conf_percent <= 100.0:
             raise ValueError("conf_percent must be in [0, 100]")
         if conf_floor < 0.0:
             raise ValueError("conf_floor must be >= 0")        # the reference's floors are 1e-5 and 0.1
+        OmniVGGT._check_mask_sky(mask_sky, predictions, scene)
+        images = predictions["images"]
+        S = (images[scene] if images.dim() == 5 else images).shape[0]
+        if frame is not None and not 0 <= frame < S:
+            raise IndexError(f"frame {frame} out of range for {S} views")
+        return S
+
+    @staticmethod
+    def _kept_views(predictions: Dict[str, object], source: str, conf_percent: float, conf_floor: float,
+                    frame: Optional[int], scene: int, mask_sky):
+        """The views point_cloud, mesh and matches work on and their keep mask, after _check_views: the scene's source, its
+        confidence times non-sky over all views, then the frame, then conf >= percentile(conf, conf_percent) and
+        conf > conf_floor.  Returns (images fp32 [F,3,H,W], extrinsic [S,3,4], points fp32 [F,H,W,3], mask uint8 [F,H,W],
+        threshold 0-d, first view f0), the images, points and mask contiguous."""
+        from . import ops
+        images, ext, points, conf = OmniVGGT._scene_source(predictions, source, scene)
+        conf = OmniVGGT._sky_conf(mask_sky, images, conf, scene)
+        f0 = 0 if frame is None else frame
+        if frame is not None:
+            images, points, conf = images[frame:frame + 1], points[frame:frame + 1], conf[frame:frame + 1]
+        mask, thr, _ = ops.conf_percentile_mask(conf.float().contiguous(), conf_percent, conf_floor)
+        if conf_percent == 0.0:
+            thr = torch.zeros((), device=images.device, dtype=torch.float32)   # same mask: conf > conf_floor >= 0 implies conf >= 0
+        return images.contiguous(), ext, points.float().contiguous(), mask, thr, f0
 
     @staticmethod
     def _scene_source(predictions: Dict[str, object], source: str, scene: int):
@@ -412,20 +438,13 @@ class OmniVGGT(nn.Module, PyTorchModelHubMixin):
         points that are not finite raise ValueError; a view with no kept point has no matches.  ``mask_sky``: as in
         ``point_cloud``."""
         from . import geometry, ops
-        OmniVGGT._check_source(source, conf_percent, conf_floor)
-        OmniVGGT._check_mask_sky(mask_sky, predictions, scene)
-        images = predictions["images"]
-        S = (images[scene] if images.dim() == 5 else images).shape[0]
+        S = OmniVGGT._check_views(predictions, source, conf_percent, conf_floor, None, scene, mask_sky)
         pair_arr = geometry.check_pairs(pairs, S)
         if len(pair_arr) == 0:
             return []
-        images, _, points, conf = OmniVGGT._scene_source(predictions, source, scene)
+        images, _, points, mask, _, _ = OmniVGGT._kept_views(predictions, source, conf_percent, conf_floor, None, scene, mask_sky)
         _, _, H, W = images.shape
-        dev = images.device
-        conf = OmniVGGT._sky_conf(mask_sky, images, conf, scene)
-        mask, _, _ = ops.conf_percentile_mask(conf.float().contiguous(), conf_percent, conf_floor)
-        mt = ops.Matcher(points.float().contiguous().view(S, H * W, 3), mask.view(S, H * W),
-                         torch.from_numpy(pair_arr).to(dev))
+        mt = ops.Matcher(points.view(S, H * W, 3), mask.view(S, H * W), torch.from_numpy(pair_arr).to(images.device))
         counts, nonfinite = mt.counts()
         if nonfinite:
             raise ValueError("kept points must be finite (cKDTree: data must be finite, check for nan or inf values)")
@@ -457,31 +476,17 @@ class OmniVGGT(nn.Module, PyTorchModelHubMixin):
         H x W is ``m == 0``).  The confidence of every view becomes conf * non-sky before the frame selection and the
         percentile, as the reference orders it; no host read is added."""
         from . import ops
-        OmniVGGT._check_source(source, conf_percent, conf_floor)
-        OmniVGGT._check_mask_sky(mask_sky, predictions, scene)
-        images, ext, points, conf = OmniVGGT._scene_source(predictions, source, scene)
-        conf = OmniVGGT._sky_conf(mask_sky, images, conf, scene)
-        S, _, H, W = images.shape
-        f0 = 0
-        if frame is not None:
-            if not 0 <= frame < S:
-                raise IndexError(f"frame {frame} out of range for {S} views")
-            f0 = frame
-            images, points, conf = images[frame:frame + 1], points[frame:frame + 1], conf[frame:frame + 1]
-        images = images.contiguous()
-        points = points.float().contiguous()
-        conf = conf.float().contiguous()
-        F = images.shape[0]
+        OmniVGGT._check_views(predictions, source, conf_percent, conf_floor, frame, scene, mask_sky)
+        images, ext, points, mask, thr, f0 = OmniVGGT._kept_views(predictions, source, conf_percent, conf_floor, frame, scene,
+                                                                  mask_sky)
+        F, _, H, W = images.shape
         dev = images.device
-
-        mask, thr, _ = ops.conf_percentile_mask(conf, conf_percent, conf_floor)
-        if conf_percent == 0.0:
-            thr = torch.zeros((), device=dev, dtype=torch.float32)   # same mask: conf > conf_floor >= 0 implies conf >= 0
         ws = ops.point_cloud_workspace(F * H * W, dev)
         cnt = ops.point_cloud_count(mask, images, ws, mask_black_bg, mask_white_bg)
         center = ops.point_cloud_center(points, ws)
-        n = int(cnt.item())
-        align = OmniVGGT._align(ext[f0].double().cpu()).to(dev)
+        host = ops.host_read(torch.cat([cnt.double().reshape(1), ext[f0].double().reshape(-1)]))   # count < 2^31: exact
+        n = int(host[0])
+        align = OmniVGGT._align(host[1:].view(3, 4)).to(dev)
         if n == 0:
             return {"points": torch.empty(0, 3, device=dev), "colors": torch.empty(0, 3, device=dev, dtype=torch.uint8),
                     "frame": torch.empty(0, device=dev, dtype=torch.int32), "conf_threshold": thr, "center": center,
@@ -521,34 +526,16 @@ class OmniVGGT(nn.Module, PyTorchModelHubMixin):
         Both add ``conf_threshold`` and ``align``, as ``point_cloud`` returns them.  The three totals and the first camera are
         read back together: the one host synchronisation.  ``mask_sky``: as in ``point_cloud``."""
         from . import ops
-        OmniVGGT._check_source(source, conf_percent, conf_floor)
+        OmniVGGT._check_views(predictions, source, conf_percent, conf_floor, frame, scene, mask_sky)
         if layout not in ("reference", "glb"):
             raise ValueError(f"layout must be 'reference' or 'glb', got {layout!r}")
-        images = predictions["images"]
-        S = (images[scene] if images.dim() == 5 else images).shape[0]
-        if frame is not None and not 0 <= frame < S:
-            raise IndexError(f"frame {frame} out of range for {S} views")
-        OmniVGGT._check_mask_sky(mask_sky, predictions, scene)
-        images, ext, points, conf = OmniVGGT._scene_source(predictions, source, scene)
-        conf = OmniVGGT._sky_conf(mask_sky, images, conf, scene)
-        _, _, H, W = images.shape
-        f0 = 0
-        if frame is not None:
-            f0 = frame
-            images, points, conf = images[frame:frame + 1], points[frame:frame + 1], conf[frame:frame + 1]
-        images = images.contiguous()
-        points = points.float().contiguous()
-        conf = conf.float().contiguous()
-        F = images.shape[0]
-        dev = images.device
-
-        mask, thr, _ = ops.conf_percentile_mask(conf, conf_percent, conf_floor)
-        if conf_percent == 0.0:
-            thr = torch.zeros((), device=dev, dtype=torch.float32)   # same mask: conf > conf_floor >= 0 implies conf >= 0
+        images, ext, points, mask, thr, f0 = OmniVGGT._kept_views(predictions, source, conf_percent, conf_floor, frame, scene,
+                                                                  mask_sky)
+        F, _, H, W = images.shape
         mesher = ops.Mesher(mask.view(-1), images, F, H, W, mask_black_bg, mask_white_bg)
         host = ops.host_read(torch.cat([mesher.totals.double(), ext[f0].double().reshape(-1)]))   # totals < 2^33: exact
         n_ref, n_used, n_fwd = (int(v) for v in host[:3].tolist())
-        align = OmniVGGT._align(host[3:].view(3, 4)).to(dev)
+        align = OmniVGGT._align(host[3:].view(3, 4)).to(images.device)
         if layout == "glb":
             pos, cols, idx = mesher.compact(points.view(-1, 3), n_used, n_fwd)
             return {"positions": pos, "colors": cols, "indices": idx, "conf_threshold": thr, "align": align}

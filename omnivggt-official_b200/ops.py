@@ -216,7 +216,7 @@ def point_cloud_count(conf_mask, images, ws, mask_black_bg: bool = False, mask_w
     assert conf_mask.is_contiguous() and images.is_contiguous() and images.dim() == 4 and images.shape[1] == 3
     F, _, H, W = images.shape
     assert conf_mask.numel() == F * H * W
-    cnt = torch.empty((), device=images.device, dtype=torch.int64)
+    cnt = torch.zeros((), device=images.device, dtype=torch.int64)
     L.check(L.lib().ovg_point_cloud_count(conf_mask.data_ptr(), images.data_ptr(), F, H, W, int(mask_black_bg), int(mask_white_bg),
                                           ws.data_ptr(), ws.numel(), cnt.data_ptr(), L.stream()))
     return cnt

@@ -133,6 +133,85 @@ def test_write_glb_empty_cloud_is_the_reference_placeholder(tmp_path):
     assert np.array_equal(p, [[1, 0, 0]]) and np.array_equal(c, [[255, 255, 255, 255]])
 
 
+@pytest.fixture()
+def dry(monkeypatch):
+    """The C library replaced by a recorder, on CPU tensors; host reads counted."""
+    from omnivggt_official_b200 import _lib, ops
+
+    class Rec:
+        def __init__(self):
+            self.calls, self.reads = [], 0
+
+        def __getattr__(self, name):
+            def fn(*a):
+                self.calls.append((name, a))
+                return 0
+            return fn
+
+    rec = Rec()
+
+    def read(t):
+        rec.calls.append(("host_read", ()))
+        rec.reads += 1
+        return t.cpu()
+
+    monkeypatch.setattr(_lib, "lib", lambda: rec)
+    monkeypatch.setattr(_lib, "stream", lambda: 0)
+    monkeypatch.setattr(ops, "_on_device", lambda t: True)
+    monkeypatch.setattr(ops, "host_read", read)
+    return rec
+
+
+def _scene(S, H, W, seed=3):
+    g = torch.Generator().manual_seed(seed)
+    ext = torch.eye(4)[:3].repeat(1, S, 1, 1)
+    ext[0, :, :, 3] = torch.arange(S, dtype=torch.float32)[:, None]          # a different camera per view
+    return {"images": torch.rand(1, S, 3, H, W, generator=g), "world_points_from_depth": torch.randn(1, S, H, W, 3, generator=g),
+            "depth_conf": 1.0 + torch.rand(1, S, H, W, generator=g), "extrinsic": ext}
+
+
+def test_dry_run_call_order_and_one_host_read(dry):
+    """conf mask -> count -> centre -> one host read of the kept count and the first camera; the same calls for 1 and 24
+    views.  The recorder's kept count is 0, so the cloud ends there."""
+    from omnivggt_official_b200 import OmniVGGT
+    seqs = []
+    for S in (1, 24):
+        dry.calls.clear()
+        out = OmniVGGT.point_cloud(_scene(S, 6, 8), mask_white_bg=True)
+        names = [n for n, _ in dry.calls]
+        assert names == ["ovg_conf_percentile_mask", "ovg_point_cloud_workspace_bytes", "ovg_point_cloud_count",
+                         "ovg_point_cloud_center", "host_read"]
+        assert dry.calls[2][1][2:7] == (S, 6, 8, 0, 1)
+        assert out["points"].shape == (0, 3) and torch.equal(out["align"], OmniVGGT._align(torch.eye(4)[:3].double()))
+        seqs.append(names)
+    assert seqs[0] == seqs[1] and dry.reads == 2
+    dry.calls.clear()
+    pred = _scene(5, 6, 8)
+    out = OmniVGGT.point_cloud(pred, frame=3)
+    assert dry.calls[2][1][2] == 1                                       # one view after the frame selection
+    assert torch.equal(out["align"], OmniVGGT._align(pred["extrinsic"][0, 3].double()))
+    assert dry.reads == 3
+
+
+def test_errors_before_any_device_work(dry):
+    from omnivggt_official_b200 import OmniVGGT
+    pred = _scene(4, 6, 8)
+    with pytest.raises(ValueError, match="source"):
+        OmniVGGT.point_cloud(pred, source="normals")
+    for pct in (-1.0, 100.5):
+        with pytest.raises(ValueError, match="conf_percent"):
+            OmniVGGT.point_cloud(pred, conf_percent=pct)
+    with pytest.raises(ValueError, match="conf_floor"):
+        OmniVGGT.point_cloud(pred, conf_floor=-1.0)
+    for f in (4, -1):
+        for mask_sky in (False, True):
+            with pytest.raises(IndexError):
+                OmniVGGT.point_cloud(pred, frame=f, mask_sky=mask_sky)
+    with pytest.raises(ValueError, match="mask_sky"):
+        OmniVGGT.point_cloud(pred, mask_sky=torch.zeros(4, 8, 6, dtype=torch.bool))
+    assert dry.calls == []
+
+
 # ------------------------------------------------------------------------------------------------------------------ GPU
 def _device_cloud(world, conf, images, extrinsic, **kw):
     from omnivggt_official_b200 import OmniVGGT
