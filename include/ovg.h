@@ -306,6 +306,21 @@ int ovg_segment_sky(const void* image, int image_u8, long long view_stride, long
 /* ovg_sky_mask_conf: conf_out[i] = conf[i] * (sky[i] ? 0.f : 1.f) over n elements, for a sky mask made elsewhere. */
 int ovg_sky_mask_conf(const float* conf, const unsigned char* sky, long long n, float* conf_out, void* stream);
 
+/* Farthest point sampling: po_utils/misc.py:114-148 (farthest_point_sample) for B batches of N points at once.  xyz fp32
+ * [B, N, 3] contiguous; inds_out int64 [B, npoint].  Per batch: distance = 1e10 for every point; step i records
+ * inds[i] = farthest (with include_ends, farthest = 0 at i = 0 and N-1 at i = 1; else start[b] at i = 0, device int64 [B]
+ * with start[b] in [0, N), an index outside reads point 0), then d = ((dx*dx + dy*dy) + dz*dz) in fp32, dx = x - x[farthest],
+ * each operation rounded (no contraction), distance = d where d < distance (a NaN d never updates), and farthest = the first
+ * index of the largest distance.  1 <= npoint <= N < 2^31 (the reference adds random noise when npoint > N).
+ * One kernel launch whatever npoint is, no host synchronisation; results are bit-identical from run to run.  N <=
+ * OVG_FPS_CTA_POINTS: one CTA per batch with every point in shared memory; above, a cooperative launch of the whole grid,
+ * split into one group of CTAs per batch, with up to OVG_FPS_CTA_POINTS points per CTA in shared memory and the rest read
+ * from global memory.  workspace: ovg_fps_workspace_bytes(B, N) bytes, 256-byte aligned. */
+#define OVG_FPS_CTA_POINTS 14336
+long long ovg_fps_workspace_bytes(int B, long long N);
+int ovg_farthest_point_sample(const float* xyz, int B, long long N, int npoint, const long long* start, int include_ends,
+                              void* workspace, long long workspace_bytes, long long* inds_out, void* stream);
+
 /* Baseline JPEG decoding on the device, bit-identical to Pillow (libjpeg-turbo's default islow IDCT, fancy upsampling and
  * YCbCr -> RGB tables).  The plan is host code (no CUDA call): it parses every file, routes it to the device or to the host
  * (OVG_JPEG_* below: anything the device cannot decode exactly goes to the host), and builds the staging stream (tables plus the

@@ -17,6 +17,7 @@
 #include "match.cuh"
 #include "mesh.cuh"
 #include "sky.cuh"
+#include "fps.cuh"
 #include "tail.cuh"
 #include "pre.cuh"
 #include "jpeg.cuh"
@@ -1169,6 +1170,71 @@ int ovg_sky_mask_conf(const float* conf, const unsigned char* sky, long long n, 
   ovg::sky_mask_conf_kernel<<<static_cast<unsigned>((n + 255) / 256), 256, 0, reinterpret_cast<cudaStream_t>(stream)>>>(
       conf, sky, n, conf_out);
   return post_launch("ovg_sky_mask_conf");
+}
+
+}  // extern "C"
+
+// -------------------------------------------------------------------------------------------------- farthest point sampling
+namespace {
+
+// FPS workspace, carved the same way by the size query and by the entry point.
+ovg::FpsParams fps_workspace(void* base, int B, long long N, long long* bytes) {
+  Arena ar(base, 0);
+  ovg::FpsParams p{};
+  p.B = B; p.N = N;
+  p.arrive = ar.get<unsigned>(B);
+  p.slots = ar.get<ovg::FpsSlot>(2LL * ovg::FPS_MAX_CTAS);
+  p.dist = ar.get<float>(static_cast<long long>(B) * N);
+  *bytes = ar.bytes();
+  return p;
+}
+
+}  // namespace
+
+extern "C" {
+
+long long ovg_fps_workspace_bytes(int B, long long N) {
+  if (B <= 0 || N <= 0) return -1;
+  long long bytes = 0;
+  fps_workspace(nullptr, B, N, &bytes);
+  return bytes;
+}
+
+int ovg_farthest_point_sample(const float* xyz, int B, long long N, int npoint, const long long* start, int include_ends,
+                              void* workspace, long long workspace_bytes, long long* inds_out, void* stream) {
+  OVG_REQUIRE(B > 0 && N > 0 && npoint > 0, "bad sizes");
+  OVG_REQUIRE(N < (1LL << 31), "N must be below 2^31");
+  OVG_REQUIRE(npoint <= N, "npoint must be <= N");
+  OVG_REQUIRE(static_cast<long long>(B) * N < (1LL << 40), "too many points");
+  OVG_REQUIRE(xyz && inds_out && (start || include_ends), "null xyz / inds_out, or no start without include_ends");
+  long long bytes = 0;
+  ovg::FpsParams p = fps_workspace(workspace, B, N, &bytes);
+  OVG_REQUIRE(workspace_ok(workspace, workspace_bytes, bytes, 256),
+              "workspace must be 256-byte aligned and ovg_fps_workspace_bytes(B, N) long");
+  p.xyz = xyz; p.start = start; p.inds = inds_out; p.npoint = npoint; p.ends = include_ends ? 1 : 0;
+  cudaStream_t st = reinterpret_cast<cudaStream_t>(stream);
+  if (N <= ovg::FPS_CTA_POINTS) {   // one CTA per batch, every point in its shared memory
+    int rc = allow_dynamic_smem<ovg::fps_cta_kernel>(ovg::FPS_SMEM_BYTES);
+    if (rc) return rc;
+    ovg::fps_cta_kernel<<<B, ovg::FPS_THREADS, static_cast<int>(N) * 16, st>>>(p);
+    return post_launch("ovg_farthest_point_sample(cta)");
+  }
+  // The grid kernel spins on the other CTAs of its group: launched cooperatively, sized by the occupancy query, so the
+  // launch fails rather than run with CTAs that are not co-resident.
+  int rc = allow_dynamic_smem<ovg::fps_grid_kernel>(ovg::FPS_SMEM_BYTES);
+  if (rc) return rc;
+  int per_sm = 0;
+  OVG_CUDA(cudaOccupancyMaxActiveBlocksPerMultiprocessor(&per_sm, ovg::fps_grid_kernel, ovg::FPS_THREADS,
+                                                         ovg::FPS_SMEM_BYTES));
+  OVG_REQUIRE(per_sm > 0, "the grid kernel does not fit on an SM");
+  const int grid = std::min(per_sm * num_sms(), ovg::FPS_MAX_CTAS);
+  p.groups = std::min(B, grid);
+  p.G = grid / p.groups;
+  OVG_CUDA(cudaMemsetAsync(p.arrive, 0, sizeof(unsigned) * B, st));
+  void* args[] = {&p};
+  OVG_CUDA(cudaLaunchCooperativeKernel(reinterpret_cast<void*>(ovg::fps_grid_kernel), dim3(grid), dim3(ovg::FPS_THREADS), args,
+                                       ovg::FPS_SMEM_BYTES, st));
+  return post_launch("ovg_farthest_point_sample(grid)");
 }
 
 }  // extern "C"

@@ -1,7 +1,8 @@
 """Geometry of point maps on the device: dense correspondence (libovg ovg_match_*, the reference's
 omnivggt/utils/geometry.py:435-451 find_reciprocal_matches), triangle meshes (libovg ovg_mesh_*, the reference's
-omnivggt/viz.py:40-89 pts3d_to_trimesh and cat_meshes) and model-free sky segmentation (libovg ovg_segment_sky, the
-reference's omnivggt/viz.py:357-393 segment_sky)."""
+omnivggt/viz.py:40-89 pts3d_to_trimesh and cat_meshes), model-free sky segmentation (libovg ovg_segment_sky, the
+reference's omnivggt/viz.py:357-393 segment_sky) and farthest point sampling (libovg ovg_farthest_point_sample, the
+reference's omnivggt/utils/po_utils/misc.py:114-148 farthest_point_sample)."""
 from __future__ import annotations
 
 import numpy as np
@@ -122,6 +123,32 @@ def segment_sky(image):
     img = img.contiguous()
     sky, _ = ops.segment_sky(img, 1, H, W, H * W * 3, 3, 1)
     return sky.view(H, W).bool()
+
+
+def farthest_point_sample(xyz, npoint: int, include_ends: bool = False, deterministic: bool = False):
+    """Drop-in for po_utils/misc.py:114-148: npoint indices of each batch of xyz [B, N, 3] (a CUDA or CPU tensor, or an array,
+    moved to the current CUDA device and used as fp32), each the point farthest from the ones before it.  Returns int64
+    [B, npoint] on the device, in selection order.
+
+    The first index is 0 when deterministic, else torch.randint(0, N, (B,)) from torch's default CPU generator, drawn as the
+    reference draws it: the same torch.manual_seed gives the same indices.  With include_ends the first two are 0 and N-1.
+    Distances are fp32 ((dx*dx + dy*dy) + dz*dz) without contraction; a NaN distance never replaces a running one; ties go to
+    the lowest index.  Limits, each a ValueError before any device work: C != 3; N == 0; npoint < 1; npoint > N (where the
+    reference adds torch.randn_like noise at every step, which cannot be reproduced)."""
+    shape = tuple(xyz.shape) if hasattr(xyz, "shape") else np.shape(xyz)
+    if len(shape) != 3 or shape[2] != 3:
+        raise ValueError(f"xyz must have shape [B, N, 3], got {shape}")
+    B, N = shape[0], shape[1]
+    if N == 0:
+        raise ValueError("xyz has no points")
+    if int(npoint) < 1 or int(npoint) > N:
+        raise ValueError(f"npoint must be in [1, N = {N}], got {npoint}")
+    start = torch.randint(0, 1 if deterministic else N, (B,), dtype=torch.long)   # misc.py:127-130, same generator draw
+    dev = _device_of(xyz)
+    if B == 0:
+        return torch.zeros(0, int(npoint), device=dev, dtype=torch.int64)
+    pts = _to(xyz, dev).float().contiguous()
+    return ops.farthest_point_sample(pts, int(npoint), start.to(dev), include_ends)
 
 
 def cat_meshes(meshes):

@@ -455,7 +455,8 @@ class OmniVGGT(nn.Module, PyTorchModelHubMixin):
     @torch.no_grad()
     def point_cloud(predictions: Dict[str, object], *, source: str = "depth", conf_percent: float = 50.0,
                     conf_floor: float = 1e-5, frame: Optional[int] = None, mask_black_bg: bool = False,
-                    mask_white_bg: bool = False, scene: int = 0, mask_sky=False) -> Dict[str, torch.Tensor]:
+                    mask_white_bg: bool = False, scene: int = 0, mask_sky=False,
+                    max_points: Optional[int] = None) -> Dict[str, torch.Tensor]:
         """The filtered, coloured point cloud of one scene, built on the device (libovg kernels).
 
         Replaces the host numpy of the reference's GLB export (visual_util.py:190-236,:320-358 predictions_to_glb) and
@@ -474,9 +475,18 @@ class OmniVGGT(nn.Module, PyTorchModelHubMixin):
         ``mask_sky`` (the reference's --mask_sky, visual_util.py:140-188): False, no sky masking; True, the sky of every view
         by ``sky_mask``; or a bool tensor [S,H,W] / [B,S,H,W], True = sky (a reference mask file m, uint8 255 = non-sky, at
         H x W is ``m == 0``).  The confidence of every view becomes conf * non-sky before the frame selection and the
-        percentile, as the reference orders it; no host read is added."""
+        percentile, as the reference orders it; no host read is added.
+
+        ``max_points`` (None: every kept point): when more than max_points points are kept, ``points``, ``colors`` and
+        ``frame`` are those of the reference's farthest_point_sample (po_utils/misc.py:114-148, deterministic, from the first
+        kept point) over the kept points, max_points of them in selection order, so every prefix is a coarser sample of the
+        whole cloud.  ``conf_threshold``, ``center``, ``scale`` and ``align`` stay those of all kept points.  A cloud with fewer
+        than max_points distinct positions repeats points, as the reference's indices do.  One more launch, no host read."""
         from . import ops
         OmniVGGT._check_views(predictions, source, conf_percent, conf_floor, frame, scene, mask_sky)
+        if max_points is not None and (isinstance(max_points, (bool, np.bool_)) or not isinstance(max_points, (int, np.integer))
+                                       or max_points < 1):
+            raise ValueError(f"max_points must be None or an integer >= 1, got {max_points!r}")
         images, ext, points, mask, thr, f0 = OmniVGGT._kept_views(predictions, source, conf_percent, conf_floor, frame, scene,
                                                                   mask_sky)
         F, _, H, W = images.shape
@@ -493,6 +503,9 @@ class OmniVGGT(nn.Module, PyTorchModelHubMixin):
                     "scale": torch.ones((), device=dev), "align": align}
         pts, cols, fr, xyz = ops.point_cloud_gather(points, mask, images, ws, n, mask_black_bg, mask_white_bg, f0)
         scale = ops.point_cloud_scale(xyz, n, ws)
+        if max_points is not None and n > max_points:
+            idx = ops.farthest_point_sample(pts[None], int(max_points), torch.zeros(1, device=dev, dtype=torch.int64))[0]
+            pts, cols, fr = pts[idx], cols[idx], fr[idx]
         return {"points": pts, "colors": cols, "frame": fr, "conf_threshold": thr, "center": center, "scale": scale,
                 "align": align}
 

@@ -289,6 +289,24 @@ def sky_mask_conf(conf, sky):
     return out
 
 
+def farthest_point_sample(xyz, npoint: int, start: Optional[torch.Tensor], include_ends: bool = False):
+    """Farthest point sampling of B batches (ovg_farthest_point_sample): xyz fp32 [B, N, 3] on the device, start int64 [B] on
+    the device (the first index of each batch; None only with include_ends), 1 <= npoint <= N.  Returns int64 [B, npoint]
+    in selection order: one library call, one kernel launch, no host read."""
+    _chk(xyz, F32, "xyz")
+    assert xyz.dim() == 3 and xyz.shape[2] == 3 and xyz.is_contiguous()
+    B, N = xyz.shape[0], xyz.shape[1]
+    if start is not None:
+        _chk(start, torch.int64, "start")
+        assert start.is_contiguous() and start.numel() == B
+    lib = L.lib()
+    ws = torch.empty(max(lib.ovg_fps_workspace_bytes(B, N), 0), device=xyz.device, dtype=torch.uint8)
+    inds = torch.empty(B, npoint, device=xyz.device, dtype=torch.int64)
+    L.check(lib.ovg_farthest_point_sample(xyz.data_ptr(), B, N, npoint, L.ptr(start), int(include_ends), ws.data_ptr(),
+                                          ws.numel(), inds.data_ptr(), L.stream()))
+    return inds
+
+
 def host_read(t: torch.Tensor) -> torch.Tensor:
     """The device-to-host read of a matching or mesh call (its one synchronisation)."""
     return t.cpu()
