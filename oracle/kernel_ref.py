@@ -1,9 +1,10 @@
 """fp64 references of the hot-path kernels, with per-element error bounds taken from where each kernel rounds.
 
-Covers the GEMM and its epilogues, the QKV epilogue, attention, LayerNorm and the camera head.  Only the maths is restated here
-(pure torch, float64 unless stated).  tests/test_kernel_bounds_gpu.py checks the CUDA kernels against these functions, and
-tests/test_kernel_ref_cpu.py checks the functions themselves: CPU emulations of each kernel's arithmetic must pass, and
-emulations with seeded mistakes must fail.
+Covers the GEMM and its epilogues, the QKV epilogue, attention, LayerNorm, the camera head, and the kernels of the DPT output:
+bilinear upsampling, the fused output tail, and the im2col copies of the patch embeddings.  Only the maths is restated here
+(pure torch, float64 unless stated).  tests/test_kernel_bounds_gpu.py and tests/test_dpt_bounds_gpu.py check the CUDA kernels
+against these functions, and tests/test_kernel_ref_cpu.py and tests/test_dpt_ref_cpu.py check the functions themselves: CPU
+emulations of each kernel's arithmetic must pass, and emulations with seeded mistakes must fail.
 
 Where the bounds come from:
   * A 16-bit store is allowed one unit in the last place (ulp) of the stored type at the reference's magnitude.  That is a full ulp,
@@ -23,6 +24,7 @@ from typing import Dict, Optional, Sequence, Tuple
 import torch
 
 F64 = torch.float64
+F32 = torch.float32
 U_BF16 = 2.0 ** -8          # unit roundoff of bf16 (8 significant bits)
 EPS32 = 2.0 ** -24          # unit roundoff of fp32
 
@@ -225,17 +227,23 @@ def headtail_ref(a, w, taps, bias, w2, b2, head_act: int, F: int, gh: int, gw: i
     K = a.shape[1] * len(taps)
     h = acc + bias.to(F64)[None]
     eh = acc_bound(absacc, K) + EPS32 * h.abs()
-    eh = torch.where(h > 0, eh, torch.where(h + eh > 0, eh, torch.zeros_like(eh)))
-    h = h.clamp(min=0)
-    w2, b2 = w2.to(F64), b2.to(F64)
-    y = h @ w2.t() + b2
-    ey = eh @ w2.abs().t() + 34 * EPS32 * (h @ w2.abs().t() + b2.abs())
     pw = gw + 2
     r = torch.arange(acc.shape[0], device=acc.device)
     fr, rem = r // ((gh + 2) * pw), r % ((gh + 2) * pw)
     yy, xx = rem // pw, rem % pw
     inner = (yy >= 1) & (yy <= gh) & (xx >= 1) & (xx <= gw)
-    y, ey = y[inner].reshape(F, gh, gw, -1), ey[inner].reshape(F, gh, gw, -1)
+    return head_post(h[inner].reshape(F, gh, gw, -1), eh[inner].reshape(F, gh, gw, -1), w2, b2, head_act)
+
+
+def head_post(h, eh, w2, b2, head_act: int, epi_c: float = 34.0):
+    """ReLU -> 1x1 conv 32 -> outc -> activations (exp / inverse-log; confidence 1 + exp), from the 3x3 conv output h [..., 32]
+    (fp64, bias included) and its error bound eh.  epi_c: fp32 roundings allowed to the 1x1 (0 when it is exact).  The
+    activations may add 2 fp32 ulp (expf; expm1f 1 ulp).  Returns (preds [..., outc-1], conf [...], bound of preds, bound of conf)."""
+    eh = torch.where(h > 0, eh, torch.where(h + eh > 0, eh, torch.zeros_like(eh)))
+    h = h.clamp(min=0)
+    w2, b2 = w2.to(device=h.device, dtype=F64), b2.to(device=h.device, dtype=F64)
+    y = h @ w2.t() + b2
+    ey = eh @ w2.abs().t() + epi_c * EPS32 * (h @ w2.abs().t() + b2.abs())
     yp, ep = y[..., :-1], ey[..., :-1]
     if head_act == 0:
         preds = torch.exp(yp)
@@ -477,3 +485,232 @@ def camera_ref(w: Dict[str, object], tokens: torch.Tensor, B: int, S: int, heads
         act[:, 7:] = act[:, 7:].clamp(min=0)
         outs.append(act)
     return torch.stack(outs)
+
+
+# ----------------------------------------------------------------------------------------------- bilinear upsampling, DPT tail
+# The resize kernels (ovg_upsample_bilinear's two kernels and the producer warps of the fused tail) compute the sample positions
+# in fp32 and blend in fp32.  The references take the positions exactly as the kernels do (sample_positions) and blend in fp64, so
+# what is left to bound is the blend:
+#   * every output is a sum of four terms w_y w_x v, and each term passes through at most four fp32 roundings on any of the
+#     kernels' evaluation orders (vertical then horizontal, horizontal then vertical, with or without FMA contraction):
+#     BLEND_ROUNDINGS * EPS32 * sum |w v| (second-order terms are below 2^-40 of it);
+#   * nvcc may contract w1 = fp32(s o) - i0 into fma(s, o, -i0), which moves w1 and w0 = 1 - w1 by up to EPS32 (|f| + 3):
+#     position_slack.
+BLEND_ROUNDINGS = 4.0001
+# tail_tables_kernel: one table entry is four fp32 FMA chains of <= 144 terms, then two adds: <= 146 roundings of a partial sum.
+TABLE_ROUNDINGS = 146
+
+
+def sample_positions(n_src: int, n_dst: int):
+    """align_corners sample positions as the kernels compute them: s = fp32(n_src - 1) / fp32(n_dst - 1), f = fp32(s o),
+    i0 = int(f), i1 = i0 + (i0 < n_src - 1), w1 = f - i0 (exact), w0 = fp32(1 - w1).  Returns (i0, i1, w0, w1, f); the weights
+    and f as fp64 [n_dst]."""
+    if n_dst > 1:
+        s = torch.tensor(float(n_src - 1), dtype=F32) / torch.tensor(float(n_dst - 1), dtype=F32)
+    else:
+        s = torch.tensor(0.0, dtype=F32)
+    f = s * torch.arange(n_dst, dtype=F32)
+    i0 = f.to(torch.int64)
+    i1 = i0 + (i0 < n_src - 1).to(torch.int64)
+    w1 = f - i0.to(F32)
+    w0 = 1.0 - w1
+    return i0, i1, w0.to(F64), w1.to(F64), f.to(F64)
+
+
+def _blend(src: torch.Tensor, H: int, W: int):
+    """fp64 bilinear blend of src [F, h, w, C] at the kernels' fp32 positions: (value, the fp32 blend's error bound, sum |w v|),
+    all [F, H, W, C]."""
+    Fr, h, w, C = src.shape
+    dev = src.device
+    yi0, yi1, wy0, wy1, fy = (t.to(dev) for t in sample_positions(h, H))
+    xi0, xi1, wx0, wx1, fx = (t.to(dev) for t in sample_positions(w, W))
+    s = src.to(F64)
+    a, b = s[:, yi0], s[:, yi1]                                                  # [F, H, w, C]
+    cy = lambda t: t[None, :, None, None]                                        # noqa: E731
+    cx = lambda t: t[None, None, :, None]                                        # noqa: E731
+    r = cy(wy0) * a + cy(wy1) * b
+    value = cx(wx0) * r[:, :, xi0] + cx(wx1) * r[:, :, xi1]
+    del r
+    ar = cy(wy0) * a.abs() + cy(wy1) * b.abs()
+    absum = cx(wx0) * ar[:, :, xi0] + cx(wx1) * ar[:, :, xi1]
+    slack = EPS32 * (cx(fx.abs()) + 3) * (ar[:, :, xi0] + ar[:, :, xi1])
+    del ar
+    bb = a.abs() + b.abs()
+    slack += EPS32 * (cy(fy.abs()) + 3) * (cx(wx0) * bb[:, :, xi0] + cx(wx1) * bb[:, :, xi1])
+    return value, BLEND_ROUNDINGS * EPS32 * absum + slack, absum
+
+
+def embedding_map(tx: Optional[torch.Tensor], ty: Optional[torch.Tensor], H: int, W: int, C: int, device=None) -> torch.Tensor:
+    """The separable position embedding as a map fp64 [H, W, C]: channels [0, C/2) = tx[x], [C/2, C) = ty[y] (zeros without)."""
+    if tx is None:
+        return torch.zeros(H, W, C, dtype=F64, device=device)
+    tx, ty = tx.to(device=device, dtype=F64), ty.to(device=device, dtype=F64)
+    return torch.cat([tx[None].expand(H, W, C // 2), ty[:, None].expand(H, W, C // 2)], -1)
+
+
+def bilinear_ref(src, H: int, W: int, tx=None, ty=None, dtype=torch.bfloat16):
+    """ovg_upsample_bilinear on the interior src [F, h, w, C] (align_corners resize + the separable table): (ref fp64
+    [F, H, W, C], bound).  The bound is one ulp of the 16-bit store plus the fp32 blend and the table add."""
+    value, err, absum = _blend(src, H, W)
+    emb = embedding_map(tx, ty, H, W, src.shape[-1], src.device)[None]
+    ref = value + emb
+    bound = ulp(ref, dtype) + err + EPS32 * (absum + emb.abs())
+    return ref, bound
+
+
+def upsample_path(w: int, C: int) -> str:
+    """Which kernel ovg_upsample_bilinear launches, restated from its launch rule: "rows" (two-pass, one source row of 32 channels
+    in 48 KB of shared memory) when C % 32 == 0 and w * 128 B <= 48 KB, else "direct"."""
+    return "rows" if C % 32 == 0 and w * 32 * 4 <= 48 * 1024 and C // 32 <= 65535 else "direct"
+
+
+def conv3x3(x: torch.Tensor, wk: torch.Tensor) -> torch.Tensor:
+    """3x3 convolution with zero padding, NHWC: x [F, H, W, C], wk [O, 3, 3, C] -> [F, H, W, O] (fp64, as nine matmuls)."""
+    Fr, H, W, C = x.shape
+    xp = torch.nn.functional.pad(x, (0, 0, 1, 1, 1, 1))
+    out = torch.zeros(Fr, H, W, wk.shape[0], dtype=x.dtype, device=x.device)
+    for ky in range(3):
+        for kx in range(3):
+            out += xp[:, ky:ky + H, kx:kx + W] @ wk[:, ky, kx].t()
+    return out
+
+
+ROW_CLASSES = ((1, 2), (0, 2), (0, 1))     # kernel taps of the other axis inside the image: first, interior, last row / column
+
+
+def tail_tables_ref(tx, ty, w3x3, H: int, W: int):
+    """tail_tables_kernel: the position embedding's image under the 3x3 kernel, split by linearity into gx [3, W, 32] (class =
+    the output row's: 0 first row, 1 interior, 2 last row; x half of the embedding) and gy [3, H, 32] (class = the output
+    column's; y half), so that conv(E)[y, x] = gx[rc(y), x] + gy[cc(x), y].  w3x3 [32, 9 * 128] in K order (ky, kx, c)."""
+    wk = w3x3.to(F64).reshape(32, 3, 3, 128)
+    out = []
+    for t, n, part in ((tx, W, 0), (ty, H, 1)):
+        tp = torch.nn.functional.pad(t.to(device=wk.device, dtype=F64), (0, 0, 1, 1))
+        g = torch.zeros(3, n, 32, dtype=F64, device=wk.device)
+        for cls, (lo, hi) in enumerate(ROW_CLASSES):
+            for ks in range(3):                                   # tap along the table's own axis
+                ws = sum((wk[:, ko, ks, :64] if part == 0 else wk[:, ks, ko, 64:]) for ko in range(lo, hi + 1))
+                g[cls] += tp[ks:ks + n] @ ws.t()
+        out.append(g)
+    return out[0], out[1]
+
+
+def dpt_tail_ref(src, tx, ty, w3x3, bias, w2, b2, head_act: int, H: int, W: int, dtype=torch.bfloat16):
+    """ovg_dpt_tail on the interior src [F, h, w, 128]: resize -> 16-bit operand -> + embedding -> 3x3 conv 128 -> 32 + bias ->
+    ReLU -> 1x1 -> activations.  Returns (preds [F, H, W, outc-1], conf [F, H, W], bound of preds, bound of conf), fp64.
+
+    The producers round the fp32 blend to 16 bits; the reference uses round(up64) as the conv operand and allows the
+    neighbouring 16-bit value only where up64 lies within the blend's error bound of a rounding point.  The embedding enters
+    in fp32 through the tables.  Pre-activation bound: tensor-core accumulation over K = 9 * 128, the two fp32 adds that join
+    the three kernel rows' partial sums, the operand flips, the tables' fp32 FMA chains and the three epilogue adds."""
+    dev = src.device
+    up, err, _ = _blend(src, H, W)
+    op = round_to(up, dtype)
+    dop = torch.maximum((round_to(up + err, dtype) - op).abs(), (round_to(up - err, dtype) - op).abs())
+    del up, err
+    wk = w3x3.to(device=dev, dtype=F64).reshape(32, 3, 3, 128)
+    wa = wk.abs()
+    emb = embedding_map(tx, ty, H, W, 128, dev)[None]
+    h = conv3x3(op + emb, wk) + bias.to(device=dev, dtype=F64)
+    absacc = conv3x3(op.abs(), wa)
+    flips = conv3x3(dop, wa)
+    del op, dop
+    abse = conv3x3(emb.abs(), wa) if tx is not None else torch.zeros_like(absacc[:1])
+    eh = acc_bound(absacc, 9 * 128) + 2 * EPS32 * absacc + flips + TABLE_ROUNDINGS * EPS32 * abse \
+        + 3 * EPS32 * (absacc + bias.to(device=dev, dtype=F64).abs() + abse)
+    return head_post(h, eh, w2, b2, head_act)
+
+
+# ----------------------------------------------------------------------------------------------- fused tail geometry
+FT_VBUF_PX = 80          # source pixels a 130-pixel strip may span (tail.cuh): the ring row and itab size
+
+
+def tail_supported(h: int, w: int, H: int, W: int, C: int = 128) -> bool:
+    """ovg_dpt_tail_supported, restated in fp32."""
+    import numpy as np
+    if C != 128 or h < 2 or w < 2 or H < h or W < w:
+        return False
+    sx = np.float32(w - 1) / np.float32(W - 1)
+    return int(sx * np.float32(129.0)) + 3 <= FT_VBUF_PX
+
+
+def tail_schedule(F: int, H: int, W: int, sms: int) -> Dict[str, int]:
+    """ovg_dpt_tail's work split on a device with `sms` SMs: 128-pixel strips, segments of seg_rows output rows (two halo rows
+    each), about three work items per SM."""
+    n_strips = (W + 127) // 128
+    segs = max(1, (3 * sms + F * n_strips - 1) // (F * n_strips))
+    segs = min(segs, H)
+    seg_rows = (H + segs - 1) // segs
+    if seg_rows < 8 and H >= 8:
+        seg_rows = 8
+    n_segs = (H + seg_rows - 1) // seg_rows
+    return dict(n_strips=n_strips, seg_rows=seg_rows, n_segs=n_segs, n_items=F * n_strips * n_segs,
+                last_strip_px=W - 128 * (n_strips - 1))
+
+
+def tail_strip(w: int, W: int, strip: int):
+    """The producer's walk for one strip, in fp32 as tail.cuh: (x_lo, x_hi, xs_lo, ns, itab) with itab a list of
+    (first strip row, pixel count) per source interval xs_lo + j, j < ns."""
+    import numpy as np
+    sx = np.float32(w - 1) / np.float32(W - 1)
+    x0 = 128 * strip
+    x_lo, x_hi = max(x0 - 1, 0), min(x0 + 128, W - 1)
+    fl = lambda X: int(sx * np.float32(X))                                     # noqa: E731
+    xs_lo = fl(x_lo)
+    xs_hi = min(fl(x_hi) + 1, w - 1)
+    ns = xs_hi - xs_lo + 1
+    itab = []
+    for j in range(ns):
+        sabs = xs_lo + j
+        Xg = max(int(np.float32(sabs) / sx) - 2, x_lo)
+        while Xg <= x_hi and fl(Xg) < sabs:
+            Xg += 1
+        n = 0
+        while Xg + n <= x_hi and fl(Xg + n) == sabs:
+            n += 1
+        itab.append((Xg - (x0 - 1), n))
+    return x_lo, x_hi, xs_lo, ns, itab
+
+
+# ----------------------------------------------------------------------------------------------- im2col of the patch embeddings
+def image_cols_ref(images: torch.Tensor, mean3, std3, patch: int, ldc: int) -> torch.Tensor:
+    """ovg_image_im2col in fp32 on the CPU: (v - mean) * istd with istd = 1 / std rounded to fp32 (the host's 1.0f / std), stored
+    as bf16 rows (k, py, px) x columns (c, ky, kx), zero-padded to ldc.  Two IEEE roundings and no contraction opportunity,
+    so this is bit-exact."""
+    K, _, H, W = images.shape
+    hp, wp = H // patch, W // patch
+    mean = torch.tensor([float(v) for v in mean3], dtype=F32)[None, :, None, None]
+    istd = (1.0 / torch.tensor([float(v) for v in std3], dtype=F32))[None, :, None, None]
+    v = (images.to(F32).cpu() - mean) * istd
+    cols = v.reshape(K, 3, hp, patch, wp, patch).permute(0, 2, 4, 1, 3, 5).reshape(K * hp * wp, 3 * patch * patch)
+    out = torch.zeros(K * hp * wp, ldc, dtype=torch.bfloat16)
+    out[:, :3 * patch * patch] = cols.to(torch.bfloat16)
+    return out
+
+
+def depth_scale_ref(depth: torch.Tensor, mask: torch.Tensor, idx_stats: Sequence[int]) -> torch.Tensor:
+    """The per-scene scale of ovg_depth_im2col from exact sums: fp32(1 / (fp32(sum / count) + 1e-8f)), 0 without a valid pixel
+    (fp32 [B]).  Equal to the kernel's bit for bit when its fp32 partial sums are exact (dyadic depths)."""
+    d = depth.to(F64).cpu()[:, list(idx_stats)]
+    m = mask.cpu()[:, list(idx_stats)] > 0
+    out = torch.zeros(d.shape[0], dtype=F32)
+    for b in range(d.shape[0]):
+        cnt = int(m[b].sum())
+        if cnt:
+            mean = torch.tensor(float(d[b][m[b]].sum()) / cnt, dtype=F64).to(F32)
+            out[b] = torch.tensor(1.0, dtype=F32) / (mean + torch.tensor(1e-8, dtype=F32))
+    return out
+
+
+def depth_cols_ref(depth: torch.Tensor, mask: torch.Tensor, scale: torch.Tensor, idx_cols: Sequence[int], patch: int):
+    """ovg_depth_im2col's rows for the views idx_cols, given the per-scene fp32 scale: [d * scale * m, m] in fp32 ((d * scale)
+    rounded, then * m; no contraction opportunity), stored as bf16 rows (b, view, py, px) x columns (ky, kx) of each half."""
+    d = depth.to(F32).cpu()[:, list(idx_cols)]
+    m = mask.to(F32).cpu()[:, list(idx_cols)]
+    B, S, H, W = d.shape
+    hp, wp = H // patch, W // patch
+    v = (d * scale.to(F32).cpu()[:, None, None, None]) * m
+
+    def unfold(t):
+        return t.reshape(B, S, hp, patch, wp, patch).permute(0, 1, 2, 4, 3, 5).reshape(B * S * hp * wp, patch * patch)
+    return torch.cat([unfold(v), unfold(m)], 1).to(torch.bfloat16)
