@@ -321,6 +321,25 @@ long long ovg_fps_workspace_bytes(int B, long long N);
 int ovg_farthest_point_sample(const float* xyz, int B, long long N, int npoint, const long long* start, int include_ends,
                               void* workspace, long long workspace_bytes, long long* inds_out, void* stream);
 
+/* Image ranking by camera distance: datasets/utils/image_ranking.py:9-140 (rotation_angle, extrinsic_distance, the batched
+ * and chunked distance matrices, compute_ranking) for N views at once.  extrinsics: element (v, r, c) at v view_stride +
+ * r row_stride + c col_stride (elements of fp64 when in_f64, else fp32); R is rows 0-2 x columns 0-2 and t is column 3 of
+ * rows 0-2, whatever convention the caller's extrinsics use.  With normalize, t = t / mean_v |t_v|: the mean is one fp64
+ * reduction in a fixed order and the quotient is rounded to the input dtype, as the reference's in-place division is.  With
+ * an fp32 output (out_f64 = 0) every operand is then rounded to fp32, as the reference's chunked path casts them.
+ * d(i, j) = degrees(arccos(clip((trace(R_i^T R_j) - 1) / 2, -1, 1))) / 180 + lambda_t |t_i - t_j| in fp64, every multiply
+ * and add rounded on its own in the reference's order (trace = (M00 + M11) + M22, Mcc summed over the rows in order), then
+ * rounded once into dists [N, N] (fp64 when out_f64, else fp32).  ranking int64 [N, k]: the first k entries of each row's
+ * stable sort of its dists (ties in index order, -0 equal to +0, NaN last), 1 <= k <= N.  No host synchronisation;
+ * results are bit-identical from run to run.  N <= OVG_RANK_CTA_VIEWS: one CTA per row with the row's keys in shared
+ * memory; above, a persistent grid sorting each row in a per-CTA scratch of the workspace.  1 <= N < 2^31.
+ * workspace: ovg_ranking_workspace_bytes(N, out_f64) bytes, 256-byte aligned. */
+#define OVG_RANK_CTA_VIEWS 8192
+long long ovg_ranking_workspace_bytes(long long N, int out_f64);
+int ovg_compute_ranking(const void* extrinsics, int in_f64, long long N, long long view_stride, long long row_stride,
+                        long long col_stride, double lambda_t, int normalize, int out_f64, long long k, void* workspace,
+                        long long workspace_bytes, long long* ranking, void* dists, void* stream);
+
 /* Baseline JPEG decoding on the device, bit-identical to Pillow (libjpeg-turbo's default islow IDCT, fancy upsampling and
  * YCbCr -> RGB tables).  The plan is host code (no CUDA call): it parses every file, routes it to the device or to the host
  * (OVG_JPEG_* below: anything the device cannot decode exactly goes to the host), and builds the staging stream (tables plus the

@@ -139,6 +139,8 @@ EXPORTS = {
     "ovg_sky_mask_conf": (C.c_int, [_vp, _vp, _ll, _vp, _vp]),
     "ovg_fps_workspace_bytes": (_ll, [_i, _ll]),
     "ovg_farthest_point_sample": (C.c_int, [_vp, _i, _ll, _i, _vp, _i, _vp, _ll, _vp, _vp]),
+    "ovg_ranking_workspace_bytes": (_ll, [_ll, _i]),
+    "ovg_compute_ranking": (C.c_int, [_vp, _i, _ll, _ll, _ll, _ll, C.c_double, _i, _i, _ll, _vp, _ll, _vp, _vp, _vp]),
     "ovg_jpeg_plan_create": (C.c_int, [_pp, C.POINTER(_ll), _i, _i, _pp]),
     "ovg_jpeg_plan_destroy": (None, [_vp]),
     "ovg_jpeg_plan_file": (C.c_int, [_vp, _i, C.POINTER(_i), C.POINTER(_i), C.POINTER(_i), C.POINTER(_i)]),

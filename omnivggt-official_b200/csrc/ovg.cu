@@ -18,6 +18,7 @@
 #include "mesh.cuh"
 #include "sky.cuh"
 #include "fps.cuh"
+#include "rank.cuh"
 #include "tail.cuh"
 #include "pre.cuh"
 #include "jpeg.cuh"
@@ -1235,6 +1236,70 @@ int ovg_farthest_point_sample(const float* xyz, int B, long long N, int npoint, 
   OVG_CUDA(cudaLaunchCooperativeKernel(reinterpret_cast<void*>(ovg::fps_grid_kernel), dim3(grid), dim3(ovg::FPS_THREADS), args,
                                        ovg::FPS_SMEM_BYTES, st));
   return post_launch("ovg_farthest_point_sample(grid)");
+}
+
+}  // extern "C"
+
+// ----------------------------------------------------------------------------------------------------------- image ranking
+namespace {
+
+// Ranking workspace, carved the same way by the size query and by the entry point: the packed operands, and on the grid
+// path one scratch of two key / index buffers per CTA.
+ovg::RankParams ranking_workspace(void* base, long long N, int out_f64, long long* bytes) {
+  Arena ar(base, 0);
+  ovg::RankParams p{};
+  p.pose = ar.get<double>(N * 12);
+  if (N > ovg::RANK_CTA_VIEWS) {
+    p.scratch_stride = (N * (2 * (out_f64 ? 8 : 4) + 8) + 255) & ~255LL;
+    p.scratch = ar.get<unsigned char>(ovg::RANK_GRID_CTAS * p.scratch_stride);
+  }
+  *bytes = ar.bytes();
+  return p;
+}
+
+template <typename T, typename K>
+int launch_ranking(const ovg::RankParams& p, cudaStream_t st) {
+  if (p.N <= ovg::RANK_CTA_VIEWS) {
+    const int smem = p.N * static_cast<int>(2 * sizeof(K) + 8);
+    const int rc = allow_dynamic_smem<ovg::rank_smem_kernel<T, K>>(ovg::RANK_CTA_VIEWS * static_cast<int>(2 * sizeof(K) + 8));
+    if (rc) return rc;
+    ovg::rank_smem_kernel<T, K><<<p.N, ovg::RANK_THREADS, smem, st>>>(p);
+    return post_launch("ovg_compute_ranking(smem)");
+  }
+  ovg::rank_grid_kernel<T, K><<<ovg::RANK_GRID_CTAS, ovg::RANK_THREADS, 0, st>>>(p);
+  return post_launch("ovg_compute_ranking(grid)");
+}
+
+}  // namespace
+
+extern "C" {
+
+long long ovg_ranking_workspace_bytes(long long N, int out_f64) {
+  if (N <= 0 || N >= (1LL << 31)) return -1;
+  long long bytes = 0;
+  ranking_workspace(nullptr, N, out_f64, &bytes);
+  return bytes;
+}
+
+int ovg_compute_ranking(const void* extrinsics, int in_f64, long long N, long long view_stride, long long row_stride,
+                        long long col_stride, double lambda_t, int normalize, int out_f64, long long k, void* workspace,
+                        long long workspace_bytes, long long* ranking, void* dists, void* stream) {
+  OVG_REQUIRE(N > 0 && N < (1LL << 31), "N must be in [1, 2^31)");
+  OVG_REQUIRE(k >= 1 && k <= N, "k must be in [1, N]");
+  OVG_REQUIRE(extrinsics && ranking && dists, "null extrinsics / ranking / dists");
+  long long bytes = 0;
+  ovg::RankParams p = ranking_workspace(workspace, N, out_f64, &bytes);
+  OVG_REQUIRE(workspace_ok(workspace, workspace_bytes, bytes, 256),
+              "workspace must be 256-byte aligned and ovg_ranking_workspace_bytes(N, out_f64) long");
+  p.ext = extrinsics; p.s0 = view_stride; p.s1 = row_stride; p.s2 = col_stride;
+  p.ranking = ranking; p.dists = dists; p.lambda = lambda_t;
+  p.N = static_cast<int>(N); p.k = static_cast<int>(k);
+  p.in_f64 = in_f64 ? 1 : 0; p.out_f64 = out_f64 ? 1 : 0; p.normalize = normalize ? 1 : 0;
+  cudaStream_t st = reinterpret_cast<cudaStream_t>(stream);
+  ovg::rank_prep_kernel<<<1, ovg::RANK_PREP_THREADS, 0, st>>>(p);
+  const int rc = post_launch("ovg_compute_ranking(prep)");
+  if (rc) return rc;
+  return p.out_f64 ? launch_ranking<double, unsigned long long>(p, st) : launch_ranking<float, unsigned>(p, st);
 }
 
 }  // extern "C"

@@ -1,8 +1,9 @@
 """Geometry of point maps on the device: dense correspondence (libovg ovg_match_*, the reference's
 omnivggt/utils/geometry.py:435-451 find_reciprocal_matches), triangle meshes (libovg ovg_mesh_*, the reference's
 omnivggt/viz.py:40-89 pts3d_to_trimesh and cat_meshes), model-free sky segmentation (libovg ovg_segment_sky, the
-reference's omnivggt/viz.py:357-393 segment_sky) and farthest point sampling (libovg ovg_farthest_point_sample, the
-reference's omnivggt/utils/po_utils/misc.py:114-148 farthest_point_sample)."""
+reference's omnivggt/viz.py:357-393 segment_sky), farthest point sampling (libovg ovg_farthest_point_sample, the
+reference's omnivggt/utils/po_utils/misc.py:114-148 farthest_point_sample) and the ranking of views by camera distance
+(libovg ovg_compute_ranking, the reference's omnivggt/datasets/utils/image_ranking.py:118-140 compute_ranking)."""
 from __future__ import annotations
 
 import numpy as np
@@ -149,6 +150,48 @@ def farthest_point_sample(xyz, npoint: int, include_ends: bool = False, determin
         return torch.zeros(0, int(npoint), device=dev, dtype=torch.int64)
     pts = _to(xyz, dev).float().contiguous()
     return ops.farthest_point_sample(pts, int(npoint), start.to(dev), include_ends)
+
+
+RANKING_CHUNKED_ABOVE = 6000     # image_ranking.py:129: the batched path switches to its fp32 chunked formula above this
+
+
+def compute_ranking(extrinsics, lambda_t: float = 1.0, normalize: bool = True, batched: bool = True, k=None):
+    """Drop-in for image_ranking.py:118-140: the camera-distance matrix of N views and, per view, every view from nearest to
+    farthest.  extrinsics [N, >=3, >=4] of float32 or float64: a CUDA or CPU tensor, or an array (moved to the current CUDA
+    device); R = E[:, :3, :3], t = E[:, :3, 3], whatever convention they use.  Returns (ranking int64 [N, k], dists [N, N])
+    on the device.
+
+    d(i, j) = degrees(arccos(clip((trace(R_i^T R_j) - 1) / 2, -1, 1))) / 180 + lambda_t |t_i - t_j|, after t / mean |t| when
+    normalize.  dists has the reference's dtype: the input's when batched and N <= 6000, float32 when batched and N > 6000
+    (computed from float32 operands, as the chunked path is), float64 when not batched.  Each entry is evaluated in fp64
+    and rounded once; where the reference computes in float32 (a float32 input, or the chunked path), lambda_t is rounded
+    to float32 as numpy does.  ranking is the stable argsort of dists: ties in index order, NaN last (the reference's
+    quicksort leaves the order of ties unspecified).  k=None returns every column; k=m returns the first m columns of the
+    same ranking, and dists in full.  Limits, each a ValueError before any device work: not 3-D, fewer than 3 rows or 4
+    columns, a dtype other than float32 / float64, k outside [1, N]."""
+    shape = tuple(extrinsics.shape) if hasattr(extrinsics, "shape") else np.shape(extrinsics)
+    if len(shape) != 3 or shape[1] < 3 or shape[2] < 4:
+        raise ValueError(f"extrinsics must have shape [N, >=3, >=4], got {shape}")
+    dtype = extrinsics.dtype if torch.is_tensor(extrinsics) else np.asarray(extrinsics).dtype
+    if dtype not in (torch.float32, torch.float64, np.float32, np.float64):
+        raise ValueError(f"extrinsics dtype must be float32 or float64, got {dtype}")
+    in_f64 = dtype in (torch.float64, np.float64)
+    N = shape[0]
+    if k is None:
+        k = N
+    elif isinstance(k, bool) or not isinstance(k, (int, np.integer)) or not 1 <= k <= N:
+        raise ValueError(f"k must be an integer in [1, N = {N}], got {k!r}")
+    if not batched:
+        out = torch.float64
+    elif N > RANKING_CHUNKED_ABOVE:
+        out = torch.float32
+    else:
+        out = torch.float64 if in_f64 else torch.float32
+    lam = float(lambda_t) if in_f64 and out == torch.float64 else float(np.float32(lambda_t))
+    dev = _device_of(extrinsics)
+    if N == 0:
+        return torch.zeros(0, 0, device=dev, dtype=torch.int64), torch.zeros(0, 0, device=dev, dtype=out)
+    return ops.compute_ranking(_to(extrinsics, dev), lam, normalize, out, int(k))
 
 
 def cat_meshes(meshes):

@@ -307,6 +307,26 @@ def farthest_point_sample(xyz, npoint: int, start: Optional[torch.Tensor], inclu
     return inds
 
 
+def compute_ranking(ext: torch.Tensor, lambda_t: float, normalize: bool, out_dtype, k: int):
+    """Camera-distance matrix and ranking of N views (ovg_compute_ranking): ext fp32 or fp64 [N, >=3, >=4] on the device (any
+    strides), out_dtype torch.float32 or torch.float64, 1 <= k <= N.  Returns (ranking int64 [N, k], dists [N, N] of
+    out_dtype): one library call, two kernel launches, no host read."""
+    if ext.dtype not in (torch.float32, torch.float64) or not _on_device(ext):
+        raise TypeError(f"ext: expected cuda float32 / float64, got {ext.device} {ext.dtype}")
+    assert ext.dim() == 3 and ext.shape[1] >= 3 and ext.shape[2] >= 4
+    assert out_dtype in (torch.float32, torch.float64)
+    N = ext.shape[0]
+    out_f64 = int(out_dtype == torch.float64)
+    lib = L.lib()
+    ws = torch.empty(max(lib.ovg_ranking_workspace_bytes(N, out_f64), 0), device=ext.device, dtype=torch.uint8)
+    ranking = torch.empty(N, k, device=ext.device, dtype=torch.int64)
+    dists = torch.empty(N, N, device=ext.device, dtype=out_dtype)
+    L.check(lib.ovg_compute_ranking(ext.data_ptr(), int(ext.dtype == torch.float64), N, *ext.stride(), float(lambda_t),
+                                    int(normalize), out_f64, k, ws.data_ptr(), ws.numel(), ranking.data_ptr(),
+                                    dists.data_ptr(), L.stream()))
+    return ranking, dists
+
+
 def host_read(t: torch.Tensor) -> torch.Tensor:
     """The device-to-host read of a matching or mesh call (its one synchronisation)."""
     return t.cpu()
