@@ -7,10 +7,17 @@
 //   * DPT 1x1 / transposed convs (heads/dpt_head.py:69-96)                              -- 1 tap
 //   * DPT 3x3 convs as 9 row-shifted GEMMs over a zero-bordered ("padded-linear") NHWC
 //     layout (heads/dpt_head.py:326-354,:379-399,:115-126)                              -- 9 taps
-// Roles: warpgroup 0 = TMA producer (one thread), warpgroups 1-2 = wgmma (64 rows of the 128-row tile each) + epilogue.
-// Pipeline: smem full/empty ring (TMA<->MMA).  The finished accumulator tile goes through an fp32 smem tile so that the
-// epilogue works on whole rows (one row per thread), as the QKV head LayerNorm and the row remaps need; the producer keeps
-// loading the next tile's K blocks meanwhile.
+// Roles (512 threads, setmaxnreg split 40 / 144 / 184 registers = the whole 64K register file):
+//   warpgroup 0     TMA producer (one thread), 40 registers
+//   warpgroups 1-2  wgmma consumers, 64 rows of the 128-row tile each; they issue MMAs and stage the accumulators, nothing else
+//                   (144 registers)
+//   warpgroup 3     epilogue: one whole accumulator row per thread, every column of the tile (184 registers)
+// Pipeline: smem full/empty ring (TMA<->MMA).  The finished accumulator tile goes through ONE fp32 smem tile (sAcc) so that
+// the epilogue works on whole rows, as the QKV head LayerNorm and the row remaps need.  Hand-off over two named barriers of
+// the 384 consumer + epilogue threads: the consumers wait for GEMM_BAR_ACC_FREE (skipped on their first tile), store the
+// accumulators and arrive on GEMM_BAR_ACC_FULL; the epilogue waits for GEMM_BAR_ACC_FULL, runs the fused epilogue and arrives on
+// GEMM_BAR_ACC_FREE (not after its last tile, so that both barriers end balanced).  The epilogue of tile i thus runs under
+// the MMAs of tile i + 1; the consumers stall only when an epilogue takes longer than a K loop.
 #pragma once
 #include "ptx.cuh"
 
@@ -73,7 +80,16 @@ struct GemmParams {
 
 constexpr int GEMM_BM = 128;
 constexpr int GEMM_BK = 64;
-constexpr int GEMM_THREADS = 384;
+constexpr int GEMM_THREADS = 512;
+constexpr int GEMM_EPI_THREAD0 = 384;     // first thread of the epilogue warpgroup
+constexpr int GEMM_BAR_ACC_FULL = 1;      // named barriers over the 256 consumer + 128 epilogue threads
+constexpr int GEMM_BAR_ACC_FREE = 2;
+// setmaxnreg split; the three warpgroups share the 64K-entry register file.  The QKV epilogue (two 64-wide heads per row at
+// BN = 128) needs the most: it spills at 168.  The wgmma warpgroups hold BN / 2 accumulators and little else.
+constexpr int GEMM_PRODUCER_REGS = 40;
+constexpr int GEMM_MMA_REGS = 144;
+constexpr int GEMM_EPI_REGS = 184;
+static_assert(128 * (GEMM_PRODUCER_REGS + 2 * GEMM_MMA_REGS + GEMM_EPI_REGS) <= 65536, "register split");
 constexpr int GEMM_A_BYTES = GEMM_BM * GEMM_BK * 2;
 
 constexpr int GEMM_QKV_TABLE_BYTES = 3 * 64 * 18 * 4 + 1024;   // QKV epilogue: rope cos / sin / -sin + q,k LayerNorm affine
@@ -126,10 +142,10 @@ __device__ __forceinline__ void acc_ld32(const float* src, uint32_t* r) {
 }
 
 // One 128 x BN accumulator tile: smem -> registers -> fused epilogue -> global.  `arow` is this thread's row of the fp32
-// accumulator tile, `m` its global row, `colhalf` selects which column chunks this warp owns.
+// accumulator tile, `m` its global row; this thread owns the column chunks cfirst, cfirst + cstep, ... of the row.
 template <int BN, int EPI>
 __device__ __forceinline__ void epilogue_tile(const GemmParams& p, const float* arow, const int m, const int n0,
-                                              const int colhalf, const float* s_rope) {
+                                              const int cfirst, const int cstep, const float* s_rope) {
   if constexpr (EPI == EPI_QKV) {
     // ---- per-row RoPE position (reference omnivggt_aggregator.py:215-224; layers/rope.py:39-59)
     int py = 0, px = 0;
@@ -153,7 +169,7 @@ __device__ __forceinline__ void epilogue_tile(const GemmParams& p, const float* 
     const long long seq = m / p.ntok;
     const long long tok = m % p.ntok;
     const int heads = p.C >> 6;
-    for (int c = colhalf; c < BN / 64; c += 2) {
+    for (int c = cfirst; c < BN / 64; c += cstep) {
       const int n = n0 + c * 64;
       if (n >= p.N) continue;                                   // warp-uniform
       if (m < p.M) {
@@ -270,7 +286,7 @@ __device__ __forceinline__ void epilogue_tile(const GemmParams& p, const float* 
         interior = (yy >= 1 && yy <= p.gh && xx >= 1 && xx <= p.gw);
       }
     }
-    for (int c = colhalf; c < BN / 32; c += 2) {
+    for (int c = cfirst; c < BN / 32; c += cstep) {
       const int n = n0 + c * 32;
       if (n >= p.N || !row_ok) continue;
       uint32_t raw[32];
@@ -438,7 +454,7 @@ gemm_kernel(const __grid_constant__ CUtensorMap tmA, const __grid_constant__ CUt
 
   if (warp < 4) {
     // ===================== TMA producer =====================
-    reg_dealloc<40>();
+    reg_dealloc<GEMM_PRODUCER_REGS>();
     if (threadIdx.x == 0) {
       int s = 0;
       uint32_t ph = 0;
@@ -459,22 +475,16 @@ gemm_kernel(const __grid_constant__ CUtensorMap tmA, const __grid_constant__ CUt
         }
       }
     }
-  } else {
-    // ===================== wgmma + epilogue (2 warpgroups, 8 warps) =====================
-    reg_alloc<232>();
+  } else if (threadIdx.x < GEMM_EPI_THREAD0) {
+    // ===================== wgmma (2 warpgroups, 8 warps) =====================
+    reg_alloc<GEMM_MMA_REGS>();
     const int cw = (warp >> 2) - 1;      // consumer warpgroup: rows [64 cw, 64 cw + 64) of the tile
-    const int e = warp - 4;              // epilogue warp 0..7
-    const int quarter = e & 3;           // epilogue rows 32 * quarter .. + 31
-    const int colhalf = e >> 2;
-    const int r = quarter * 32 + lane;
     const int frow = cw * 64 + (warp & 3) * 16 + (lane >> 2);   // accumulator fragment rows frow, frow + 8
     const int fcol = 2 * (lane & 3);
     int s = 0;
     uint32_t ph = 0;
     float acc[BN / 2];
     for (int tile = blockIdx.x; tile < num_tiles; tile += gridDim.x) {
-      const int m0 = (tile / n_tiles) * GEMM_BM;
-      const int n0 = (tile % n_tiles) * BN;
       int prev = -1;
       for (int kb = 0; kb < p.k_blocks; ++kb) {
         mbar_wait_quiet(&full[s], ph);      // no printf call site: it would serialise the wgmma pipeline
@@ -498,14 +508,25 @@ gemm_kernel(const __grid_constant__ CUtensorMap tmA, const __grid_constant__ CUt
       wgmma_wait<0>();
       fence_regs<BN / 2>(acc);
       if (lane == 0) mbar_arrive(&empty[prev]);
-      named_sync(1, 256);                // every epilogue thread is done with the previous tile's accumulators
+      // the epilogue warpgroup is done with the previous tile's accumulators (it has read sAcc in full)
+      if (tile != static_cast<int>(blockIdx.x)) named_sync(GEMM_BAR_ACC_FREE, 384);
 #pragma unroll
       for (int j = 0; j < BN / 8; ++j) {
         *reinterpret_cast<float2*>(sAcc + frow * Cfg::ACC_LD + 8 * j + fcol) = make_float2(acc[4 * j], acc[4 * j + 1]);
         *reinterpret_cast<float2*>(sAcc + (frow + 8) * Cfg::ACC_LD + 8 * j + fcol) = make_float2(acc[4 * j + 2], acc[4 * j + 3]);
       }
-      named_sync(1, 256);
-      epilogue_tile<BN, EPI>(p, sAcc + r * Cfg::ACC_LD, m0 + r, n0, colhalf, s_rope);
+      named_arrive(GEMM_BAR_ACC_FULL, 384);
+    }
+  } else {
+    // ===================== epilogue (1 warpgroup): row r of every tile, all BN columns =====================
+    reg_alloc<GEMM_EPI_REGS>();
+    const int r = threadIdx.x - GEMM_EPI_THREAD0;
+    for (int tile = blockIdx.x; tile < num_tiles; tile += gridDim.x) {
+      const int m0 = (tile / n_tiles) * GEMM_BM;
+      const int n0 = (tile % n_tiles) * BN;
+      named_sync(GEMM_BAR_ACC_FULL, 384);
+      epilogue_tile<BN, EPI>(p, sAcc + r * Cfg::ACC_LD, m0 + r, n0, 0, 1, s_rope);
+      if (tile + static_cast<int>(gridDim.x) < num_tiles) named_arrive(GEMM_BAR_ACC_FREE, 384);
     }
   }
 }
@@ -522,8 +543,9 @@ constexpr int HT_B_TILE = 32 * 128;                  // one [32 x 64] 16-bit wei
 constexpr int HT_B_BYTES = 18 * HT_B_TILE;           // 9 taps x 2 K blocks
 constexpr int HT_ACC_LD = 36;
 constexpr int HT_SMEM_BYTES = HT_STAGES * HT_A_BYTES + HT_B_BYTES + GEMM_BM * HT_ACC_LD * 4 + 1024 + 256;
+constexpr int HT_THREADS = 384;   // producer warpgroup + 2 wgmma warpgroups that also run the epilogue
 
-__global__ void __launch_bounds__(GEMM_THREADS, 1)
+__global__ void __launch_bounds__(HT_THREADS, 1)
 headtail_kernel(const __grid_constant__ CUtensorMap tmA, const __grid_constant__ CUtensorMap tmB, const GemmParams p) {
   extern __shared__ uint8_t smem_raw[];
   uint8_t* smem = reinterpret_cast<uint8_t*>((reinterpret_cast<uintptr_t>(smem_raw) + 1023) & ~uintptr_t(1023));
@@ -625,7 +647,7 @@ headtail_kernel(const __grid_constant__ CUtensorMap tmA, const __grid_constant__
         *reinterpret_cast<float2*>(sAcc + (frow + 8) * HT_ACC_LD + 8 * j + fcol) = make_float2(acc[4 * j + 2], acc[4 * j + 3]);
       }
       named_sync(1, 256);
-      epilogue_tile<32, EPI_HEADTAIL>(p, sAcc + r * HT_ACC_LD, m0 + r, 0, e >> 2, nullptr);
+      epilogue_tile<32, EPI_HEADTAIL>(p, sAcc + r * HT_ACC_LD, m0 + r, 0, e >> 2, 2, nullptr);
     }
   }
 }

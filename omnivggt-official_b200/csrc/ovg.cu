@@ -314,7 +314,7 @@ int ovg_gemm(const ovg_gemm_args* a, void* stream) {
       if (rc) return rc;
       const int tiles = (p.M + ovg::GEMM_BM - 1) / ovg::GEMM_BM;
       const int grid = tiles < num_sms() ? tiles : num_sms();
-      ovg::headtail_kernel<<<grid, ovg::GEMM_THREADS, ovg::HT_SMEM_BYTES, st>>>(ta136, tb, p);
+      ovg::headtail_kernel<<<grid, ovg::HT_THREADS, ovg::HT_SMEM_BYTES, st>>>(ta136, tb, p);
       return post_launch("ovg_gemm(headtail)");
     }
     default: return fail(OVG_E_INVALID, "ovg_gemm: unknown epilogue");

@@ -88,6 +88,11 @@ __device__ __forceinline__ void reg_dealloc() { asm volatile("setmaxnreg.dec.syn
 __device__ __forceinline__ void named_sync(int id, int nthreads) {
   asm volatile("bar.sync %0, %1;" ::"r"(id), "r"(nthreads) : "memory");
 }
+// arrive on a named barrier without waiting for it; the calling thread's prior shared-memory writes are visible to the threads
+// that wait on it (bar.sync) once it completes
+__device__ __forceinline__ void named_arrive(int id, int nthreads) {
+  asm volatile("bar.arrive %0, %1;" ::"r"(id), "r"(nthreads) : "memory");
+}
 
 // ------------------------------------------------------------------ wgmma (sm_90a)
 // Shared-memory matrix descriptor, 128B swizzle (tile rows are 128 B = 64 16-bit elements, 8-row groups of 1024 B).
