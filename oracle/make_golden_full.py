@@ -2,22 +2,29 @@
 camera head, both DPT heads; reference omnivggt/models/omnivggt.py:10-68) once per case at 518 x 518 on CPU fp32 and store
 its outputs (build container only; TEST INFRASTRUCTURE).
 
-    python oracle/make_golden_full.py            # ~6 min, ~12 GB of host memory
+    python oracle/make_golden_full.py [case ...]   # all six: ~10 min on 8 cores, peak host memory 17.2 GB (full_cfg5)
 
-Cases (BASELINE.json configs):
-  full_cfg1      configs[0]: 1 scene x 4 views @ 518^2, images only
-  full_aux_s3    configs[2]-shaped: 1 scene x 3 views @ 518^2, depth + camera aux on every view
-  full_mixed_s5  configs[4]-shaped: 1 scene x 5 views @ 518^2, partial depth_gt_index / camera_gt_index
+Cases (bench.CONFIGS / BASELINE.json configs):
+  full_cfg1      cfg1: 1 scene x 4 views, images only
+  full_aux_s3    cfg3-shaped: 1 scene x 3 views, depth + camera aux on every view
+  full_mixed_s5  cfg5-shaped: 1 scene x 5 views, partial depth_gt_index / camera_gt_index
+  full_cfg2      cfg2: 1 scene x 8 views, images only (the reference's DPT heads take all 8 frames in one chunk)
+  full_cfg3      cfg3: 1 scene x 8 views, depth + camera aux on every view
+  full_cfg5      cfg5: 1 scene x 24 views, the sparse index lists of bench.CONFIGS["cfg5"] (3 DPT chunks of 8 frames)
+All at 518 x 518; the index lists of full_cfg2/3/5 are read from bench.CONFIGS so they cannot drift from what bench.py runs.
 
 Weights are oracle/synth.make_state_dict(schema, seed 0) over the reference's own 1 505-key schema (stored as
 tests/golden/full.schema.json, names + shapes only), so the GPU tests rebuild the identical state dict without the
-reference.  Dense outputs are stored on a pixel lattice (every STRIDE-th row / column, fp32): the fixtures stay small
-and the comparison still covers every frame, every output channel and the whole image extent.
+reference.  Dense outputs are stored at the row x column lists of oracle/full_golden.lines (recorded in full_index.json):
+stride 7 from 3 for the first three cases, stride 13 from 6 for full_cfg2 / full_cfg3 and stride 15 from 7 for full_cfg5
+(13 and 15 are coprime to the 14-pixel patch, so every position inside a patch is sampled), each plus the two outermost lines
+per side.  Every fixture stays under 1 MB.
 """
 from __future__ import annotations
 
 import json
 import os
+import resource
 import sys
 import time
 
@@ -26,30 +33,39 @@ from safetensors.torch import save_file
 
 HERE = os.path.dirname(os.path.abspath(__file__))
 sys.path.insert(0, os.path.dirname(HERE))
+from bench import CONFIGS  # noqa: E402
+from oracle.full_golden import GOLDEN, lines, sample  # noqa: E402
 from oracle.ref_shims import import_reference  # noqa: E402
 from oracle.synth import make_inputs, make_state_dict  # noqa: E402
 
-GOLDEN = os.path.join(os.path.dirname(HERE), "tests", "golden")
-STRIDE = 7   # 518 = 74 * 7
+H = W = 518
 
-# name -> (S, depth_gt_index, camera_gt_index, input seed)
+
+def _bench(cfg):
+    c = CONFIGS[cfg]
+    return c["S"], list(c["depth_idx"]), list(c["cam_idx"])
+
+
+# name -> (S, depth_gt_index, camera_gt_index, input seed, stride, offset)
 CASES = {
-    "full_cfg1": (4, [], [], 11),
-    "full_aux_s3": (3, [0, 1, 2], [0, 1, 2], 12),
-    "full_mixed_s5": (5, [0, 3], [0, 2, 4], 13),
+    "full_cfg1": (4, [], [], 11, 7, 3),
+    "full_aux_s3": (3, [0, 1, 2], [0, 1, 2], 12, 7, 3),
+    "full_mixed_s5": (5, [0, 3], [0, 2, 4], 13, 7, 3),
+    "full_cfg2": (*_bench("cfg2"), 14, 13, 6),
+    "full_cfg3": (*_bench("cfg3"), 15, 13, 6),
+    "full_cfg5": (*_bench("cfg5"), 16, 15, 7),       # 24 views: the sparser stride keeps the fixture under 1 MB
 }
 
 
-def lattice(t: torch.Tensor) -> torch.Tensor:
-    """[B,S,H,W,...] -> every STRIDE-th pixel (offset STRIDE // 2)."""
-    o = STRIDE // 2
-    return t[:, :, o::STRIDE, o::STRIDE].contiguous().clone()
+def peak_rss_gb() -> float:
+    return resource.getrusage(resource.RUSAGE_SELF).ru_maxrss / 2**20     # ru_maxrss is in KiB on Linux
 
 
 def main():
     import_reference()
     from omnivggt.models.omnivggt import OmniVGGT as RefOmniVGGT
     torch.set_num_threads(os.cpu_count() or 8)
+    only = set(sys.argv[1:]) or set(CASES)
     t0 = time.time()
     m = RefOmniVGGT().eval()
     schema = {k: list(t.shape) for k, t in m.state_dict().items()}
@@ -59,26 +75,28 @@ def main():
     with open(os.path.join(GOLDEN, "full.schema.json"), "w") as f:
         json.dump({"schema": schema}, f, indent=0, sort_keys=True)
     print(f"reference OmniVGGT built: {len(schema)} tensors, {time.time() - t0:.0f} s", flush=True)
-    index = {}
-    for name, (S, didx, cidx, seed) in CASES.items():
-        inp = make_inputs(1, S, 518, 518, seed=seed)
+    path = os.path.join(GOLDEN, "full_index.json")
+    index = json.load(open(path)) if os.path.exists(path) else {}
+    index = {k: v for k, v in index.items() if k in CASES}
+    for name, (S, didx, cidx, seed, stride, offset) in CASES.items():
+        if name not in only:
+            continue
+        inp = make_inputs(1, S, H, W, seed=seed)
         t0 = time.time()
         with torch.no_grad():
             out = m(images=inp["images"], extrinsics=inp["extrinsics"], intrinsics=inp["intrinsics"], depth=inp["depth"],
                     mask=inp["mask"], depth_gt_index=list(didx), camera_gt_index=list(cidx))
         dt = time.time() - t0
-        store = {"pose_enc": out["pose_enc"].contiguous().clone()}
-        for i, p in enumerate(out["pose_enc_list"]):
-            store[f"pose_enc_list.{i}"] = p.contiguous().clone()
-        for k in ("depth", "depth_conf", "world_points", "world_points_conf"):
-            store[k] = lattice(out[k].float())
+        rows, cols = lines(H, stride, offset), lines(W, stride, offset)
+        store = sample(out, rows, cols)
         save_file(store, os.path.join(GOLDEN, f"{name}.safetensors"))
         stats = {k: [float(v.abs().mean()), float(v.abs().max())] for k, v in store.items() if "list" not in k}
-        index[name] = dict(S=S, H=518, W=518, depth_gt_index=didx, camera_gt_index=cidx, input_seed=seed, weight_seed=0,
-                           stride=STRIDE, cpu_forward_s=round(dt, 1), stats=stats)
-        print(name, f"{dt:.0f} s", stats, flush=True)
-    with open(os.path.join(GOLDEN, "full_index.json"), "w") as f:
-        json.dump(index, f, indent=1, sort_keys=True)
+        index[name] = dict(S=S, H=H, W=W, depth_gt_index=didx, camera_gt_index=cidx, input_seed=seed, weight_seed=0,
+                           stride=stride, offset=offset, rows=rows, cols=cols, cpu_forward_s=round(dt, 1), stats=stats)
+        with open(path, "w") as f:        # after every case, so a long run leaves the finished cases usable
+            json.dump(index, f, indent=1, sort_keys=True)
+        print(name, f"{dt:.0f} s, peak host memory {peak_rss_gb():.1f} GB", stats, flush=True)
+        del out, store
 
 
 if __name__ == "__main__":
