@@ -340,6 +340,34 @@ int ovg_compute_ranking(const void* extrinsics, int in_f64, long long N, long lo
                         long long col_stride, double lambda_t, int normalize, int out_f64, long long k, void* workspace,
                         long long workspace_bytes, long long* ranking, void* dists, void* stream);
 
+/* Similarity alignment (Umeyama 1991, eqs. 40-42, uniform weights) of n corresponding points, and its application to one
+ * view set's predictions, so that overlapping view sets of a long capture can be put into one frame.
+ * ovg_sim3_estimate: src, dst fp32 [n, 3]; keep uint8 [n] or NULL (keep all); a pair with a non-finite coordinate is dropped
+ *     as if its keep byte were 0.  Over the kept pairs: mu_s, mu_d the means, Sigma = (1/n) sum (d - mu_d)(s - mu_s)^T,
+ *     sigma^2 = (1/n) sum |s - mu_s|^2, Sigma = U D V^T by a one-sided Jacobi SVD in fp64 (one thread, cyclic pairs, until a
+ *     sweep rotates nothing), S = diag(1, 1, -1) when det U det V < 0 else I, R = U S V^T, c = tr(D S) / sigma^2,
+ *     t = mu_d - c R mu_s.  out_sim3 fp64 [4, 4] = [[c R, t], [0, 0, 0, 1]] minimises sum |d - (c R s + t)|^2.  out_stats
+ *     fp64 [4] = kept count, status, RMS of |d - (c R s + t)| over the kept pairs (0 when none), c.  Status (out_sim3 is
+ *     then the identity and c = 1): 0 estimated, 1 fewer than 3 kept pairs, 2 sigma^2 == 0, 3 the second singular value is
+ *     not above 1e-12 times the first.  Every sum is fp64 over a fixed grid, then in a fixed order: results are
+ *     bit-identical from run to run.  Five launches, no host synchronisation.  workspace: ovg_sim3_workspace_bytes(n) bytes,
+ *     256-byte aligned.
+ * ovg_sim3_apply: maps views x hw pixels of one view set by sim3 = [[A, t], [0, 1]], with c = sqrt((A00^2 + A10^2) + A20^2)
+ *     and R = A / c.  Every value is evaluated in fp64 from the fp32 input, each product and sum rounded on its own in the
+ *     order written, and rounded to fp32 once:
+ *       points fp32 [views * hw, 3] (points, points2):  p'_r = ((A_r0 x + A_r1 y) + A_r2 z) + t_r
+ *       depth fp32 [views * hw]:                        d' = c d
+ *       world-to-camera extrinsics fp32 [views, 3, 4]:  R'_rj = (E_r0 R_j0 + E_r1 R_j1) + E_r2 R_j2 (R' = R_E R^T),
+ *                                                       t'_r = c E_r3 - ((R'_r0 t_0 + R'_r1 t_1) + R'_r2 t_2), R' unrounded
+ *     so unprojecting d' through (K, [R' | t']) gives p' up to fp32 rounding.  Any input pair may be NULL (skipped); outputs
+ *     may be slices of larger tensors but must not overlap the inputs.  One launch. */
+long long ovg_sim3_workspace_bytes(long long n);
+int ovg_sim3_estimate(const float* src, const float* dst, const unsigned char* keep, long long n, void* workspace,
+                      long long workspace_bytes, double* out_sim3, double* out_stats, void* stream);
+int ovg_sim3_apply(const double* sim3, int views, long long hw, const float* points_in, float* points_out,
+                   const float* points2_in, float* points2_out, const float* depth_in, float* depth_out,
+                   const float* ext_in, float* ext_out, void* stream);
+
 /* Baseline JPEG decoding on the device, bit-identical to Pillow (libjpeg-turbo's default islow IDCT, fancy upsampling and
  * YCbCr -> RGB tables).  The plan is host code (no CUDA call): it parses every file, routes it to the device or to the host
  * (OVG_JPEG_* below: anything the device cannot decode exactly goes to the host), and builds the staging stream (tables plus the

@@ -141,6 +141,9 @@ EXPORTS = {
     "ovg_farthest_point_sample": (C.c_int, [_vp, _i, _ll, _i, _vp, _i, _vp, _ll, _vp, _vp]),
     "ovg_ranking_workspace_bytes": (_ll, [_ll, _i]),
     "ovg_compute_ranking": (C.c_int, [_vp, _i, _ll, _ll, _ll, _ll, C.c_double, _i, _i, _ll, _vp, _ll, _vp, _vp, _vp]),
+    "ovg_sim3_workspace_bytes": (_ll, [_ll]),
+    "ovg_sim3_estimate": (C.c_int, [_vp, _vp, _vp, _ll, _vp, _ll, _vp, _vp, _vp]),
+    "ovg_sim3_apply": (C.c_int, [_vp, _i, _ll, _vp, _vp, _vp, _vp, _vp, _vp, _vp, _vp, _vp]),
     "ovg_jpeg_plan_create": (C.c_int, [_pp, C.POINTER(_ll), _i, _i, _pp]),
     "ovg_jpeg_plan_destroy": (None, [_vp]),
     "ovg_jpeg_plan_file": (C.c_int, [_vp, _i, C.POINTER(_i), C.POINTER(_i), C.POINTER(_i), C.POINTER(_i)]),

@@ -19,6 +19,7 @@
 #include "sky.cuh"
 #include "fps.cuh"
 #include "rank.cuh"
+#include "sim3.cuh"
 #include "tail.cuh"
 #include "pre.cuh"
 #include "jpeg.cuh"
@@ -1300,6 +1301,73 @@ int ovg_compute_ranking(const void* extrinsics, int in_f64, long long N, long lo
   const int rc = post_launch("ovg_compute_ranking(prep)");
   if (rc) return rc;
   return p.out_f64 ? launch_ranking<double, unsigned long long>(p, st) : launch_ranking<float, unsigned>(p, st);
+}
+
+}  // extern "C"
+
+// ------------------------------------------------------------------------------------------------------ Sim(3) alignment
+namespace {
+
+// Sim(3) workspace, carved the same way by the size query and by the entry point: the partials of the three passes and the
+// solved transform.  Its size does not depend on n.
+ovg::Sim3Params sim3_workspace(void* base, long long* bytes) {
+  Arena ar(base, 0);
+  ovg::Sim3Params p{};
+  p.part0 = ar.get<double>(ovg::SIM3_BLOCKS * ovg::SIM3_P0);
+  p.part1 = ar.get<double>(ovg::SIM3_BLOCKS * ovg::SIM3_P1);
+  p.part2 = ar.get<double>(ovg::SIM3_BLOCKS);
+  p.solved = ar.get<double>(12);
+  *bytes = ar.bytes();
+  return p;
+}
+
+}  // namespace
+
+extern "C" {
+
+long long ovg_sim3_workspace_bytes(long long n) {
+  if (n < 0) return -1;
+  long long bytes = 0;
+  sim3_workspace(nullptr, &bytes);
+  return bytes;
+}
+
+int ovg_sim3_estimate(const float* src, const float* dst, const unsigned char* keep, long long n, void* workspace,
+                      long long workspace_bytes, double* out_sim3, double* out_stats, void* stream) {
+  OVG_REQUIRE(n >= 0, "n must be >= 0");
+  OVG_REQUIRE((src && dst) || n == 0, "null src / dst");
+  OVG_REQUIRE(out_sim3 && out_stats, "null out_sim3 / out_stats");
+  long long bytes = 0;
+  ovg::Sim3Params p = sim3_workspace(workspace, &bytes);
+  OVG_REQUIRE(workspace_ok(workspace, workspace_bytes, bytes, 256),
+              "workspace must be 256-byte aligned and ovg_sim3_workspace_bytes(n) long");
+  p.src = src; p.dst = dst; p.keep = keep; p.n = n; p.sim3 = out_sim3; p.stats = out_stats;
+  cudaStream_t st = reinterpret_cast<cudaStream_t>(stream);
+  ovg::sim3_means_kernel<<<ovg::SIM3_BLOCKS, ovg::SIM3_THREADS, 0, st>>>(p);
+  int rc = post_launch("ovg_sim3_estimate(means)");
+  if (rc) return rc;
+  ovg::sim3_moments_kernel<<<ovg::SIM3_BLOCKS, ovg::SIM3_THREADS, 0, st>>>(p);
+  if ((rc = post_launch("ovg_sim3_estimate(moments)"))) return rc;
+  ovg::sim3_solve_kernel<<<1, 32, 0, st>>>(p);
+  if ((rc = post_launch("ovg_sim3_estimate(solve)"))) return rc;
+  ovg::sim3_residual_kernel<<<ovg::SIM3_BLOCKS, ovg::SIM3_THREADS, 0, st>>>(p);
+  if ((rc = post_launch("ovg_sim3_estimate(residual)"))) return rc;
+  ovg::sim3_finish_kernel<<<1, 32, 0, st>>>(p);
+  return post_launch("ovg_sim3_estimate(finish)");
+}
+
+int ovg_sim3_apply(const double* sim3, int views, long long hw, const float* points_in, float* points_out,
+                   const float* points2_in, float* points2_out, const float* depth_in, float* depth_out,
+                   const float* ext_in, float* ext_out, void* stream) {
+  OVG_REQUIRE(sim3 && views > 0 && hw > 0, "bad arguments");
+  OVG_REQUIRE(!points_in == !points_out && !points2_in == !points2_out && !depth_in == !depth_out && !ext_in == !ext_out,
+              "each input needs its output and each output its input");
+  ovg::Sim3ApplyParams p{sim3, {points_in, points2_in}, {points_out, points2_out}, depth_in, depth_out, ext_in, ext_out,
+                         static_cast<long long>(views) * hw, views};
+  long long blocks = (p.n_pix + 255) / 256;
+  if (blocks > num_sms() * 8LL) blocks = num_sms() * 8LL;          // grid-stride inside
+  ovg::sim3_apply_kernel<<<static_cast<int>(blocks), 256, 0, reinterpret_cast<cudaStream_t>(stream)>>>(p);
+  return post_launch("ovg_sim3_apply");
 }
 
 }  // extern "C"

@@ -2,8 +2,10 @@
 omnivggt/utils/geometry.py:435-451 find_reciprocal_matches), triangle meshes (libovg ovg_mesh_*, the reference's
 omnivggt/viz.py:40-89 pts3d_to_trimesh and cat_meshes), model-free sky segmentation (libovg ovg_segment_sky, the
 reference's omnivggt/viz.py:357-393 segment_sky), farthest point sampling (libovg ovg_farthest_point_sample, the
-reference's omnivggt/utils/po_utils/misc.py:114-148 farthest_point_sample) and the ranking of views by camera distance
-(libovg ovg_compute_ranking, the reference's omnivggt/datasets/utils/image_ranking.py:118-140 compute_ranking)."""
+reference's omnivggt/utils/po_utils/misc.py:114-148 farthest_point_sample), the ranking of views by camera distance
+(libovg ovg_compute_ranking, the reference's omnivggt/datasets/utils/image_ranking.py:118-140 compute_ranking) and the
+similarity alignment of corresponding points (libovg ovg_sim3_estimate, Umeyama's method as the reference's
+omnivggt/utils/vo_eval.py:190-233 reaches it through evo)."""
 from __future__ import annotations
 
 import numpy as np
@@ -192,6 +194,36 @@ def compute_ranking(extrinsics, lambda_t: float = 1.0, normalize: bool = True, b
     if N == 0:
         return torch.zeros(0, 0, device=dev, dtype=torch.int64), torch.zeros(0, 0, device=dev, dtype=out)
     return ops.compute_ranking(_to(extrinsics, dev), lam, normalize, out, int(k))
+
+
+SIM3_STATUS = {1: "fewer than 3 kept pairs", 2: "the source points all coincide (sigma^2 == 0)",
+               3: "the points are collinear or coincide (second singular value <= 1e-12 x the first)"}
+
+
+def align_sim3(src, dst, keep=None):
+    """The similarity transform that best maps src onto dst: fp64 [4, 4] [[c R, t], [0, 1]] on the device, minimising
+    sum |dst - (c R src + t)|^2 over the kept pairs (Umeyama 1991, eqs. 40-42; what evo's umeyama_alignment computes with
+    correct_scale, and what the reference's vo_eval reaches through align=True, correct_scale=True).
+
+    src, dst [N, 3]: CUDA tensors, or arrays (moved to the current CUDA device), used as fp32.  keep [N] (bool or integer,
+    non-zero = kept) or None.  Pairs with a non-finite coordinate are dropped.  Aligns predicted point maps to ground truth,
+    or a predicted trajectory of camera centres to a reference one (the ATE alignment).  Raises ValueError when fewer than 3
+    pairs are kept or the kept points are coincident or collinear; reading that status is the call's one host read."""
+    _check_shape(src, "src")
+    _check_shape(dst, "dst")
+    n = (src.shape if hasattr(src, "shape") else np.shape(src))[0]
+    if (dst.shape if hasattr(dst, "shape") else np.shape(dst))[0] != n:
+        raise ValueError("src and dst must have the same number of points")
+    if keep is not None and tuple(keep.shape if hasattr(keep, "shape") else np.shape(keep)) != (n,):
+        raise ValueError(f"keep must have shape [{n}]")
+    dev = _device_of(src, dst, keep)
+    s, d = (_to(p, dev).to(torch.float32).contiguous() for p in (src, dst))
+    k = None if keep is None else (_to(keep, dev) != 0).to(torch.uint8).contiguous()
+    sim3, stats = ops.sim3_estimate(s, d, k)
+    status = int(ops.host_read(stats[1]))
+    if status:
+        raise ValueError(f"align_sim3: degenerate input: {SIM3_STATUS[status]}")
+    return sim3
 
 
 def cat_meshes(meshes):

@@ -35,6 +35,21 @@ _HEADS = ("camera_head", "depth_head", "point_head")
 _DPT_HEADS = (("depth_head", 0), ("point_head", 1))          # name, head_act (exp / inverse-log)
 
 
+def chunk_schedule(S: int, chunk: int, overlap: int) -> List[Tuple[int, int]]:
+    """The view sets (start, end) of OmniVGGT.reconstruct over S views: one set when S <= chunk; else starts 0, step,
+    2 step, ... (step = chunk - overlap) while start + chunk < S, then a last set at S - chunk.  Every set has chunk views
+    and shares at least overlap views with the views before it."""
+    if S <= chunk:
+        return [(0, S)]
+    out = [(a, a + chunk) for a in range(0, S - chunk, chunk - overlap)]
+    return out + [(S - chunk, S)]
+
+
+def chunk_index(idx: Optional[Sequence[int]], start: int, end: int) -> List[int]:
+    """A view set's members of a list of global view indices, as indices into the set."""
+    return [int(i) - start for i in (idx or []) if start <= int(i) < end]
+
+
 class OmniVGGT(nn.Module, PyTorchModelHubMixin):
     def __init__(self, img_size: int = 518, patch_size: int = 14, embed_dim: int = 1024, *, depth: int = 24,
                  patch_embed: str = "dinov2_vitl14_reg", dino_depth: int = 24, dino_heads: int = 16,
@@ -555,6 +570,118 @@ class OmniVGGT(nn.Module, PyTorchModelHubMixin):
         faces, face_colors = mesher.faces(n_ref)
         return {"vertices": points.view(-1, 3).clone(), "face_colors": face_colors, "faces": faces, "conf_threshold": thr,
                 "align": align}
+
+    # ---------------------------------------------------------------------------------------------- long captures
+    @torch.no_grad()
+    def reconstruct(self, images: torch.Tensor, extrinsics: torch.Tensor = None, intrinsics: torch.Tensor = None,
+                    depth: torch.Tensor = None, mask: torch.Tensor = None, depth_gt_index: list = None,
+                    camera_gt_index: list = None, *, chunk: int = 24, overlap: int = 8, source: str = "depth",
+                    conf_percent: float = 50.0) -> Dict[str, object]:
+        """One scene longer than one forward, as overlapping view sets merged into the frame and scale of the first.
+
+        Views are taken in the given order (permute them first for an unordered collection, e.g. by
+        ``geometry.compute_ranking``).  The view sets are ``chunk_schedule(S, chunk, overlap)``: each has ``chunk`` views (so
+        every forward replays one CUDA graph) and shares at least ``overlap`` views with the views before it.
+        ``depth_gt_index`` / ``camera_gt_index`` hold global view indices; each view set gets its members, re-indexed.
+
+        Per view set: the forward on its views, then the cameras decoded and the depth unprojected as ``postprocess`` does.
+        The first set is kept as it is.  Each later set is aligned by the similarity (libovg ovg_sim3_estimate) that maps its
+        points of the views it shares with the merge onto the merged points of those views, over the pixels kept on both
+        sides by point_cloud's rule (conf >= percentile(conf over those views, conf_percent) and conf > 1e-5), with
+        ``source`` selecting the points as in ``point_cloud``.  Its new views are then mapped into the merge (libovg
+        ovg_sim3_apply: points, depth and extrinsics in fp64, rounded once; intrinsics and confidences copied).  A view kept
+        by several sets keeps the outputs of the first.  Only one set's raw outputs are held at a time.
+
+        Returns a dict with B = 1 that ``point_cloud``, ``mesh``, ``matches`` and ``sky_mask`` take as it is: ``images``,
+        ``extrinsic``, ``intrinsic``, ``depth``, ``depth_conf``, ``world_points_from_depth`` and, with the point head,
+        ``world_points`` / ``world_points_conf``; ``chunks`` [(start, end)]; ``sim3`` fp64 [n_chunks, 4, 4] mapping each set
+        into the first set's frame; ``align_pairs`` and ``align_rmse`` fp64 [n_chunks] (0 for the first set).  ``pose_enc``
+        is not returned: it is normalised per view set.  The alignment statistics are read once per set boundary, and a
+        degenerate overlap raises ValueError naming the set and its views.  Errors accumulate along the chain of sets (no
+        loop closure)."""
+        from . import ops
+        if self._cp is not None:
+            raise RuntimeError("reconstruct runs its view sets on one GPU; under enable_context_parallel() call the model itself")
+        if images.dim() == 4:
+            images = images.unsqueeze(0)
+        if images.dim() != 5 or images.shape[0] != 1:
+            raise ValueError(f"reconstruct takes one scene (B = 1), got images of shape {tuple(images.shape)}")
+        for name, v in (("chunk", chunk), ("overlap", overlap)):
+            if isinstance(v, (bool, np.bool_)) or not isinstance(v, (int, np.integer)):
+                raise ValueError(f"{name} must be an integer, got {v!r}")
+        if chunk < 2:
+            raise ValueError(f"chunk must be >= 2, got {chunk}")
+        if not 1 <= overlap < chunk:
+            raise ValueError(f"overlap must be in [1, chunk - 1 = {chunk - 1}], got {overlap}")
+        if source not in ("depth", "pointmap"):
+            raise ValueError(f"source must be 'depth' or 'pointmap', got {source!r}")
+        if source == "pointmap" and self.point_head is None:
+            raise ValueError("source='pointmap' needs the point head (it is set to None)")
+        if self.camera_head is None or self.depth_head is None:
+            raise ValueError("reconstruct needs the camera head and the depth head")
+        if not 0.0 <= conf_percent <= 100.0:
+            raise ValueError("conf_percent must be in [0, 100]")
+        S, H, W = images.shape[1], images.shape[-2], images.shape[-1]
+        for name, idx in (("depth_gt_index", depth_gt_index), ("camera_gt_index", camera_gt_index)):
+            if any(not 0 <= int(i) < S for i in (idx or [])):
+                raise IndexError(f"{name} {list(idx)} out of range for {S} views")
+        chunks = chunk_schedule(S, chunk, overlap)
+        merged: Dict[str, torch.Tensor] = {}
+        sims, stats_all = [], []
+        for k, (a, b) in enumerate(chunks):
+            di, ci = chunk_index(depth_gt_index, a, b), chunk_index(camera_gt_index, a, b)
+            part = (lambda t: None if t is None else t[:, a:b])
+            raw = self(images[:, a:b], part(extrinsics), part(intrinsics), part(depth), part(mask), depth_gt_index=di,
+                       camera_gt_index=ci)
+            n = b - a
+            ext, intr, c2w = ops.pose_decode(raw["pose_enc"][0].float().contiguous(), H, W)
+            r = {"extrinsic": ext, "intrinsic": intr, "depth": raw["depth"][0], "depth_conf": raw["depth_conf"][0],
+                 "world_points_from_depth": ops.unproject_depth(raw["depth"][0].float().reshape(n, H, W), intr, c2w, H, W)}
+            if "world_points" in raw:
+                r["world_points"], r["world_points_conf"] = raw["world_points"][0], raw["world_points_conf"][0]
+            del raw
+            if k == 0:
+                dev = ext.device
+                merged = {key: torch.empty((1, S) + tuple(v.shape[1:]), device=dev, dtype=torch.float32) for key, v in r.items()}
+                for key, v in r.items():
+                    merged[key][0, :n].copy_(v)
+                sims.append(torch.eye(4, device=dev, dtype=torch.float64))
+                stats_all.append(torch.zeros(4, device=dev, dtype=torch.float64))
+                continue
+            sim3, stats = self._merge_view_set(merged, r, k, a, chunks[k - 1][1], b, source, conf_percent)
+            sims.append(sim3)
+            stats_all.append(stats)
+        stats = torch.stack(stats_all)
+        merged.update(images=images, chunks=chunks, sim3=torch.stack(sims), align_pairs=stats[:, 0].clone(),
+                      align_rmse=stats[:, 2].clone())
+        return merged
+
+    @staticmethod
+    def _merge_view_set(merged: Dict[str, torch.Tensor], r: Dict[str, torch.Tensor], k: int, a: int, n0: int, b: int,
+                        source: str, conf_percent: float):
+        """Aligns view set k (views a..b-1, outputs r in its own frame) on its views a..n0-1 that are merged already and
+        writes its views n0..b-1 into the merged tensors.  Returns (sim3, stats) on the device; the status is read here."""
+        from . import geometry, ops
+        pkey, ckey = ("world_points_from_depth", "depth_conf") if source == "depth" else ("world_points", "world_points_conf")
+        m_src, _, _ = ops.conf_percentile_mask(r[ckey][:n0 - a].contiguous(), conf_percent, 1e-5)
+        m_dst, _, _ = ops.conf_percentile_mask(merged[ckey][0, a:n0].contiguous(), conf_percent, 1e-5)
+        sim3, stats = ops.sim3_estimate(r[pkey][:n0 - a].reshape(-1, 3), merged[pkey][0, a:n0].reshape(-1, 3),
+                                        (m_src & m_dst).view(-1))
+        status = int(ops.host_read(stats)[1])
+        if status:
+            raise ValueError(f"view set {k} (views {a}..{b - 1}) cannot be aligned on its shared views {a}..{n0 - 1}: "
+                             f"{geometry.SIM3_STATUS[status]}")
+        new = slice(n0 - a, b - a)
+        H, W = r["depth"].shape[1:3]
+        ops.sim3_apply(sim3, b - n0, H * W,
+                       points=[(r[key][new], merged[key][0, n0:b]) for key in ("world_points_from_depth", "world_points")
+                               if key in r],
+                       depth=(r["depth"][new], merged["depth"][0, n0:b]),
+                       ext=(r["extrinsic"][new], merged["extrinsic"][0, n0:b]))
+        for key in ("intrinsic", "depth_conf", "world_points_conf"):
+            if key in r:
+                merged[key][0, n0:b].copy_(r[key][new])
+        return sim3, stats
 
     # ---------------------------------------------------------------------------------------------- CUDA graph replay
     def _forward_graphed(self, eng, impl, images, extrinsics, intrinsics, depth, mask, depth_idx, cam_idx):

@@ -327,6 +327,45 @@ def compute_ranking(ext: torch.Tensor, lambda_t: float, normalize: bool, out_dty
     return ranking, dists
 
 
+def sim3_estimate(src: torch.Tensor, dst: torch.Tensor, keep: Optional[torch.Tensor] = None):
+    """Umeyama similarity (ovg_sim3_estimate) mapping src onto dst: fp32 [n, 3] contiguous on the device, keep uint8 [n] or
+    None.  Returns (sim3 fp64 [4, 4], stats fp64 [4] = kept count, status, RMS residual, c): five launches, no host read."""
+    _chk(src, F32, "src")
+    _chk(dst, F32, "dst")
+    assert src.dim() == 2 and src.shape[1] == 3 and src.shape == dst.shape and src.is_contiguous() and dst.is_contiguous()
+    n = src.shape[0]
+    if keep is not None:
+        _chk(keep, torch.uint8, "keep")
+        assert keep.is_contiguous() and keep.numel() == n
+    lib = L.lib()
+    ws = torch.empty(lib.ovg_sim3_workspace_bytes(n), device=src.device, dtype=torch.uint8)
+    sim3 = torch.empty(4, 4, device=src.device, dtype=torch.float64)
+    stats = torch.empty(4, device=src.device, dtype=torch.float64)
+    L.check(lib.ovg_sim3_estimate(src.data_ptr(), dst.data_ptr(), L.ptr(keep), n, ws.data_ptr(), ws.numel(), sim3.data_ptr(),
+                                  stats.data_ptr(), L.stream()))
+    return sim3, stats
+
+
+def sim3_apply(sim3: torch.Tensor, views: int, hw: int, points=(), depth=None, ext=None) -> None:
+    """ovg_sim3_apply: points = up to two (in, out) pairs of fp32 [views * hw, 3], depth = (in, out) fp32 [views * hw],
+    ext = (in, out) fp32 [views, 3, 4] world-to-camera; every tensor contiguous on the device, the outputs typically slices of
+    merged tensors.  sim3 fp64 [4, 4] on the device.  One launch."""
+    _chk(sim3, torch.float64, "sim3")
+    assert sim3.shape == (4, 4) and sim3.is_contiguous() and len(points) <= 2
+    pairs = list(points) + [None] * (2 - len(points))
+    sizes = [views * hw * 3] * 2 + [views * hw, views * 12]
+    flat = []
+    for pair, size in zip(pairs + [depth, ext], sizes):
+        if pair is None:
+            flat += [None, None]
+            continue
+        for t in pair:
+            _chk(t, F32, "sim3_apply operand")
+            assert t.is_contiguous() and t.numel() == size, (tuple(t.shape), size)
+        flat += [pair[0].data_ptr(), pair[1].data_ptr()]
+    L.check(L.lib().ovg_sim3_apply(sim3.data_ptr(), views, hw, *flat, L.stream()))
+
+
 def host_read(t: torch.Tensor) -> torch.Tensor:
     """The device-to-host read of a matching or mesh call (its one synchronisation)."""
     return t.cpu()
