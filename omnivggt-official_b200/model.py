@@ -176,6 +176,11 @@ class OmniVGGT(nn.Module, PyTorchModelHubMixin):
             raise ValueError(f"Expected 3 input channels, got {Cin}")                 # omnivggt_aggregator.py:139-140
         assert H % self.patch_size == 0, f"Input image height {H} is not a multiple of patch height {self.patch_size}"
         assert W % self.patch_size == 0, f"Input image width {W} is not a multiple of patch width: {self.patch_size}"
+        # The fused RoPE epilogue holds 64 positions per axis (patch rows / columns + 1), so 63 patches = 882 px per side.
+        # Refused here, before the DINOv2 patchifier or any other kernel runs, for every entry point that reaches the aggregator.
+        limit = 63 * self.patch_size
+        if max(H, W) > limit:
+            raise ValueError(f"{H}x{W} input: at most {limit} px per side (the fused RoPE epilogue holds 64 positions per axis)")
         depth_idx = list(depth_gt_index) if depth_gt_index is not None else []
         cam_idx = list(camera_gt_index) if camera_gt_index is not None else []
         if len(depth_idx):

@@ -260,7 +260,20 @@ def head_post(h, eh, w2, b2, head_act: int, epi_c: float = 34.0):
 # ----------------------------------------------------------------------------------------------- attention
 def attention_ref(q, k, v):
     """softmax_j(q . k_j) v_j with q in log2 units (pre-scaled by log2(e)/sqrt(64)); q [B,H,nq,64], k, v [B,H,nkv,64].
-    Returns (out fp64 [B, nq, H*64], bound fp64 [B, nq, H*64])."""
+    Returns (out fp64 [B, nq, H*64], bound fp64 [B, nq, H*64]).  One (batch, head) at a time: the fp64 scores of a 10 410-token
+    global attention take 0.9 GB per head, so all 16 heads at once would need about 14 GB before temporaries."""
+    B, H, nq, D = q.shape
+    out = torch.empty(B, nq, H, D, dtype=F64, device=q.device)
+    bound = torch.empty_like(out)
+    for b in range(B):
+        for h in range(H):
+            o, e = _attention_ref_slice(q[b:b + 1, h:h + 1], k[b:b + 1, h:h + 1], v[b:b + 1, h:h + 1])
+            out[b, :, h], bound[b, :, h] = o[0], e[0]
+    return out.view(B, nq, H * D), bound.view(B, nq, H * D)
+
+
+def _attention_ref_slice(q, k, v):
+    """attention_ref of q, k, v [B, H, n, 64] in one piece."""
     q, k, v = q.to(F64), k.to(F64), v.to(F64)
     B, H, nq, D = q.shape
     nkv = k.shape[2]

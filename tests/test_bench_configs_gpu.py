@@ -1,8 +1,9 @@
 """The configurations bench.py times, against the unmodified reference's outputs (tests/golden/full_cfg2/3/5, checked by
 oracle/full_golden.py per view, per border line and per output).
 
-bench.py times CUDA-graph replays, so for cfg2, cfg3 and cfg5 the replay (third call of a signature) must equal the eager
-forward bit for bit and pass the same bars.  cfg4 runs several scenes per forward call: the full_cfg2 inputs as scene 3 of a
+bench.py times CUDA-graph replays, so for cfg2, cfg3 and cfg5, and for the 392 x 518 and 882 x 518 inputs of
+full_land_s10 and full_tall_s3, the replay (third call of a signature) must equal the eager forward bit for bit and pass the
+same bars.  cfg4 runs several scenes per forward call: the full_cfg2 inputs as scene 3 of a
 B = 4 call must give what the reference gives for them alone."""
 import pytest
 import torch
@@ -18,7 +19,7 @@ def _inputs(meta, B=1, seed=None):
     return make_inputs(B, meta["S"], meta["H"], meta["W"], seed=meta["input_seed"] if seed is None else seed)
 
 
-@pytest.mark.parametrize("case", ["full_cfg2", "full_cfg3", "full_cfg5"])
+@pytest.mark.parametrize("case", ["full_cfg2", "full_cfg3", "full_cfg5", "full_land_s10", "full_tall_s3"])
 def test_full_size_graph_replay_matches_eager_and_reference(case):
     meta = FULL_INDEX[case]
     m = full_model()

@@ -17,7 +17,7 @@ CASES = sorted(INDEX)
 BENCH_CASES = {"full_cfg1": "cfg1", "full_cfg2": "cfg2", "full_cfg3": "cfg3", "full_cfg5": "cfg5"}
 # Worst rel-L2 of an output over one view or border line, over all full-size cases on the H100 with the fp16 heads
 # (DESIGN.md §2).
-MEASURED_REL = 7.6e-3
+MEASURED_REL = 7.7e-3
 
 
 def noisy(ref, case):
@@ -118,11 +118,17 @@ def test_fixture_layout(case):
     assert meta["cpu_forward_s"] > 0
 
 
-@pytest.mark.parametrize("name", ["full_cfg2", "full_cfg3", "full_cfg5"])
+@pytest.mark.parametrize("name", ["full_cfg2", "full_cfg3", "full_cfg5", "full_land_s10", "full_wide_s5", "full_tall_s3"])
 def test_new_cases_cover_every_position_in_a_patch(name):
     meta = INDEX[name]
-    for ln in (meta["rows"], meta["cols"]):
-        assert {x % PATCH for x in ln if 1 < x < meta["H"] - 2} == set(range(PATCH))
+    for ln, n in ((meta["rows"], meta["H"]), (meta["cols"], meta["W"])):
+        assert {x % PATCH for x in ln if 1 < x < n - 2} == set(range(PATCH))
+
+
+@pytest.mark.parametrize("name,H,W", [("full_land_s10", 392, 518), ("full_wide_s5", 294, 518), ("full_tall_s3", 882, 518)])
+def test_non_square_cases_are_the_loader_shapes(name, H, W):
+    """4:3 and 16:9 photos and the tallest input the engine accepts, as the loaders produce them (width 518, height scaled)."""
+    assert (INDEX[name]["H"], INDEX[name]["W"]) == (H, W)
 
 
 def test_sample_takes_the_listed_rows_and_columns():

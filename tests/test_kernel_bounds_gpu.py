@@ -281,9 +281,23 @@ def _positions(M, T, nspecial, wp):
     return torch.where((t >= nspecial)[:, None], pos, torch.zeros_like(pos))
 
 
-@pytest.mark.parametrize("C,frames,hp,wp,bn", [(128, 3, 4, 4, 0), (1024, 2, 37, 37, 0), (1024, 2, 29, 30, 512), (256, 4, 3, 5, 0)])
+def _rope_recipe(maxpos):
+    """The reference's RoPE frequency tables (layers/rope.py:103-114: fp32 angles position x 100^-(2i/32), then cos and sin),
+    computed on the CPU; the halves the reference concatenates are equal, so one half [maxpos, 16] is kept."""
+    exponents = torch.arange(0, 32, 2).float() / 32
+    inv_freq = 1.0 / (100.0 ** exponents)
+    angles = torch.einsum("i,j->ij", torch.arange(maxpos, dtype=inv_freq.dtype), inv_freq)
+    return angles, angles.cos(), angles.sin()
+
+
+# (37, 37) and (29, 30): square and near-square 518-pixel grids; 28 x 37, 21 x 37 and 63 x 37: the 392-, 294- and 882-pixel-high
+# inputs of a 518-pixel width, the last one reading row 63, the last of the 64 table rows the engine's RoPE holds.
+@pytest.mark.parametrize("C,frames,hp,wp,bn", [(128, 3, 4, 4, 0), (1024, 2, 37, 37, 0), (1024, 2, 29, 30, 512), (256, 4, 3, 5, 0),
+                                               (1024, 2, 28, 37, 0), (1024, 2, 21, 37, 0), (1024, 1, 63, 37, 0)])
 def test_gemm_qkv_norm_rope_per_element(C, frames, hp, wp, bn):
-    """EPI_QKV with LayerNorm(64) on q / k and 2-D RoPE, frame-wise sequences."""
+    """EPI_QKV with LayerNorm(64) on q / k and 2-D RoPE, frame-wise sequences.  The device's RoPE tables, which the fp64
+    reference takes as given, are first checked against the reference's recipe on the CPU: within 4 fp32 ulps of the angle (the
+    device's pow, reciprocal and product may each round differently) plus 4 of the value (cosf / sinf)."""
     ops = _ops()
     heads, T = C // 64, hp * wp + 5
     M = frames * T
@@ -291,7 +305,15 @@ def test_gemm_qkv_norm_rope_per_element(C, frames, hp, wp, bn):
     w = _randn(3 * C, C, scale=C ** -0.5, seed=2, dtype=BF16)
     bias = _randn(3 * C, scale=0.1, seed=3)
     ln = [1 + 0.1 * _randn(64, seed=4), 0.1 * _randn(64, seed=5), 1 + 0.1 * _randn(64, seed=6), 0.1 * _randn(64, seed=7)]
-    cos, sin = ops.rope_tables(max(hp, wp) + 1, "cuda")
+    maxpos = max(hp, wp) + 1
+    assert maxpos <= 64
+    cos, sin = ops.rope_tables(maxpos, "cuda")
+    angles, rcos, rsin = _rope_recipe(maxpos)
+    assert cos.shape == sin.shape == (maxpos, 16) and cos.dtype == sin.dtype == F32
+    for name, got, ref in (("cos", cos, rcos), ("sin", sin, rsin)):
+        bound = 4 * R.ulp(angles, F32) + 4 * R.ulp(ref, F32)
+        r = R.check_bound(got, ref.double(), bound, f"RoPE {name} table, {maxpos} positions", ("position", "frequency"))
+        _margin(f"RoPE {name} table {maxpos} positions", r)
     q, k, v = (torch.zeros(frames, heads, T, 64, device="cuda", dtype=BF16) for _ in range(3))
     ops.qkv_proj(a, w, bias, *ln, q, k, v, ntok=T, T=T, nspecial=5, wp=wp, rope_cos=cos, rope_sin=sin, block_n=bn)
     qscale = float(torch.tensor((1.0 / math.sqrt(64.0)) * math.log2(math.e), dtype=F32))
@@ -336,6 +358,9 @@ def _attn_shape(path, sms):
         return 2, 3, 300, 1374, False
     if path == "cross_persistent":
         return 4, 16, 700, 1374, False
+    if path in REAL_SHAPES:
+        B, H, n = REAL_SHAPES[path]
+        return B, H, n, n, True
     parts = int(path[-1])
     n = 24 * 128 + 37                                   # 25 KV tiles (>= 24: split allowed), ragged last tile
     for h in range(1, 400):
@@ -345,6 +370,11 @@ def _attn_shape(path, sms):
 
 
 PATHS = ["plain", "persistent", "split2", "split3", "split4", "cross_plain", "cross_persistent"]
+# (batch, heads, tokens) as the model launches attention for 294-, 392- and 882-pixel-high inputs of a 518-pixel width with 5, 10
+# and 3 views: frame attention over each view's T = hp * wp + 5 tokens, global attention over a scene's S * T.  They leave ragged
+# last tiles other than the 518 x 518 ones, and whichever path this device's launch rule picks for them is the one tested.
+REAL_SHAPES = {"frame 294x518": (5, 16, 782), "global 294x518": (1, 16, 3910), "frame 392x518": (10, 16, 1041),
+               "global 392x518": (1, 16, 10410), "frame 882x518": (3, 16, 2336), "global 882x518": (1, 16, 7008)}
 
 
 def _run_attention(q, k, v, B, H, nq, nkv, scratch):
@@ -368,8 +398,9 @@ def _run_attention(q, k, v, B, H, nq, nkv, scratch):
 
 def _check_path(path, sms, B, H, nq, nkv, scratch, launches, written):
     kind, parts = R.attention_path(B, H, nq, nkv, sms, scratch)
-    assert kind == {"plain": "plain", "persistent": "persistent", "cross_plain": "plain", "cross_persistent": "persistent"}.get(
-        path, "split")
+    if path not in REAL_SHAPES:
+        assert kind == {"plain": "plain", "persistent": "persistent", "cross_plain": "plain", "cross_persistent": "persistent"}.get(
+            path, "split")
     assert launches == (2 if kind == "split" else 1), launches
     if kind == "split":      # exactly the partial results of `parts` KV ranges per tail tile were written
         assert written == R.split_scratch_bytes(B, H, nq, sms, parts), (written, parts)
@@ -401,14 +432,15 @@ def test_attention_rounding_rows(path, sms):
     _margin(f"attention rounding rows {path}", r)
 
 
-@pytest.mark.parametrize("n", [1, 33, 127, 128, 129, 1374, 9000])
+@pytest.mark.parametrize("n", [1, 33, 127, 128, 129, 1374, 9000] + sorted(n for *_, n in REAL_SHAPES.values()))
 def test_attention_uniform_rows_exact(n, sms):
     """Every probability exactly 1: out = the column mean of v, bit for bit (a key the mask should drop would take nearly all the
-    weight).  9000 keys with scratch also run the split path where this device's cost rule splits them."""
-    B, H = 1, 2
+    weight).  9000 keys with scratch also run the split path where this device's cost rule splits them.  The frame and global
+    lengths of the non-square inputs (REAL_SHAPES) run at the model's batch and 16 heads."""
+    B, H = next(((b, h) for b, h, m in REAL_SHAPES.values() if m == n), (1, 2))
     q, k, v, exp = R.uniform_case(B, H, n, seed=n)
     out, launches, _ = _run_attention(q, k, v, B, H, n, n, True)
-    print(f"uniform n={n}: {R.attention_path(B, H, n, n, sms, True)}, {launches} launch(es)")
+    print(f"uniform B={B} H={H} n={n}: {R.attention_path(B, H, n, n, sms, True)}, {launches} launch(es)")
     bad = (out.cpu() != exp).any(-1).nonzero()
     assert bad.numel() == 0, f"{bad.shape[0]} rows differ, first (batch, row) {tuple(bad[0].tolist())}"
 
@@ -429,10 +461,10 @@ def _rand_attn(B, H, nq, nkv, kind, seed):
 
 
 @pytest.mark.parametrize("kind", ["random", "peaky", "spike"])
-@pytest.mark.parametrize("path", PATHS)
+@pytest.mark.parametrize("path", PATHS + list(REAL_SHAPES))
 def test_attention_per_element(path, kind, sms):
-    """Random, peaky and late-spike inputs within the per-element bound on every path; the split result agrees with the unsplit
-    one within the bound, and repeated runs are bit-identical."""
+    """Random, peaky and late-spike inputs within the per-element bound on every path and at the frame and global shapes of
+    the non-square inputs; the split result agrees with the unsplit one within the bound, and repeated runs are bit-identical."""
     B, H, nq, nkv, scratch = _attn_shape(path, sms)
     q, k, v = _rand_attn(B, H, nq, nkv, kind, seed=3)
     out, launches, written = _run_attention(q, k, v, B, H, nq, nkv, scratch)

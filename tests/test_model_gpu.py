@@ -227,11 +227,13 @@ def set_heads(m, dpt_dtype):
         m._invalidate()
 
 
-@pytest.mark.parametrize("case,dpt_dtype", [(c, "fp16") for c in sorted(FULL_INDEX)] + [("full_cfg1", "bf16"), ("full_cfg2", "bf16")])
+@pytest.mark.parametrize("case,dpt_dtype", [(c, "fp16") for c in sorted(FULL_INDEX)]
+                         + [("full_cfg1", "bf16"), ("full_cfg2", "bf16"), ("full_land_s10", "bf16")])
 def test_full_size_matches_reference_golden(case, dpt_dtype):
-    """bench.py's cfg1, cfg2, cfg3 and cfg5 (4, 8, 8 and 24 views) and aux-shaped siblings: the full model on the CUDA path
-    against outputs of the UNMODIFIED reference forward (omnivggt/models/omnivggt.py:20-68, CPU fp32; generated by
-    oracle/make_golden_full.py).  Dense outputs are compared at the stored row and column lists, image borders included."""
+    """bench.py's cfg1, cfg2, cfg3 and cfg5 (4, 8, 8 and 24 views), aux-shaped siblings and the non-square inputs the loaders
+    produce (392 x 518, 294 x 518 and 882 x 518, the largest accepted): the full model on the CUDA path against outputs of the
+    UNMODIFIED reference forward (omnivggt/models/omnivggt.py:20-68, CPU fp32; generated by oracle/make_golden_full.py).
+    Dense outputs are compared at the stored row and column lists, image borders included."""
     meta = FULL_INDEX[case]
     m = full_model()
     set_heads(m, dpt_dtype)
@@ -239,6 +241,60 @@ def test_full_size_matches_reference_golden(case, dpt_dtype):
     out = m(depth_gt_index=meta["depth_gt_index"], camera_gt_index=meta["camera_gt_index"], **inp)
     torch.cuda.synchronize()
     full_size_check(case, out, f"heads={dpt_dtype}")
+
+
+SIZE_SEQUENCE = ["full_cfg1", "full_tall_s3", "full_wide_s5", "full_land_s10", "full_cfg1"]
+
+
+@pytest.mark.parametrize("graphs", [False, True], ids=["eager", "graphs"])
+def test_full_size_image_size_changes_between_calls(graphs):
+    """One model across image sizes: 518 x 518, 882 x 518, 294 x 518, 392 x 518, then 518 x 518 again.  A larger size regrows
+    the workspaces, and each size adds its RoPE and UV tables.  With CUDA graphs each size runs until its third call, which is
+    captured and replayed; the last 518 x 518 call replays the graph captured before the workspaces grew.  Every call passes
+    the reference bars, and the second 518 x 518 result equals the first bit for bit."""
+    m = full_model()
+    set_heads(m, "fp16")
+    use = m.use_cuda_graph
+    m.use_cuda_graph, m._graphs = graphs, {}
+    first = None
+    try:
+        for i, case in enumerate(SIZE_SEQUENCE):
+            meta = FULL_INDEX[case]
+            inp = {k: v.cuda() for k, v in make_inputs(1, meta["S"], meta["H"], meta["W"], seed=meta["input_seed"]).items()}
+            kw = dict(depth_gt_index=meta["depth_gt_index"], camera_gt_index=meta["camera_gt_index"])
+            for _ in range(3 if graphs and case not in SIZE_SEQUENCE[:i] else 1):
+                out = m(**inp, **kw)
+            torch.cuda.synchronize()
+            if graphs:
+                assert len(m._graphs) == len(set(SIZE_SEQUENCE[:i + 1])), len(m._graphs)
+                assert all(e["graph"] is not None for e in m._graphs.values()), "graph was not captured"
+            full_size_check(case, out, f"heads=fp16 {'graph replay' if graphs else 'eager'}, call {i + 1} of the size sequence")
+            if first is None:
+                first = {k: out[k].clone() for k in KEYS}
+            elif case == SIZE_SEQUENCE[0]:
+                for k in KEYS:
+                    assert torch.equal(out[k], first[k]), k
+    finally:
+        m.use_cuda_graph, m._graphs = use, {}
+        torch.cuda.empty_cache()
+
+
+def test_input_above_882_pixels_is_refused_before_any_kernel():
+    """The fused RoPE epilogue holds 64 positions per axis, so 63 patches = 882 px is the most a side may have (full_tall_s3
+    runs 882).  A 896-pixel side is refused with a ValueError naming the limit before the patchifier or any other libovg
+    kernel runs, by forward, the aggregator component call and reconstruct."""
+    from omnivggt_official_b200 import _lib as L
+    m = full_model()
+    for H, W in ((896, 518), (518, 896)):
+        inp = {k: v.cuda() for k, v in make_inputs(1, 2, H, W, seed=7).items()}
+        torch.cuda.synchronize()
+        n0 = L.lib().ovg_launch_count()
+        for call in (lambda: m(**inp), lambda: m.aggregator(**inp, depth_gt_index=[0], camera_gt_index=[1]),
+                     lambda: m.reconstruct(**inp, chunk=2, overlap=1)):
+            with pytest.raises(ValueError, match=f"{H}x{W} input: at most 882 px per side"):
+                call()
+        torch.cuda.synchronize()
+        assert L.lib().ovg_launch_count() == n0
 
 
 @pytest.mark.parametrize("S,didx,cidx", [(8, list(range(8)), list(range(8))),          # BASELINE.json configs[2]
