@@ -12,17 +12,22 @@ from test_host_cpu import mini_model
 
 
 class _Recorder:
+    """Records every call and its arguments.  Workspace size queries get a positive size, so that every workspace is a real
+    buffer whose pointer can be checked (test_poison_cpu.py); every other call returns 0 (OVG_OK)."""
+
     def __init__(self):
         self.calls = []
+        self.args = []
         self.descs = {}
 
     def __getattr__(self, name):
         def fn(*a):
             self.calls.append(name)
+            self.args.append((name, a))
             if name.endswith("_create"):
                 d = a[0]._obj                       # ctypes.byref(desc)
                 self.descs[name] = type(d).from_buffer_copy(d)
-            return 0
+            return 4096 if name.endswith("_workspace_bytes") else 0
         return fn
 
 

@@ -50,6 +50,26 @@ def model(variant):
     return _MODELS[variant]
 
 
+def reduced_golden_check(case, out, keys=KEYS, log=False):
+    """The outputs ``keys`` of a forward of the reduced golden ``case`` against the reference's: shape, dtype, finiteness and
+    relative L2 under TOL; pose_enc also max-abs 5e-2.  ``log``: print the errors and append them to the parity log first."""
+    ref = load_file(os.path.join(GOLDEN, f"{case}.safetensors"))
+    errs = {k: rel(out[k], ref[k]) for k in keys}
+    if log:
+        print(case, json.dumps(errs))
+        d = os.path.join(os.path.dirname(GOLDEN), os.pardir, "gpurun_out")
+        if os.path.isdir(d):
+            with open(os.path.join(d, "model_parity_mini.txt"), "a") as f:
+                f.write(case + " " + json.dumps({k: round(v, 5) for k, v in errs.items()}) + "\n")
+    for k in keys:
+        assert out[k].shape == ref[k].shape and out[k].dtype == torch.float32 and out[k].is_cuda
+        assert torch.isfinite(out[k]).all(), k
+        assert errs[k] < TOL, (k, errs)
+    if "pose_enc" in keys:
+        assert (out["pose_enc"].cpu() - ref["pose_enc"]).abs().max() < 5e-2
+    return errs
+
+
 @pytest.mark.parametrize("case", sorted(INDEX))
 def test_matches_reference_golden(case):
     meta = INDEX[case]
@@ -57,18 +77,7 @@ def test_matches_reference_golden(case):
     inp = {k: v.cuda() for k, v in make_inputs(meta["B"], meta["S"], meta["H"], meta["W"], seed=meta["input_seed"]).items()}
     out = m(depth_gt_index=meta["depth_gt_index"], camera_gt_index=meta["camera_gt_index"], **inp)
     torch.cuda.synchronize()
-    ref = load_file(os.path.join(GOLDEN, f"{case}.safetensors"))
-    errs = {k: rel(out[k], ref[k]) for k in KEYS}
-    print(case, json.dumps(errs))
-    d = os.path.join(os.path.dirname(GOLDEN), os.pardir, "gpurun_out")
-    if os.path.isdir(d):
-        with open(os.path.join(d, "model_parity_mini.txt"), "a") as f:
-            f.write(case + " " + json.dumps({k: round(v, 5) for k, v in errs.items()}) + "\n")
-    for k in KEYS:
-        assert out[k].shape == ref[k].shape and out[k].dtype == torch.float32 and out[k].is_cuda
-        assert torch.isfinite(out[k]).all(), k
-        assert errs[k] < TOL, (k, errs)
-    assert (out["pose_enc"].cpu() - ref["pose_enc"]).abs().max() < 5e-2
+    reduced_golden_check(case, out, log=True)
     assert len(out["pose_enc_list"]) == 4 and out["images"].shape == (meta["B"], meta["S"], 3, meta["H"], meta["W"])
 
 
@@ -203,9 +212,10 @@ def full_model():
     return _FULL["m"]
 
 
-def full_size_check(case, out, label):
+def full_size_check(case, out, label, log=True):
     """Compare a full-size forward with the reference fixture of `case` (oracle/full_golden.py: aggregate, per view, per border
-    line, per pose_enc_list entry, pose_enc max-abs per view), log the worst values and assert the bars of the heads' format."""
+    line, per pose_enc_list entry, pose_enc max-abs per view), log the worst values and assert the bars of the heads' format.
+    ``log=False``: print the worst values but leave the parity log to the parity tests."""
     meta = FULL_INDEX[case]
     for k in KEYS[1:]:
         assert torch.isfinite(out[k]).all(), k
@@ -215,7 +225,7 @@ def full_size_check(case, out, label):
             + json.dumps(w))
     print(line)
     d = os.path.join(os.path.dirname(GOLDEN), os.pardir, "gpurun_out")
-    if os.path.isdir(d):
+    if log and os.path.isdir(d):
         with open(os.path.join(d, "model_parity_full.txt"), "a") as f:
             f.write(line + "\n")
     full_golden.check(metrics, FULL_BARS_BF16_HEADS if "bf16" in label else full_golden.BARS)

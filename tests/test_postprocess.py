@@ -105,13 +105,18 @@ def test_model_postprocess_api():
     inp = {k: v.cuda() for k, v in make_inputs(1, 3, 56, 56, seed=4).items()}
     pred = m.postprocess(m(depth_gt_index=[1], camera_gt_index=[0], **inp), conf_percent=25.0)
     torch.cuda.synchronize()
-    H = W = 56
+    check_postprocess_against_oracle(pred, 25.0)
+
+
+def check_postprocess_against_oracle(pred, pct):
+    """The keys postprocess added to the predictions of one scene against the oracle on the same predictions."""
+    H, W = pred["images"].shape[-2:]
     ext, intr = PO.pose_encoding_to_extri_intri(pred["pose_enc"].cpu().numpy(), H, W)
     assert np.allclose(pred["extrinsic"].cpu().numpy(), ext, rtol=1e-4, atol=1e-5)
     assert np.allclose(pred["intrinsic"].cpu().numpy(), intr, rtol=1e-4, atol=1e-3)
     world = PO.unproject_depth_map_to_point_map(pred["depth"][0, ..., 0].cpu().numpy(), ext[0], intr[0])
     got = pred["world_points_from_depth"][0].cpu().numpy()
     assert np.abs(got - world).max() <= 1e-4 * np.abs(world).max()
-    mask, thr = PO.conf_percentile_mask(pred["depth_conf"].cpu().numpy(), 25.0)
+    mask, thr = PO.conf_percentile_mask(pred["depth_conf"].cpu().numpy(), pct)
     assert abs(pred["conf_threshold"].item() - float(thr)) <= 1e-6 * abs(float(thr))
     assert (pred["conf_mask"].cpu().numpy() != mask).sum() <= 2 and pred["conf_mask"].shape == pred["depth_conf"].shape

@@ -76,10 +76,16 @@ def test_tap_and_index_tables_match_the_libraries():
 def test_gpu_pipeline_matches_oracle_bit_for_bit(name, tmp_path):
     from omnivggt_official_b200 import preprocess as PP
     d = make_folder(str(tmp_path), name, seed=0)
-    imgs, cams, deps, tr = _read_folder(d)
-    ref = PO.load_views(imgs, cams, [x.T if t else x for x, t in zip(deps, tr)])
     out = PP.load_images_and_cameras(d["images"], d["cameras"], d["depths"])
     torch.cuda.synchronize()
+    check_pipeline_against_oracle(name, d, out)
+
+
+def check_pipeline_against_oracle(name, d, out):
+    """load_images_and_cameras' tuple for the synthetic folder d (make_folder(..., name)) against the oracle loader, and the
+    image and depth digests of the reference's loader when Pillow is the pinned build."""
+    imgs, cams, deps, tr = _read_folder(d)
+    ref = PO.load_views(imgs, cams, [x.T if t else x for x, t in zip(deps, tr)])
     assert out[5] == ref[5] and out[6] == ref[6]
     assert torch.equal(out[0].cpu(), torch.from_numpy(ref[0]))                      # images: bit-exact
     assert torch.equal(out[3].cpu(), torch.from_numpy(ref[3])) and torch.equal(out[4].cpu(), torch.from_numpy(ref[4]))
