@@ -11,7 +11,8 @@
 //   warpgroup 0     TMA producer (one thread), 40 registers
 //   warpgroups 1-2  wgmma consumers, 64 rows of the 128-row tile each; they issue MMAs and stage the accumulators, nothing else
 //                   (144 registers)
-//   warpgroup 3     epilogue: one whole accumulator row per thread, every column of the tile (184 registers)
+//   warpgroup 3     epilogue: one whole accumulator row per thread, every column of the tile (184 registers); the residual
+//                   epilogue instead walks the tile row by row across each warp, so that its fp32 read-modify-write is coalesced
 // Pipeline: smem full/empty ring (TMA<->MMA).  The finished accumulator tile goes through ONE fp32 smem tile (sAcc) so that
 // the epilogue works on whole rows, as the QKV head LayerNorm and the row remaps need.  Hand-off over two named barriers of
 // the 384 consumer + epilogue threads: the consumers wait for GEMM_BAR_ACC_FREE (skipped on their first tile), store the
@@ -45,7 +46,7 @@ struct GemmParams {
   int rowmap;  // RowMap
   int gh, gw;  // source grid (rows are (frame, y, x)); RM_PAD: interior size of the padded domain
   int ps, cout;  // RM_PIXSHUF: stride (= kernel) and output channels
-  // ---- EPI_RESID:  out(fp32)[row,n] += gamma[n] * (acc + bias[n]),  row = row_index ? row_index[m] : m
+  // ---- EPI_RESID (epilogue_resid_tile):  out(fp32)[row,n] += gamma[n] * (acc + bias[n]),  row = row_index ? row_index[m] : m
   const float* gamma;
   const int* row_index;
   // ---- EPI_QKV (layers/attention.py:52-58 fused: bias, q/k LayerNorm(64), 2-D RoPE, head-major bf16)
@@ -260,14 +261,12 @@ __device__ __forceinline__ void epilogue_tile(const GemmParams& p, const float* 
     }
   } else {
     // ---- row mapping
-    bool row_ok = m < p.M;
+    static_assert(EPI == EPI_BF16 || EPI == EPI_HEADTAIL, "EPI_RESID runs epilogue_resid_tile");
+    const bool row_ok = m < p.M;
     bool interior = true;  // RM_PAD: border rows are written as zeros
     long long drow = m;
     int fr = 0, yy = 0, xx = 0;
-    if (EPI == EPI_RESID) {
-      if (p.row_index && row_ok) drow = p.row_index[m];
-    }
-    if (EPI == EPI_BF16 || EPI == EPI_HEADTAIL) {
+    {
       if (p.rowmap == RM_DENSE2PAD || p.rowmap == RM_PIXSHUF) {
         const int hw = p.gh * p.gw;
         fr = m / hw;
@@ -295,20 +294,7 @@ __device__ __forceinline__ void epilogue_tile(const GemmParams& p, const float* 
 #pragma unroll
       for (int i = 0; i < 32; ++i) v[i] = __uint_as_float(raw[i]);
 
-      if constexpr (EPI == EPI_RESID) {
-        float* x = reinterpret_cast<float*>(p.out) + drow * p.ldo + n;
-#pragma unroll
-        for (int i = 0; i < 8; ++i) {
-          float4 xv = reinterpret_cast<float4*>(x)[i];
-          const float4 g = __ldg(reinterpret_cast<const float4*>(p.gamma + n) + i);
-          const float4 b = __ldg(reinterpret_cast<const float4*>(p.bias + n) + i);
-          xv.x += g.x * (v[4 * i + 0] + b.x);
-          xv.y += g.y * (v[4 * i + 1] + b.y);
-          xv.z += g.z * (v[4 * i + 2] + b.z);
-          xv.w += g.w * (v[4 * i + 3] + b.w);
-          reinterpret_cast<float4*>(x)[i] = xv;
-        }
-      } else if constexpr (EPI == EPI_HEADTAIL) {
+      if constexpr (EPI == EPI_HEADTAIL) {
         if (!interior) continue;
 #pragma unroll
         for (int i = 0; i < 32; ++i) v[i] = fmaxf(v[i] + __ldg(p.bias + i), 0.f);
@@ -405,6 +391,96 @@ __device__ __forceinline__ void epilogue_tile(const GemmParams& p, const float* 
   }
 }
 
+// EPI_RESID over one 128 x BN tile by the epilogue warpgroup: x[row, n] += gamma[n] * (acc + bias[n]) in fp32.  Epilogue warp
+// `ew` takes rows [32 ew, 32 ew + 32); each warp access covers whole rows, BN / 4 lanes per row with one float4 each, so a row
+// segment of x is one contiguous 4 * BN-byte load and store (a row per thread would touch 32 rows per access and use half of each
+// 32-byte sector).  RES_INFLIGHT accesses are issued before the first is used: one warp per scheduler has to cover the HBM latency alone.
+constexpr int RES_INFLIGHT = 8;
+template <int BN>
+__device__ __forceinline__ void epilogue_resid_tile(const GemmParams& p, const float* sAcc, const int m0, const int n0,
+                                                    const int ew, const int lane) {
+  constexpr int LPR = BN / 4;           // lanes per row
+  constexpr int RPA = 32 / LPR;         // rows per warp access
+  static_assert(32 % (RPA * RES_INFLIGHT) == 0, "rows per warp");
+  const int c = 4 * (lane % LPR);
+  const int n = n0 + c;
+  if (n >= p.N) return;                 // N % 32 == 0: a float4 is wholly inside or outside
+  const float4 g = __ldg(reinterpret_cast<const float4*>(p.gamma + n));
+  const float4 b = __ldg(reinterpret_cast<const float4*>(p.bias + n));
+  for (int j0 = 0; j0 < 32; j0 += RPA * RES_INFLIGHT) {
+    float4 xv[RES_INFLIGHT], a[RES_INFLIGHT];
+    float* x[RES_INFLIGHT];
+#pragma unroll
+    for (int u = 0; u < RES_INFLIGHT; ++u) {
+      const int r = 32 * ew + j0 + u * RPA + lane / LPR;
+      const int m = m0 + r;
+      x[u] = nullptr;
+      if (m < p.M) {
+        const long long drow = p.row_index ? p.row_index[m] : m;
+        x[u] = reinterpret_cast<float*>(p.out) + drow * p.ldo + n;
+        xv[u] = *reinterpret_cast<const float4*>(x[u]);
+        a[u] = *reinterpret_cast<const float4*>(sAcc + r * GemmCfg<BN>::ACC_LD + c);
+      }
+    }
+#pragma unroll
+    for (int u = 0; u < RES_INFLIGHT; ++u) {
+      if (x[u] == nullptr) continue;
+      xv[u].x += g.x * (a[u].x + b.x);
+      xv[u].y += g.y * (a[u].y + b.y);
+      xv[u].z += g.z * (a[u].z + b.z);
+      xv[u].w += g.w * (a[u].w + b.w);
+      *reinterpret_cast<float4*>(x[u]) = xv[u];
+    }
+  }
+}
+
+// The two wgmma warpgroups of gemm_kernel: the K loop of every tile, then the accumulators into sAcc for the epilogue warpgroup.
+// The operand type is a template argument, so that each K block is one straight run of wgmmas: with the choice between the bf16 and
+// the fp16 form made at run time inside the loop, ptxas put a warpgroup fence in front of every wgmma and made each one wait on
+// the scoreboard.
+template <int BN, bool F16>
+__device__ __forceinline__ void gemm_mma_loop(const GemmParams& p, uint8_t* sA, uint8_t* sB, float* sAcc, uint64_t* full,
+                                              uint64_t* empty, const int num_tiles, const int warp, const int lane) {
+  using Cfg = GemmCfg<BN>;
+  constexpr int STAGES = Cfg::STAGES;
+  const int cw = (warp >> 2) - 1;      // consumer warpgroup: rows [64 cw, 64 cw + 64) of the tile
+  const int frow = cw * 64 + (warp & 3) * 16 + (lane >> 2);   // accumulator fragment rows frow, frow + 8
+  const int fcol = 2 * (lane & 3);
+  int s = 0;
+  uint32_t ph = 0;
+  float acc[BN / 2];
+  for (int tile = blockIdx.x; tile < num_tiles; tile += gridDim.x) {
+    int prev = -1;
+    for (int kb = 0; kb < p.k_blocks; ++kb) {
+      mbar_wait_quiet(&full[s], ph);      // no printf call site: it would serialise the wgmma pipeline
+      const uint64_t adesc = make_sw128_desc(smem_u32(sA + s * GEMM_A_BYTES + cw * 64 * 128));
+      const uint64_t bdesc = make_sw128_desc(smem_u32(sB + s * Cfg::B_BYTES));
+      wgmma_fence();
+#pragma unroll
+      for (int k = 0; k < GEMM_BK / 16; ++k) wgmma_ss<BN, F16>(acc, adesc + 2 * k, bdesc + 2 * k, (kb | k) != 0);
+      wgmma_commit();
+      wgmma_wait<1>();                 // the previous K block's MMAs are done: release its stage
+      if (prev >= 0 && lane == 0) mbar_arrive(&empty[prev]);
+      prev = s;
+      if (++s == STAGES) {
+        s = 0;
+        ph ^= 1;
+      }
+    }
+    wgmma_wait<0>();
+    fence_regs<BN / 2>(acc);
+    if (lane == 0) mbar_arrive(&empty[prev]);
+    // the epilogue warpgroup is done with the previous tile's accumulators (it has read sAcc in full)
+    if (tile != static_cast<int>(blockIdx.x)) named_sync(GEMM_BAR_ACC_FREE, 384);
+#pragma unroll
+    for (int j = 0; j < BN / 8; ++j) {
+      *reinterpret_cast<float2*>(sAcc + frow * Cfg::ACC_LD + 8 * j + fcol) = make_float2(acc[4 * j], acc[4 * j + 1]);
+      *reinterpret_cast<float2*>(sAcc + (frow + 8) * Cfg::ACC_LD + 8 * j + fcol) = make_float2(acc[4 * j + 2], acc[4 * j + 3]);
+    }
+    named_arrive(GEMM_BAR_ACC_FULL, 384);
+  }
+}
+
 template <int BN, int EPI>
 __global__ void __launch_bounds__(GEMM_THREADS, 1)
 gemm_kernel(const __grid_constant__ CUtensorMap tmA, const __grid_constant__ CUtensorMap tmB, const GemmParams p) {
@@ -478,44 +554,12 @@ gemm_kernel(const __grid_constant__ CUtensorMap tmA, const __grid_constant__ CUt
   } else if (threadIdx.x < GEMM_EPI_THREAD0) {
     // ===================== wgmma (2 warpgroups, 8 warps) =====================
     reg_alloc<GEMM_MMA_REGS>();
-    const int cw = (warp >> 2) - 1;      // consumer warpgroup: rows [64 cw, 64 cw + 64) of the tile
-    const int frow = cw * 64 + (warp & 3) * 16 + (lane >> 2);   // accumulator fragment rows frow, frow + 8
-    const int fcol = 2 * (lane & 3);
-    int s = 0;
-    uint32_t ph = 0;
-    float acc[BN / 2];
-    for (int tile = blockIdx.x; tile < num_tiles; tile += gridDim.x) {
-      int prev = -1;
-      for (int kb = 0; kb < p.k_blocks; ++kb) {
-        mbar_wait_quiet(&full[s], ph);      // no printf call site: it would serialise the wgmma pipeline
-        const uint64_t adesc = make_sw128_desc(smem_u32(sA + s * GEMM_A_BYTES + cw * 64 * 128));
-        const uint64_t bdesc = make_sw128_desc(smem_u32(sB + s * Cfg::B_BYTES));
-        wgmma_fence();
-#pragma unroll
-        for (int k = 0; k < GEMM_BK / 16; ++k) {
-          if (p.f16) wgmma_ss<BN, true>(acc, adesc + 2 * k, bdesc + 2 * k, (kb | k) != 0);
-          else wgmma_ss<BN, false>(acc, adesc + 2 * k, bdesc + 2 * k, (kb | k) != 0);
-        }
-        wgmma_commit();
-        wgmma_wait<1>();                 // the previous K block's MMAs are done: release its stage
-        if (prev >= 0 && lane == 0) mbar_arrive(&empty[prev]);
-        prev = s;
-        if (++s == STAGES) {
-          s = 0;
-          ph ^= 1;
-        }
-      }
-      wgmma_wait<0>();
-      fence_regs<BN / 2>(acc);
-      if (lane == 0) mbar_arrive(&empty[prev]);
-      // the epilogue warpgroup is done with the previous tile's accumulators (it has read sAcc in full)
-      if (tile != static_cast<int>(blockIdx.x)) named_sync(GEMM_BAR_ACC_FREE, 384);
-#pragma unroll
-      for (int j = 0; j < BN / 8; ++j) {
-        *reinterpret_cast<float2*>(sAcc + frow * Cfg::ACC_LD + 8 * j + fcol) = make_float2(acc[4 * j], acc[4 * j + 1]);
-        *reinterpret_cast<float2*>(sAcc + (frow + 8) * Cfg::ACC_LD + 8 * j + fcol) = make_float2(acc[4 * j + 2], acc[4 * j + 3]);
-      }
-      named_arrive(GEMM_BAR_ACC_FULL, 384);
+    // Only EPI_BF16 / EPI_HEADTAIL take fp16 operands; the others are bf16 at compile time.
+    if constexpr (EPI == EPI_BF16 || EPI == EPI_HEADTAIL) {
+      if (p.f16) gemm_mma_loop<BN, true>(p, sA, sB, sAcc, full, empty, num_tiles, warp, lane);
+      else gemm_mma_loop<BN, false>(p, sA, sB, sAcc, full, empty, num_tiles, warp, lane);
+    } else {
+      gemm_mma_loop<BN, false>(p, sA, sB, sAcc, full, empty, num_tiles, warp, lane);
     }
   } else {
     // ===================== epilogue (1 warpgroup): row r of every tile, all BN columns =====================
@@ -525,7 +569,8 @@ gemm_kernel(const __grid_constant__ CUtensorMap tmA, const __grid_constant__ CUt
       const int m0 = (tile / n_tiles) * GEMM_BM;
       const int n0 = (tile % n_tiles) * BN;
       named_sync(GEMM_BAR_ACC_FULL, 384);
-      epilogue_tile<BN, EPI>(p, sAcc + r * Cfg::ACC_LD, m0 + r, n0, 0, 1, s_rope);
+      if constexpr (EPI == EPI_RESID) epilogue_resid_tile<BN>(p, sAcc, m0, n0, r >> 5, lane);
+      else epilogue_tile<BN, EPI>(p, sAcc + r * Cfg::ACC_LD, m0 + r, n0, 0, 1, s_rope);
       if (tile + static_cast<int>(gridDim.x) < num_tiles) named_arrive(GEMM_BAR_ACC_FREE, 384);
     }
   }
