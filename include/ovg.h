@@ -261,6 +261,40 @@ int ovg_match_gather(const int* pairs, int P, int V, long long cap, int W, const
 int ovg_match_pair(const int* pairs, int P, int V, long long cap, int pair, const void* workspace, long long workspace_bytes,
                    unsigned char* reciprocal, long long* nn, void* stream);
 
+/* Multi-view tracks for a COLMAP sparse model ("star tracks"; no counterpart in the reference), on a match workspace after
+ * ovg_match_query, with the same pairs, V, cap and P.  Node (v, k) is kept point k of view v.  Views anchor in order
+ * a = 0 .. V-1: every kept node of view a that no earlier step claimed gathers its partners, the reciprocal match of k in each
+ * view j > a of a pair (a, j) when that node is unclaimed too; with 1 + partners >= min_views the anchor and its partners
+ * become one new track and are claimed.  Tracks are numbered by (anchor view, anchor kept index), and a track's observations
+ * go in ascending view order, anchor first: at most one observation per view, every node in at most one track.  Each pair's
+ * reciprocal matching is one-to-one, so a step is fully parallel and no atomic decides anything: results are bit-identical
+ * from run to run.  The number of kernel launches grows with V, not with P.  V * cap < 2^31.
+ * pairs: device int32 [P, 2] = (i, j), i < j, unique and sorted by (i, j); pair_off: device int32 [V + 1], the pairs of
+ * anchor a are pairs[pair_off[a], pair_off[a + 1]).  One workspace of ovg_tracks_workspace_bytes(V, cap) bytes (256-byte
+ * aligned) serves both calls; run them in order on the stream of the match calls.
+ * ovg_tracks_assign: the tracks, 1 <= min_views <= V.  counts_out: device int64 [3] = tracks, observations, then 1 if a kept
+ *     point is not finite.  Reading it back to size the outputs is the one host synchronisation of a call. */
+long long ovg_tracks_workspace_bytes(int V, long long cap);
+int ovg_tracks_assign(const int* pairs, const int* pair_off, int P, int V, long long cap, int min_views, const void* match_workspace,
+                      long long match_workspace_bytes, void* workspace, long long workspace_bytes, long long* counts_out,
+                      void* stream);
+/* ovg_tracks_gather: n_tracks tracks and n_obs observations as counted.  images fp32 [V, 3, H, W] (cap = H W), extrinsic fp32
+ * [V, 3, 4] world-to-camera [R | t], intrinsic fp32 [V, 3, 3].  Pixel (x, y) of a kept row r is (r % W, r / W); its centre is
+ * (x + 0.5, y + 0.5), COLMAP's convention, while the intrinsics keep the reference's (unprojection through (x - cx) / fx,
+ * utils/geometry.py:236-264), so COLMAP's principal point is (cx + 0.5, cy + 0.5).
+ * Per track: points fp64 [n, 3] = the sum of the observations' points in observation order, divided once; colors uint8 [n, 3]
+ * = the anchor pixel's uint8(trunc(x * 255)); error fp64 [n] = the mean distance between the projection of the point
+ * (fp64, every operation rounded on its own: ((r0 px + r1 py) + r2 pz) + t per row, u = fx (X / Z) + (cx + 0.5)) and the
+ * pixel centre, +inf when some observation sees the point at Z <= 0; offsets int64 [n + 1] into the observations.
+ * Per observation: view int32, xy int64 [m, 2] and point2d int32, the rank of the node in its view's list below.
+ * Per view: view_offsets int64 [V + 1] and the claimed nodes in row-major pixel order, view_track int32 [m] and view_xy int64
+ * [m, 2]. */
+int ovg_tracks_gather(const float* images, const float* extrinsic, const float* intrinsic, int V, long long cap, int P, int W,
+                      long long n_tracks, long long n_obs, const void* match_workspace, long long match_workspace_bytes,
+                      void* workspace, long long workspace_bytes, double* points, unsigned char* colors, double* error,
+                      long long* offsets, int* view, long long* xy, int* point2d, long long* view_offsets, int* view_track,
+                      long long* view_xy, void* stream);
+
 /* Triangle mesh of point maps: viz.py:40-89 (pts3d_to_trimesh per view, cat_meshes across views) for F views at once.
  * Pixels are numbered i = (f H + y) W + x.  The quad at (y, x), y < H-1, x < W-1, gives the TL triangle (tl, tr, bl) and the BR
  * triangle (tr, bl, br); a triangle is kept when its three vertices are.  Reference layout: per view, the kept TL triangles,

@@ -130,6 +130,10 @@ EXPORTS = {
     "ovg_match_query": (C.c_int, [_vp, _i, _i, _ll, _vp, _ll, _vp, _vp]),
     "ovg_match_gather": (C.c_int, [_vp, _i, _i, _ll, _i, _vp, _ll, _vp, _vp, _vp]),
     "ovg_match_pair": (C.c_int, [_vp, _i, _i, _ll, _i, _vp, _ll, _vp, _vp, _vp]),
+    "ovg_tracks_workspace_bytes": (_ll, [_i, _ll]),
+    "ovg_tracks_assign": (C.c_int, [_vp, _vp, _i, _i, _ll, _i, _vp, _ll, _vp, _ll, _vp, _vp]),
+    "ovg_tracks_gather": (C.c_int, [_vp, _vp, _vp, _i, _ll, _i, _i, _ll, _ll, _vp, _ll, _vp, _ll, _vp, _vp, _vp, _vp, _vp, _vp, _vp,
+                                    _vp, _vp, _vp, _vp]),
     "ovg_mesh_workspace_bytes": (_ll, [_i, _i, _i]),
     "ovg_mesh_count": (C.c_int, [_vp, _vp, _i, _i, _i, _i, _i, _vp, _ll, _vp, _vp]),
     "ovg_mesh_faces": (C.c_int, [_vp, _vp, _i, _i, _i, _i, _vp, _ll, _vp, _vp, _vp]),

@@ -1,4 +1,4 @@
-// Ordered stream compaction, shared by the point cloud, the mesh and the matches: kept items land in the order of numpy's
+// Ordered stream compaction, shared by the point cloud, the mesh, the matches and the tracks: kept items land in the order of numpy's
 // boolean indexing and no atomic ever decides an output slot, so runs are bit-identical.  Block b of a count / gather kernel
 // owns the tile [b COMPACT_TILE, (b + 1) COMPACT_TILE) of its items, walked in COMPACT_ITERS chunks of COMPACT_THREADS
 // consecutive items.  The count kernel stores the tile's kept count (tile_sum), a scan turns the counts into tile offsets
@@ -58,6 +58,38 @@ __device__ __forceinline__ void chunk_ranks(const bool (&flag)[S], unsigned int 
     sum[s] = pre[s][COMPACT_THREADS / 32];
   }
   __syncthreads();                                 // pre is rewritten by the next chunk
+}
+
+// chunk_ranks for per-thread counts instead of flags: rank[s] = the sum of val[s] over the threads before this one in the
+// chunk, sum[s] = the chunk's total.  An inclusive shuffle scan within a warp, a scan over the warps.
+template <int S>
+__device__ __forceinline__ void chunk_sums(const unsigned int (&val)[S], unsigned int (&rank)[S], unsigned int (&sum)[S]) {
+  __shared__ unsigned int pre[S][COMPACT_THREADS / 32 + 1];
+  const int lane = threadIdx.x & 31, warp = threadIdx.x >> 5;
+  unsigned int inc[S];
+#pragma unroll
+  for (int s = 0; s < S; ++s) {
+    inc[s] = val[s];
+#pragma unroll
+    for (int o = 1; o < 32; o <<= 1) {
+      const unsigned int t = __shfl_up_sync(0xffffffffu, inc[s], o);
+      if (lane >= o) inc[s] += t;
+    }
+    if (lane == 31) pre[s][warp + 1] = inc[s];
+  }
+  __syncthreads();
+  if (threadIdx.x < S) {
+    pre[threadIdx.x][0] = 0;
+#pragma unroll
+    for (int w = 1; w <= COMPACT_THREADS / 32; ++w) pre[threadIdx.x][w] += pre[threadIdx.x][w - 1];
+  }
+  __syncthreads();
+#pragma unroll
+  for (int s = 0; s < S; ++s) {
+    rank[s] = pre[s][warp] + inc[s] - val[s];
+    sum[s] = pre[s][COMPACT_THREADS / 32];
+  }
+  __syncthreads();
 }
 
 // One block of 1024 threads: exclusive scan of cnt[0, len) into out (out may be cnt when Tin is Tout), runs per thread,

@@ -15,6 +15,7 @@
 #include "gemm.cuh"
 #include "post.cuh"
 #include "match.cuh"
+#include "tracks.cuh"
 #include "mesh.cuh"
 #include "sky.cuh"
 #include "fps.cuh"
@@ -1011,6 +1012,106 @@ int ovg_match_pair(const int* pairs, int P, int V, long long cap, int pair, cons
   ovg::MatchOut o{1, nullptr, nullptr, pair, reciprocal, nn};
   ovg::match_pair_kernel<<<static_cast<unsigned>((cap + 255) / 256), 256, 0, reinterpret_cast<cudaStream_t>(stream)>>>(p, o);
   return post_launch("ovg_match_pair");
+}
+
+}  // extern "C"
+
+// ------------------------------------------------------------------------------------------------------------- star tracks
+namespace {
+
+// Track workspace, carved the same way by the size query and by both entry points.
+long long tracks_workspace(void* base, int V, long long cap, ovg::TrackParams* p) {
+  Arena ar(base, 0);
+  const long long nodes = V * cap;
+  const long long tiles = ovg::compact_tiles(cap) * (V > 2 ? V : 2);
+  p->claim = ar.get<int>(nodes);
+  p->rank = ar.get<int>(nodes);
+  p->obs = ar.get<int>(nodes);
+  p->track_start = ar.get<int>(nodes);
+  p->tile_count = ar.get<unsigned int>(tiles);
+  p->tile_offset = ar.get<unsigned long long>(tiles);
+  p->scan_total = ar.get<unsigned long long>(1);
+  p->totals = ar.get<unsigned long long>(4);
+  return ar.bytes();
+}
+
+int tracks_check(int V, long long cap, int P, const void* match_ws, long long match_ws_bytes, void* workspace,
+                 long long workspace_bytes, ovg::TrackParams* p) {
+  OVG_REQUIRE(V > 0 && cap > 0 && static_cast<long long>(V) * cap < (1LL << 31), "V * cap must be below 2^31");
+  int rc = match_check(V, cap, P, match_ws, match_ws_bytes, &p->m);
+  if (rc) return rc;
+  OVG_REQUIRE(workspace_ok(workspace, workspace_bytes, tracks_workspace(nullptr, V, cap, p), 256),
+              "workspace must be 256-byte aligned and ovg_tracks_workspace_bytes(V, cap) long");
+  tracks_workspace(workspace, V, cap, p);
+  return OVG_OK;
+}
+
+}  // namespace
+
+extern "C" {
+
+long long ovg_tracks_workspace_bytes(int V, long long cap) {
+  ovg::TrackParams p{};
+  return (V > 0 && cap > 0) ? tracks_workspace(nullptr, V, cap, &p) : -1;
+}
+
+int ovg_tracks_assign(const int* pairs, const int* pair_off, int P, int V, long long cap, int min_views, const void* match_workspace,
+                      long long match_workspace_bytes, void* workspace, long long workspace_bytes, long long* counts_out,
+                      void* stream) {
+  ovg::TrackParams p{};
+  int rc = tracks_check(V, cap, P, match_workspace, match_workspace_bytes, workspace, workspace_bytes, &p);
+  if (rc) return rc;
+  OVG_REQUIRE(pairs && pair_off && counts_out, "null pairs / pair_off / counts_out");
+  OVG_REQUIRE(min_views >= 1 && min_views <= V, "min_views must be in [1, V]");
+  p.m.pairs = pairs;
+  p.pair_off = pair_off;
+  p.min_views = min_views;
+  cudaStream_t st = reinterpret_cast<cudaStream_t>(stream);
+  OVG_CUDA(cudaMemsetAsync(p.claim, 0xFF, 4LL * V * cap, st));
+  OVG_CUDA(cudaMemsetAsync(p.totals, 0, 2 * sizeof(unsigned long long), st));
+  const int tiles = p.m.tiles;
+  for (int a = 0; a < V; ++a) {
+    ovg::track_count_kernel<<<tiles, ovg::COMPACT_THREADS, 0, st>>>(p, a);
+    if ((rc = post_launch("ovg_tracks_assign(count)"))) return rc;
+    ovg::tile_scan_kernel<<<1, 1024, 0, st>>>(p.tile_count, p.tile_offset, p.scan_total, 2LL * tiles);
+    if ((rc = post_launch("ovg_tracks_assign(scan)"))) return rc;
+    ovg::track_write_kernel<<<tiles, ovg::COMPACT_THREADS, 0, st>>>(p, a);
+    if ((rc = post_launch("ovg_tracks_assign(write)"))) return rc;
+  }
+  ovg::track_counts_kernel<<<1, 1, 0, st>>>(p, counts_out);
+  return post_launch("ovg_tracks_assign(counts)");
+}
+
+int ovg_tracks_gather(const float* images, const float* extrinsic, const float* intrinsic, int V, long long cap, int P, int W,
+                      long long n_tracks, long long n_obs, const void* match_workspace, long long match_workspace_bytes,
+                      void* workspace, long long workspace_bytes, double* points, unsigned char* colors, double* error,
+                      long long* offsets, int* view, long long* xy, int* point2d, long long* view_offsets, int* view_track,
+                      long long* view_xy, void* stream) {
+  ovg::TrackParams p{};
+  int rc = tracks_check(V, cap, P, match_workspace, match_workspace_bytes, workspace, workspace_bytes, &p);
+  if (rc) return rc;
+  OVG_REQUIRE(W > 0 && cap % W == 0, "cap must be H * W");
+  OVG_REQUIRE(n_tracks >= 0 && n_tracks <= n_obs && n_obs <= static_cast<long long>(V) * cap, "bad track counts");
+  OVG_REQUIRE(offsets && view_offsets, "null offsets / view_offsets");
+  OVG_REQUIRE(n_tracks == 0 || (images && extrinsic && intrinsic && points && colors && error && view && xy && point2d &&
+                                view_track && view_xy), "null operand");
+  const ovg::TrackOut o{images, extrinsic, intrinsic, W, n_tracks, n_obs, points, colors, error, offsets, view, xy, point2d,
+                        view_offsets, view_track, view_xy};
+  cudaStream_t st = reinterpret_cast<cudaStream_t>(stream);
+  const dim3 grid(p.m.tiles, V);
+  ovg::track_claimed_kernel<<<grid, ovg::COMPACT_THREADS, 0, st>>>(p);
+  if ((rc = post_launch("ovg_tracks_gather(claimed count)"))) return rc;
+  ovg::tile_scan_kernel<<<1, 1024, 0, st>>>(p.tile_count, p.tile_offset, p.scan_total, static_cast<long long>(V) * p.m.tiles);
+  if ((rc = post_launch("ovg_tracks_gather(scan)"))) return rc;
+  ovg::track_view_kernel<<<grid, ovg::COMPACT_THREADS, 0, st>>>(p, o);
+  if ((rc = post_launch("ovg_tracks_gather(views)"))) return rc;
+  if (n_tracks == 0) {
+    OVG_CUDA(cudaMemsetAsync(offsets, 0, sizeof(long long), st));
+    return OVG_OK;
+  }
+  ovg::track_point_kernel<<<static_cast<unsigned>((n_tracks + ovg::TRACK_POINT_THREADS - 1) / ovg::TRACK_POINT_THREADS),
+                            ovg::TRACK_POINT_THREADS, 0, st>>>(p, o);
+  return post_launch("ovg_tracks_gather(points)");
 }
 
 }  // extern "C"

@@ -473,6 +473,74 @@ class OmniVGGT(nn.Module, PyTorchModelHubMixin):
 
     @staticmethod
     @torch.no_grad()
+    def tracks(predictions: Dict[str, object], pairs=None, *, source: str = "depth", conf_percent: float = 50.0,
+               conf_floor: float = 1e-5, scene: int = 0, mask_sky=False, min_views: int = 2) -> Dict[str, torch.Tensor]:
+        """Multi-view tracks of one scene for a COLMAP sparse model (``colmap.write_colmap``), built on the device from the
+        reciprocal matches of ``matches``; no counterpart in the reference.
+
+        ``source``, the keep mask, ``mask_sky`` and ``pairs`` are those of ``matches``; (i, j) and (j, i) are one pair and
+        duplicates are merged.  Star tracks: views anchor in order a = 0 .. S-1; every kept pixel of view a not yet in a
+        track gathers its partners, its reciprocal match in each view j > a of a pair (a, j) that is not in a track either,
+        and when 1 + partners >= ``min_views`` (in [1, S]; 1 turns every remaining kept pixel into a one-view point) they
+        become one new track.  Tracks are numbered by (anchor view, anchor pixel in row-major order); each has at most one
+        observation per view, in ascending view order, and every pixel is in at most one track.  Matches are not chained
+        across pairs: reciprocal nearest neighbours of different pairs are not transitive.
+
+        Returns on the device, per track: ``points`` fp64 [n, 3] (the mean of the observations' points, not rounded to
+        fp32), ``colors`` uint8 [n, 3] (the anchor pixel's, as ``point_cloud`` computes colours), ``error`` fp64 [n] (mean
+        reprojection distance in pixels, COLMAP's pixel-centre convention, +inf when a camera sees the point behind it) and
+        ``offsets`` int64 [n + 1]; per observation: ``view`` int32 [m], ``xy`` int64 [m, 2] (x, y) and ``point2d`` int32
+        [m] (rank of the pixel in its view's list); per view: ``view_offsets`` int64 [S + 1], ``view_track`` int32 [m] and
+        ``view_xy`` int64 [m, 2], each view's pixels in tracks in row-major order; and the ``extrinsic`` / ``intrinsic``
+        used, decoded from ``pose_enc`` where the predictions do not hold them.  The counts are the one host read; kept
+        points that are not finite raise ValueError."""
+        from . import geometry, ops
+        S = OmniVGGT._check_views(predictions, source, conf_percent, conf_floor, None, scene, mask_sky)
+        if isinstance(min_views, (bool, np.bool_)) or not isinstance(min_views, (int, np.integer)) or not 1 <= min_views <= S:
+            raise ValueError(f"min_views must be an integer in [1, {S}], got {min_views!r}")
+        pair_arr = geometry.check_pairs(pairs, S)
+        pair_arr = np.unique(np.sort(pair_arr, axis=1), axis=0).astype(np.int32).reshape(-1, 2)
+        H, W = predictions["images"].shape[-2:]
+        if S * H * W >= 2 ** 31:
+            raise ValueError(f"tracks need views * H * W < 2^31, got {S} x {H} x {W}")
+        ext, intr = OmniVGGT._scene_cameras(predictions, scene, H, W)
+        images, _, points, mask, _, _ = OmniVGGT._kept_views(predictions, source, conf_percent, conf_floor, None, scene, mask_sky)
+        # the pairs of anchor a are pair_arr[pair_off[a]:pair_off[a + 1]]; the matcher sizes its workspace by at least one
+        # pair, so without pairs it queries view 0 against itself, which no anchor reads
+        pair_off = np.searchsorted(pair_arr[:, 0], np.arange(S + 1)).astype(np.int32)
+        queried = pair_arr if len(pair_arr) else np.zeros((1, 2), np.int32)
+        dev = images.device
+        packed = torch.from_numpy(np.concatenate([queried.ravel(), pair_off])).to(dev)
+        mt = ops.Matcher(points.view(S, H * W, 3), mask.view(S, H * W), packed[:queried.size].view(-1, 2))
+        tr = ops.Tracker(mt, packed[queried.size:], min_views)
+        n, m, nonfinite = tr.counts()
+        if nonfinite:
+            raise ValueError("kept points must be finite (cKDTree: data must be finite, check for nan or inf values)")
+        out = tr.gather(images, ext, intr, W, n, m)
+        out.update(extrinsic=ext, intrinsic=intr)
+        return out
+
+    @staticmethod
+    def _scene_cameras(predictions: Dict[str, object], scene: int, H: int, W: int):
+        """(extrinsic fp32 [S,3,4], intrinsic fp32 [S,3,3]) of one scene, contiguous: the predictions' own, or those that
+        ``postprocess`` decodes from ``pose_enc`` where they are missing."""
+        from . import ops
+        cams = {}
+        for key, trailing in (("extrinsic", 2), ("intrinsic", 2)):
+            if key in predictions:
+                t = predictions[key]
+                cams[key] = (t[scene] if t.dim() == trailing + 2 else t).float().contiguous()
+        if len(cams) < 2:
+            if "pose_enc" not in predictions:
+                raise ValueError("tracks need extrinsic and intrinsic, or pose_enc to decode them from")
+            pose = predictions["pose_enc"]
+            ext, intr, _ = ops.pose_decode((pose[scene] if pose.dim() == 3 else pose).float().contiguous(), H, W)
+            cams.setdefault("extrinsic", ext)
+            cams.setdefault("intrinsic", intr)
+        return cams["extrinsic"], cams["intrinsic"]
+
+    @staticmethod
+    @torch.no_grad()
     def point_cloud(predictions: Dict[str, object], *, source: str = "depth", conf_percent: float = 50.0,
                     conf_floor: float = 1e-5, frame: Optional[int] = None, mask_black_bg: bool = False,
                     mask_white_bg: bool = False, scene: int = 0, mask_sky=False,

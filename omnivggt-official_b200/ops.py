@@ -464,3 +464,51 @@ class Matcher:
             L.check(L.lib().ovg_match_pair(self.pairs.data_ptr(), self.P, self.V, self.cap, k, self.ws.data_ptr(), self.ws.numel(),
                                            rec.data_ptr(), nn.data_ptr(), L.stream()))
         return rec.bool(), nn
+
+
+class Tracker:
+    """Star tracks (ovg_tracks_*) over a Matcher's reciprocal matches: the Matcher's pairs must be (i, j) with i < j, unique and
+    sorted, and pair_off int32 [V + 1] on the device gives each anchor view's range of them.  Assigns the tracks on
+    construction (ovg_tracks_assign); ``counts()`` is the one host read, in place of the Matcher's."""
+
+    def __init__(self, matcher: Matcher, pair_off: torch.Tensor, min_views: int):
+        _chk(pair_off, torch.int32, "pair_off")
+        assert pair_off.is_contiguous() and pair_off.numel() == matcher.V + 1
+        self.mt = matcher
+        lib = L.lib()
+        dev = matcher.ws.device
+        self.ws = torch.empty(lib.ovg_tracks_workspace_bytes(matcher.V, matcher.cap), device=dev, dtype=torch.uint8)
+        self._counts = torch.empty(3, device=dev, dtype=torch.int64)
+        L.check(lib.ovg_tracks_assign(matcher.pairs.data_ptr(), pair_off.data_ptr(), matcher.P, matcher.V, matcher.cap,
+                                      int(min_views), matcher.ws.data_ptr(), matcher.ws.numel(), self.ws.data_ptr(),
+                                      self.ws.numel(), self._counts.data_ptr(), L.stream()))
+
+    def counts(self):
+        """(tracks, observations, whether a kept point is not finite): the one host read."""
+        n, m, bad = host_read(self._counts).tolist()
+        return n, m, bool(bad)
+
+    def gather(self, images: torch.Tensor, extrinsic: torch.Tensor, intrinsic: torch.Tensor, W: int, n: int, m: int):
+        """The tracks' outputs (ovg_tracks_gather) as a dict of device tensors; images fp32 [V, 3, H, W], extrinsic fp32
+        [V, 3, 4], intrinsic fp32 [V, 3, 3], contiguous."""
+        mt = self.mt
+        for t, name, shape in ((images, "images", (mt.V, 3, mt.cap // W, W)), (extrinsic, "extrinsic", (mt.V, 3, 4)),
+                               (intrinsic, "intrinsic", (mt.V, 3, 3))):
+            _chk(t, F32, name)
+            assert t.is_contiguous() and tuple(t.shape) == shape, (name, tuple(t.shape), shape)
+        dev = self.ws.device
+        out = {"points": torch.empty(n, 3, device=dev, dtype=torch.float64),
+               "colors": torch.empty(n, 3, device=dev, dtype=torch.uint8),
+               "error": torch.empty(n, device=dev, dtype=torch.float64),
+               "offsets": torch.empty(n + 1, device=dev, dtype=torch.int64),
+               "view": torch.empty(m, device=dev, dtype=torch.int32),
+               "xy": torch.empty(m, 2, device=dev, dtype=torch.int64),
+               "point2d": torch.empty(m, device=dev, dtype=torch.int32),
+               "view_offsets": torch.empty(mt.V + 1, device=dev, dtype=torch.int64),
+               "view_track": torch.empty(m, device=dev, dtype=torch.int32),
+               "view_xy": torch.empty(m, 2, device=dev, dtype=torch.int64)}
+        L.check(L.lib().ovg_tracks_gather(
+            images.data_ptr(), extrinsic.data_ptr(), intrinsic.data_ptr(), mt.V, mt.cap, mt.P, W, n, m, mt.ws.data_ptr(),
+            mt.ws.numel(), self.ws.data_ptr(), self.ws.numel(), *(t.data_ptr() if t.numel() else None for t in out.values()),
+            L.stream()))
+        return out
