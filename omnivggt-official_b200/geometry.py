@@ -66,6 +66,11 @@ def check_pairs(pairs, S: int):
     return np.array(out, dtype=np.int32).reshape(-1, 2)
 
 
+def _is_int(v) -> bool:
+    """v is a Python or numpy integer and not a bool (which Python counts as an int)."""
+    return isinstance(v, (int, np.integer)) and not isinstance(v, (bool, np.bool_))
+
+
 def _device_of(*xs):
     dev = next((x.device for x in xs if torch.is_tensor(x) and x.is_cuda), None)
     return dev if dev is not None else torch.device("cuda", torch.cuda.current_device())
@@ -181,7 +186,7 @@ def compute_ranking(extrinsics, lambda_t: float = 1.0, normalize: bool = True, b
     N = shape[0]
     if k is None:
         k = N
-    elif isinstance(k, bool) or not isinstance(k, (int, np.integer)) or not 1 <= k <= N:
+    elif not _is_int(k) or not 1 <= k <= N:
         raise ValueError(f"k must be an integer in [1, N = {N}], got {k!r}")
     if not batched:
         out = torch.float64

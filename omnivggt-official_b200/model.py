@@ -16,7 +16,6 @@ import warnings
 import weakref
 from typing import Dict, List, Optional, Sequence, Tuple
 
-import numpy as np
 import torch
 import torch.nn as nn
 
@@ -26,7 +25,9 @@ except Exception:  # pragma: no cover
     class PyTorchModelHubMixin:  # type: ignore
         pass
 
+from . import scene as SC          # not "scene": the scene functions take an argument of that name
 from . import torch_parts as TP
+from .geometry import _is_int
 from .params import AggregatorParams, CameraHeadParams, Component, DPTParams, init_parameters
 
 _RESNET_MEAN = (0.485, 0.456, 0.406)   # reference models/aggregator.py:22-23
@@ -301,348 +302,15 @@ class OmniVGGT(nn.Module, PyTorchModelHubMixin):
             return eng.camera_head(cam.view(B * S, -1), B, S, iters=num_iterations)
         return TP.camera_head(self.camera_head, cam, iters=num_iterations, dtype=self.camera_dtype)
 
-    # ---------------------------------------------------------------------------------------------- post-processing
-    @torch.no_grad()
-    def postprocess(self, predictions: Dict[str, object], conf_percent: float = 50.0, use_point_map: bool = False
-                    ) -> Dict[str, object]:
-        """What reference inference.py does on the host right after the forward, on the device (libovg kernels):
-        ``extrinsic`` / ``intrinsic`` from ``pose_enc`` (inference.py:360-365 -> utils/pose_enc.py:65-130),
-        ``world_points_from_depth`` by unprojecting the predicted depth with the predicted cameras (visual_util.py:42-73 ->
-        utils/geometry.py:151-264), and the confidence filter of the viewer (inference.py:132-133): ``conf_mask`` =
-        conf >= percentile(conf, conf_percent) & conf > 0.1 with ``conf_threshold`` / ``conf_kept``, over
-        ``world_points_conf`` if ``use_point_map`` else ``depth_conf`` (inference.py:95-100).  Adds the keys in place."""
-        from . import ops
-        pose = predictions["pose_enc"]
-        H, W = predictions["images"].shape[-2:]
-        B, S = pose.shape[:2]
-        ext, intr, c2w = ops.pose_decode(pose.float(), H, W)
-        predictions["extrinsic"], predictions["intrinsic"] = ext, intr
-        depth = predictions["depth"].float().reshape(B * S, H, W)
-        world = ops.unproject_depth(depth, intr.view(B * S, 3, 3), c2w.view(B * S, 3, 4), H, W)
-        predictions["world_points_from_depth"] = world.view(B, S, H, W, 3)
-        conf = predictions["world_points_conf" if use_point_map else "depth_conf"].float()
-        mask, thr, cnt = ops.conf_percentile_mask(conf, conf_percent, 0.1)
-        predictions["conf_mask"], predictions["conf_threshold"], predictions["conf_kept"] = mask.bool(), thr, cnt
-        return predictions
-
-    @staticmethod
-    def _check_views(predictions: Dict[str, object], source: str, conf_percent: float, conf_floor: float,
-                     frame: Optional[int], scene: int, mask_sky) -> int:
-        """The argument checks of point_cloud, mesh and matches, before any library call; returns the scene's view count."""
-        if source not in ("depth", "pointmap"):
-            raise ValueError(f"source must be 'depth' or 'pointmap', got {source!r}")
-        if not 0.0 <= conf_percent <= 100.0:
-            raise ValueError("conf_percent must be in [0, 100]")
-        if conf_floor < 0.0:
-            raise ValueError("conf_floor must be >= 0")        # the reference's floors are 1e-5 and 0.1
-        OmniVGGT._check_mask_sky(mask_sky, predictions, scene)
-        images = predictions["images"]
-        S = (images[scene] if images.dim() == 5 else images).shape[0]
-        if frame is not None and not 0 <= frame < S:
-            raise IndexError(f"frame {frame} out of range for {S} views")
-        return S
-
-    @staticmethod
-    def _kept_views(predictions: Dict[str, object], source: str, conf_percent: float, conf_floor: float,
-                    frame: Optional[int], scene: int, mask_sky):
-        """The views point_cloud, mesh and matches work on and their keep mask, after _check_views: the scene's source, its
-        confidence times non-sky over all views, then the frame, then conf >= percentile(conf, conf_percent) and
-        conf > conf_floor.  Returns (images fp32 [F,3,H,W], extrinsic [S,3,4], points fp32 [F,H,W,3], mask uint8 [F,H,W],
-        threshold 0-d, first view f0), the images, points and mask contiguous."""
-        from . import ops
-        images, ext, points, conf = OmniVGGT._scene_source(predictions, source, scene)
-        conf = OmniVGGT._sky_conf(mask_sky, images, conf, scene)
-        f0 = 0 if frame is None else frame
-        if frame is not None:
-            images, points, conf = images[frame:frame + 1], points[frame:frame + 1], conf[frame:frame + 1]
-        mask, thr, _ = ops.conf_percentile_mask(conf.float().contiguous(), conf_percent, conf_floor)
-        if conf_percent == 0.0:
-            thr = torch.zeros((), device=images.device, dtype=torch.float32)   # same mask: conf > conf_floor >= 0 implies conf >= 0
-        return images.contiguous(), ext, points.float().contiguous(), mask, thr, f0
-
-    @staticmethod
-    def _scene_source(predictions: Dict[str, object], source: str, scene: int):
-        """(images fp32 [S,3,H,W], extrinsic [S,3,4], points [S,H,W,3], conf [S,H,W]) of one scene.  ``source="depth"``:
-        ``world_points_from_depth`` (unprojected here when ``postprocess`` has not run) with ``depth_conf``; ``"pointmap"``:
-        ``world_points`` with ``world_points_conf``."""
-        from . import ops
-
-        def scene_of(t, trailing):                             # [B, S, ...] or [S, ...] -> [S, ...] of the scene
-            return t[scene] if t.dim() == trailing + 2 else t
-
-        images = scene_of(predictions["images"], 3).float()
-        S, _, H, W = images.shape
-        if "extrinsic" in predictions:
-            ext = scene_of(predictions["extrinsic"], 2).float()
-            c2w = None
-        else:
-            ext, intr, c2w = ops.pose_decode(scene_of(predictions["pose_enc"], 1).float().contiguous(), H, W)
-        if source == "pointmap":
-            points = scene_of(predictions["world_points"], 3)
-            conf = scene_of(predictions["world_points_conf"], 2)
-        else:
-            if "world_points_from_depth" in predictions:
-                points = scene_of(predictions["world_points_from_depth"], 3)
-            else:
-                if c2w is None:
-                    ext, intr, c2w = ops.pose_decode(scene_of(predictions["pose_enc"], 1).float().contiguous(), H, W)
-                depth = scene_of(predictions["depth"], 3).float().reshape(S, H, W)
-                points = ops.unproject_depth(depth, intr, c2w, H, W)
-            conf = scene_of(predictions["depth_conf"], 2)
-        return images, ext, points, conf
-
-    @staticmethod
-    def _segment_views(images: torch.Tensor, conf: Optional[torch.Tensor] = None):
-        """ops.segment_sky over the views of images fp32 [S,3,H,W], read in place when each channel plane is contiguous."""
-        from . import ops
-        S, _, H, W = images.shape
-        if images.stride(3) != 1 or images.stride(2) != W:
-            images = images.contiguous()
-        return ops.segment_sky(images, S, H, W, images.stride(0), 1, images.stride(1), conf)
-
-    @staticmethod
-    @torch.no_grad()
-    def sky_mask(predictions: Dict[str, object], *, scene: int = 0) -> torch.Tensor:
-        """The sky of every view of one scene: the reference's model-free segment_sky (viz.py:357-393) on the images the model
-        saw, ``predictions["images"]`` fp32 [S,3,H,W] (or [B,S,3,H,W]), all views in one call with no host read.  Returns bool
-        [S, H, W] on the device, True = sky; ``point_cloud``, ``mesh`` and ``matches`` take it as ``mask_sky``."""
-        images = predictions["images"]
-        images = (images[scene] if images.dim() == 5 else images).float()
-        sky, _ = OmniVGGT._segment_views(images)
-        return sky.bool()
-
-    @staticmethod
-    def _check_mask_sky(mask_sky, predictions: Dict[str, object], scene: int) -> None:
-        """mask_sky is a bool, or a bool tensor [S, H, W] / [B, S, H, W] (True = sky) on the images' device."""
-        if isinstance(mask_sky, (bool, np.bool_)):
-            return
-        if not torch.is_tensor(mask_sky) or mask_sky.dtype != torch.bool:
-            raise ValueError(f"mask_sky must be a bool or a bool tensor, got {getattr(mask_sky, 'dtype', type(mask_sky))}")
-        images = predictions["images"]
-        want = (tuple(images.shape[:2]) if images.dim() == 5 else (images.shape[0],)) + tuple(images.shape[-2:])
-        if mask_sky.dim() == 4 and images.dim() == 5:
-            ok = tuple(mask_sky.shape) == want
-        else:
-            ok = tuple(mask_sky.shape) == want[-3:]
-        if not ok:
-            raise ValueError(f"mask_sky must have shape [S, H, W] = {list(want[-3:])}"
-                             + (f" or [B, S, H, W] = {list(want)}" if images.dim() == 5 else "") + f", got {list(mask_sky.shape)}")
-        if mask_sky.device != images.device:
-            raise ValueError(f"mask_sky is on {mask_sky.device}, the images on {images.device}")
-
-    @staticmethod
-    def _sky_conf(mask_sky, images: torch.Tensor, conf: torch.Tensor, scene: int) -> torch.Tensor:
-        """conf [S,H,W] of the scene times non-sky, over all S views, as visual_util.py:186-188 does before the frame selection
-        and the percentile.  mask_sky False: conf unchanged, no launch."""
-        from . import ops
-        if isinstance(mask_sky, (bool, np.bool_)):
-            if not mask_sky:
-                return conf
-            _, out = OmniVGGT._segment_views(images, conf.float().contiguous())
-            return out
-        sky = mask_sky[scene] if mask_sky.dim() == 4 else mask_sky
-        return ops.sky_mask_conf(conf.float().contiguous(), sky.contiguous().view(torch.uint8))
-
-    @staticmethod
-    @torch.no_grad()
-    def matches(predictions: Dict[str, object], pairs=None, *, source: str = "depth", conf_percent: float = 50.0,
-                conf_floor: float = 1e-5, scene: int = 0, mask_sky=False) -> List[Dict[str, object]]:
-        """Dense cross-view correspondences of one scene by reciprocal nearest neighbours of the predicted points (the
-        DUSt3R-family recipe on utils/geometry.py:435-451 find_reciprocal_matches and :15-37 xy_grid), on the device.
-
-        ``source`` and the keep mask are ``point_cloud``'s: conf >= percentile(conf over the scene's S views, conf_percent) and
-        conf > conf_floor.  For each pair (i, j) (default: every i < j), P1 and P2 are the kept points of views i and j in
-        row-major order, and the result is ``{"xy_i", "xy_j", "count"}`` with ``xy_j = grid_j[kept_j][reciprocal_in_P2]`` and
-        ``xy_i = grid_i[kept_i][nn2_in_P1][reciprocal_in_P2]``: int64 [count, 2] (x, y) pixel coordinates on the device.
-        Every view's index is built once; all pairs are queried in one pass; the match counts are the one host read.  Kept
-        points that are not finite raise ValueError; a view with no kept point has no matches.  ``mask_sky``: as in
-        ``point_cloud``."""
-        from . import geometry, ops
-        S = OmniVGGT._check_views(predictions, source, conf_percent, conf_floor, None, scene, mask_sky)
-        pair_arr = geometry.check_pairs(pairs, S)
-        if len(pair_arr) == 0:
-            return []
-        images, _, points, mask, _, _ = OmniVGGT._kept_views(predictions, source, conf_percent, conf_floor, None, scene, mask_sky)
-        _, _, H, W = images.shape
-        mt = ops.Matcher(points.view(S, H * W, 3), mask.view(S, H * W), torch.from_numpy(pair_arr).to(images.device))
-        counts, nonfinite = mt.counts()
-        if nonfinite:
-            raise ValueError("kept points must be finite (cKDTree: data must be finite, check for nan or inf values)")
-        xy_i, xy_j = mt.gather(sum(counts), W)
-        return [{"xy_i": a, "xy_j": b, "count": c} for a, b, c in zip(xy_i.split(counts), xy_j.split(counts), counts)]
-
-    @staticmethod
-    @torch.no_grad()
-    def tracks(predictions: Dict[str, object], pairs=None, *, source: str = "depth", conf_percent: float = 50.0,
-               conf_floor: float = 1e-5, scene: int = 0, mask_sky=False, min_views: int = 2) -> Dict[str, torch.Tensor]:
-        """Multi-view tracks of one scene for a COLMAP sparse model (``colmap.write_colmap``), built on the device from the
-        reciprocal matches of ``matches``; no counterpart in the reference.
-
-        ``source``, the keep mask, ``mask_sky`` and ``pairs`` are those of ``matches``; (i, j) and (j, i) are one pair and
-        duplicates are merged.  Star tracks: views anchor in order a = 0 .. S-1; every kept pixel of view a not yet in a
-        track gathers its partners, its reciprocal match in each view j > a of a pair (a, j) that is not in a track either,
-        and when 1 + partners >= ``min_views`` (in [1, S]; 1 turns every remaining kept pixel into a one-view point) they
-        become one new track.  Tracks are numbered by (anchor view, anchor pixel in row-major order); each has at most one
-        observation per view, in ascending view order, and every pixel is in at most one track.  Matches are not chained
-        across pairs: reciprocal nearest neighbours of different pairs are not transitive.
-
-        Returns on the device, per track: ``points`` fp64 [n, 3] (the mean of the observations' points, not rounded to
-        fp32), ``colors`` uint8 [n, 3] (the anchor pixel's, as ``point_cloud`` computes colours), ``error`` fp64 [n] (mean
-        reprojection distance in pixels, COLMAP's pixel-centre convention, +inf when a camera sees the point behind it) and
-        ``offsets`` int64 [n + 1]; per observation: ``view`` int32 [m], ``xy`` int64 [m, 2] (x, y) and ``point2d`` int32
-        [m] (rank of the pixel in its view's list); per view: ``view_offsets`` int64 [S + 1], ``view_track`` int32 [m] and
-        ``view_xy`` int64 [m, 2], each view's pixels in tracks in row-major order; and the ``extrinsic`` / ``intrinsic``
-        used, decoded from ``pose_enc`` where the predictions do not hold them.  The counts are the one host read; kept
-        points that are not finite raise ValueError."""
-        from . import geometry, ops
-        S = OmniVGGT._check_views(predictions, source, conf_percent, conf_floor, None, scene, mask_sky)
-        if isinstance(min_views, (bool, np.bool_)) or not isinstance(min_views, (int, np.integer)) or not 1 <= min_views <= S:
-            raise ValueError(f"min_views must be an integer in [1, {S}], got {min_views!r}")
-        pair_arr = geometry.check_pairs(pairs, S)
-        pair_arr = np.unique(np.sort(pair_arr, axis=1), axis=0).astype(np.int32).reshape(-1, 2)
-        H, W = predictions["images"].shape[-2:]
-        if S * H * W >= 2 ** 31:
-            raise ValueError(f"tracks need views * H * W < 2^31, got {S} x {H} x {W}")
-        ext, intr = OmniVGGT._scene_cameras(predictions, scene, H, W)
-        images, _, points, mask, _, _ = OmniVGGT._kept_views(predictions, source, conf_percent, conf_floor, None, scene, mask_sky)
-        # the pairs of anchor a are pair_arr[pair_off[a]:pair_off[a + 1]]; the matcher sizes its workspace by at least one
-        # pair, so without pairs it queries view 0 against itself, which no anchor reads
-        pair_off = np.searchsorted(pair_arr[:, 0], np.arange(S + 1)).astype(np.int32)
-        queried = pair_arr if len(pair_arr) else np.zeros((1, 2), np.int32)
-        dev = images.device
-        packed = torch.from_numpy(np.concatenate([queried.ravel(), pair_off])).to(dev)
-        mt = ops.Matcher(points.view(S, H * W, 3), mask.view(S, H * W), packed[:queried.size].view(-1, 2))
-        tr = ops.Tracker(mt, packed[queried.size:], min_views)
-        n, m, nonfinite = tr.counts()
-        if nonfinite:
-            raise ValueError("kept points must be finite (cKDTree: data must be finite, check for nan or inf values)")
-        out = tr.gather(images, ext, intr, W, n, m)
-        out.update(extrinsic=ext, intrinsic=intr)
-        return out
-
-    @staticmethod
-    def _scene_cameras(predictions: Dict[str, object], scene: int, H: int, W: int):
-        """(extrinsic fp32 [S,3,4], intrinsic fp32 [S,3,3]) of one scene, contiguous: the predictions' own, or those that
-        ``postprocess`` decodes from ``pose_enc`` where they are missing."""
-        from . import ops
-        cams = {}
-        for key, trailing in (("extrinsic", 2), ("intrinsic", 2)):
-            if key in predictions:
-                t = predictions[key]
-                cams[key] = (t[scene] if t.dim() == trailing + 2 else t).float().contiguous()
-        if len(cams) < 2:
-            if "pose_enc" not in predictions:
-                raise ValueError("tracks need extrinsic and intrinsic, or pose_enc to decode them from")
-            pose = predictions["pose_enc"]
-            ext, intr, _ = ops.pose_decode((pose[scene] if pose.dim() == 3 else pose).float().contiguous(), H, W)
-            cams.setdefault("extrinsic", ext)
-            cams.setdefault("intrinsic", intr)
-        return cams["extrinsic"], cams["intrinsic"]
-
-    @staticmethod
-    @torch.no_grad()
-    def point_cloud(predictions: Dict[str, object], *, source: str = "depth", conf_percent: float = 50.0,
-                    conf_floor: float = 1e-5, frame: Optional[int] = None, mask_black_bg: bool = False,
-                    mask_white_bg: bool = False, scene: int = 0, mask_sky=False,
-                    max_points: Optional[int] = None) -> Dict[str, torch.Tensor]:
-        """The filtered, coloured point cloud of one scene, built on the device (libovg kernels).
-
-        Replaces the host numpy of the reference's GLB export (visual_util.py:190-236,:320-358 predictions_to_glb) and
-        viewer (inference.py:96-151).  ``source="depth"``: ``world_points_from_depth`` (computed here when ``postprocess``
-        has not run) with ``depth_conf``, as ``--save_glb`` uses it; ``"pointmap"``: ``world_points`` with
-        ``world_points_conf``.  ``frame``: keep only that view, selected before the percentile (visual_util.py:190-194).
-        Kept: conf >= percentile(conf, conf_percent) (0 for conf_percent == 0, visual_util.py:206-207) and conf > conf_floor,
-        minus black / white background pixels when asked.  ``conf_floor=0.1`` reproduces the viewer's initial mask
-        (inference.py:132-133); its frame dropdown is ``cloud["frame"] == i`` on the ``frame=None`` cloud.
-
-        Returns ``points`` fp32 [n,3], ``colors`` uint8 [n,3], ``frame`` int32 [n] (numpy boolean-indexing order),
-        ``conf_threshold`` (0-d), ``center`` fp32 [3] (mean of all points of the selected views, inference.py:111),
-        ``scale`` (0-d, ||p95 - p5||, 1.0 when nothing is kept) and ``align`` fp64 [4,4] = inv(E0) diag(1,-1,-1,1) R_y(180)
-        with E0 the first selected camera (visual_util.py:320-341).  The kept count and E0 are the only device-to-host reads.
-
-        ``mask_sky`` (the reference's --mask_sky, visual_util.py:140-188): False, no sky masking; True, the sky of every view
-        by ``sky_mask``; or a bool tensor [S,H,W] / [B,S,H,W], True = sky (a reference mask file m, uint8 255 = non-sky, at
-        H x W is ``m == 0``).  The confidence of every view becomes conf * non-sky before the frame selection and the
-        percentile, as the reference orders it; no host read is added.
-
-        ``max_points`` (None: every kept point): when more than max_points points are kept, ``points``, ``colors`` and
-        ``frame`` are those of the reference's farthest_point_sample (po_utils/misc.py:114-148, deterministic, from the first
-        kept point) over the kept points, max_points of them in selection order, so every prefix is a coarser sample of the
-        whole cloud.  ``conf_threshold``, ``center``, ``scale`` and ``align`` stay those of all kept points.  A cloud with fewer
-        than max_points distinct positions repeats points, as the reference's indices do.  One more launch, no host read."""
-        from . import ops
-        OmniVGGT._check_views(predictions, source, conf_percent, conf_floor, frame, scene, mask_sky)
-        if max_points is not None and (isinstance(max_points, (bool, np.bool_)) or not isinstance(max_points, (int, np.integer))
-                                       or max_points < 1):
-            raise ValueError(f"max_points must be None or an integer >= 1, got {max_points!r}")
-        images, ext, points, mask, thr, f0 = OmniVGGT._kept_views(predictions, source, conf_percent, conf_floor, frame, scene,
-                                                                  mask_sky)
-        F, _, H, W = images.shape
-        dev = images.device
-        ws = ops.point_cloud_workspace(F * H * W, dev)
-        cnt = ops.point_cloud_count(mask, images, ws, mask_black_bg, mask_white_bg)
-        center = ops.point_cloud_center(points, ws)
-        host = ops.host_read(torch.cat([cnt.double().reshape(1), ext[f0].double().reshape(-1)]))   # count < 2^31: exact
-        n = int(host[0])
-        align = OmniVGGT._align(host[1:].view(3, 4)).to(dev)
-        if n == 0:
-            return {"points": torch.empty(0, 3, device=dev), "colors": torch.empty(0, 3, device=dev, dtype=torch.uint8),
-                    "frame": torch.empty(0, device=dev, dtype=torch.int32), "conf_threshold": thr, "center": center,
-                    "scale": torch.ones((), device=dev), "align": align}
-        pts, cols, fr, xyz = ops.point_cloud_gather(points, mask, images, ws, n, mask_black_bg, mask_white_bg, f0)
-        scale = ops.point_cloud_scale(xyz, n, ws)
-        if max_points is not None and n > max_points:
-            idx = ops.farthest_point_sample(pts[None], int(max_points), torch.zeros(1, device=dev, dtype=torch.int64))[0]
-            pts, cols, fr = pts[idx], cols[idx], fr[idx]
-        return {"points": pts, "colors": cols, "frame": fr, "conf_threshold": thr, "center": center, "scale": scale,
-                "align": align}
-
-    @staticmethod
-    def _align(e0: torch.Tensor) -> torch.Tensor:
-        """inv(E0) diag(1,-1,-1,1) R_y(180), fp64 [4,4] on the host, from the host camera E0 [3,4] (visual_util.py:320-341)."""
-        e = torch.eye(4, dtype=torch.float64)
-        e[:3, :4] = e0
-        gl = torch.diag(torch.tensor([1.0, -1.0, -1.0, 1.0], dtype=torch.float64))
-        rot_y = torch.diag(torch.tensor([-1.0, 1.0, -1.0, 1.0], dtype=torch.float64))
-        return torch.linalg.inv(e) @ gl @ rot_y
-
-    @staticmethod
-    @torch.no_grad()
-    def mesh(predictions: Dict[str, object], *, source: str = "depth", conf_percent: float = 50.0, conf_floor: float = 1e-5,
-             frame: Optional[int] = None, mask_black_bg: bool = False, mask_white_bg: bool = False, scene: int = 0,
-             layout: str = "reference", mask_sky=False) -> Dict[str, torch.Tensor]:
-        """The coloured triangle mesh of one scene's point maps, built on the device (libovg kernels): the DUSt3R-family
-        recipe of viz.py:40-89, ``cat_meshes([pts3d_to_trimesh(colors[f], points[f], keep[f]) for f in views])``.
-
-        ``source``, ``conf_percent``, ``conf_floor``, ``frame``, the background masks and ``scene`` select the views and the
-        kept pixels exactly as in ``point_cloud``; colours are (images * 255).astype(uint8).  Every pixel quad gives two
-        triangles, (tl, tr, bl) and (tr, bl, br); a triangle is kept when its three pixels are.
-
-        ``layout="reference"``: ``vertices`` fp32 [F*H*W, 3] (every point of the selected views), ``face_colors`` uint8 [n, 3]
-        and ``faces`` int64 [n, 3], as viz.py returns them: per view the kept (tl, tr, bl) triangles, the same reversed, the kept
-        (tr, bl, br) triangles, the same reversed, each in row-major order; colours from tl and br.
-        ``layout="glb"``: ``positions`` fp32 [m, 3] and ``colors`` uint8 [m, 3] of the vertices the forward triangles use, in
-        index order, each with its own pixel's colour, and ``indices`` int32 [k, 3] of the forward triangles only, for
-        ``glb.write_mesh_glb`` (whose material is double-sided in place of the reversed copies).
-        Both add ``conf_threshold`` and ``align``, as ``point_cloud`` returns them.  The three totals and the first camera are
-        read back together: the one host synchronisation.  ``mask_sky``: as in ``point_cloud``."""
-        from . import ops
-        OmniVGGT._check_views(predictions, source, conf_percent, conf_floor, frame, scene, mask_sky)
-        if layout not in ("reference", "glb"):
-            raise ValueError(f"layout must be 'reference' or 'glb', got {layout!r}")
-        images, ext, points, mask, thr, f0 = OmniVGGT._kept_views(predictions, source, conf_percent, conf_floor, frame, scene,
-                                                                  mask_sky)
-        F, _, H, W = images.shape
-        mesher = ops.Mesher(mask.view(-1), images, F, H, W, mask_black_bg, mask_white_bg)
-        host = ops.host_read(torch.cat([mesher.totals.double(), ext[f0].double().reshape(-1)]))   # totals < 2^33: exact
-        n_ref, n_used, n_fwd = (int(v) for v in host[:3].tolist())
-        align = OmniVGGT._align(host[3:].view(3, 4)).to(images.device)
-        if layout == "glb":
-            pos, cols, idx = mesher.compact(points.view(-1, 3), n_used, n_fwd)
-            return {"positions": pos, "colors": cols, "indices": idx, "conf_threshold": thr, "align": align}
-        faces, face_colors = mesher.faces(n_ref)
-        return {"vertices": points.view(-1, 3).clone(), "face_colors": face_colors, "faces": faces, "conf_threshold": thr,
-                "align": align}
+    # ---------------------------------------------------------------------------------------------- post-processing (scene.py)
+    postprocess = staticmethod(SC.postprocess)
+    sky_mask = staticmethod(SC.sky_mask)
+    point_cloud = staticmethod(SC.point_cloud)
+    mesh = staticmethod(SC.mesh)
+    matches = staticmethod(SC.matches)
+    tracks = staticmethod(SC.tracks)
+    _kept_views = staticmethod(SC._kept_views)          # their shared helpers, reached from the class as before
+    _align = staticmethod(SC._align)
 
     # ---------------------------------------------------------------------------------------------- long captures
     @torch.no_grad()
@@ -672,7 +340,6 @@ class OmniVGGT(nn.Module, PyTorchModelHubMixin):
         is not returned: it is normalised per view set.  The alignment statistics are read once per set boundary, and a
         degenerate overlap raises ValueError naming the set and its views.  Errors accumulate along the chain of sets (no
         loop closure)."""
-        from . import ops
         if self._cp is not None:
             raise RuntimeError("reconstruct runs its view sets on one GPU; under enable_context_parallel() call the model itself")
         if images.dim() == 4:
@@ -680,7 +347,7 @@ class OmniVGGT(nn.Module, PyTorchModelHubMixin):
         if images.dim() != 5 or images.shape[0] != 1:
             raise ValueError(f"reconstruct takes one scene (B = 1), got images of shape {tuple(images.shape)}")
         for name, v in (("chunk", chunk), ("overlap", overlap)):
-            if isinstance(v, (bool, np.bool_)) or not isinstance(v, (int, np.integer)):
+            if not _is_int(v):
                 raise ValueError(f"{name} must be an integer, got {v!r}")
         if chunk < 2:
             raise ValueError(f"chunk must be >= 2, got {chunk}")
@@ -707,9 +374,9 @@ class OmniVGGT(nn.Module, PyTorchModelHubMixin):
             raw = self(images[:, a:b], part(extrinsics), part(intrinsics), part(depth), part(mask), depth_gt_index=di,
                        camera_gt_index=ci)
             n = b - a
-            ext, intr, c2w = ops.pose_decode(raw["pose_enc"][0].float().contiguous(), H, W)
+            ext, intr, world = SC.decode_cameras(raw["pose_enc"][0], raw["depth"][0], H, W)
             r = {"extrinsic": ext, "intrinsic": intr, "depth": raw["depth"][0], "depth_conf": raw["depth_conf"][0],
-                 "world_points_from_depth": ops.unproject_depth(raw["depth"][0].float().reshape(n, H, W), intr, c2w, H, W)}
+                 "world_points_from_depth": world}
             if "world_points" in raw:
                 r["world_points"], r["world_points_conf"] = raw["world_points"][0], raw["world_points_conf"][0]
             del raw

@@ -46,7 +46,7 @@ GUARD = 4096                 # keeps the 256-byte workspace and 16-byte TMA alig
 GUARD_BYTE = 0x5A
 PATTERNS = ("nan", "zero", "finite")
 _BYTES = {"nan": (0xFF, 0xFF), "zero": (0x00, 0x00), "finite": (0x3F, 0xFF)}     # (float tensors, other tensors)
-PACKAGE_MODULES = ("ops", "engine", "model", "geometry", "preprocess", "pipeline", "torch_parts")
+PACKAGE_MODULES = ("ops", "engine", "model", "scene", "geometry", "preprocess", "pipeline", "torch_parts")
 
 
 def _kind(frame, shape, dtype) -> str:

@@ -56,8 +56,9 @@ def main():
     ap.add_argument("--reps", type=int, default=3)
     ap.add_argument("--single-max", type=int, default=192)
     args = ap.parse_args()
-    from omnivggt_official_b200 import OmniVGGT, ops
+    from omnivggt_official_b200 import OmniVGGT
     from omnivggt_official_b200.model import chunk_schedule
+    from omnivggt_official_b200.scene import decode_cameras
     from oracle.synth import make_inputs
     H = W = 518
     with torch.device("cuda"):
@@ -81,10 +82,10 @@ def main():
         merged = {k: v.clone() for k, v in out.items() if torch.is_tensor(v) and k not in ("images", "sim3", "align_pairs",
                                                                                             "align_rmse")}
         raw = m(images[:, a:b])
-        ext, intr, c2w = ops.pose_decode(raw["pose_enc"][0].float().contiguous(), H, W)
+        ext, intr, world = decode_cameras(raw["pose_enc"][0], raw["depth"][0], H, W)
         r = {"extrinsic": ext, "intrinsic": intr, "depth": raw["depth"][0], "depth_conf": raw["depth_conf"][0],
              "world_points": raw["world_points"][0], "world_points_conf": raw["world_points_conf"][0],
-             "world_points_from_depth": ops.unproject_depth(raw["depth"][0].float().reshape(b - a, H, W), intr, c2w, H, W)}
+             "world_points_from_depth": world}
         del raw, out
         row["boundary_ms"] = round(_events(lambda: OmniVGGT._merge_view_set(merged, r, 1, a, n0, b, "depth", 50.0),
                                            max(args.reps, 5)), 3)
