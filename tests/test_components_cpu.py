@@ -1,5 +1,5 @@
 """Component calls and heads set to None (CPU): the module against a recorder in place of the C library, as in
-test_dryrun_cpu.py, but recording every call's arguments.  What is checked: which heads get a libovg handle, which entry points a
+test_dryrun_cpu.py, looking at every call's arguments.  What is checked: which heads get a libovg handle, which entry points a
 forward or a component call issues and with which pointers, the output keys for every subset of heads (reference
 models/omnivggt.py:46-62), and that the owner back-references leave the parameter / state-dict / module tree unchanged."""
 import copy
@@ -11,38 +11,11 @@ import torch
 
 from conftest import golden_schema
 from oracle.synth import make_inputs
-from test_host_cpu import mini_model
+from ovg_support import dry, mini_model  # noqa: F401  (fixture)
 
 HEADS = ("camera_head", "depth_head", "point_head")
 KEYS = {"camera_head": ("pose_enc", "pose_enc_list"), "depth_head": ("depth", "depth_conf"),
         "point_head": ("world_points", "world_points_conf")}
-
-
-class _ArgRecorder:
-    def __init__(self):
-        self.calls = []
-
-    def __getattr__(self, name):
-        def fn(*a):
-            self.calls.append((name, a))
-            return 0
-        return fn
-
-    def count(self, name):
-        return sum(n == name for n, _ in self.calls)
-
-    def args(self, name):
-        return [a for n, a in self.calls if n == name]
-
-
-@pytest.fixture()
-def dry(monkeypatch):
-    from omnivggt_official_b200 import _lib, ops
-    rec = _ArgRecorder()
-    monkeypatch.setattr(_lib, "lib", lambda: rec)
-    monkeypatch.setattr(_lib, "stream", lambda: 0)
-    monkeypatch.setattr(ops, "_on_device", lambda t: True)
-    return rec
 
 
 def _model(variant="mini_conv"):

@@ -16,7 +16,8 @@ from safetensors.torch import load_file
 from conftest import GOLDEN, golden_index, golden_schema
 from oracle import omnivggt_oracle as O
 from oracle.synth import make_inputs, make_state_dict
-from test_model_gpu import build, rel
+from ovg_support import rel
+from test_model_gpu import build
 
 pytestmark = pytest.mark.gpu
 INDEX = golden_index()
@@ -97,7 +98,7 @@ def test_exported_layers_match_the_reference_tokens(case):
     assert ps == 5 and len(layers) == 4
     for t in layers:
         assert t.shape == (B, S, T, 256) and t.dtype == torch.float32 and t.is_cuda and torch.isfinite(t).all()
-    errs = {"agg_first": rel(layers[0], ref["agg_first"]), "agg_last": rel(layers[-1], ref["agg_last"])}
+    errs = {"agg_first": rel(layers[0], ref["agg_first"], host=True), "agg_last": rel(layers[-1], ref["agg_last"], host=True)}
     _record(f"exported layers {case} " + json.dumps({k: round(v, 6) for k, v in errs.items()}))
     assert errs["agg_first"] < TOL and errs["agg_last"] < TOL, errs
 
@@ -125,9 +126,9 @@ def test_reference_tokens_into_these_heads():
     got["depth"], got["depth_conf"] = m.depth_head(gpu_tokens, images, ns)
     got["world_points"], got["world_points_conf"] = m.point_head(gpu_tokens, images, ns)
     poses = m.camera_head(tokens)                                  # CPU tensors are moved to the device
-    errs = {k: rel(got[k], want[k]) for k in want}
+    errs = {k: rel(got[k], want[k], host=True) for k in want}
     for i in range(4):
-        errs[f"pose_enc_list.{i}"] = rel(poses[i], want_pose[i])
+        errs[f"pose_enc_list.{i}"] = rel(poses[i], want_pose[i], host=True)
     _record("oracle tokens into heads " + json.dumps({k: round(v, 6) for k, v in errs.items()}))
     for k, e in errs.items():
         assert e < TOL, (k, errs)

@@ -11,41 +11,17 @@ import torch
 import torch.nn.functional as Fn
 
 from oracle import kernel_ref as R
+from ovg_support import guarded, guards_ok, lib_module, margin, ops_module
 
 pytestmark = pytest.mark.gpu
 
 BF16, F16, F32, F64 = torch.bfloat16, torch.float16, torch.float32, torch.float64
-GUARD = 4096
 SENT = -7.0e30          # fp32 sentinel: an element the kernel should have written and did not is far outside any bound
-
-
-def _ops():
-    from omnivggt_official_b200 import ops
-    return ops
-
-
-def _L():
-    from omnivggt_official_b200 import _lib
-    return _lib
 
 
 @pytest.fixture(scope="module")
 def sms():
     return torch.cuda.get_device_properties(0).multi_processor_count
-
-
-def _margin(name, r):
-    print(f"margin {name}: {r:.3f}")
-
-
-def _guarded(n, dtype, fill):
-    buf = torch.full((GUARD + n + GUARD,), fill, device="cuda", dtype=dtype)
-    return buf, buf[GUARD:GUARD + n]
-
-
-def _guards_ok(buf, fill):
-    ref = torch.full((GUARD,), fill, device="cuda", dtype=buf.dtype)
-    return torch.equal(buf[:GUARD], ref) and torch.equal(buf[-GUARD:], ref)
 
 
 def _kernels(fn):
@@ -88,17 +64,17 @@ def _dyadic_bits(n_src, n_dst):
 def _upsample(src, H, W, tx, ty, dtype, fill=-3.0):
     """ovg_upsample_bilinear on the interior src [F, h, w, C] (cpu fp64 / 16-bit values), output between guards.  Returns the
     interior [F, H, W, C] and the kernels launched; asserts the border is zero and the guards are intact."""
-    ops = _ops()
+    ops = ops_module()
     Fr, h, w, C = src.shape
     xp = Fn.pad(src.to(F64), (0, 0, 1, 1, 1, 1)).to(dtype).cuda()
-    buf, flat = _guarded(Fr * (H + 2) * (W + 2) * C, dtype, fill)
+    buf, flat = guarded(Fr * (H + 2) * (W + 2) * C, dtype, fill)
     txd = tx.float().cuda() if tx is not None else None
     tyd = ty.float().cuda() if ty is not None else None
     names = _kernels(lambda: ops.upsample_bilinear(xp, flat, txd, tyd, Fr, h, w, H, W, C))
     out = flat.view(Fr, H + 2, W + 2, C)
     border = out.clone()
     border[:, 1:-1, 1:-1] = 0
-    assert (border == 0).all() and _guards_ok(buf, fill)
+    assert (border == 0).all() and guards_ok(buf, fill)
     want = "upsample_rows_kernel" if R.upsample_path(w, C) == "rows" else "upsample_bilinear_kernel"
     assert _ran(names, want) and not _ran(names, "upsample_rows_kernel" if want != "upsample_rows_kernel" else
                                           "upsample_bilinear_kernel"), names
@@ -164,7 +140,7 @@ def test_upsample_bound(name, Fr, h, w, H, W, C, tables, dtype):
     out, path = _upsample(src, H, W, tx, ty, dtype)
     ref, bound = R.bilinear_ref(src.cuda(), H, W, tx, ty, dtype)
     r, f = R.check_rounded(out, ref, bound, dtype, f"upsample {name} ({path})", ("frame", "y", "x", "c"))
-    _margin(f"upsample {name} {dtype} ({path})", r)
+    margin(f"upsample {name} {dtype} ({path})", r)
     print(f"  equal to round(ref): {f:.5f}")
 
 
@@ -188,7 +164,7 @@ def test_upsample_fp16_saturates(C):
 def _tail(src, tx, ty, wb, b1, w2, b2, act, H, W, dtype, names=False):
     """ovg_dpt_tail through the C entry point: guarded preds, conf and scratch.  Returns (preds, conf, gx, gy) on the device
     (gx, gy: the tables read back from the scratch; None without tables)."""
-    L = _L()
+    L = lib_module()
     Fr, h, w, C = src.shape
     outc = w2.shape[0]
     xp = Fn.pad(src.to(F64), (0, 0, 1, 1, 1, 1)).to(dtype).cuda().contiguous()
@@ -196,9 +172,9 @@ def _tail(src, tx, ty, wb, b1, w2, b2, act, H, W, dtype, names=False):
     b1d, w2d, b2d = b1.float().cuda(), w2.float().cuda().contiguous(), b2.float().cuda()
     txd = tx.float().cuda().contiguous() if tx is not None else None
     tyd = ty.float().cuda().contiguous() if ty is not None else None
-    pbuf, preds = _guarded(Fr * H * W * (outc - 1), F32, SENT)
-    cbuf, conf = _guarded(Fr * H * W, F32, SENT)
-    sbuf, scratch = _guarded(L.lib().ovg_dpt_tail_scratch_bytes(H, W) // 4, F32, SENT)
+    pbuf, preds = guarded(Fr * H * W * (outc - 1), F32, SENT)
+    cbuf, conf = guarded(Fr * H * W, F32, SENT)
+    sbuf, scratch = guarded(L.lib().ovg_dpt_tail_scratch_bytes(H, W) // 4, F32, SENT)
 
     def run():
         L.check(L.lib().ovg_dpt_tail(xp.data_ptr(), L.ptr(txd), L.ptr(tyd), wbd.data_ptr(), b1d.data_ptr(), w2d.data_ptr(),
@@ -208,7 +184,7 @@ def _tail(src, tx, ty, wb, b1, w2, b2, act, H, W, dtype, names=False):
     if not names:
         run()
     torch.cuda.synchronize()
-    assert _guards_ok(pbuf, SENT) and _guards_ok(cbuf, SENT) and _guards_ok(sbuf, SENT)
+    assert guards_ok(pbuf, SENT) and guards_ok(cbuf, SENT) and guards_ok(sbuf, SENT)
     if ks is not None:
         assert _ran(ks, "fusedtail_kernel") and _ran(ks, "tail_tables_kernel") == (tx is not None), ks
     gx = gy = None
@@ -244,7 +220,7 @@ def test_dpt_tail_exact(h, w, H, W, outc, act, dtype, tables, sms):
         assert sch["n_strips"] >= 3 and sch["last_strip_px"] == 1, sch
     if H < 8:
         assert sch["seg_rows"] < 8, sch
-    assert R.tail_supported(h, w, H, W) and _L().lib().ovg_dpt_tail_supported(h, w, H, W, 128) == 1
+    assert R.tail_supported(h, w, H, W) and lib_module().lib().ovg_dpt_tail_supported(h, w, H, W, 128) == 1
     src, _, _, b = _exact_inputs(Fr, h, w, H, W, 128, seed=h * 100 + W)
     g = _gen(W)
     qt = 4
@@ -272,7 +248,7 @@ def test_dpt_tail_exact(h, w, H, W, outc, act, dtype, tables, sms):
         assert torch.equal(gx.double().cpu(), rgx) and torch.equal(gy.double().cpu(), rgy)
     r1 = R.check_bound(preds, rp, bp, "tail preds (exact tier)", ("frame", "y", "x", "c"))
     r2 = R.check_bound(conf, rc, bc, "tail conf (exact tier)", ("frame", "y", "x"))
-    _margin(f"dpt tail exact {h}x{w}->{H}x{W} outc={outc} act={act} {dtype} (libm ulps / 2)", max(r1, r2))
+    margin(f"dpt tail exact {h}x{w}->{H}x{W} outc={outc} act={act} {dtype} (libm ulps / 2)", max(r1, r2))
 
 
 def _span(w, W):
@@ -309,8 +285,8 @@ def test_dpt_tail_bound(name, Fr, h, w, H, W, outc, act, dtype, tables, sms):
     if W == "span80":
         W = _span80_W(w)
         assert _span(w, W) == 80 and _span(w, W - 1) > 80
-        assert _L().lib().ovg_dpt_tail_supported(h, w, H, W - 1, 128) == 0
-    assert _L().lib().ovg_dpt_tail_supported(h, w, H, W, 128) == 1
+        assert lib_module().lib().ovg_dpt_tail_supported(h, w, H, W - 1, 128) == 0
+    assert lib_module().lib().ovg_dpt_tail_supported(h, w, H, W, 128) == 1
     sch = R.tail_schedule(Fr, H, W, sms)
     if W in (256, 384):
         assert W - 128 * (sch["n_strips"] - 1) + 1 == 129              # zrow: the last row of the A stage
@@ -328,7 +304,7 @@ def test_dpt_tail_bound(name, Fr, h, w, H, W, outc, act, dtype, tables, sms):
     r1 = R.check_bound(preds, rp, bp, f"tail preds {name}", ("frame", "y", "x", "c"))
     r2 = R.check_bound(conf, rc, bc, f"tail conf {name}", ("frame", "y", "x"))
     print(f"tail {name}: F={Fr} {h}x{w}->{H}x{W} schedule {sch}")
-    _margin(f"dpt tail {name} {dtype}", max(r1, r2))
+    margin(f"dpt tail {name} {dtype}", max(r1, r2))
     if Fr == 3:   # no atomics: a second run is bit-identical
         p2, c2, _, _ = _tail(src, tx, ty, wb, b1, w2, b2, act, H, W, dtype)
         assert torch.equal(p2, preds) and torch.equal(c2, conf)
@@ -338,14 +314,14 @@ def test_dpt_tail_bound(name, Fr, h, w, H, W, outc, act, dtype, tables, sms):
 @pytest.mark.parametrize("C", [8, 256, 1024, 2048])
 def test_im2col3x3s2_exact(C):
     """dst = F.unfold(pad 1, stride 2) of the NHWC input, rows (f, oy, ox) x columns (tap, c), bit for bit, between guards."""
-    ops = _ops()
+    ops = ops_module()
     Fr = 2
     sizes = (1, 2, 3, 19, 37, 38)
     for h in sizes:
         for w in sizes:
             src = torch.randn(Fr, h, w, C, device="cuda").to(BF16)
             oh, ow = (h - 1) // 2 + 1, (w - 1) // 2 + 1
-            buf, flat = _guarded(Fr * oh * ow * 9 * C, BF16, -3.0)
+            buf, flat = guarded(Fr * oh * ow * 9 * C, BF16, -3.0)
             ops.im2col3x3s2(src, flat, Fr, h, w, C)
             u = Fn.unfold(src.float().permute(0, 3, 1, 2), 3, padding=1, stride=2)           # [F, C*9, oh*ow]
             exp = u.view(Fr, C, 9, oh * ow).permute(0, 3, 2, 1).reshape(Fr * oh * ow, 9 * C).to(BF16)
@@ -353,7 +329,7 @@ def test_im2col3x3s2_exact(C):
             got = flat.view(Fr * oh * ow, 9 * C)
             bad = (got != exp).nonzero()
             assert bad.numel() == 0, f"h={h} w={w} C={C}: first mismatch (row, col) {tuple(bad[0].tolist())}"
-            assert _guards_ok(buf, -3.0), (h, w, C)
+            assert guards_ok(buf, -3.0), (h, w, C)
 
 
 # ldc 592: the DINOv2 patchifier's row stride (3 x 14^2 = 588 rounded up to a multiple of 8), at the 392- and 882-pixel-high
@@ -363,14 +339,14 @@ def test_im2col3x3s2_exact(C):
 def test_image_im2col_exact(patch, H, W, ldc):
     """ovg_image_im2col bit for bit against the fp32 restatement: the patch-14 template and the runtime-patch kernel, H != W,
     padding columns (ldc > 3 patch^2) pre-filled with a sentinel must come back zero."""
-    L = _L()
+    L = lib_module()
     import ctypes
     K = 3
     g = torch.Generator(device="cuda").manual_seed(patch + H)
     images = torch.rand(K, 3, H, W, generator=g, device="cuda")
     mean3, std3 = (0.485, 0.456, 0.406), (0.229, 0.224, 0.225)
     rows = K * (H // patch) * (W // patch)
-    buf, flat = _guarded(rows * ldc, BF16, -3.0)
+    buf, flat = guarded(rows * ldc, BF16, -3.0)
     m = (ctypes.c_float * 3)(*mean3)
     s = (ctypes.c_float * 3)(*std3)
     names = _kernels(lambda: L.check(L.lib().ovg_image_im2col(images.data_ptr(), ctypes.cast(m, ctypes.c_void_p),
@@ -381,25 +357,25 @@ def test_image_im2col_exact(patch, H, W, ldc):
     got = flat.view(rows, ldc).cpu()
     bad = (got != exp).nonzero()
     assert bad.numel() == 0, f"first mismatch (row, col) {tuple(bad[0].tolist())}: {got[tuple(bad[0])]} vs {exp[tuple(bad[0])]}"
-    assert _guards_ok(buf, -3.0)
+    assert guards_ok(buf, -3.0)
 
 
 def _depth_call(depth, mask, idx_stats, idx_cols, B, S, H, W, patch, ldc, fill=-3.0):
     """ovg_depth_im2col with separate view lists; returns (scale fp32 [B], cols [rows, 2 patch^2]) after checking the guards
     and the untouched columns [2 patch^2, ldc)."""
-    L = _L()
+    L = lib_module()
     pp = patch * patch
     i_s = torch.tensor(idx_stats, dtype=torch.int32, device="cuda")
     i_c = torch.tensor(idx_cols, dtype=torch.int32, device="cuda")
     scratch = torch.zeros(L.DEPTH_SCRATCH_DOUBLES(B), device="cuda", dtype=F64)
     rows = B * len(idx_cols) * (H // patch) * (W // patch)
-    buf, flat = _guarded(rows * ldc, BF16, fill)
+    buf, flat = guarded(rows * ldc, BF16, fill)
     names = _kernels(lambda: L.check(L.lib().ovg_depth_im2col(depth.data_ptr(), mask.data_ptr(), i_s.data_ptr(), len(idx_stats),
                                                               i_c.data_ptr(), len(idx_cols), scratch.data_ptr(), flat.data_ptr(),
                                                               ldc, B, S, H, W, patch, L.stream())))
     assert _ran(names, "depth_im2col_kernel<14>" if patch == 14 else "depth_im2col_kernel<0>"), names
     cols = flat.view(rows, ldc)
-    assert _guards_ok(buf, fill) and (cols[:, 2 * pp:] == fill).all()
+    assert guards_ok(buf, fill) and (cols[:, 2 * pp:] == fill).all()
     scale = scratch.view(F32)[2 * B * 1024 * 2:2 * B * 1024 * 2 + B].cpu()
     return scale, cols[:, :2 * pp].cpu()
 
@@ -473,6 +449,6 @@ def test_depth_im2col_bound():
                          .permute(0, 1, 3, 2, 4).reshape(-1, patch * patch)], 1).cpu()
         bound = R.ulp(ref, BF16) + (rel_scale + 2 * R.EPS32) * ref.abs()
         r, f = R.check_rounded(cols, ref, bound, BF16, f"depth im2col rows {name}", ("row", "col"))
-        _margin(f"depth_im2col scale {name}", r_s)
-        _margin(f"depth_im2col rows {name}", r)
+        margin(f"depth_im2col scale {name}", r_s)
+        margin(f"depth_im2col rows {name}", r)
         print(f"  equal to round(ref): {f:.5f}")

@@ -2,43 +2,11 @@
 SEQUENCES live in C++ (csrc/runtime.inc) and are covered by the -m gpu goldens; what is checked here is the Python side of the
 runtime API: one handle per component, one forward call per component and DPT chunk, descriptors filled from the packed
 weights, shapes of the returned dict -- for every aux / chunking / shape path."""
-import ctypes
-
 import pytest
 import torch
 
 from oracle.synth import make_inputs
-from test_host_cpu import mini_model
-
-
-class _Recorder:
-    """Records every call and its arguments.  Workspace size queries get a positive size, so that every workspace is a real
-    buffer whose pointer can be checked (test_poison_cpu.py); every other call returns 0 (OVG_OK)."""
-
-    def __init__(self):
-        self.calls = []
-        self.args = []
-        self.descs = {}
-
-    def __getattr__(self, name):
-        def fn(*a):
-            self.calls.append(name)
-            self.args.append((name, a))
-            if name.endswith("_create"):
-                d = a[0]._obj                       # ctypes.byref(desc)
-                self.descs[name] = type(d).from_buffer_copy(d)
-            return 4096 if name.endswith("_workspace_bytes") else 0
-        return fn
-
-
-@pytest.fixture()
-def dry(monkeypatch):
-    from omnivggt_official_b200 import _lib, ops
-    rec = _Recorder()
-    monkeypatch.setattr(_lib, "lib", lambda: rec)
-    monkeypatch.setattr(_lib, "stream", lambda: 0)
-    monkeypatch.setattr(ops, "_on_device", lambda t: True)
-    return rec
+from ovg_support import dry_workspaces, mini_model  # noqa: F401  (fixture "dry")
 
 
 def test_runtime_calls_dino_backend(dry):
@@ -49,7 +17,7 @@ def test_runtime_calls_dino_backend(dry):
     inp = make_inputs(1, 2, 42, 70, seed=1)
     out = m(images=inp["images"])
     assert out["depth"].shape == (1, 2, 42, 70, 1)
-    n = dry.calls.count
+    n = dry.count
     assert n("ovg_dino_create") == 1 and n("ovg_dino_forward") == 1 and n("ovg_aggregator_forward") == 1
     d = dry.descs["ovg_dino_create"]
     assert (d.C, d.registers, d.depth, d.patch, d.kpad) == (128, 4, 2, 14, 592) and d.blocks[1].w_fc2 and not d.blocks[0].qn_w
@@ -64,7 +32,7 @@ def test_runtime_calls(dry, B, S, H, W, didx, cidx):
     out = m(depth_gt_index=didx, camera_gt_index=cidx, **inp)
     assert out["depth"].shape == (B, S, H, W, 1) and out["world_points"].shape == (B, S, H, W, 3)
     assert out["depth_conf"].shape == (B, S, H, W) and out["pose_enc"].shape == (B, S, 9)
-    n = dry.calls.count
+    n = dry.count
     assert n("ovg_aggregator_create") == 1 and n("ovg_dpt_create") == 2 and n("ovg_dino_create") == 0
     assert n("ovg_aggregator_forward") == 1 and n("ovg_dpt_forward") == 2 * -(-B * S // 8)      # chunks of 8 frames per head
     assert n("ovg_camera_create") == 1 and n("ovg_camera_forward") == 1

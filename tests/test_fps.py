@@ -2,7 +2,6 @@
 of the drop-in and of point_cloud(max_points=...) on a recorded library (CPU), and the libovg kernel against the oracles
 on every path it takes (GPU)."""
 import ctypes
-import hashlib
 import json
 import os
 
@@ -13,6 +12,7 @@ import torch
 from conftest import GOLDEN
 from oracle import fps_oracle as FO
 from oracle.make_golden_fps import make_cases
+from ovg_support import install, parse_glb, scene, sha256
 
 CASES = make_cases()
 
@@ -20,10 +20,6 @@ CASES = make_cases()
 def _gold():
     with open(os.path.join(GOLDEN, "fps.json")) as f:
         return json.load(f)
-
-
-def _sha(a) -> str:
-    return hashlib.sha256(np.ascontiguousarray(a).tobytes()).hexdigest()
 
 
 def _seeded_start(k):
@@ -37,11 +33,11 @@ def _seeded_start(k):
 @pytest.mark.parametrize("name", sorted(CASES))
 def test_oracle_matches_reference_golden(name):
     g, k = _gold()[name], CASES[name]
-    assert _sha(k["xyz"]) == g["xyz_sha256"], "make_cases no longer reproduces the input"
+    assert sha256(k["xyz"]) == g["xyz_sha256"], "make_cases no longer reproduces the input"
     start = None if k["deterministic"] else _seeded_start(k).numpy()
     idx = FO.farthest_point_sample(k["xyz"], k["npoint"], k["include_ends"], start)
     assert list(idx.shape) == g["inds_shape"] and idx.dtype == np.int64
-    assert _sha(idx) == g["inds_sha256"]
+    assert sha256(idx) == g["inds_sha256"]
 
 
 def test_torch_restatement_matches_numpy_oracle_on_cpu():
@@ -54,36 +50,20 @@ def test_torch_restatement_matches_numpy_oracle_on_cpu():
 
 @pytest.fixture()
 def dry(monkeypatch):
-    """The C library replaced by a recorder, on CPU tensors; host reads counted.  The recorded sampler writes index 0."""
-    from omnivggt_official_b200 import _lib, geometry, ops
-
-    class Rec:
-        def __init__(self):
-            self.calls, self.reads, self.count = [], 0, 0
-
-        def __getattr__(self, name):
-            def fn(*a):
-                self.calls.append((name, a))
-                if name == "ovg_farthest_point_sample":
-                    ctypes.memset(a[8], 0, a[1] * a[3] * 8)
-                return 0
-            return fn
-
-    rec = Rec()
+    """The C library replaced by a recorder, on CPU tensors.  The recorded sampler writes index 0; a host read returns the
+    tensor with its first element set to ``dry.kept``, the kept count of point_cloud."""
+    from omnivggt_official_b200 import geometry
 
     def read(t):
-        rec.calls.append(("host_read", ()))
-        rec.reads += 1
         t = t.cpu().clone()
-        t.view(-1)[0] = rec.count                            # the kept count of point_cloud
+        t.view(-1)[0] = fake.kept
         return t
 
-    monkeypatch.setattr(_lib, "lib", lambda: rec)
-    monkeypatch.setattr(_lib, "stream", lambda: 0)
-    monkeypatch.setattr(ops, "_on_device", lambda t: True)
-    monkeypatch.setattr(ops, "host_read", read)
+    zero_indices = {"ovg_farthest_point_sample": lambda a: ctypes.memset(a[8], 0, a[1] * a[3] * 8)}
+    fake = install(monkeypatch, read=read, effects=zero_indices)
+    fake.kept = 0
     monkeypatch.setattr(geometry, "_device_of", lambda *xs: torch.device("cpu"))
-    return rec
+    return fake
 
 
 def test_dry_run_drop_in_is_one_call_without_host_read(dry):
@@ -93,11 +73,11 @@ def test_dry_run_drop_in_is_one_call_without_host_read(dry):
         for ends in (False, True):
             dry.calls.clear()
             idx = farthest_point_sample(xyz, npoint, include_ends=ends, deterministic=npoint == 7)
-            assert [n for n, _ in dry.calls] == ["ovg_fps_workspace_bytes", "ovg_farthest_point_sample"]
+            assert dry.names() == ["ovg_fps_workspace_bytes", "ovg_farthest_point_sample"]
             a = dry.calls[1][1]
             assert a[1:4] == (3, 500, npoint) and a[5] == int(ends)
             assert idx.shape == (3, npoint) and idx.dtype == torch.int64
-    assert dry.reads == 0
+    assert len(dry.reads) == 0
 
 
 def test_drop_in_draws_the_start_as_the_reference_does(dry, monkeypatch):
@@ -115,26 +95,19 @@ def test_drop_in_draws_the_start_as_the_reference_does(dry, monkeypatch):
         assert torch.equal(seen[-1], want) and torch.equal(torch.rand(1), after)
 
 
-def _scene(S, H, W, seed=3):
-    g = torch.Generator().manual_seed(seed)
-    ext = torch.eye(4)[:3].repeat(1, S, 1, 1)
-    return {"images": torch.rand(1, S, 3, H, W, generator=g), "world_points_from_depth": torch.randn(1, S, H, W, 3, generator=g),
-            "depth_conf": 1.0 + torch.rand(1, S, H, W, generator=g), "extrinsic": ext}
-
-
 def test_dry_run_point_cloud_max_points(dry):
     """max_points adds one sampler call after the gather when more points are kept, and no host read."""
     from omnivggt_official_b200 import OmniVGGT
     base = ["ovg_conf_percentile_mask", "ovg_point_cloud_workspace_bytes", "ovg_point_cloud_count", "ovg_point_cloud_center",
             "host_read", "ovg_point_cloud_gather"] + ["ovg_point_cloud_scale"]
-    dry.count = 50
+    dry.kept = 50
     for max_points, sampled in ((None, False), (50, False), (200, False), (49, True), (1, True), (10, True)):
         dry.calls.clear()
-        dry.reads = 0
-        out = OmniVGGT.point_cloud(_scene(2, 6, 8), max_points=max_points)
-        names = [n for n, _ in dry.calls]
+        dry.reads.clear()
+        out = OmniVGGT.point_cloud(scene(2, 6, 8), max_points=max_points)
+        names = dry.names()
         assert names == base + (["ovg_fps_workspace_bytes", "ovg_farthest_point_sample"] if sampled else []), names
-        assert dry.reads == 1
+        assert len(dry.reads) == 1
         n = max_points if sampled else 50
         assert out["points"].shape == (n, 3) and out["colors"].shape == (n, 3) and out["frame"].shape == (n,)
         if sampled:
@@ -151,7 +124,7 @@ def test_errors_before_any_library_call(dry):
                               (np.zeros((1, 10, 3)), 11, "npoint")):
         with pytest.raises(ValueError, match=what):
             farthest_point_sample(xyz, npoint)
-    pred = _scene(2, 6, 8)
+    pred = scene(2, 6, 8)
     for bad in (0, -1, 2.5, True, "10"):
         with pytest.raises((ValueError, TypeError), match="max_points"):
             OmniVGGT.point_cloud(pred, max_points=bad)
@@ -170,7 +143,7 @@ def test_kernel_matches_golden(name):
     idx = farthest_point_sample(torch.from_numpy(k["xyz"]).cuda(), k["npoint"], k["include_ends"], k["deterministic"])
     idx = idx.cpu().numpy()
     assert idx.dtype == np.int64 and list(idx.shape) == g["inds_shape"]
-    assert _sha(idx) == g["inds_sha256"]
+    assert sha256(idx) == g["inds_sha256"]
     o = FO.farthest_point_sample(k["xyz"], k["npoint"], k["include_ends"], None if start is None else start.numpy())
     assert np.array_equal(idx, o)
 
@@ -231,7 +204,7 @@ def test_runs_are_bit_identical():
 
 
 def _cuda_scene(S, H, W, seed):
-    return {k: v.cuda() for k, v in _scene(S, H, W, seed).items()}
+    return {k: v.cuda() for k, v in scene(S, H, W, seed).items()}
 
 
 @pytest.mark.gpu
@@ -239,7 +212,7 @@ def _cuda_scene(S, H, W, seed):
 def test_point_cloud_max_points_is_the_sampled_full_cloud(S, H, W, m, tmp_path):
     from omnivggt_official_b200 import OmniVGGT
     from omnivggt_official_b200.glb import write_glb
-    from test_point_cloud import _parse_glb, _read_cloud
+    from test_point_cloud import _read_cloud
     pred = _cuda_scene(S, H, W, seed=S)
     pred["world_points_from_depth"][0, 0, :4] = 0.5               # repeated positions
     full = OmniVGGT.point_cloud(pred, mask_black_bg=True)
@@ -257,7 +230,7 @@ def test_point_cloud_max_points_is_the_sampled_full_cloud(S, H, W, m, tmp_path):
             assert torch.equal(same[k], full[k]), (big, k)
     path = tmp_path / "sampled.glb"
     write_glb(str(path), sampled)
-    p, c = _read_cloud(*_parse_glb(path.read_bytes()))
+    p, c = _read_cloud(*parse_glb(path.read_bytes()))
     assert np.array_equal(p, sampled["points"].cpu().numpy()) and np.array_equal(c[:, :3], sampled["colors"].cpu().numpy())
 
 

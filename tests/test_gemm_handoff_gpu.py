@@ -16,17 +16,13 @@ import torch
 from oracle import kernel_ref as R
 
 sys.path.insert(0, os.path.dirname(os.path.abspath(__file__)))
-from test_kernel_bounds_gpu import _guarded, _guards_ok, _margin, _positions, _randn  # noqa: E402
+from ovg_support import guarded, guards_ok, margin, ops_module, randn  # noqa: E402
+from test_kernel_bounds_gpu import _positions  # noqa: E402
 
 pytestmark = pytest.mark.gpu
 
 BF16, F16, F64 = torch.bfloat16, torch.float16, torch.float64
 FILL = -3.0
-
-
-def _ops():
-    from omnivggt_official_b200 import ops
-    return ops
 
 
 @pytest.fixture(scope="module")
@@ -53,12 +49,12 @@ def _int_gpu(rows, n, K, seed):
 @pytest.mark.parametrize("bn", [64, 128])
 def test_handoff_bf16_exact(bn, dtype, K, sms):
     """EPI_BF16, identity rows, ragged last row tile, guards around the output."""
-    ops = _ops()
+    ops = ops_module()
     N = 256
     M = 128 * _m_tiles(sms, N // bn) - 37
     a, b = _int_gpu(M, N, K, seed=K + bn)
     bias = torch.randint(-300, 300, (N,)).double().cuda()
-    buf, flat = _guarded(M * N, dtype, FILL)
+    buf, flat = guarded(M * N, dtype, FILL)
     ops.gemm(a.to(dtype), b.to(dtype), epi=ops.L.EPI_BF16, bias=bias.float(), out=flat, ldo=N, block_n=bn)
     acc, _ = R.gemm_acc(a, b)
     exp = R.round_to(acc + bias[None], dtype)
@@ -66,23 +62,23 @@ def test_handoff_bf16_exact(bn, dtype, K, sms):
     got = flat.view(M, N).double()
     bad = (got != exp).nonzero()
     assert bad.numel() == 0, f"{bad.shape[0]} mismatches, first at (row, col) {tuple(bad[0].tolist())}"
-    assert _guards_ok(buf, FILL)
+    assert guards_ok(buf, FILL)
 
 
 def test_handoff_gelu_per_element(sms):
     """EPI_BF16 with the exact-erf GELU, fc1-shaped (N = 1024, K = 1024) at 128 x 128 tiles."""
-    ops = _ops()
+    ops = ops_module()
     N, K = 1024, 1024
     M = 128 * _m_tiles(sms, N // 128) - 5
-    a = _randn(M, K, seed=1, dtype=BF16)
-    w = _randn(N, K, scale=K ** -0.5, seed=2, dtype=BF16)
-    bias = _randn(N, seed=3)
+    a = randn(M, K, seed=1, dtype=BF16)
+    w = randn(N, K, scale=K ** -0.5, seed=2, dtype=BF16)
+    bias = randn(N, seed=3)
     out = torch.empty(M, N, device="cuda", dtype=BF16)
     ops.gemm(a, w, epi=ops.L.EPI_BF16, bias=bias, act=ops.L.ACT_GELU, out=out, ldo=N, block_n=128)
     ref, bound = R.linear_ref(a, w, bias, act="gelu", out_dtype=BF16)
     torch.cuda.synchronize()
     r, f = R.check_rounded(out, ref, bound, BF16, f"GEMM+GELU {M}x{N}x{K}", ("row", "col"))
-    _margin(f"handoff GEMM+GELU {M}x{N}x{K}", r)
+    margin(f"handoff GEMM+GELU {M}x{N}x{K}", r)
 
 
 @pytest.mark.parametrize("K", [64, 512])
@@ -90,7 +86,7 @@ def test_handoff_gelu_per_element(sms):
 @pytest.mark.parametrize("scatter", [False, True])
 def test_handoff_resid_exact(scatter, bn, K, sms):
     """EPI_RESID: x[row] += gamma (acc + bias) in fp32 with power-of-two gamma, rows direct or scattered through row_index."""
-    ops = _ops()
+    ops = ops_module()
     N = 256
     M = 128 * _m_tiles(sms, N // bn) - 11
     a, b = _int_gpu(M, N, K, seed=M + K)
@@ -116,16 +112,16 @@ def test_handoff_resid_exact(scatter, bn, K, sms):
 @pytest.mark.parametrize("bn", [64, 128])
 def test_handoff_qkv_norm_rope(bn, sms):
     """EPI_QKV with the q / k LayerNorm(64) and 2-D RoPE at the aggregator's token layout (37 x 37 patches + 5 special tokens)."""
-    ops = _ops()
+    ops = ops_module()
     C, hp, wp = 256, 37, 37
     heads, T = C // 64, hp * wp + 5
     frames = -(-128 * _m_tiles(sms, 3 * C // bn) // T)
     M = frames * T
     assert -(-M // 128) * (3 * C // bn) >= 3 * sms
-    a = _randn(M, C, seed=1, dtype=BF16)
-    w = _randn(3 * C, C, scale=C ** -0.5, seed=2, dtype=BF16)
-    bias = _randn(3 * C, scale=0.1, seed=3)
-    ln = [1 + 0.1 * _randn(64, seed=4), 0.1 * _randn(64, seed=5), 1 + 0.1 * _randn(64, seed=6), 0.1 * _randn(64, seed=7)]
+    a = randn(M, C, seed=1, dtype=BF16)
+    w = randn(3 * C, C, scale=C ** -0.5, seed=2, dtype=BF16)
+    bias = randn(3 * C, scale=0.1, seed=3)
+    ln = [1 + 0.1 * randn(64, seed=4), 0.1 * randn(64, seed=5), 1 + 0.1 * randn(64, seed=6), 0.1 * randn(64, seed=7)]
     cos, sin = ops.rope_tables(max(hp, wp) + 1, "cuda")
     q, k, v = (torch.zeros(frames, heads, T, 64, device="cuda", dtype=BF16) for _ in range(3))
     ops.qkv_proj(a, w, bias, *ln, q, k, v, ntok=T, T=T, nspecial=5, wp=wp, rope_cos=cos, rope_sin=sin, block_n=bn)
@@ -134,14 +130,14 @@ def test_handoff_qkv_norm_rope(bn, sms):
     torch.cuda.synchronize()
     for name, out, ref, bnd in zip("qkv", (q, k, v), refs, bnds):
         r, f = R.check_rounded(out, ref, bnd, BF16, f"QKV {name} bn={bn}", ("seq", "head", "tok", "col"))
-        _margin(f"handoff QKV {name} bn={bn}", r)
+        margin(f"handoff QKV {name} bn={bn}", r)
 
 
 @pytest.mark.parametrize("dtype", [BF16, F16])
 def test_handoff_pad_taps_skips_exact(dtype, sms):
     """RM_PAD, a 3 x 3 conv as 9 row-shifted taps over a zero-bordered grid with two skips and ReLU: border rows written as zeros,
     interior = relu(taps + bias + skips)."""
-    ops = _ops()
+    ops = ops_module()
     gh, gw, Cin, N, bn = 78, 78, 64, 128, 64
     per_frame = (gh + 2) * (gw + 2)
     F = -(-128 * _m_tiles(sms, N // bn) // per_frame)
@@ -153,11 +149,11 @@ def test_handoff_pad_taps_skips_exact(dtype, sms):
     b = torch.randint(-8, 9, (N, 9 * Cin), generator=g).double().cuda()
     s1, s2 = (torch.randint(-64, 65, (rows, N), generator=g).double().cuda() for _ in range(2))
     bias = torch.randint(-200, 200, (N,), generator=g).double().cuda()
-    buf, flat = _guarded(rows * N, dtype, FILL)
+    buf, flat = guarded(rows * N, dtype, FILL)
     ops.gemm(a.to(dtype), b.to(dtype), taps=taps, epi=ops.L.EPI_BF16, bias=bias.float(), act=ops.L.ACT_RELU, out=flat, ldo=N,
              skip1=s1.to(dtype), skip2=s2.to(dtype), rowmap=ops.L.ROWS_PAD, gh=gh, gw=gw, block_n=bn)
     acc, _ = R.gemm_acc(a, b, taps)
     exp = R.round_to((acc + bias[None] + s1 + s2).clamp(min=0), dtype).reshape(F, gh + 2, gw + 2, N)
     exp[:, 0], exp[:, -1], exp[:, :, 0], exp[:, :, -1] = 0.0, 0.0, 0.0, 0.0
     torch.cuda.synchronize()
-    assert torch.equal(flat.view(F, gh + 2, gw + 2, N).double(), exp) and _guards_ok(buf, FILL)
+    assert torch.equal(flat.view(F, gh + 2, gw + 2, N).double(), exp) and guards_ok(buf, FILL)

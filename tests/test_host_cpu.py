@@ -15,19 +15,7 @@ import torch
 from conftest import GOLDEN, ROOT, golden_index, golden_schema
 from oracle import omnivggt_oracle as O
 from oracle.synth import make_inputs, make_state_dict
-
-
-def mini_model(variant="mini_conv"):
-    from omnivggt_official_b200 import OmniVGGT
-    v = golden_schema(variant)["variant"]
-    kw = dict(img_size=v["img_size"], embed_dim=v["embed_dim"], depth=v["depth"], dpt_features=v["features"],
-              dpt_out_channels=v["out_channels"], dpt_layers=tuple(range(v["depth"]))[-4:], camera_heads=v["cam_heads"],
-              camera_trunk_depth=v["cam_trunk"])
-    if v["patch_embed"] == "conv":
-        kw.update(patch_embed="conv")
-    else:
-        kw.update(patch_embed="dino", dino_depth=2, dino_heads=2)
-    return OmniVGGT(**kw)
+from ovg_support import mini_model
 
 
 def test_library_exports_every_declared_symbol_and_abi_version():

@@ -10,41 +10,16 @@ import pytest
 import torch
 
 from oracle import kernel_ref as R
+from ovg_support import guarded, guards_ok, lib_module, margin, ops_module, randn
 
 pytestmark = pytest.mark.gpu
 
 BF16, F16, F32, F64 = torch.bfloat16, torch.float16, torch.float32, torch.float64
-GUARD = 4096
-
-
-def _ops():
-    from omnivggt_official_b200 import ops
-    return ops
-
-
-def _L():
-    from omnivggt_official_b200 import _lib
-    return _lib
 
 
 @pytest.fixture(scope="module")
 def sms():
     return torch.cuda.get_device_properties(0).multi_processor_count
-
-
-def _margin(name, r):
-    print(f"margin {name}: {r:.3f}")
-
-
-def _guarded(n, dtype, fill):
-    """A flat buffer with `n` elements between two sentinel guards: (buffer, the n-element middle)."""
-    buf = torch.full((GUARD + n + GUARD,), fill, device="cuda", dtype=dtype)
-    return buf, buf[GUARD:GUARD + n]
-
-
-def _guards_ok(buf, fill):
-    ref = torch.full((GUARD,), fill, device="cuda", dtype=buf.dtype)
-    return torch.equal(buf[:GUARD], ref) and torch.equal(buf[-GUARD:], ref)
 
 
 def _act(x, act):
@@ -72,14 +47,14 @@ IDENT = [(1, 32, 8, 0), (63, 32, 56, 0), (64, 96, 72, 64), (65, 160, 392, 128), 
 def test_gemm_exact_ident(M, N, K, bn, dtype, act):
     """EPI_BF16, identity rows: strided A (lda > a_cols, the extra columns hold 99s), strided output (ldo > N, sentinels between
     the rows), guards around the output, row 0 on round-to-nearest-even ties (and fp16 saturation)."""
-    ops = _ops()
+    ops = ops_module()
     a, b = R.int_operands(M, N, K, seed=M * 7 + K, extra_cols=24)
     a[:, K:] = 99.0
     a[0, :K] = 0.0
     a[0, 0] = 1.0
     bias = _int_bias(b, N, dtype)
     ldo, fill = N + 32, -3.0
-    buf, flat = _guarded(M * ldo, dtype, fill)
+    buf, flat = guarded(M * ldo, dtype, fill)
     ops.gemm(a.to(dtype).cuda()[:, :K], b.to(dtype).cuda(), epi=ops.L.EPI_BF16, bias=bias.float().cuda(), act=ACT[act],
              out=flat, ldo=ldo, block_n=bn)
     acc, _ = R.gemm_acc(a[:, :K], b)
@@ -91,36 +66,36 @@ def test_gemm_exact_ident(M, N, K, bn, dtype, act):
     bad = (got != exp).nonzero()
     assert bad.numel() == 0, f"{bad.shape[0]} mismatches, first at (row, col) {tuple(bad[0].tolist())}: " \
                              f"{got[tuple(bad[0])]:.1f} vs {exp[tuple(bad[0])]:.1f}"
-    assert (out[:, N:] == fill).all() and _guards_ok(buf, fill)
+    assert (out[:, N:] == fill).all() and guards_ok(buf, fill)
 
 
 @pytest.mark.parametrize("waves", ["sms-1", "sms", "sms+1", "2sms+1"])
 def test_gemm_exact_scheduler_edges(waves, sms):
     """Tile counts at the edges of the persistent scheduler: SMs - 1, SMs, SMs + 1 and 2 SMs + 1 tiles of 128 x 128."""
-    ops = _ops()
+    ops = ops_module()
     tiles = {"sms-1": sms - 1, "sms": sms, "sms+1": sms + 1, "2sms+1": 2 * sms + 1}[waves]
     M, N, K = 128 * (tiles - 1) + 1 if waves.endswith("+1") else 128 * tiles, 128, 64
     a, b = R.int_operands(M, N, K, seed=tiles)
     bias = torch.randint(-300, 300, (N,)).double()
-    buf, flat = _guarded(M * N, BF16, -3.0)
+    buf, flat = guarded(M * N, BF16, -3.0)
     ops.gemm(a.to(BF16).cuda(), b.to(BF16).cuda(), epi=ops.L.EPI_BF16, bias=bias.float().cuda(), out=flat, ldo=N, block_n=128)
     acc = (a.cuda() @ b.cuda().t())
     torch.cuda.synchronize()
-    assert torch.equal(flat.view(M, N).double(), R.round_to(acc + bias.cuda()[None], BF16)) and _guards_ok(buf, -3.0)
+    assert torch.equal(flat.view(M, N).double(), R.round_to(acc + bias.cuda()[None], BF16)) and guards_ok(buf, -3.0)
 
 
 @pytest.mark.parametrize("act", ["none", "relu"])
 @pytest.mark.parametrize("dtype", [BF16, F16])
 def test_gemm_exact_dense2pad_table(dtype, act):
     """RM_DENSE2PAD with the additive table: rows (frame, y, x) land inside the zero-bordered map; the border stays untouched."""
-    ops = _ops()
+    ops = ops_module()
     F, gh, gw, K, N = 3, 5, 7, 72, 96
     M = F * gh * gw
     a, b = R.int_operands(M, N, K, seed=11)
     bias = torch.randint(-200, 200, (N,)).double()
     table = torch.randint(-500, 500, (gh * gw, N)).double()
     fill = -3.0
-    buf, flat = _guarded(F * (gh + 2) * (gw + 2) * N, dtype, fill)
+    buf, flat = guarded(F * (gh + 2) * (gw + 2) * N, dtype, fill)
     ops.gemm(a.to(dtype).cuda(), b.to(dtype).cuda(), epi=ops.L.EPI_BF16, bias=bias.float().cuda(), act=ACT[act],
              table=table.float().cuda(), table_rows=gh * gw, out=flat, ldo=N, rowmap=ops.L.ROWS_DENSE2PAD, gh=gh, gw=gw, block_n=64)
     acc, _ = R.gemm_acc(a, b)
@@ -130,7 +105,7 @@ def test_gemm_exact_dense2pad_table(dtype, act):
     assert torch.equal(out[:, 1:-1, 1:-1].double().cpu(), exp)
     border = out.clone()
     border[:, 1:-1, 1:-1] = fill
-    assert (border == fill).all() and _guards_ok(buf, fill)
+    assert (border == fill).all() and guards_ok(buf, fill)
 
 
 @pytest.mark.parametrize("act", ["none", "relu"])
@@ -138,7 +113,7 @@ def test_gemm_exact_dense2pad_table(dtype, act):
 def test_gemm_exact_pad_taps_skips(dtype, act):
     """RM_PAD, 9 row-shifted taps over a zero-bordered grid whose border rows hold non-zero values: the taps of the first and last
     rows read past both ends of a_rows (zero fill), border outputs are written as zeros, interior = taps + bias + two skips."""
-    ops = _ops()
+    ops = ops_module()
     F, gh, gw, Cin, N = 3, 6, 9, 64, 160
     rows = F * (gh + 2) * (gw + 2)
     taps = [(ky - 1) * (gw + 2) + (kx - 1) for ky in range(3) for kx in range(3)]
@@ -148,21 +123,21 @@ def test_gemm_exact_pad_taps_skips(dtype, act):
     s1, s2 = (torch.randint(-64, 65, (rows, N), generator=g).double() for _ in range(2))
     bias = torch.randint(-200, 200, (N,), generator=g).double()
     fill = -3.0
-    buf, flat = _guarded(rows * N, dtype, fill)
+    buf, flat = guarded(rows * N, dtype, fill)
     ops.gemm(a.to(dtype).cuda(), b.to(dtype).cuda(), taps=taps, epi=ops.L.EPI_BF16, bias=bias.float().cuda(), act=ACT[act],
              out=flat, ldo=N, skip1=s1.to(dtype).cuda(), skip2=s2.to(dtype).cuda(), rowmap=ops.L.ROWS_PAD, gh=gh, gw=gw, block_n=128)
     acc, _ = R.gemm_acc(a, b, taps)
     exp = R.round_to(_act(acc + bias[None] + s1 + s2, act), dtype).reshape(F, gh + 2, gw + 2, N)
     exp[:, 0], exp[:, -1], exp[:, :, 0], exp[:, :, -1] = 0.0, 0.0, 0.0, 0.0
     torch.cuda.synchronize()
-    assert torch.equal(flat.view(F, gh + 2, gw + 2, N).double().cpu(), exp) and _guards_ok(buf, fill)
+    assert torch.equal(flat.view(F, gh + 2, gw + 2, N).double().cpu(), exp) and guards_ok(buf, fill)
 
 
 @pytest.mark.parametrize("dtype", [BF16, F16])
 def test_gemm_exact_pixel_shuffle(dtype):
     """RM_PIXSHUF: column (ky, kx, c) of row (frame, y, x) lands at pixel (y ps + ky, x ps + kx) of the bordered output, bias and
     skip indexed by the output channel; the border stays untouched."""
-    ops = _ops()
+    ops = ops_module()
     F, gh, gw, ps, cout, K = 2, 3, 4, 2, 32, 64
     M, N = F * gh * gw, ps * ps * cout
     a, b = R.int_operands(M, N, K, seed=13)
@@ -170,7 +145,7 @@ def test_gemm_exact_pixel_shuffle(dtype):
     oh, ow = gh * ps + 2, gw * ps + 2
     skip = torch.randint(-64, 65, (F, oh, ow, cout)).double()
     fill = -3.0
-    buf, flat = _guarded(F * oh * ow * cout, dtype, fill)
+    buf, flat = guarded(F * oh * ow * cout, dtype, fill)
     ops.gemm(a.to(dtype).cuda(), b.to(dtype).cuda(), epi=ops.L.EPI_BF16, bias=bias.float().cuda(), out=flat, ldo=cout,
              skip1=skip.to(dtype).cuda(), rowmap=ops.L.ROWS_PIXSHUF, gh=gh, gw=gw, ps=ps, cout=cout)
     acc, _ = R.gemm_acc(a, b)
@@ -181,7 +156,7 @@ def test_gemm_exact_pixel_shuffle(dtype):
     assert torch.equal(out[:, 1:-1, 1:-1].double().cpu(), exp)
     border = out.clone()
     border[:, 1:-1, 1:-1] = fill
-    assert (border == fill).all() and _guards_ok(buf, fill)
+    assert (border == fill).all() and guards_ok(buf, fill)
 
 
 @pytest.mark.parametrize("M,N,K,bn", [(300, 96, 392, 64), (129, 160, 4096, 128), (65, 32, 8, 0)])
@@ -189,7 +164,7 @@ def test_gemm_exact_pixel_shuffle(dtype):
 def test_gemm_exact_resid(M, N, K, bn, scatter):
     """EPI_RESID: x[row] += gamma (acc + bias) in fp32, exact with integer x, acc, bias and power-of-two gamma; with row_index
     the rows are scattered through a permutation."""
-    ops = _ops()
+    ops = ops_module()
     a, b = R.int_operands(M, N, K, seed=M + K)
     g = torch.Generator().manual_seed(N)
     bias = torch.randint(-200, 200, (N,), generator=g).double()
@@ -213,11 +188,11 @@ def test_gemm_exact_resid(M, N, K, bn, scatter):
 def test_gemm_exact_qkv_plain(nb, ntok, C, bn):
     """EPI_QKV with qk_norm = rope = 0 (the DINOv2 blocks): bias, q times a power-of-two qscale, head-major [nb, heads, ntok, 64]
     outputs with guards."""
-    ops = _ops()
+    ops = ops_module()
     M, heads = nb * ntok, C // 64
     a, b = R.int_operands(M, 3 * C, C, seed=ntok)
     bias = torch.randint(-200, 200, (3 * C,)).double()
-    bufs = [_guarded(M * C, BF16, -3.0) for _ in range(3)]
+    bufs = [guarded(M * C, BF16, -3.0) for _ in range(3)]
     q, k, v = (f.view(nb, heads, ntok, 64) for _, f in bufs)
     ops.gemm(a.to(BF16).cuda(), b.to(BF16).cuda(), epi=ops.L.EPI_QKV, bias=bias.float().cuda(), q_out=q, k_out=k, v_out=v, C=C,
              ntok=ntok, T=ntok, nspecial=0, wp=1, maxpos=0, qk_norm=0, rope=0, qscale=0.125, block_n=bn)
@@ -226,30 +201,25 @@ def test_gemm_exact_qkv_plain(nb, ntok, C, bn):
     torch.cuda.synchronize()
     assert torch.equal(q.double().cpu(), R.round_to(t[0] * 0.125, BF16))
     assert torch.equal(k.double().cpu(), R.round_to(t[1], BF16)) and torch.equal(v.double().cpu(), R.round_to(t[2], BF16))
-    assert all(_guards_ok(buf, -3.0) for buf, _ in bufs)
+    assert all(guards_ok(buf, -3.0) for buf, _ in bufs)
 
 
 # ----------------------------------------------------------------------------------------------- GEMM, realistic inputs
-def _randn(*s, scale=1.0, seed=0, dtype=F32):
-    g = torch.Generator(device="cuda").manual_seed(seed)
-    return (torch.randn(*s, generator=g, device="cuda") * scale).to(dtype)
-
-
 def test_gemm_accumulation_constant():
     """The raw fp32 accumulator (EPI_RESID with gamma 1, bias 0 into zeros) against the exact dot products: the largest
     |acc - exact| / (sqrt(K) 2^-24 sum|a||b|) must stay at least 4x below ACC_C."""
-    ops = _ops()
+    ops = ops_module()
     worst = 0.0
     for M, N, K in [(300, 256, 64), (1000, 384, 192), (515, 1024, 1024), (515, 1024, 4096), (2748, 1024, 1024)]:
-        a = _randn(M, K, seed=1, dtype=BF16)
-        w = _randn(N, K, scale=K ** -0.5, seed=2, dtype=BF16)
+        a = randn(M, K, seed=1, dtype=BF16)
+        w = randn(N, K, scale=K ** -0.5, seed=2, dtype=BF16)
         x = torch.zeros(M, N, device="cuda")
         ops.linear_resid(a, w, torch.zeros(N, device="cuda"), torch.ones(N, device="cuda"), x)
         acc, absacc = R.gemm_acc(a, w)
         r = float(((x.double() - acc).abs() / (math.sqrt(K) * R.EPS32 * absacc)).max())
         print(f"accumulation constant, M={M} N={N} K={K}: {r:.4f}")
         worst = max(worst, r)
-    _margin("accumulation constant / ACC_C", worst / R.ACC_C)
+    margin("accumulation constant / ACC_C", worst / R.ACC_C)
     assert worst <= R.ACC_C / 4, worst
 
 
@@ -257,10 +227,10 @@ def test_gemm_accumulation_constant():
                                             (77, 96, 392, 64, BF16), (2748, 3072, 1024, 512, BF16), (5000, 1024, 128, 512, BF16),
                                             (300, 256, 128, 0, F16), (2748, 1024, 1024, 512, F16)])
 def test_gemm_gelu_per_element(M, N, K, bn, dtype):
-    ops = _ops()
-    a = _randn(M, K, seed=1, dtype=dtype)
-    w = _randn(N, K, scale=K ** -0.5, seed=2, dtype=dtype)
-    bias = _randn(N, seed=3)
+    ops = ops_module()
+    a = randn(M, K, seed=1, dtype=dtype)
+    w = randn(N, K, scale=K ** -0.5, seed=2, dtype=dtype)
+    bias = randn(N, seed=3)
     out = torch.empty(M, N, device="cuda", dtype=dtype)
     ops.gemm(a, w, epi=ops.L.EPI_BF16, bias=bias, act=ops.L.ACT_GELU, out=out, ldo=N, block_n=bn)
     ref, bound = R.linear_ref(a, w, bias, act="gelu", out_dtype=dtype)
@@ -270,7 +240,7 @@ def test_gemm_gelu_per_element(M, N, K, bn, dtype):
     # N(0, 1.3^2) inputs and 98.3 % of those below -1.  Truncating stores match about half.
     min_match = 0.97 if dtype == F16 else 0.99
     r, f = R.check_rounded(out, ref, bound, dtype, f"GEMM+GELU {M}x{N}x{K}", ("row", "col"), min_match)
-    _margin(f"GEMM+GELU {M}x{N}x{K} {dtype}", r)
+    margin(f"GEMM+GELU {M}x{N}x{K} {dtype}", r)
     print(f"  equal to round(ref): {f:.5f}")
 
 
@@ -298,13 +268,13 @@ def test_gemm_qkv_norm_rope_per_element(C, frames, hp, wp, bn):
     """EPI_QKV with LayerNorm(64) on q / k and 2-D RoPE, frame-wise sequences.  The device's RoPE tables, which the fp64
     reference takes as given, are first checked against the reference's recipe on the CPU: within 4 fp32 ulps of the angle (the
     device's pow, reciprocal and product may each round differently) plus 4 of the value (cosf / sinf)."""
-    ops = _ops()
+    ops = ops_module()
     heads, T = C // 64, hp * wp + 5
     M = frames * T
-    a = _randn(M, C, seed=1, dtype=BF16)
-    w = _randn(3 * C, C, scale=C ** -0.5, seed=2, dtype=BF16)
-    bias = _randn(3 * C, scale=0.1, seed=3)
-    ln = [1 + 0.1 * _randn(64, seed=4), 0.1 * _randn(64, seed=5), 1 + 0.1 * _randn(64, seed=6), 0.1 * _randn(64, seed=7)]
+    a = randn(M, C, seed=1, dtype=BF16)
+    w = randn(3 * C, C, scale=C ** -0.5, seed=2, dtype=BF16)
+    bias = randn(3 * C, scale=0.1, seed=3)
+    ln = [1 + 0.1 * randn(64, seed=4), 0.1 * randn(64, seed=5), 1 + 0.1 * randn(64, seed=6), 0.1 * randn(64, seed=7)]
     maxpos = max(hp, wp) + 1
     assert maxpos <= 64
     cos, sin = ops.rope_tables(maxpos, "cuda")
@@ -313,7 +283,7 @@ def test_gemm_qkv_norm_rope_per_element(C, frames, hp, wp, bn):
     for name, got, ref in (("cos", cos, rcos), ("sin", sin, rsin)):
         bound = 4 * R.ulp(angles, F32) + 4 * R.ulp(ref, F32)
         r = R.check_bound(got, ref.double(), bound, f"RoPE {name} table, {maxpos} positions", ("position", "frequency"))
-        _margin(f"RoPE {name} table {maxpos} positions", r)
+        margin(f"RoPE {name} table {maxpos} positions", r)
     q, k, v = (torch.zeros(frames, heads, T, 64, device="cuda", dtype=BF16) for _ in range(3))
     ops.qkv_proj(a, w, bias, *ln, q, k, v, ntok=T, T=T, nspecial=5, wp=wp, rope_cos=cos, rope_sin=sin, block_n=bn)
     qscale = float(torch.tensor((1.0 / math.sqrt(64.0)) * math.log2(math.e), dtype=F32))
@@ -321,20 +291,20 @@ def test_gemm_qkv_norm_rope_per_element(C, frames, hp, wp, bn):
     torch.cuda.synchronize()
     for name, out, ref, bnd in zip("qkv", (q, k, v), refs, bnds):
         r, f = R.check_rounded(out, ref, bnd, BF16, f"QKV {name} C={C}", ("seq", "head", "tok", "col"))
-        _margin(f"QKV {name} C={C} {hp}x{wp}", r)
+        margin(f"QKV {name} C={C} {hp}x{wp}", r)
 
 
 @pytest.mark.parametrize("dtype", [BF16, F16])
 @pytest.mark.parametrize("outc,act", [(2, 0), (4, 1)])
 def test_headtail_per_element(outc, act, dtype):
     """EPI_HEADTAIL (row-shift kernel): 3x3 conv 128 -> 32 + ReLU + 1x1 + activations, fp32 outputs, against the bound."""
-    ops = _ops()
+    ops = ops_module()
     Fr, h, w, Cin = 2, 14, 28, 128
-    x = _randn(Fr, h + 2, w + 2, Cin, seed=1)
+    x = randn(Fr, h + 2, w + 2, Cin, seed=1)
     x[:, 0], x[:, -1], x[:, :, 0], x[:, :, -1] = 0, 0, 0, 0
     xp = x.to(dtype)
-    wb = _randn(32, 9 * Cin, scale=(9 * Cin) ** -0.5, seed=2, dtype=dtype)
-    b1, w2, b2 = _randn(32, scale=0.1, seed=3), _randn(outc, 32, scale=32 ** -0.5, seed=4), _randn(outc, scale=0.1, seed=5)
+    wb = randn(32, 9 * Cin, scale=(9 * Cin) ** -0.5, seed=2, dtype=dtype)
+    b1, w2, b2 = randn(32, scale=0.1, seed=3), randn(outc, 32, scale=32 ** -0.5, seed=4), randn(outc, scale=0.1, seed=5)
     preds = torch.zeros(Fr, h, w, outc - 1, device="cuda")
     conf = torch.zeros(Fr, h, w, device="cuda")
     taps = [(ky - 1) * (w + 2) + (kx - 1) for ky in range(3) for kx in range(3)]
@@ -344,7 +314,7 @@ def test_headtail_per_element(outc, act, dtype):
     torch.cuda.synchronize()
     r1 = R.check_bound(preds, rp, bp, "HEADTAIL preds", ("frame", "y", "x", "c"))
     r2 = R.check_bound(conf, rc, bc, "HEADTAIL conf", ("frame", "y", "x"))
-    _margin(f"HEADTAIL outc={outc} act={act} {dtype}", max(r1, r2))
+    margin(f"HEADTAIL outc={outc} act={act} {dtype}", max(r1, r2))
 
 
 # ----------------------------------------------------------------------------------------------- attention
@@ -379,7 +349,7 @@ REAL_SHAPES = {"frame 294x518": (5, 16, 782), "global 294x518": (1, 16, 3910), "
 
 def _run_attention(q, k, v, B, H, nq, nkv, scratch):
     """ovg_attention on the device; returns (out, launches, scratch bytes written)."""
-    ops, L = _ops(), _L()
+    ops, L = ops_module(), lib_module()
     out = torch.zeros(B, nq, H * 64, device="cuda", dtype=BF16)
     s = None
     if scratch:
@@ -429,7 +399,7 @@ def test_attention_rounding_rows(path, sms):
     out, *_ = _run_attention(q, k, v, B, H, nq, nkv, scratch)
     ref, bound = R.attention_ref(q.cuda(), k.cuda(), v.cuda())
     r, f = R.check_rounded(out, ref, bound, BF16, f"attention rounding rows ({path})", ("batch", "row", "col"))
-    _margin(f"attention rounding rows {path}", r)
+    margin(f"attention rounding rows {path}", r)
 
 
 @pytest.mark.parametrize("n", [1, 33, 127, 128, 129, 1374, 9000] + sorted(n for *_, n in REAL_SHAPES.values()))
@@ -471,14 +441,14 @@ def test_attention_per_element(path, kind, sms):
     _check_path(path, sms, B, H, nq, nkv, scratch, launches, written)
     ref, bound = R.attention_ref(q.cuda(), k.cuda(), v.cuda())
     r = R.check_bound(out, ref, bound, f"attention {kind} ({path})", ("batch", "row", "col"))
-    _margin(f"attention {kind} {path}", r)
+    margin(f"attention {kind} {path}", r)
     again, *_ = _run_attention(q, k, v, B, H, nq, nkv, scratch)
     assert torch.equal(out, again)
     if scratch:
         plain, *_ = _run_attention(q, k, v, B, H, nq, nkv, False)
         R.check_bound(plain, ref, bound, f"attention {kind} unsplit", ("batch", "row", "col"))
         rr = R.check_bound(out, plain.double(), 2 * bound, f"attention {kind} split vs unsplit", ("batch", "row", "col"))
-        _margin(f"attention {kind} split vs unsplit (2x bound)", rr)
+        margin(f"attention {kind} split vs unsplit (2x bound)", rr)
 
 
 # ----------------------------------------------------------------------------------------------- LayerNorm
@@ -488,7 +458,7 @@ def test_attention_per_element(path, kind, sms):
 def test_layernorm_per_element(C, in_dtype, out_dtype):
     """Rows with a common offset of 1000 x their spread, near-constant rows where eps dominates, ordinary rows; strided input and
     output (ld > C, sentinels in the gap) and the row gather that drops special tokens."""
-    ops = _ops()
+    ops = ops_module()
     g = torch.Generator().manual_seed(C)
     rows = 6 * 21
     x = torch.randn(rows, C, generator=g, dtype=F64) * 3 + 0.5
@@ -511,7 +481,7 @@ def test_layernorm_per_element(C, in_dtype, out_dtype):
         torch.cuda.synchronize()
         r = R.check_bound(obuf[:, :C], ref, bound, f"LayerNorm C={C}", ("row", "col"))
         assert (obuf[:, C:] == fill).all()
-        _margin(f"LayerNorm C={C} {in_dtype}->{out_dtype} gather={gather}", r)
+        margin(f"LayerNorm C={C} {in_dtype}->{out_dtype} gather={gather}", r)
 
 
 # ----------------------------------------------------------------------------------------------- camera head
@@ -536,7 +506,7 @@ def test_camera_head_against_fp64(embed_dim, heads):
     D = 2 * embed_dim
     worst = 0.0
     for S in (1, 3, 24):
-        tok = _randn(2, S, 1, D, seed=S)
+        tok = randn(2, S, 1, D, seed=S)
         out = torch.stack(m.camera_head([tok], num_iterations=4))            # [4, B, S, 9]
         ref = R.camera_ref(eng.cam, tok.reshape(2 * S, D), 2, S, heads)
         e = R.camera_error(out.reshape(4, 2 * S, 9), ref)
@@ -546,4 +516,4 @@ def test_camera_head_against_fp64(embed_dim, heads):
         for bi in range(2):
             alone = torch.stack(m.camera_head([tok[bi:bi + 1]], num_iterations=4))
             assert torch.equal(alone[:, 0], out[:, bi]), (S, bi)
-    _margin(f"camera head D={D} heads={heads} (error / CAM_TOL)", worst / R.CAM_TOL)
+    margin(f"camera head D={D} heads={heads} (error / CAM_TOL)", worst / R.CAM_TOL)

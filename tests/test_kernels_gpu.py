@@ -6,24 +6,11 @@ import pytest
 import torch
 import torch.nn.functional as F
 
+from ovg_support import ops_module, randn, rel
+
 pytestmark = pytest.mark.gpu
 
 BF16, F32 = torch.bfloat16, torch.float32
-
-
-def _ops():
-    from omnivggt_official_b200 import ops
-    return ops
-
-
-def rel(a, b):
-    a, b = a.float(), b.float()
-    return ((a - b).norm() / b.norm().clamp(min=1e-12)).item()
-
-
-def randn(*s, scale=1.0, seed=0, dtype=F32):
-    g = torch.Generator(device="cuda").manual_seed(seed)
-    return (torch.randn(*s, generator=g, device="cuda") * scale).to(dtype)
 
 
 # ----------------------------------------------------------------------------------------------- GEMM
@@ -36,7 +23,7 @@ def randn(*s, scale=1.0, seed=0, dtype=F32):
                                       (5000, 1024, 128, 512), (4000, 1280, 64, 512), (19000, 256, 64, 512),
                                       (2748, 384, 192, 384), (1500, 128, 2048, 384), (300, 256, 128, 384)])
 def test_gemm_bf16_bias_gelu(M, N, K, bn):
-    ops = _ops()
+    ops = ops_module()
     a = randn(M, K, seed=1, dtype=BF16)
     w = randn(N, K, scale=K ** -0.5, seed=2, dtype=BF16)
     bias = randn(N, seed=3)
@@ -51,7 +38,7 @@ def test_gemm_bf16_bias_gelu(M, N, K, bn):
 @pytest.mark.parametrize("M,N,K,bn", [(5000, 1024, 128, 512), (10992, 1024, 256, 512)])
 def test_gemm_resid_split_tail(M, N, K, bn):
     """Residual epilogue (fp32 read-modify-write) over a tile count with a short last wave."""
-    ops = _ops()
+    ops = ops_module()
     a = randn(M, K, seed=1, dtype=BF16)
     w = randn(N, K, scale=K ** -0.5, seed=2, dtype=BF16)
     bias, gamma = randn(N, seed=3), randn(N, seed=4)
@@ -64,7 +51,7 @@ def test_gemm_resid_split_tail(M, N, K, bn):
 
 @pytest.mark.parametrize("bn", [0, 512])
 def test_gemm_resid_rowindex(bn):
-    ops = _ops()
+    ops = ops_module()
     M, N, K = 1374 * 2, 1024, 1024
     a = randn(M, K, seed=1, dtype=BF16)
     w = randn(N, K, scale=K ** -0.5, seed=2, dtype=BF16)
@@ -103,7 +90,7 @@ def _rope_ref(t, pos, base=100.0):
 def test_gemm_qkv_epilogue(C, frames, hp, wp, S, bn):
     """QKV linear + q/k LayerNorm(64) + 2-D RoPE + head-major layout vs reference formulas
     (layers/attention.py:52-58, layers/rope.py:154-188)."""
-    ops = _ops()
+    ops = ops_module()
     heads, T = C // 64, hp * wp + 5
     M = frames * T
     a = randn(M, C, seed=1, dtype=BF16)
@@ -140,7 +127,7 @@ def test_gemm_qkv_epilogue(C, frames, hp, wp, S, bn):
                                            (1, 3, 64), (1, 2, 129), (1, 2, 257), (1, 2, 320), (2, 3, 385)])
 def test_attention(batch, heads, n):
     """vs softmax(q k^T / 8) v in fp32 (layers/attention.py:61-66).  bf16 P and bf16 output: rel-L2 < 1e-2."""
-    ops = _ops()
+    ops = ops_module()
     q = randn(batch, heads, n, 64, seed=1)
     k = randn(batch, heads, n, 64, seed=2)
     v = randn(batch, heads, n, 64, seed=3)
@@ -175,7 +162,7 @@ def test_attention_global_sizes_of_baseline_configs(heads, n):
     """BASELINE.json configs[1] / configs[4]: the global attention of 8 views (L = 10 992, 172 KV steps) and of 24 views
     (L = 32 976, 516 KV steps), 16 heads, against fp32 SDPA (reference layers/attention.py:61-66) -- same 1e-2 bar as the
     small shapes; the long accumulation (fp32 O / l in registers, online rescaling) is what is under test."""
-    ops = _ops()
+    ops = ops_module()
     q = randn(1, heads, n, 64, seed=1)
     k = randn(1, heads, n, 64, seed=2)
     v = randn(1, heads, n, 64, seed=3)
@@ -211,7 +198,7 @@ def test_attention_split_tail_shapes(batch, heads, n):
     688 tiles leave a last wave of 28 tiles, split in 3 parts; 1 376 tiles over two batch entries leave 56, split in 2; 497 tiles leave
     101, which the cost rule does not split, so that case checks the unsplit path with scratch given.  test_kernel_bounds_gpu.py
     asserts which path each of its shapes takes on the device it runs on."""
-    ops = _ops()
+    ops = ops_module()
     q = randn(batch, heads, n, 64, seed=1) * 1.5
     k = randn(batch, heads, n, 64, seed=2)
     v = randn(batch, heads, n, 64, seed=3)
@@ -230,7 +217,7 @@ def test_attention_split_tail_shapes(batch, heads, n):
 
 def test_attention_peaky_rows_rescale():
     """Large, growing logits force the lazy-rescale path (running max grows by > 8 between KV tiles)."""
-    ops = _ops()
+    ops = ops_module()
     batch, heads, n = 1, 2, 1024
     q = randn(batch, heads, n, 64, seed=1)
     k = randn(batch, heads, n, 64, seed=2) * torch.linspace(0.2, 6.0, n, device="cuda")[None, None, :, None]
@@ -249,7 +236,7 @@ def test_attention_peaky_rows_rescale():
 def test_attention_late_spike_overflow(spike_at):
     """One key far down the sequence whose logit exceeds everything before it by > 2^128: exp2 against the previous
     maximum would overflow, the kernel must rescale O / l to the new maximum (and keep earlier / later steps exact)."""
-    ops = _ops()
+    ops = ops_module()
     batch, heads, n = 1, 2, 700
     q = randn(batch, heads, n, 64, seed=1) * 0.3 + 2.0
     k = randn(batch, heads, n, 64, seed=2) * 0.3
@@ -269,7 +256,7 @@ def test_attention_late_spike_overflow(spike_at):
 # ----------------------------------------------------------------------------------------------- LayerNorm & co
 @pytest.mark.parametrize("C", [128, 256, 1024, 2048])
 def test_layernorm(C):
-    ops = _ops()
+    ops = ops_module()
     x = randn(777, C, seed=1) * 3 + 0.5
     w, b = 1 + 0.1 * randn(C, seed=2), 0.1 * randn(C, seed=3)
     out = torch.empty(777, C, device="cuda", dtype=BF16)
@@ -285,7 +272,7 @@ def test_layernorm(C):
 
 
 def test_assemble_and_inject():
-    ops = _ops()
+    ops = ops_module()
     B, S, P, R, C = 2, 3, 16, 4, 128
     K, T = B * S, P + R + 1
     patch, cam, reg = randn(K, P, C, seed=1), randn(2, C, seed=2), randn(2, R, C, seed=3)
@@ -313,7 +300,7 @@ def test_assemble_and_inject():
 
 
 def test_depth_im2col_matches_reference_normalisation():
-    ops = _ops()
+    ops = ops_module()
     B, S, H, W, patch = 2, 4, 28, 42, 14
     idx = torch.tensor([0, 2, 3], device="cuda", dtype=torch.int32)
     depth = 0.5 + 4 * torch.rand(B, S, H, W, device="cuda")
@@ -321,7 +308,7 @@ def test_depth_im2col_matches_reference_normalisation():
     mask[1] = 0          # scene without valid pixels -> zeros (omnivggt_aggregator.py:121-122)
     Sd, hp, wp = 3, H // patch, W // patch
     cols = torch.zeros(B * Sd * hp * wp, 2 * patch * patch, device="cuda", dtype=BF16)
-    scratch = torch.zeros(_ops().L.DEPTH_SCRATCH_DOUBLES(B), device="cuda", dtype=torch.float64)
+    scratch = torch.zeros(ops_module().L.DEPTH_SCRATCH_DOUBLES(B), device="cuda", dtype=torch.float64)
     ops.depth_im2col(depth, mask, idx, scratch, cols, B, S, Sd, H, W, patch)
     d, m = depth[:, idx.long()], mask[:, idx.long()]
     norm = torch.zeros_like(d)
@@ -348,7 +335,7 @@ def _from_pad(p):  # -> NCHW fp32 interior
 def test_conv3x3_taps_with_skips_relu(Fr, h, w, Cin, Cout, bn):
     """3x3 conv as 9 row-shifted GEMMs over the zero-bordered layout + bias + two skips + ReLU
     (heads/dpt_head.py:379-399)."""
-    ops = _ops()
+    ops = ops_module()
     x = randn(Fr, Cin, h, w, seed=1)
     wt = randn(Cout, Cin, 3, 3, scale=(9 * Cin) ** -0.5, seed=2)
     bias = randn(Cout, seed=3)
@@ -372,7 +359,7 @@ def test_conv3x3_taps_with_skips_relu(Fr, h, w, Cin, Cout, bn):
                                                 (4, 256, 256, 37, 37, 512)])
 def test_conv_transpose_pixel_shuffle(ps, Cin, Cout, h, w, bn):
     """ConvTranspose2d(k = s) as one GEMM with a pixel-shuffle store (heads/dpt_head.py:84-89)."""
-    ops = _ops()
+    ops = ops_module()
     Fr = 2
     x = randn(Fr, Cin, h, w, seed=1)
     wt = randn(Cin, Cout, ps, ps, scale=Cin ** -0.5, seed=2)
@@ -388,7 +375,7 @@ def test_conv_transpose_pixel_shuffle(ps, Cin, Cout, h, w, bn):
 
 
 def test_dense2pad_with_table():
-    ops = _ops()
+    ops = ops_module()
     Fr, h, w, Cin, Cout = 3, 5, 7, 256, 128
     a = randn(Fr * h * w, Cin, seed=1, dtype=BF16)
     wb = randn(Cout, Cin, scale=Cin ** -0.5, seed=2, dtype=BF16)
@@ -401,7 +388,7 @@ def test_dense2pad_with_table():
 
 
 def test_im2col_s2_and_conv():
-    ops = _ops()
+    ops = ops_module()
     Fr, h, w, C, Cout = 2, 7, 5, 64, 64
     x = randn(Fr, C, h, w, seed=1)
     wt = randn(Cout, C, 3, 3, scale=(9 * C) ** -0.5, seed=2)
@@ -417,7 +404,7 @@ def test_im2col_s2_and_conv():
 
 @pytest.mark.parametrize("h,w,H,W,C", [(4, 4, 8, 8, 64), (19, 19, 37, 37, 256), (8, 12, 14, 21, 128), (1, 1, 3, 3, 64)])
 def test_upsample_bilinear(h, w, H, W, C):
-    ops = _ops()
+    ops = ops_module()
     Fr = 2
     x = randn(Fr, C, h, w, seed=1)
     tx, ty = randn(W, C // 2, seed=2), randn(H, C // 2, seed=3)
@@ -436,7 +423,7 @@ def test_upsample_bilinear(h, w, H, W, C):
 @pytest.mark.parametrize("outc,act", [(2, 0), (4, 1)])
 def test_head_tail(outc, act):
     """3x3 conv 128->32 + ReLU + 1x1 32->outc + activations (heads/dpt_head.py:121-126; heads/head_act.py:61-125)."""
-    ops = _ops()
+    ops = ops_module()
     Fr, h, w, Cin = 2, 14, 28, 128
     x = randn(Fr, Cin, h, w, seed=1)
     w1 = randn(32, Cin, 3, 3, scale=(9 * Cin) ** -0.5, seed=2)
@@ -466,7 +453,7 @@ F16 = torch.float16
 @pytest.mark.parametrize("M,N,K,bn", [(300, 256, 128, 0), (1000, 384, 192, 128), (77, 96, 392, 64), (2748, 1024, 1024, 512),
                                       (5000, 1024, 128, 512), (2748, 384, 192, 384)])
 def test_fp16_gemm_bias_gelu(M, N, K, bn):
-    ops = _ops()
+    ops = ops_module()
     a = randn(M, K, seed=1, dtype=F16)
     w = randn(N, K, scale=K ** -0.5, seed=2, dtype=F16)
     bias = randn(N, seed=3)
@@ -479,7 +466,7 @@ def test_fp16_gemm_bias_gelu(M, N, K, bn):
 
 @pytest.mark.parametrize("Fr,h,w,Cin,Cout,bn", [(2, 9, 7, 64, 64, 0), (1, 37, 37, 256, 256, 512), (2, 30, 30, 256, 128, 384)])
 def test_fp16_conv3x3_taps_with_skips_relu(Fr, h, w, Cin, Cout, bn):
-    ops = _ops()
+    ops = ops_module()
     x = randn(Fr, Cin, h, w, seed=1)
     wt = randn(Cout, Cin, 3, 3, scale=(9 * Cin) ** -0.5, seed=2)
     bias = randn(Cout, seed=3)
@@ -501,7 +488,7 @@ def test_fp16_conv3x3_taps_with_skips_relu(Fr, h, w, Cin, Cout, bn):
 
 def test_fp16_stores_saturate_instead_of_overflowing():
     """|acc| > 65504 is stored as +-65504, never inf (cvt.rn.satfinite.f16x2.f32)."""
-    ops = _ops()
+    ops = ops_module()
     a = torch.full((256, 64), 64.0, device="cuda", dtype=F16)
     w = torch.full((64, 64), 32.0, device="cuda", dtype=F16)
     w[1::2] = -32.0
@@ -514,7 +501,7 @@ def test_fp16_stores_saturate_instead_of_overflowing():
 
 @pytest.mark.parametrize("h,w,H,W,C", [(4, 4, 8, 8, 64), (19, 19, 37, 37, 256), (8, 12, 14, 21, 144)])
 def test_fp16_upsample_bilinear(h, w, H, W, C):
-    ops = _ops()
+    ops = ops_module()
     Fr = 2
     x = randn(Fr, C, h, w, seed=1)
     tx, ty = randn(W, C // 2, seed=2), randn(H, C // 2, seed=3)
@@ -530,7 +517,7 @@ def test_fp16_upsample_bilinear(h, w, H, W, C):
 
 
 def test_fp16_layernorm_out_and_head_tail():
-    ops = _ops()
+    ops = ops_module()
     C, T, P = 2048, 21, 16
     xb = randn(4 * T, C, seed=4, dtype=BF16)
     out = torch.empty(4 * P, C, device="cuda", dtype=F16)
@@ -561,7 +548,7 @@ def test_fp16_layernorm_out_and_head_tail():
 def test_dpt_tail_fused(Fr, h, w, H, W, outc, act, dtype):
     """ovg_dpt_tail: resize + position embedding + 3x3 conv 128->32 + ReLU + 1x1 + activations in one kernel (the H x W x 128 map
     is never written) against PyTorch fp32 (heads/dpt_head.py:242-260), and against the two-kernel path it replaces."""
-    ops = _ops()
+    ops = ops_module()
     Cin = 128
     assert ops.L.lib().ovg_dpt_tail_supported(h, w, H, W, Cin) == 1
     x = randn(Fr, Cin, h, w, seed=1)
@@ -618,7 +605,7 @@ def test_c_host_drives_the_runtime(tmp_path):
 def test_attention_own_queries_against_all_keys():
     """ovg_attention with nq < nkv: a window of the query rows against ALL keys equals the same rows of the full self-attention bit
     for bit (what a rank of the context-parallel global block computes)."""
-    ops = _ops()
+    ops = ops_module()
     heads, n, lo, hi = 4, 1374 * 2, 1374, 1374 + 700
     q = randn(1, heads, n, 64, seed=1, dtype=BF16) * 0.18
     k = randn(1, heads, n, 64, seed=2, dtype=BF16)
@@ -646,7 +633,7 @@ def test_attention_own_queries_against_all_keys():
 def test_qkv_epilogue_stores_kv_rows_into_peer_buffers():
     """EPI_QKV with k_peers / v_peers: the K / V rows of this rank's tokens land in every listed full-length buffer at the rank's
     token offset (here both "peers" are local allocations) and equal what the plain epilogue writes; q stays local."""
-    ops = _ops()
+    ops = ops_module()
     C, T, frames, hp, wp = 256, 25, 2, 4, 5
     heads, M = C // 64, frames * T
     a = randn(M, C, seed=1, dtype=BF16)

@@ -2,7 +2,6 @@
 padded with white.  CPU: the numpy oracle against the UNMODIFIED reference's outputs on seeded PNG lists (tests/golden/
 load_fn.json), the package's geometry against where the oracle places each image, the errors, and a dry run of the library calls.
 GPU: libovg against the oracle and the golden, bit for bit; ovg_preprocess_image_canvas on its own; the output feeding the model."""
-import hashlib
 import json
 import os
 import types
@@ -15,6 +14,7 @@ from conftest import GOLDEN
 from oracle import load_fn_oracle as LO
 from oracle import preprocess_oracle as PO
 from oracle.make_golden_load_fn import CASES, MODES, write_case
+from ovg_support import install, sha256
 
 GOLD = json.load(open(os.path.join(GOLDEN, "load_fn.json")))
 CASE_MODES = [(c, m) for c in sorted(CASES) for m in MODES]
@@ -22,10 +22,6 @@ CASE_MODES = [(c, m) for c in sorted(CASES) for m in MODES]
 # (h, w): landscape, portrait, square, upscaled, width already 518, exact sizes, extreme aspect ratios, odd sizes
 SWEEP = [(480, 640), (500, 300), (400, 400), (60, 100), (700, 518), (392, 518), (518, 392), (518, 518), (37, 500), (500, 37),
          (1000, 999), (999, 1000), (29, 31), (203, 1001), (1001, 203), (14, 14)]
-
-
-def _sha(a):
-    return hashlib.sha256(np.ascontiguousarray(a).tobytes()).hexdigest()
 
 
 def _pillow_matches():
@@ -47,26 +43,12 @@ def oracle_placement(sizes, mode):
     return x.shape, boxes
 
 
-class _ArgRecorder:
-    def __init__(self):
-        self.calls = []
-
-    def __getattr__(self, name):
-        def fn(*a):
-            self.calls.append((name, a))
-            return 0
-        return fn
-
-
 @pytest.fixture()
 def dry(monkeypatch):
-    """The C library replaced by a recorder, on CPU tensors (as in test_components_cpu.py)."""
-    from omnivggt_official_b200 import _lib
-    rec = _ArgRecorder()
-    monkeypatch.setattr(_lib, "lib", lambda: rec)
-    monkeypatch.setattr(_lib, "stream", lambda: 0)
+    """The C library replaced by a recorder, on CPU tensors; the stream synchronisations of the loader do nothing."""
+    fake = install(monkeypatch)
     monkeypatch.setattr(torch.cuda, "current_stream", lambda *a: types.SimpleNamespace(synchronize=lambda: None))
-    return rec
+    return fake
 
 
 @pytest.mark.parametrize("case,mode", CASE_MODES)
@@ -76,8 +58,8 @@ def test_oracle_matches_reference_golden(case, mode, tmp_path):
     g = GOLD[case][mode]
     x = LO.load_and_preprocess_images(write_case(str(tmp_path), case), mode)
     assert list(x.shape) == g["shape"] and x.dtype == np.float32
-    assert _sha(x) == g["f32_sha256"]
-    assert _sha(np.rint(x.astype(np.float64) * 255).astype(np.uint8)) == g["u8_sha256"]
+    assert sha256(x) == g["f32_sha256"]
+    assert sha256(np.rint(x.astype(np.float64) * 255).astype(np.uint8)) == g["u8_sha256"]
 
 
 @pytest.mark.parametrize("mode", MODES)
@@ -127,7 +109,7 @@ def test_dry_run_arguments(dry, case, mode, tmp_path, capsys):
     assert list(out.shape) == g["shape"] and out.dtype == torch.float32
     sizes = [PP.decode_rgb(p).shape[:2] for p in sorted(paths)]
     shape, boxes = oracle_placement(sizes, mode)
-    assert [n for n, _ in dry.calls] == ["ovg_preprocess_image_canvas"] * len(paths)
+    assert dry.names() == ["ovg_preprocess_image_canvas"] * len(paths)
     for i, ((h, w), box, (_, a)) in enumerate(zip(sizes, boxes, dry.calls)):
         nw, nh = LO.resized_size(w, h, mode)
         crop = (nh - 518) // 2 if mode == "crop" and nh > 518 else 0
@@ -150,7 +132,7 @@ def test_gpu_matches_oracle_and_golden(case, mode, tmp_path, capsys):
     ref = LO.load_and_preprocess_images(paths, mode)
     assert torch.equal(out.cpu(), torch.from_numpy(ref))
     if _pillow_matches():
-        assert _sha(out.cpu().numpy()) == GOLD[case][mode]["f32_sha256"]
+        assert sha256(out.cpu().numpy()) == GOLD[case][mode]["f32_sha256"]
 
 
 @pytest.mark.gpu

@@ -3,7 +3,6 @@ CPU: the numpy oracle against the UNMODIFIED reference's outputs on a seeded cas
 large-set oracle against the definition, a dry run of the library calls, and the errors.
 GPU: libovg's ovg_match_* against the oracle bit for bit, against cKDTree on two 518^2 views, a 24-view scene against per-pair
 calls, and OmniVGGT.matches on the mini model."""
-import hashlib
 import json
 import os
 import types
@@ -15,14 +14,11 @@ import torch
 from conftest import GOLDEN
 from oracle import matches_oracle as MO
 from oracle.make_golden_matches import make_cases, surface_views
+from ovg_support import install, sha256
 
 GOLD = json.load(open(os.path.join(GOLDEN, "matches.json")))
 CASES = make_cases()
 NAMES = sorted(CASES)
-
-
-def _sha(a) -> str:
-    return hashlib.sha256(np.ascontiguousarray(a).tobytes()).hexdigest()
 
 
 def _check_against_golden(name, rec, nn2, count):
@@ -31,10 +27,10 @@ def _check_against_golden(name, rec, nn2, count):
     g = GOLD[name]
     P1, P2 = CASES[name]
     assert (len(rec), len(nn2)) == (g["m"], g["m"])
-    assert _sha(np.sqrt(MO.d2_of(P2, P1, nn2))) == g["dist2_sha256"]
+    assert sha256(np.sqrt(MO.d2_of(P2, P1, nn2))) == g["dist2_sha256"]
     if not g["has_ties"]:
         assert count == g["count"]
-        assert _sha(np.asarray(rec, bool)) == g["reciprocal_sha256"] and _sha(np.asarray(nn2, np.int64)) == g["nn2_in_P1_sha256"]
+        assert sha256(np.asarray(rec, bool)) == g["reciprocal_sha256"] and sha256(np.asarray(nn2, np.int64)) == g["nn2_in_P1_sha256"]
 
 
 def _scene(S, H, W, seed=5):
@@ -54,7 +50,7 @@ def test_oracle_matches_reference_golden(name):
     rec, nn2, count = MO.find_reciprocal_matches(P1, P2)
     _check_against_golden(name, rec, nn2, count)
     nn1, _ = MO.nn_brute(P1, P2)
-    assert _sha(np.sqrt(MO.d2_of(P1, P2, nn1))) == GOLD[name]["dist1_sha256"]
+    assert sha256(np.sqrt(MO.d2_of(P1, P2, nn1))) == GOLD[name]["dist1_sha256"]
 
 
 @pytest.mark.parametrize("name", ["duplicates", "all_equal_same", "surface", "point_cloud_01", "far_outlier"])
@@ -68,30 +64,8 @@ def test_kdtree_oracle_equals_definition(name):
 
 @pytest.fixture()
 def dry(monkeypatch):
-    """The C library replaced by a recorder, on CPU tensors; host reads counted."""
-    from omnivggt_official_b200 import _lib, ops
-
-    class Rec:
-        def __init__(self):
-            self.calls, self.reads = [], 0
-
-        def __getattr__(self, name):
-            def fn(*a):
-                self.calls.append((name, a))
-                return 0
-            return fn
-
-    rec = Rec()
-
-    def read(t):
-        rec.reads += 1
-        return t.cpu()
-
-    monkeypatch.setattr(_lib, "lib", lambda: rec)
-    monkeypatch.setattr(_lib, "stream", lambda: 0)
-    monkeypatch.setattr(ops, "_on_device", lambda t: True)
-    monkeypatch.setattr(ops, "host_read", read)
-    return rec
+    """The C library replaced by a recorder, on CPU tensors; host reads are recorded in ``reads`` only."""
+    return install(monkeypatch, read_in_calls=False)
 
 
 @pytest.mark.parametrize("pairs", [[(0, 1)], [(3, 1), (0, 2)], None])
@@ -101,13 +75,12 @@ def test_dry_run_builds_once_and_reads_once(dry, pairs):
     S, H, W = 6, 8, 10
     out = OmniVGGT.matches(_scene(S, H, W), pairs)
     P = len(pairs) if pairs is not None else S * (S - 1) // 2
-    assert [n for n, _ in dry.calls] == ["ovg_conf_percentile_mask", "ovg_match_workspace_bytes", "ovg_match_index",
-                                         "ovg_match_query"]
+    assert dry.names() == ["ovg_conf_percentile_mask", "ovg_match_workspace_bytes", "ovg_match_index", "ovg_match_query"]
     _, idx = dry.calls[2]
     assert idx[2:5] == (S, H * W, P)
     _, q = dry.calls[3]
     assert q[1:4] == (P, S, H * W)
-    assert dry.reads == 1
+    assert len(dry.reads) == 1
     assert len(out) == P and all(o["count"] == 0 for o in out)
 
 

@@ -3,10 +3,7 @@ CPU: the numpy oracle against the UNMODIFIED reference's outputs (tests/golden/m
 reference layout, the .glb writer, a dry run of the library calls, and the errors.
 GPU: libovg's ovg_mesh_* / OmniVGGT.mesh / the geometry drop-ins against the oracle bit for bit, 24 views of 518^2, single
 views, repeats, and the mini model."""
-import hashlib
-import json
 import os
-import struct
 
 import numpy as np
 import pytest
@@ -17,6 +14,7 @@ from conftest import GOLDEN
 from oracle import mesh_oracle as MO
 from oracle.make_golden_cloud import GLB_CASES
 from oracle.make_golden_mesh import cloud_inputs, glb_case_views, make_cases
+from ovg_support import dry, parse_glb, scene, sha256  # noqa: F401  (fixture)
 
 GOLD = {k: v.numpy() for k, v in load_file(os.path.join(GOLDEN, "mesh.safetensors")).items()}
 CASES = make_cases()
@@ -24,14 +22,10 @@ NAMES = sorted(CASES)
 KEYS = ("vertices", "face_colors", "faces")
 
 
-def _sha(a) -> bytes:
-    return hashlib.sha256(np.ascontiguousarray(a).tobytes()).digest()
-
-
 def _check_golden(key, m):
     assert len(m["faces"]) == int(GOLD[f"{key}_count"])
     for k in KEYS:
-        assert _sha(m[k]) == GOLD[f"{key}_{k}_sha256"].tobytes(), (key, k)
+        assert sha256(m[k], hex=False) == GOLD[f"{key}_{k}_sha256"].tobytes(), (key, k)
 
 
 def _np(d):
@@ -89,20 +83,6 @@ def test_glb_layout_expands_to_the_forward_faces(i):
     assert 2 * len(glb["indices"]) == n_ref
 
 
-def _parse_glb(data: bytes):
-    magic, version, total = struct.unpack_from("<III", data, 0)
-    assert magic == 0x46546C67 and version == 2 and total == len(data)
-    jlen, jtype = struct.unpack_from("<II", data, 12)
-    assert jtype == 0x4E4F534A and jlen % 4 == 0
-    doc = json.loads(data[20:20 + jlen].decode())
-    off = 20 + jlen
-    if off == total:
-        return doc, b""
-    blen, btype = struct.unpack_from("<II", data, off)
-    assert btype == 0x004E4942 and blen % 4 == 0 and off + 8 + blen == total
-    return doc, data[off + 8:off + 8 + blen]
-
-
 def _read_mesh(doc, binary):
     prim = doc["meshes"][0]["primitives"][0]
     assert prim["mode"] == 4
@@ -136,7 +116,7 @@ def test_write_mesh_glb_parses(tmp_path):
                 "indices": torch.from_numpy(np.searchsorted(used, idx).astype(np.int32)), "align": o["align"]}
         path = tmp_path / "mesh.glb"
         write_mesh_glb(str(path), mesh)
-        doc, binary = _parse_glb(path.read_bytes())
+        doc, binary = parse_glb(path.read_bytes())
         assert doc["asset"]["version"] == "2.0" and doc["scenes"][doc["scene"]]["nodes"] == [0]
         p, c, i = _read_mesh(doc, binary)
         assert np.array_equal(p[i], o["positions"][idx]) and np.array_equal(c[:, :3], o["colors"][used])
@@ -150,11 +130,11 @@ def test_write_mesh_glb_empty_and_non_finite(tmp_path):
     path = tmp_path / "empty.glb"
     write_mesh_glb(str(path), {"positions": np.zeros((0, 3), np.float32), "colors": np.zeros((0, 3), np.uint8),
                                "indices": np.zeros((0, 3), np.int32), "align": np.eye(4)})
-    doc, binary = _parse_glb(path.read_bytes())
+    doc, binary = parse_glb(path.read_bytes())
     assert binary == b"" and doc["scenes"] == [{}] and doc["scene"] == 0 and "meshes" not in doc
     pos = np.array([[0, 0, 0], [1, 0, 0], [0, 1, 0]], np.float32)
     mesh = {"positions": pos, "colors": np.zeros((3, 3), np.uint8), "indices": np.array([[0, 1, 2]], np.int32)}
-    _read_mesh(*_parse_glb(mesh_glb_bytes(mesh)))
+    _read_mesh(*parse_glb(mesh_glb_bytes(mesh)))
     for bad in (np.nan, np.inf, -np.inf):
         pos[1, 2] = bad
         with pytest.raises(ValueError, match="finite"):
@@ -162,41 +142,6 @@ def test_write_mesh_glb_empty_and_non_finite(tmp_path):
     pos[1, 2] = 0.0
     with pytest.raises(ValueError, match="indices"):
         mesh_glb_bytes({**mesh, "indices": np.array([[0, 1, 3]], np.int32)})
-
-
-@pytest.fixture()
-def dry(monkeypatch):
-    """The C library replaced by a recorder, on CPU tensors; host reads counted."""
-    from omnivggt_official_b200 import _lib, ops
-
-    class Rec:
-        def __init__(self):
-            self.calls, self.reads = [], 0
-
-        def __getattr__(self, name):
-            def fn(*a):
-                self.calls.append((name, a))
-                return 0
-            return fn
-
-    rec = Rec()
-
-    def read(t):
-        rec.calls.append(("host_read", ()))
-        rec.reads += 1
-        return t.cpu()
-
-    monkeypatch.setattr(_lib, "lib", lambda: rec)
-    monkeypatch.setattr(_lib, "stream", lambda: 0)
-    monkeypatch.setattr(ops, "_on_device", lambda t: True)
-    monkeypatch.setattr(ops, "host_read", read)
-    return rec
-
-
-def _scene(S, H, W, seed=3):
-    g = torch.Generator().manual_seed(seed)
-    return {"images": torch.rand(1, S, 3, H, W, generator=g), "world_points_from_depth": torch.randn(1, S, H, W, 3, generator=g),
-            "depth_conf": 1.0 + torch.rand(1, S, H, W, generator=g), "extrinsic": torch.eye(4)[:3].repeat(1, S, 1, 1)}
 
 
 @pytest.mark.parametrize("layout", ["reference", "glb"])
@@ -207,23 +152,23 @@ def test_dry_run_call_order_and_launches(dry, layout):
     seqs = []
     for S in (1, 24):
         dry.calls.clear()
-        out = OmniVGGT.mesh(_scene(S, 6, 8), layout=layout, mask_white_bg=True)
-        names = [n for n, _ in dry.calls]
+        out = OmniVGGT.mesh(scene(S, 6, 8), layout=layout, mask_white_bg=True)
+        names = dry.names()
         assert names == ["ovg_conf_percentile_mask", "ovg_mesh_workspace_bytes", "ovg_mesh_count", "host_read", last]
         _, cnt = dry.calls[2]
         assert cnt[2:7] == (S, 6, 8, 0, 1)
         seqs.append(names)
         assert "align" in out and "conf_threshold" in out
-    assert seqs[0] == seqs[1] and dry.reads == 2
+    assert seqs[0] == seqs[1] and len(dry.reads) == 2
     dry.calls.clear()
-    OmniVGGT.mesh(_scene(5, 6, 8), frame=3)
+    OmniVGGT.mesh(scene(5, 6, 8), frame=3)
     assert dry.calls[2][1][2] == 1                                       # one view after the frame selection
 
 
 def test_errors_before_any_device_work(dry):
     from omnivggt_official_b200 import OmniVGGT
     from omnivggt_official_b200.geometry import cat_meshes, pts3d_to_trimesh
-    pred = _scene(4, 6, 8)
+    pred = scene(4, 6, 8)
     with pytest.raises(ValueError, match="source"):
         OmniVGGT.mesh(pred, source="normals")
     for pct in (-1.0, 100.5):

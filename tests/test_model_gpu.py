@@ -16,16 +16,12 @@ from safetensors.torch import load_file
 from conftest import GOLDEN, golden_index, golden_schema
 from oracle import full_golden
 from oracle.synth import make_inputs, make_state_dict
+from ovg_support import rel
 
 pytestmark = pytest.mark.gpu
 INDEX = golden_index()
 TOL = 2e-2
 KEYS = ("pose_enc", "depth", "depth_conf", "world_points", "world_points_conf")
-
-
-def rel(a, b):
-    a, b = a.float().cpu(), b.float().cpu()
-    return ((a - b).norm() / b.norm().clamp(min=1e-12)).item()
 
 
 def build(variant, dino_dtype=torch.float32):
@@ -54,7 +50,7 @@ def reduced_golden_check(case, out, keys=KEYS, log=False):
     """The outputs ``keys`` of a forward of the reduced golden ``case`` against the reference's: shape, dtype, finiteness and
     relative L2 under TOL; pose_enc also max-abs 5e-2.  ``log``: print the errors and append them to the parity log first."""
     ref = load_file(os.path.join(GOLDEN, f"{case}.safetensors"))
-    errs = {k: rel(out[k], ref[k]) for k in keys}
+    errs = {k: rel(out[k], ref[k], host=True) for k in keys}
     if log:
         print(case, json.dumps(errs))
         d = os.path.join(os.path.dirname(GOLDEN), os.pardir, "gpurun_out")
@@ -104,7 +100,7 @@ def test_batch_independence_and_determinism():
     one = m(depth_gt_index=[1], camera_gt_index=[0, 2], **{k: v[1:2] for k, v in inp.items()})
     for k in KEYS:
         assert torch.equal(both[k], again[k]), k
-        assert rel(both[k][1:2], one[k]) < 2e-3, (k, rel(both[k][1:2], one[k]))
+        assert rel(both[k][1:2], one[k], host=True) < 2e-3, (k, rel(both[k][1:2], one[k], host=True))
 
 
 def test_cuda_graph_replay_matches_eager():
@@ -163,7 +159,7 @@ def test_view_permutation_equivariance():
     a = m(**inp, depth_gt_index=[], camera_gt_index=[])
     b = m(**{k: v[:, perm] for k, v in inp.items()}, depth_gt_index=[], camera_gt_index=[])
     for k in KEYS:
-        assert rel(b[k], a[k][:, perm]) < 1e-2, (k, rel(b[k], a[k][:, perm]))
+        assert rel(b[k], a[k][:, perm], host=True) < 1e-2, (k, rel(b[k], a[k][:, perm], host=True))
 
 
 @pytest.mark.parametrize("aux", [False, True])
@@ -184,7 +180,7 @@ def test_full_width_vs_oracle(aux):
     out = m(depth_gt_index=didx, camera_gt_index=cidx, **{k: v.cuda() for k, v in inp.items()})
     torch.cuda.synchronize()
     ref = omnivggt_forward(sd, depth_gt_index=didx, camera_gt_index=cidx, cfg=OracleConfig(dpt_layers=(0, 1, 2, 3)), **inp)
-    errs = {k: rel(out[k], ref[k]) for k in KEYS}
+    errs = {k: rel(out[k], ref[k], host=True) for k in KEYS}
     print("full_width", aux, json.dumps(errs))
     for k in KEYS:
         assert errs[k] < TOL, errs
@@ -331,6 +327,6 @@ def test_full_size_configs_properties(S, didx, cidx):
             assert torch.equal(o[k], a[k]), k
     assert (a["depth"] > 0).all() and (a["depth_conf"] >= 1).all() and (a["world_points_conf"] >= 1).all()
     b = m(depth_gt_index=[], camera_gt_index=[], **inp)
-    assert rel(b["depth"], a["depth"]) > 1e-4 and rel(b["pose_enc"], a["pose_enc"]) > 1e-4
+    assert rel(b["depth"], a["depth"], host=True) > 1e-4 and rel(b["pose_enc"], a["pose_enc"], host=True) > 1e-4
     del m
     torch.cuda.empty_cache()

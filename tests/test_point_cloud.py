@@ -1,9 +1,6 @@
 """Point cloud and GLB export: the numpy oracle against the unmodified reference's GLB export and viewer (CPU), the .glb
 writer (CPU), and the libovg point-cloud kernels / OmniVGGT.point_cloud against the oracle (GPU)."""
-import hashlib
-import json
 import os
-import struct
 
 import numpy as np
 import pytest
@@ -13,10 +10,7 @@ from safetensors.torch import load_file
 from conftest import GOLDEN
 from oracle import pointcloud_oracle as PC
 from oracle.make_golden_cloud import GLB_CASES, VIEWER_CASES, make_cloud_inputs
-
-
-def _sha(a) -> bytes:
-    return hashlib.sha256(np.ascontiguousarray(a).tobytes()).digest()
+from ovg_support import dry, parse_glb, scene, sha256  # noqa: F401  (fixture)
 
 
 def _gold():
@@ -26,7 +20,7 @@ def _gold():
     inp = make_cloud_inputs()
     for k in ("images", "depth_conf", "world_points", "world_points_conf"):
         g[k] = inp[k][0].numpy()
-        assert _sha(g[k]) == g[f"{k}_sha256"].tobytes(), f"make_cloud_inputs no longer reproduces {k}"
+        assert sha256(g[k], hex=False) == g[f"{k}_sha256"].tobytes(), f"make_cloud_inputs no longer reproduces {k}"
     return g
 
 
@@ -53,12 +47,12 @@ def test_oracle_matches_reference_glb_export(i):
     o = PC.point_cloud(world, conf, g["images"], g["extrinsic"], pct, 1e-5, frame, black, white)
     if len(o["points"]) == 0:                                    # the reference's placeholder (visual_util.py:226-229)
         assert int(g[f"glb{i}_count"]) == 1 and o["scale"] == 1.0
-        assert _sha(np.array([[1, 0, 0]])) == g[f"glb{i}_points_sha256"].tobytes()
-        assert _sha(np.array([[255, 255, 255]])) == g[f"glb{i}_colors_sha256"].tobytes()
+        assert sha256(np.array([[1, 0, 0]]), hex=False) == g[f"glb{i}_points_sha256"].tobytes()
+        assert sha256(np.array([[255, 255, 255]]), hex=False) == g[f"glb{i}_colors_sha256"].tobytes()
     else:
         assert len(o["points"]) == int(g[f"glb{i}_count"]) and o["points"].dtype == np.float32
-        assert _sha(o["points"]) == g[f"glb{i}_points_sha256"].tobytes()
-        assert _sha(o["colors"]) == g[f"glb{i}_colors_sha256"].tobytes()
+        assert sha256(o["points"], hex=False) == g[f"glb{i}_points_sha256"].tobytes()
+        assert sha256(o["colors"], hex=False) == g[f"glb{i}_colors_sha256"].tobytes()
         assert set(np.unique(o["frame"])) <= ({0, 1, 2} if frame is None else {frame})
         assert (np.diff(o["frame"]) >= 0).all()
     assert float(o["scale"] * 0.05) == float(g[f"glb{i}_radius"])          # cam_width = scene_scale * 0.05, fp32
@@ -73,20 +67,8 @@ def test_oracle_matches_reference_viewer(i):
     pct, black, white = VIEWER_CASES[i]
     o = PC.point_cloud(g["world_points_from_depth"], g["depth_conf"], g["images"], g["extrinsic"], pct, 0.1, None, black, white)
     assert len(o["points"]) == int(g[f"viewer{i}_count"])
-    assert _sha(o["points"] - o["center"]) == g[f"viewer{i}_points_sha256"].tobytes()
-    assert _sha(o["colors"]) == g[f"viewer{i}_colors_sha256"].tobytes()
-
-
-def _parse_glb(data: bytes):
-    magic, version, total = struct.unpack_from("<III", data, 0)
-    assert magic == 0x46546C67 and version == 2 and total == len(data)
-    jlen, jtype = struct.unpack_from("<II", data, 12)
-    assert jtype == 0x4E4F534A and jlen % 4 == 0
-    doc = json.loads(data[20:20 + jlen].decode())
-    off = 20 + jlen
-    blen, btype = struct.unpack_from("<II", data, off)
-    assert btype == 0x004E4942 and blen % 4 == 0 and off + 8 + blen == total
-    return doc, data[off + 8:off + 8 + blen]
+    assert sha256(o["points"] - o["center"], hex=False) == g[f"viewer{i}_points_sha256"].tobytes()
+    assert sha256(o["colors"], hex=False) == g[f"viewer{i}_colors_sha256"].tobytes()
 
 
 def _read_cloud(doc, binary):
@@ -116,7 +98,7 @@ def test_write_glb_round_trip(tmp_path):
         cloud = {"points": torch.from_numpy(o["points"][:n]), "colors": torch.from_numpy(o["colors"][:n]), "align": o["align"]}
         path = tmp_path / "scene.glb"
         write_glb(str(path), cloud)
-        doc, binary = _parse_glb(path.read_bytes())
+        doc, binary = parse_glb(path.read_bytes())
         assert doc["asset"]["version"] == "2.0"
         p, c = _read_cloud(doc, binary)
         assert np.array_equal(p, o["points"][:n]) and np.array_equal(c[:, :3], o["colors"][:n]) and (c[:, 3] == 255).all()
@@ -128,46 +110,9 @@ def test_write_glb_empty_cloud_is_the_reference_placeholder(tmp_path):
     from omnivggt_official_b200.glb import write_glb
     path = tmp_path / "empty.glb"
     write_glb(str(path), {"points": np.zeros((0, 3), np.float32), "colors": np.zeros((0, 3), np.uint8), "align": np.eye(4)})
-    doc, binary = _parse_glb(path.read_bytes())
+    doc, binary = parse_glb(path.read_bytes())
     p, c = _read_cloud(doc, binary)
     assert np.array_equal(p, [[1, 0, 0]]) and np.array_equal(c, [[255, 255, 255, 255]])
-
-
-@pytest.fixture()
-def dry(monkeypatch):
-    """The C library replaced by a recorder, on CPU tensors; host reads counted."""
-    from omnivggt_official_b200 import _lib, ops
-
-    class Rec:
-        def __init__(self):
-            self.calls, self.reads = [], 0
-
-        def __getattr__(self, name):
-            def fn(*a):
-                self.calls.append((name, a))
-                return 0
-            return fn
-
-    rec = Rec()
-
-    def read(t):
-        rec.calls.append(("host_read", ()))
-        rec.reads += 1
-        return t.cpu()
-
-    monkeypatch.setattr(_lib, "lib", lambda: rec)
-    monkeypatch.setattr(_lib, "stream", lambda: 0)
-    monkeypatch.setattr(ops, "_on_device", lambda t: True)
-    monkeypatch.setattr(ops, "host_read", read)
-    return rec
-
-
-def _scene(S, H, W, seed=3):
-    g = torch.Generator().manual_seed(seed)
-    ext = torch.eye(4)[:3].repeat(1, S, 1, 1)
-    ext[0, :, :, 3] = torch.arange(S, dtype=torch.float32)[:, None]          # a different camera per view
-    return {"images": torch.rand(1, S, 3, H, W, generator=g), "world_points_from_depth": torch.randn(1, S, H, W, 3, generator=g),
-            "depth_conf": 1.0 + torch.rand(1, S, H, W, generator=g), "extrinsic": ext}
 
 
 def test_dry_run_call_order_and_one_host_read(dry):
@@ -177,25 +122,25 @@ def test_dry_run_call_order_and_one_host_read(dry):
     seqs = []
     for S in (1, 24):
         dry.calls.clear()
-        out = OmniVGGT.point_cloud(_scene(S, 6, 8), mask_white_bg=True)
-        names = [n for n, _ in dry.calls]
+        out = OmniVGGT.point_cloud(scene(S, 6, 8, distinct_cameras=True), mask_white_bg=True)
+        names = dry.names()
         assert names == ["ovg_conf_percentile_mask", "ovg_point_cloud_workspace_bytes", "ovg_point_cloud_count",
                          "ovg_point_cloud_center", "host_read"]
         assert dry.calls[2][1][2:7] == (S, 6, 8, 0, 1)
         assert out["points"].shape == (0, 3) and torch.equal(out["align"], OmniVGGT._align(torch.eye(4)[:3].double()))
         seqs.append(names)
-    assert seqs[0] == seqs[1] and dry.reads == 2
+    assert seqs[0] == seqs[1] and len(dry.reads) == 2
     dry.calls.clear()
-    pred = _scene(5, 6, 8)
+    pred = scene(5, 6, 8, distinct_cameras=True)
     out = OmniVGGT.point_cloud(pred, frame=3)
     assert dry.calls[2][1][2] == 1                                       # one view after the frame selection
     assert torch.equal(out["align"], OmniVGGT._align(pred["extrinsic"][0, 3].double()))
-    assert dry.reads == 3
+    assert len(dry.reads) == 3
 
 
 def test_errors_before_any_device_work(dry):
     from omnivggt_official_b200 import OmniVGGT
-    pred = _scene(4, 6, 8)
+    pred = scene(4, 6, 8, distinct_cameras=True)
     with pytest.raises(ValueError, match="source"):
         OmniVGGT.point_cloud(pred, source="normals")
     for pct in (-1.0, 100.5):
@@ -256,7 +201,8 @@ def test_point_cloud_kernels_match_golden(i):
         assert float(d["scale"]) == 1.0 and d["colors"].shape == (0, 3)
     elif float(d["conf_threshold"]) == float(g[f"glb{i}_thr"]):
         assert len(d["points"]) == int(g[f"glb{i}_count"])
-        assert _sha(d["points"]) == g[f"glb{i}_points_sha256"].tobytes() and _sha(d["colors"]) == g[f"glb{i}_colors_sha256"].tobytes()
+        assert sha256(d["points"], hex=False) == g[f"glb{i}_points_sha256"].tobytes()
+        assert sha256(d["colors"], hex=False) == g[f"glb{i}_colors_sha256"].tobytes()
 
 
 @pytest.mark.gpu
@@ -269,7 +215,7 @@ def test_point_cloud_reproduces_viewer(i):
     _check_against_oracle(d, g["world_points_from_depth"], g["depth_conf"], g["images"], g["extrinsic"], pct, 0.1, None,
                           black, white)
     if len(d["points"]) == int(g[f"viewer{i}_count"]):       # recentring: the centre is checked against the oracle above
-        assert _sha(d["colors"]) == g[f"viewer{i}_colors_sha256"].tobytes()
+        assert sha256(d["colors"], hex=False) == g[f"viewer{i}_colors_sha256"].tobytes()
 
 
 def _large_inputs(S=24, H=518, W=518, seed=7):

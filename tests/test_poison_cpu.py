@@ -6,8 +6,7 @@ import pytest
 import torch
 
 from oracle.synth import make_inputs
-from test_dryrun_cpu import dry  # noqa: F401  (fixture)
-from test_host_cpu import mini_model
+from ovg_support import dry_workspaces, mini_model, scene  # noqa: F401  (fixture "dry")
 from test_poison_gpu import GUARD, GUARD_BYTE, PACKAGE_MODULES, poison  # noqa: F401  (fixture)
 
 
@@ -84,7 +83,7 @@ def _pointers(name, args):
 def _coverage(rec, P, want):
     ranges = P.ranges()
     seen = set()
-    for name, args in rec.args:
+    for name, args in rec.calls:
         if name.endswith(("_create", "_destroy", "_workspace_bytes")):
             continue
         assert name in PTR_ARGS, f"{name}: entry point without a workspace / output map in PTR_ARGS"
@@ -104,7 +103,7 @@ def test_dry_run_forward_allocates_through_the_proxy(dry, poison):
         inp = make_inputs(1, 9, 28, 28, seed=1)
         out = m(depth_gt_index=[4], camera_gt_index=[0, 3], **inp)
         assert out["depth"].shape == (1, 9, 28, 28, 1)
-        assert dry.calls.count("ovg_dpt_forward") == 4
+        assert dry.count("ovg_dpt_forward") == 4
         assert {"agg_ws", "dino_ws", "cam.ws", "depth_head.ws", "point_head.ws"} <= set(m._engine.ws.bufs)
         _coverage(dry, P, {"ovg_aggregator_forward", "ovg_dino_forward", "ovg_dpt_forward", "ovg_camera_forward"})
         assert P.guards_broken() == []
@@ -112,7 +111,6 @@ def test_dry_run_forward_allocates_through_the_proxy(dry, poison):
 
 def test_dry_run_point_cloud_allocates_through_the_proxy(dry, poison):
     from omnivggt_official_b200 import OmniVGGT
-    from test_point_cloud import _scene
     with poison("nan", devices=("cpu",)) as P:
-        OmniVGGT.point_cloud(_scene(3, 6, 8), mask_black_bg=True)
+        OmniVGGT.point_cloud(scene(3, 6, 8, distinct_cameras=True), mask_black_bg=True)
         _coverage(dry, P, {"ovg_conf_percentile_mask", "ovg_point_cloud_count", "ovg_point_cloud_center"})

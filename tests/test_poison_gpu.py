@@ -35,12 +35,15 @@ Which launch first writes each stateful region, per entry point (read from csrc/
                w2c / K: camera_prepare_kernel, zeros for a view without a camera; depth and mask maps are torch.zeros.
 Context parallelism is not covered: its peer flags and epoch counter are persistent by design and it needs two GPUs."""
 import contextlib
+import functools
 import importlib
 import sys
 
 import numpy as np
 import pytest
 import torch
+
+from ovg_support import randn, scene
 
 GUARD = 4096                 # keeps the 256-byte workspace and 16-byte TMA alignment of the allocator's blocks
 GUARD_BYTE = 0x5A
@@ -448,8 +451,7 @@ def test_point_cloud_filter_modes(kind):
 
 
 def _scene_cuda(S=3, H=40, W=48, seed=3):
-    from test_point_cloud import _scene
-    return {k: v.cuda() for k, v in _scene(S, H, W, seed).items()}
+    return {k: v.cuda() for k, v in scene(S, H, W, seed, distinct_cameras=True).items()}
 
 
 def _host_sky(images):
@@ -652,9 +654,7 @@ def test_load_images_and_cameras(name, tmp_path):
 
 
 # ------------------------------------------------------------------------------------------------------------------ kernel entry points
-def _randn(*s, scale=1.0, seed=0):
-    g = torch.Generator().manual_seed(seed)
-    return (torch.randn(*s, generator=g) * scale).cuda()
+_randn = functools.partial(randn, host_rng=True)
 
 
 def _to_pad(x, dtype):

@@ -1,7 +1,6 @@
 """Input pipeline (SURVEY.md section 8f rank 4).  CPU: the oracle (Pillow / OpenCV calls as in the reference + the restated tap and
 index tables) against the UNMODIFIED reference loader's outputs on the seeded synthetic folders (tests/golden/preprocess.json).
 GPU: the libovg kernels against the oracle, bit for bit on images / depth / mask."""
-import hashlib
 import json
 import os
 
@@ -12,12 +11,9 @@ import torch
 from conftest import GOLDEN
 from oracle import preprocess_oracle as PO
 from oracle.synth_folder import FOLDERS, make_folder
+from ovg_support import sha256
 
 GOLD = json.load(open(os.path.join(GOLDEN, "preprocess.json")))
-
-
-def _sha(a):
-    return hashlib.sha256(np.ascontiguousarray(a).tobytes()).hexdigest()
 
 
 def _read_folder(d):
@@ -53,8 +49,8 @@ def test_oracle_matches_reference_loader(name, tmp_path):
     deps = [d.T if t else d for d, t in zip(deps, tr)]          # the reference transposes PNG depth (visual_util.py:771)
     images, extr, intr, dep, mask, didx, cidx = PO.load_views(imgs, cams, deps)
     assert list(images.shape) == g["images_shape"] and didx == g["depth_indices"] and cidx == g["camera_indices"]
-    assert _sha(images.astype(np.float32)) == g["images_f32_sha256"]
-    assert _sha(dep.astype(np.float32)) == g["depth_sha256"] and _sha(mask.astype(np.float32)) == g["mask_sha256"]
+    assert sha256(images.astype(np.float32)) == g["images_f32_sha256"]
+    assert sha256(dep.astype(np.float32)) == g["depth_sha256"] and sha256(mask.astype(np.float32)) == g["mask_sha256"]
     assert np.allclose(extr, np.array(g["extrinsics"]), atol=2e-6) and np.allclose(intr, np.array(g["intrinsics"]), rtol=1e-5, atol=1e-3)
 
 
@@ -92,7 +88,7 @@ def check_pipeline_against_oracle(name, d, out):
     assert np.allclose(out[1].cpu().numpy(), ref[1], atol=2e-6) and np.allclose(out[2].cpu().numpy(), ref[2], rtol=1e-6, atol=1e-4)
     if PIL_version_matches():
         g = GOLD[name]
-        assert _sha(out[0].cpu().numpy()) == g["images_f32_sha256"] and _sha(out[3].cpu().numpy()) == g["depth_sha256"]
+        assert sha256(out[0].cpu().numpy()) == g["images_f32_sha256"] and sha256(out[3].cpu().numpy()) == g["depth_sha256"]
 
 
 def PIL_version_matches():

@@ -1,7 +1,6 @@
 """Image ranking by camera distance: the numpy oracle against the unmodified reference's compute_ranking (CPU), the
 validation and call pattern of the drop-in on a recorded library (CPU), and the libovg kernels against the goldens and the
 oracle on both regimes (GPU)."""
-import hashlib
 import json
 import os
 
@@ -12,6 +11,7 @@ import torch
 from conftest import GOLDEN
 from oracle import ranking_oracle as RO
 from oracle.make_golden_ranking import make_cases, poses, trajectory
+from ovg_support import install, sha256
 
 CASES = make_cases()
 CTA = 8192           # OVG_RANK_CTA_VIEWS: one CTA per row with the keys in shared memory up to here, the grid above
@@ -36,7 +36,7 @@ def _truth(k, rows=None):
 def test_golden_inputs_are_reproduced(name):
     m = _meta()[name]
     E = CASES[name]["E"]
-    assert hashlib.sha256(np.ascontiguousarray(E).tobytes()).hexdigest() == m["E_sha256"]
+    assert sha256(E) == m["E_sha256"]
     assert list(E.shape) == m["E_shape"] and str(E.dtype) == m["E_dtype"]
 
 
@@ -81,31 +81,11 @@ def test_numpy_restatement_matches_the_reference(name):
 
 @pytest.fixture()
 def dry(monkeypatch):
-    """The C library replaced by a recorder, on CPU tensors; host reads counted."""
-    from omnivggt_official_b200 import _lib, geometry, ops
-
-    class Rec:
-        def __init__(self):
-            self.calls = []
-
-        def __getattr__(self, name):
-            def fn(*a):
-                self.calls.append((name, a))
-                return 0
-            return fn
-
-    rec = Rec()
-
-    def read(t):
-        rec.calls.append(("host_read", ()))
-        return t.cpu()
-
-    monkeypatch.setattr(_lib, "lib", lambda: rec)
-    monkeypatch.setattr(_lib, "stream", lambda: 0)
-    monkeypatch.setattr(ops, "_on_device", lambda t: True)
-    monkeypatch.setattr(ops, "host_read", read)
+    """The C library replaced by a recorder, on CPU tensors; host reads recorded."""
+    from omnivggt_official_b200 import geometry
+    fake = install(monkeypatch)
     monkeypatch.setattr(geometry, "_device_of", lambda *xs: torch.device("cpu"))
-    return rec
+    return fake
 
 
 @pytest.mark.parametrize("N,dtype,batched,out", [(50, np.float64, True, torch.float64), (50, np.float32, True, torch.float32),
@@ -120,7 +100,7 @@ def test_dry_run_is_one_call_without_host_read(dry, N, dtype, batched, out):
         for lam, normalize in ((1.0, True), (0.1, False)):
             dry.calls.clear()
             ranking, dists = compute_ranking(E, lambda_t=lam, normalize=normalize, batched=batched, k=k)
-            assert [n for n, _ in dry.calls] == ["ovg_ranking_workspace_bytes", "ovg_compute_ranking"]
+            assert dry.names() == ["ovg_ranking_workspace_bytes", "ovg_compute_ranking"]
             assert dry.calls[0][1] == (N, int(out == torch.float64))
             a = dry.calls[1][1]
             f32_compute = dtype == np.float32 or out == torch.float32

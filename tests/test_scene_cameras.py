@@ -7,6 +7,8 @@ import itertools
 import pytest
 import torch
 
+from ovg_support import install
+
 B, S, H, W = 2, 3, 4, 5
 SCENE = 1
 OWN, DECODED = 10.0, 20.0          # translations (plus the view index) of the predictions' and of the decoded extrinsics
@@ -27,37 +29,22 @@ def tracks_decodes(has_ext, has_intr, unproject):
 
 @pytest.fixture()
 def dry(monkeypatch):
-    from omnivggt_official_b200 import _lib, ops
-
-    class Rec:
-        def __init__(self):
-            self.calls, self.reads, self.decoded = [], [], []
-
-        def __getattr__(self, name):
-            def fn(*a):
-                self.calls.append((name, a))
-                return 0
-            return fn
-
-    rec = Rec()
+    from omnivggt_official_b200 import ops
 
     def read(t):                  # counts read zero; the fp64 reads of point_cloud and mesh carry E0 and read as they are
-        rec.reads.append(t.cpu())
         return t.cpu() if t.dtype == torch.float64 else torch.zeros_like(t, device="cpu")
 
     def pose_decode(pose_enc, h, w):
         assert pose_enc.dtype == torch.float32 and tuple(pose_enc.shape) == (S, 9) and (h, w) == (H, W)
         assert (pose_enc == SCENE).all()
         cams = _cameras(DECODED, DECODED_K) + (torch.full((S, 3, 4), DECODED_C2W),)
-        rec.decoded.append(cams)                                # kept alive: their pointers identify them
+        fake.decoded.append(cams)                               # kept alive: their pointers identify them
         return cams
 
-    monkeypatch.setattr(_lib, "lib", lambda: rec)
-    monkeypatch.setattr(_lib, "stream", lambda: 0)
-    monkeypatch.setattr(ops, "_on_device", lambda t: True)
-    monkeypatch.setattr(ops, "host_read", read)
+    fake = install(monkeypatch, read=read, read_in_calls=False)
+    fake.decoded = []
     monkeypatch.setattr(ops, "pose_decode", pose_decode)
-    return rec
+    return fake
 
 
 def _predictions(has_ext, has_intr, has_wpfd):

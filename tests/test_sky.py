@@ -5,7 +5,6 @@ cv2 over every colour, its opening against scipy and its component selection aga
 the errors.
 GPU: libovg's ovg_segment_sky through geometry.segment_sky and OmniVGGT.sky_mask against the oracle bit for bit, large and
 adversarial masks, repeats, and mask_sky on point_cloud / mesh / matches and the mini model."""
-import hashlib
 import os
 
 import numpy as np
@@ -17,6 +16,7 @@ from conftest import GOLDEN
 from oracle import sky_oracle as SO
 from oracle.make_golden_cloud import GLB_CASES
 from oracle.make_golden_sky import ground, make_cases, sky_cloud_inputs
+from ovg_support import dry, scene, sha256  # noqa: F401  (fixture)
 
 GOLD = {k: v.numpy() for k, v in load_file(os.path.join(GOLDEN, "sky.safetensors")).items()}
 CASES = make_cases()
@@ -24,11 +24,7 @@ NAMES = sorted(CASES)
 
 
 def _bits_sha(mask) -> bytes:
-    return hashlib.sha256(np.packbits(np.ascontiguousarray(mask, dtype=bool)).tobytes()).digest()
-
-
-def _sha(a) -> bytes:
-    return hashlib.sha256(np.ascontiguousarray(a).tobytes()).digest()
+    return sha256(np.packbits(np.ascontiguousarray(mask, dtype=bool)), hex=False)
 
 
 def _check_golden(name, mask):
@@ -40,8 +36,8 @@ def _check_glb_golden(i, points, colors):
     if len(points) == 0:
         points, colors = np.array([[1, 0, 0]]), np.array([[255, 255, 255]])
     assert len(points) == int(GOLD[f"glb{i}_count"]), i
-    assert _sha(points) == GOLD[f"glb{i}_points_sha256"].tobytes(), i
-    assert _sha(colors) == GOLD[f"glb{i}_colors_sha256"].tobytes(), i
+    assert sha256(points, hex=False) == GOLD[f"glb{i}_points_sha256"].tobytes(), i
+    assert sha256(colors, hex=False) == GOLD[f"glb{i}_colors_sha256"].tobytes(), i
 
 
 def _source(g, src):
@@ -67,7 +63,7 @@ def test_cases_cover_the_contract():
 
 def test_oracle_views_and_glb_clouds_match_reference_golden():
     g = sky_cloud_inputs()
-    assert _sha(g["images"]) == GOLD["images_sha256"].tobytes()
+    assert sha256(g["images"], hex=False) == GOLD["images_sha256"].tobytes()
     sky = SO.sky_of_views(g["images"])
     assert _bits_sha(sky) == GOLD["views_sky_sha256"].tobytes() and sky.any()
     for i, (src, pct, frame, black, white) in enumerate(GLB_CASES):
@@ -119,58 +115,19 @@ def test_oracle_selection_matches_cv2_components():
             assert np.array_equal(SO.select_components(mask), np.isin(labels, sel)), mask.shape
 
 
-@pytest.fixture()
-def dry(monkeypatch):
-    """The C library replaced by a recorder, on CPU tensors; host reads counted."""
-    from omnivggt_official_b200 import _lib, ops
-
-    class Rec:
-        def __init__(self):
-            self.calls, self.reads = [], 0
-
-        def __getattr__(self, name):
-            def fn(*a):
-                self.calls.append((name, a))
-                return 0
-            return fn
-
-    rec = Rec()
-
-    def read(t):
-        rec.calls.append(("host_read", ()))
-        rec.reads += 1
-        return t.cpu()
-
-    monkeypatch.setattr(_lib, "lib", lambda: rec)
-    monkeypatch.setattr(_lib, "stream", lambda: 0)
-    monkeypatch.setattr(ops, "_on_device", lambda t: True)
-    monkeypatch.setattr(ops, "host_read", read)
-    return rec
-
-
-def _scene(S, H, W, seed=3):
-    g = torch.Generator().manual_seed(seed)
-    return {"images": torch.rand(1, S, 3, H, W, generator=g), "world_points_from_depth": torch.randn(1, S, H, W, 3, generator=g),
-            "depth_conf": 1.0 + torch.rand(1, S, H, W, generator=g), "extrinsic": torch.eye(4)[:3].repeat(1, S, 1, 1)}
-
-
-def _names(dry):
-    return [n for n, _ in dry.calls]
-
-
 def test_dry_run_launches_do_not_depend_on_views(dry, monkeypatch):
     from omnivggt_official_b200 import OmniVGGT, geometry
     monkeypatch.setattr(geometry, "_device_of", lambda *xs: torch.device("cpu"))
     seqs = []
     for S in (1, 24):
         dry.calls.clear()
-        sky = OmniVGGT.sky_mask(_scene(S, 6, 8))
+        sky = OmniVGGT.sky_mask(scene(S, 6, 8))
         assert sky.shape == (S, 6, 8) and sky.dtype == torch.bool
-        assert _names(dry) == ["ovg_sky_workspace_bytes", "ovg_segment_sky"]
+        assert dry.names() == ["ovg_sky_workspace_bytes", "ovg_segment_sky"]
         a = dry.calls[1][1]
         assert a[1:8] == (0, 3 * 6 * 8, 1, 6 * 8, S, 6, 8) and a[8] is None     # fp32 [S,3,H,W] read in place
-        seqs.append(_names(dry))
-    assert seqs[0] == seqs[1] and dry.reads == 0
+        seqs.append(dry.names())
+    assert seqs[0] == seqs[1] and len(dry.reads) == 0
     dry.calls.clear()
     geometry.segment_sky(np.zeros((5, 7, 3), np.uint8))
     assert dry.calls[1][1][1:8] == (1, 5 * 7 * 3, 3, 1, 1, 5, 7)
@@ -201,13 +158,13 @@ def test_dry_run_mask_sky_adds_no_host_read_and_false_adds_no_launch(dry, monkey
     monkeypatch.setattr(ops.Matcher, "counts", lambda self: ([0] * self.P, False))
     syncs = _host_syncs(monkeypatch)
     fn = getattr(OmniVGGT, method)
-    pred = _scene(3, 6, 8)
+    pred = scene(3, 6, 8)
     base = None
     for mask_sky in (False, True, torch.zeros(3, 6, 8, dtype=torch.bool), torch.zeros(1, 3, 6, 8, dtype=torch.bool)):
         dry.calls.clear()
         syncs[0] = 0
         fn(pred, mask_sky=mask_sky)
-        names = _names(dry)
+        names = dry.names()
         if base is None:
             base = (names, syncs[0])
             assert not any("sky" in n for n in names)
@@ -225,7 +182,7 @@ def test_dry_run_mask_sky_adds_no_host_read_and_false_adds_no_launch(dry, monkey
 def test_errors_before_any_device_work(dry, monkeypatch):
     from omnivggt_official_b200 import OmniVGGT, geometry
     monkeypatch.setattr(geometry, "_device_of", lambda *xs: torch.device("cpu"))
-    pred = _scene(3, 6, 8)
+    pred = scene(3, 6, 8)
     for bad in (np.zeros((4, 5)), np.zeros((4, 5, 4)), np.zeros((2, 4, 5, 3)), torch.zeros(3, 4, 5)):
         with pytest.raises(ValueError, match="shape"):
             geometry.segment_sky(bad)

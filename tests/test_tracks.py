@@ -25,6 +25,7 @@ from conftest import GOLDEN
 from oracle import matches_oracle as MO
 from oracle import tracks_oracle as TO
 from oracle.make_golden_matches import surface_views
+from ovg_support import host_zeros, install
 
 INT_KEYS = ("offsets", "view", "xy", "point2d", "view_offsets", "view_track", "view_xy", "colors")
 
@@ -202,30 +203,8 @@ def test_write_colmap_errors(tmp_path):
 
 @pytest.fixture()
 def dry(monkeypatch):
-    """The C library replaced by a recorder, on CPU tensors; host reads counted (they read zeros)."""
-    from omnivggt_official_b200 import _lib, ops
-
-    class Rec:
-        def __init__(self):
-            self.calls, self.reads = [], 0
-
-        def __getattr__(self, name):
-            def fn(*a):
-                self.calls.append((name, a))
-                return 0
-            return fn
-
-    rec = Rec()
-
-    def read(t):
-        rec.reads += 1
-        return torch.zeros_like(t, device="cpu")
-
-    monkeypatch.setattr(_lib, "lib", lambda: rec)
-    monkeypatch.setattr(_lib, "stream", lambda: 0)
-    monkeypatch.setattr(ops, "_on_device", lambda t: True)
-    monkeypatch.setattr(ops, "host_read", read)
-    return rec
+    """The C library replaced by a recorder, on CPU tensors; host reads read zeros and are recorded in ``reads`` only."""
+    return install(monkeypatch, read=host_zeros, read_in_calls=False)
 
 
 def _scene(S, H, W, seed=5):
@@ -242,12 +221,11 @@ def test_dry_run_reads_once(dry, pairs, P):
     from omnivggt_official_b200 import OmniVGGT
     S, H, W = 6, 8, 10
     out = OmniVGGT.tracks(_scene(S, H, W), pairs, min_views=1)
-    assert [n for n, _ in dry.calls] == ["ovg_conf_percentile_mask", "ovg_match_workspace_bytes", "ovg_match_index",
-                                         "ovg_match_query", "ovg_tracks_workspace_bytes", "ovg_tracks_assign",
-                                         "ovg_tracks_gather"]
+    assert dry.names() == ["ovg_conf_percentile_mask", "ovg_match_workspace_bytes", "ovg_match_index", "ovg_match_query",
+                           "ovg_tracks_workspace_bytes", "ovg_tracks_assign", "ovg_tracks_gather"]
     _, a = dry.calls[5]
     assert a[2:6] == (max(P, 1), S, H * W, 1)
-    assert dry.reads == 1
+    assert len(dry.reads) == 1
     assert out["points"].shape == (0, 3) and out["offsets"].shape == (1,) and out["view_offsets"].shape == (S + 1,)
     assert out["extrinsic"].shape == (S, 3, 4) and out["intrinsic"].shape == (S, 3, 3)
 
