@@ -295,6 +295,38 @@ int ovg_tracks_gather(const float* images, const float* extrinsic, const float* 
                       long long* offsets, int* view, long long* xy, int* point2d, long long* view_offsets, int* view_track,
                       long long* view_xy, void* stream);
 
+/* Bundle adjustment of tracks (ovg_tracks_*): reference lines: none, the reference has no bundle adjuster; the problem is
+ * COLMAP's default PINHOLE bundle adjustment.  Residual of observation o (track p, view v): X = R_v P_p + t_v, r_o =
+ * (fx X/Z + cx + 0.5 - ox, fy Y/Z + cy + 0.5 - oy), the operation order of ovg_tracks_gather's error; cost 1/2 sum rho(|r|^2)
+ * with rho(s) = s (OVG_BA_LOSS_TRIVIAL) or c^2 log(1 + s / c^2), c = loss_scale (OVG_BA_LOSS_CAUCHY; finite and > 0 for
+ * either loss), the normal equations weighted by rho'(s) (IRLS).  Parameters: per view R <- Exp(dw) R, t <- t + dt, fx and fy when refine_focal; per point
+ * P <- P + dP.  Gauge: view 0's pose and the coordinate k of view 1's translation with the largest |t1 - R1 R0^T t0|_k are
+ * held.  A track with one observation, or seen at Z <= 0 at the start, is held and left out of the cost.
+ * Levenberg-Marquardt as Ceres' LevenbergMarquardtStrategy: (H + D / mu) delta = -g, D = clamp(diag H, 1e-6, 1e32), mu = 1e4
+ * at the start; a step is accepted when (F(x) - F(x + delta)) / (-g^T delta - delta^T H delta / 2) > 1e-3 and no refined
+ * observation has Z <= 0; then mu /= max(1/3, 1 - (2 rho - 1)^3), nu = 2, else mu /= nu, nu *= 2.  Stops: a relative
+ * decrease <= 1e-6, |g|inf <= 1e-10, |delta| <= 1e-8 (|x| + 1e-8) with x the refined translations, focal lengths and points,
+ * mu < 1e-32, or `iterations` steps.  Linear solve: the points eliminated (Schur complement), S dc = b by PCG from 0 with the
+ * exact per-view diagonal blocks of S as preconditioner (Cholesky), stopped at |r| <= 1e-10 |b| or 500 iterations.
+ * points fp64 [n, 3]; offsets int64 [n + 1] into the observations; view int32 [m] in [0, V); observations fp64 [m, 2] in
+ * COLMAP's pixel frame (pixel centres at x + 0.5); extrinsic fp32 [V, 3, 4] world-to-camera; intrinsic fp32 [V, 3, 3].
+ * 2 <= V <= 256.  Outputs: points_out fp64 [n, 3], extrinsic_out fp64 [V, 3, 4], intrinsic_out fp64 [V, 3, 3] (fx, fy
+ * refined, the rest copied), error_out fp64 [n] (ovg_tracks_gather's error at the refined parameters), cost_out fp64 [2]
+ * (initial, final), stats_out int64 [4] = steps, accepted steps, PCG iterations, status (0 converged, 1 iterations reached,
+ * 2 the trust region collapsed, 3 nothing to refine); trace_out fp64 [iterations] = the cost after each step, NaN after the
+ * last, or NULL.  Launches: 9 + 6 per iteration, the PCG one cooperative launch per step whatever its iteration count; after
+ * a stop the remaining launches return at once.  No host synchronisation.  Every sum has a fixed order and no float atomic
+ * is used: results are bit-identical from run to run, and every output and workspace byte read is written first in the call
+ * (the workspace may hold anything).  One workspace of ovg_ba_workspace_bytes(V, n, m) bytes, 256-byte aligned. */
+#define OVG_BA_LOSS_TRIVIAL 0
+#define OVG_BA_LOSS_CAUCHY 1
+long long ovg_ba_workspace_bytes(int V, long long n_tracks, long long n_obs);
+int ovg_bundle_adjust(const double* points, const long long* offsets, const int* view, const double* observations,
+                      const float* extrinsic, const float* intrinsic, int V, long long n_tracks, long long n_obs, int iterations,
+                      int refine_focal, int loss, double loss_scale, void* workspace, long long workspace_bytes,
+                      double* points_out, double* extrinsic_out, double* intrinsic_out, double* error_out, double* cost_out,
+                      long long* stats_out, double* trace_out, void* stream);
+
 /* Triangle mesh of point maps: viz.py:40-89 (pts3d_to_trimesh per view, cat_meshes across views) for F views at once.
  * Pixels are numbered i = (f H + y) W + x.  The quad at (y, x), y < H-1, x < W-1, gives the TL triangle (tl, tr, bl) and the BR
  * triangle (tr, bl, br); a triangle is kept when its three vertices are.  Reference layout: per view, the kept TL triangles,

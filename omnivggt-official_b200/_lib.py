@@ -134,6 +134,9 @@ EXPORTS = {
     "ovg_tracks_assign": (C.c_int, [_vp, _vp, _i, _i, _ll, _i, _vp, _ll, _vp, _ll, _vp, _vp]),
     "ovg_tracks_gather": (C.c_int, [_vp, _vp, _vp, _i, _ll, _i, _i, _ll, _ll, _vp, _ll, _vp, _ll, _vp, _vp, _vp, _vp, _vp, _vp, _vp,
                                     _vp, _vp, _vp, _vp]),
+    "ovg_ba_workspace_bytes": (_ll, [_i, _ll, _ll]),
+    "ovg_bundle_adjust": (C.c_int, [_vp, _vp, _vp, _vp, _vp, _vp, _i, _ll, _ll, _i, _i, _i, C.c_double, _vp, _ll, _vp, _vp, _vp, _vp,
+                                    _vp, _vp, _vp, _vp]),
     "ovg_mesh_workspace_bytes": (_ll, [_i, _i, _i]),
     "ovg_mesh_count": (C.c_int, [_vp, _vp, _i, _i, _i, _i, _i, _vp, _ll, _vp, _vp]),
     "ovg_mesh_faces": (C.c_int, [_vp, _vp, _i, _i, _i, _i, _vp, _ll, _vp, _vp, _vp]),

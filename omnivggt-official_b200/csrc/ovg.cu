@@ -1,5 +1,6 @@
 // libovg C ABI (include/ovg.h): argument validation, TMA descriptor cache, kernel launches.
 #include <atomic>
+#include <cmath>
 #include <cstdlib>
 #include <mutex>
 #include <string>
@@ -16,6 +17,7 @@
 #include "post.cuh"
 #include "match.cuh"
 #include "tracks.cuh"
+#include "ba.cuh"
 #include "mesh.cuh"
 #include "sky.cuh"
 #include "fps.cuh"
@@ -1112,6 +1114,123 @@ int ovg_tracks_gather(const float* images, const float* extrinsic, const float* 
   ovg::track_point_kernel<<<static_cast<unsigned>((n_tracks + ovg::TRACK_POINT_THREADS - 1) / ovg::TRACK_POINT_THREADS),
                             ovg::TRACK_POINT_THREADS, 0, st>>>(p, o);
   return post_launch("ovg_tracks_gather(points)");
+}
+
+}  // extern "C"
+
+// ------------------------------------------------------------------------------------------------------- bundle adjustment
+namespace {
+
+// Bundle-adjustment workspace, carved the same way by the size query and by the entry point.
+long long ba_workspace(void* base, int V, long long n, long long m, ovg::BaParams* p) {
+  Arena ar(base, 0);
+  p->tblocks = static_cast<int>(std::max(1LL, (n + ovg::BA_THREADS - 1) / ovg::BA_THREADS));
+  p->vtiles = static_cast<int>(std::max(1LL, ovg::compact_tiles(m)));
+  p->st = ar.get<ovg::BaState>(1);
+  p->cam = ar.get<double>(2LL * V * ovg::BA_CAM);
+  p->mask = ar.get<double>(static_cast<long long>(V) * ovg::BA_NP);
+  p->dcam = ar.get<double>(static_cast<long long>(V) * ovg::BA_NP);
+  p->pts = ar.get<double>(6 * n);
+  p->dp = ar.get<double>(3 * n);
+  p->vinv = ar.get<double>(9 * n);
+  p->y = ar.get<double>(3 * n);
+  p->gp = ar.get<double>(3 * n);
+  p->zt = ar.get<double>(3 * n);
+  p->incl = ar.get<unsigned char>(n);
+  p->ob = ar.get<ovg::BaObs>(m);
+  p->obs_track = ar.get<int>(m);
+  p->view_obs = ar.get<int>(m);
+  p->view_off = ar.get<long long>(V + 1);
+  p->gmax = ar.get<double>(p->tblocks);
+  p->vpart = ar.get<double>(static_cast<long long>(V) * ovg::BA_BLOCK_CHUNKS * ovg::BA_ENTRIES);
+  p->vsum = ar.get<double>(static_cast<long long>(V) * ovg::BA_ENTRIES);
+  p->bpart = ar.get<double>(static_cast<long long>(V) * ovg::BA_PCG_CHUNKS * ovg::BA_NP);
+  p->epart = ar.get<double>(static_cast<long long>(p->tblocks) * ovg::BA_EVAL);
+  p->tile_count = ar.get<unsigned int>(static_cast<long long>(V) * p->vtiles);
+  p->tile_offset = ar.get<unsigned long long>(static_cast<long long>(V) * p->vtiles);
+  p->scan_total = ar.get<unsigned long long>(1);
+  return ar.bytes();
+}
+
+bool ba_sizes_ok(int V, long long n, long long m) {
+  return V >= 2 && V <= ovg::BA_MAX_VIEWS && n >= 0 && m >= 0 && n < (1LL << 31) && m < (1LL << 31);
+}
+
+}  // namespace
+
+extern "C" {
+
+long long ovg_ba_workspace_bytes(int V, long long n_tracks, long long n_obs) {
+  ovg::BaParams p{};
+  return ba_sizes_ok(V, n_tracks, n_obs) ? ba_workspace(nullptr, V, n_tracks, n_obs, &p) : -1;
+}
+
+int ovg_bundle_adjust(const double* points, const long long* offsets, const int* view, const double* observations,
+                      const float* extrinsic, const float* intrinsic, int V, long long n_tracks, long long n_obs, int iterations,
+                      int refine_focal, int loss, double loss_scale, void* workspace, long long workspace_bytes,
+                      double* points_out, double* extrinsic_out, double* intrinsic_out, double* error_out, double* cost_out,
+                      long long* stats_out, double* trace_out, void* stream) {
+  OVG_REQUIRE(ba_sizes_ok(V, n_tracks, n_obs), "need 2 <= V <= 256 and 0 <= n_tracks, n_obs < 2^31");
+  OVG_REQUIRE(iterations >= 1, "iterations must be >= 1");
+  OVG_REQUIRE(loss == OVG_BA_LOSS_TRIVIAL || loss == OVG_BA_LOSS_CAUCHY, "unknown loss");
+  OVG_REQUIRE(std::isfinite(loss_scale) && loss_scale > 0.0, "loss_scale must be finite and > 0");
+  OVG_REQUIRE(offsets && extrinsic && intrinsic && extrinsic_out && intrinsic_out && cost_out && stats_out, "null operand");
+  OVG_REQUIRE(n_tracks == 0 || (points && points_out && error_out), "null points / points_out / error_out");
+  OVG_REQUIRE(n_obs == 0 || (view && observations), "null view / observations");
+  ovg::BaParams p{};
+  OVG_REQUIRE(workspace_ok(workspace, workspace_bytes, ba_workspace(nullptr, V, n_tracks, n_obs, &p), 256),
+              "workspace must be 256-byte aligned and ovg_ba_workspace_bytes(V, n_tracks, n_obs) long");
+  ba_workspace(workspace, V, n_tracks, n_obs, &p);
+  p.V = V; p.n = n_tracks; p.m = n_obs; p.iterations = iterations; p.refine_focal = refine_focal ? 1 : 0;
+  p.cauchy = loss == OVG_BA_LOSS_CAUCHY; p.c2 = loss_scale * loss_scale;
+  p.points = points; p.offsets = offsets; p.view = view; p.obs = observations; p.ext = extrinsic; p.intr = intrinsic;
+  p.points_out = points_out; p.ext_out = extrinsic_out; p.intr_out = intrinsic_out; p.error_out = error_out;
+  p.cost_out = cost_out; p.stats_out = stats_out; p.trace = trace_out;
+  // the PCG spins on the other CTAs: launched cooperatively with the grid the occupancy query allows
+  const int smem = ovg::BA_VIEW_SMEM * V * static_cast<int>(sizeof(double));
+  int rc = allow_dynamic_smem<ovg::ba_pcg_kernel>(ovg::BA_VIEW_SMEM * ovg::BA_MAX_VIEWS * static_cast<int>(sizeof(double)));
+  if (rc) return rc;
+  int per_sm = 0;
+  OVG_CUDA(cudaOccupancyMaxActiveBlocksPerMultiprocessor(&per_sm, ovg::ba_pcg_kernel, ovg::BA_PCG_THREADS, smem));
+  OVG_REQUIRE(per_sm > 0, "the PCG kernel does not fit on an SM");
+  const int grid = per_sm * num_sms();
+  cudaStream_t st = reinterpret_cast<cudaStream_t>(stream);
+  const unsigned tb = static_cast<unsigned>(p.tblocks);
+  const dim3 vgrid(p.vtiles, V);
+  ovg::ba_init_kernel<<<1, 1, 0, st>>>(p);
+  if ((rc = post_launch("ovg_bundle_adjust(init)"))) return rc;
+  ovg::ba_track_init_kernel<<<tb, ovg::BA_THREADS, 0, st>>>(p);
+  if ((rc = post_launch("ovg_bundle_adjust(track init)"))) return rc;
+  ovg::ba_view_count_kernel<<<vgrid, ovg::COMPACT_THREADS, 0, st>>>(p);
+  if ((rc = post_launch("ovg_bundle_adjust(view count)"))) return rc;
+  ovg::tile_scan_kernel<<<1, 1024, 0, st>>>(p.tile_count, p.tile_offset, p.scan_total, static_cast<long long>(V) * p.vtiles);
+  if ((rc = post_launch("ovg_bundle_adjust(scan)"))) return rc;
+  ovg::ba_view_gather_kernel<<<vgrid, ovg::COMPACT_THREADS, 0, st>>>(p);
+  if ((rc = post_launch("ovg_bundle_adjust(view gather)"))) return rc;
+  ovg::ba_eval_kernel<<<tb, ovg::BA_THREADS, 0, st>>>(p, 0);
+  if ((rc = post_launch("ovg_bundle_adjust(initial cost)"))) return rc;
+  ovg::ba_control_kernel<<<1, ovg::BA_PCG_THREADS, 0, st>>>(p, 1);
+  if ((rc = post_launch("ovg_bundle_adjust(initial control)"))) return rc;
+  void* args[] = {&p};
+  for (int i = 0; i < iterations; ++i) {                     // after a stop every kernel returns at once
+    ovg::ba_track_kernel<<<tb, ovg::BA_THREADS, 0, st>>>(p);
+    if ((rc = post_launch("ovg_bundle_adjust(tracks)"))) return rc;
+    ovg::ba_view_block_kernel<<<dim3(ovg::BA_BLOCK_CHUNKS, V), ovg::BA_BLOCK_THREADS, 0, st>>>(p);
+    if ((rc = post_launch("ovg_bundle_adjust(view blocks)"))) return rc;
+    ovg::ba_view_reduce_kernel<<<V, ovg::BA_BLOCK_THREADS, 0, st>>>(p);
+    if ((rc = post_launch("ovg_bundle_adjust(view sums)"))) return rc;
+    OVG_CUDA(cudaLaunchCooperativeKernel(reinterpret_cast<void*>(ovg::ba_pcg_kernel), dim3(grid), dim3(ovg::BA_PCG_THREADS),
+                                         args, smem, st));
+    if ((rc = post_launch("ovg_bundle_adjust(pcg)"))) return rc;
+    ovg::ba_eval_kernel<<<tb, ovg::BA_THREADS, 0, st>>>(p, 1);
+    if ((rc = post_launch("ovg_bundle_adjust(trial cost)"))) return rc;
+    ovg::ba_control_kernel<<<1, ovg::BA_PCG_THREADS, 0, st>>>(p, 0);
+    if ((rc = post_launch("ovg_bundle_adjust(control)"))) return rc;
+  }
+  ovg::ba_output_kernel<<<tb, ovg::BA_THREADS, 0, st>>>(p);
+  if ((rc = post_launch("ovg_bundle_adjust(points)"))) return rc;
+  ovg::ba_finish_kernel<<<1, 32, 0, st>>>(p);
+  return post_launch("ovg_bundle_adjust(finish)");
 }
 
 }  // extern "C"

@@ -7,6 +7,7 @@
 //   track_claimed_kernel  tile counts of the claimed nodes of every view
 //   track_view_kernel     per view, the ordered compaction of the claimed nodes: track, pixel and rank of each
 //   track_point_kernel    one thread per track: fp64 mean, colour, reprojection error, and the observations' outputs
+// track_reproject is the per-observation reprojection, shared with the bundle adjuster (ba.cuh).
 // A partner of anchor (a, k) is the reciprocal match jj of k in view j > a of pair (a, j), if (j, jj) is unclaimed.  Each pair's
 // reciprocal matching is one-to-one, so a node of view j can only be the partner of one anchor of view a: inside a step no two
 // threads read or write the same claim, and nothing is decided by an atomic.  Sums run in a fixed order: results are
@@ -182,11 +183,31 @@ __global__ void __launch_bounds__(COMPACT_THREADS) track_view_kernel(const Track
   }
 }
 
+// The reprojection of point c through camera (E world -> camera [R | t] row-major [3, 4], K [3, 3]) against the observation
+// (ox, oy) in COLMAP's pixel frame, every fp64 operation rounded on its own:
+//   (X, Y, Z) = R c + t, each row ((r0 c0 + r1 c1) + r2 c2) + t;  du = (fx (X / Z) + (cx + 0.5)) - ox;  dv likewise.
+// Returns Z <= 0 (the camera sees the point behind it).  T is the cameras' element type: fp32 for tracks, fp64 for the bundle
+// adjuster; an fp32 camera widened to fp64 gives the same bits either way.
+template <typename T>
+__device__ __forceinline__ bool track_reproject(const T* E, const T* K, const double c[3], double ox, double oy, double X[3],
+                                                double& du, double& dv) {
+#pragma unroll
+  for (int r = 0; r < 3; ++r)
+    X[r] = __dadd_rn(__dadd_rn(__dadd_rn(__dmul_rn(static_cast<double>(E[4 * r]), c[0]),
+                                         __dmul_rn(static_cast<double>(E[4 * r + 1]), c[1])),
+                               __dmul_rn(static_cast<double>(E[4 * r + 2]), c[2])),
+                     static_cast<double>(E[4 * r + 3]));
+  const double u = __dadd_rn(__dmul_rn(static_cast<double>(K[0]), __ddiv_rn(X[0], X[2])), __dadd_rn(static_cast<double>(K[2]), 0.5));
+  const double w = __dadd_rn(__dmul_rn(static_cast<double>(K[4]), __ddiv_rn(X[1], X[2])), __dadd_rn(static_cast<double>(K[5]), 0.5));
+  du = __dsub_rn(u, ox);
+  dv = __dsub_rn(w, oy);
+  return X[2] <= 0.0;
+}
+
 // grid ceil(n / TRACK_POINT_THREADS), after track_view_kernel.  Position: the fp64 sum of the observations' points in
-// observation order, divided once by their count.  Error: the mean over the observations of the distance between the
-// projection of that position and the pixel centre (x + 0.5, y + 0.5), every fp64 operation rounded on its own:
-//   (X, Y, Z) = R p + t, each row ((r0 px + r1 py) + r2 pz) + t;  u = fx (X / Z) + (cx + 0.5);  v = fy (Y / Z) + (cy + 0.5);
-//   e = sqrt((u - (x + 0.5))^2 + (v - (y + 0.5))^2), summed in observation order and divided once; +inf when some Z <= 0.
+// observation order, divided once by their count.  Error: the mean over the observations of the distance sqrt(du^2 + dv^2)
+// of track_reproject against the pixel centre (x + 0.5, y + 0.5), summed in observation order and divided once; +inf when
+// some Z <= 0.
 __global__ void __launch_bounds__(TRACK_POINT_THREADS) track_point_kernel(const TrackParams p, const TrackOut o) {
   const long long t = static_cast<long long>(blockIdx.x) * TRACK_POINT_THREADS + threadIdx.x;
   if (t >= o.n) return;
@@ -224,23 +245,10 @@ __global__ void __launch_bounds__(TRACK_POINT_THREADS) track_point_kernel(const 
   for (long long q = b; q < e; ++q) {
     const int node = p.obs[q];
     const int v = static_cast<int>(node / cap);
-    const float* E = o.extrinsic + 12 * v;
-    const float* K = o.intrinsic + 9 * v;
-    double X[3];
-#pragma unroll
-    for (int r = 0; r < 3; ++r)
-      X[r] = __dadd_rn(__dadd_rn(__dadd_rn(__dmul_rn(static_cast<double>(E[4 * r]), c[0]),
-                                           __dmul_rn(static_cast<double>(E[4 * r + 1]), c[1])),
-                                 __dmul_rn(static_cast<double>(E[4 * r + 2]), c[2])),
-                       static_cast<double>(E[4 * r + 3]));
-    behind |= X[2] <= 0.0;
-    const double u = __dadd_rn(__dmul_rn(static_cast<double>(K[0]), __ddiv_rn(X[0], X[2])),
-                               __dadd_rn(static_cast<double>(K[2]), 0.5));
-    const double w = __dadd_rn(__dmul_rn(static_cast<double>(K[4]), __ddiv_rn(X[1], X[2])),
-                               __dadd_rn(static_cast<double>(K[5]), 0.5));
     const long long pix = __float_as_int(p.m.pts[node].w);
-    const double du = __dsub_rn(u, static_cast<double>(pix % o.W) + 0.5);
-    const double dv = __dsub_rn(w, static_cast<double>(pix / o.W) + 0.5);
+    double X[3], du, dv;
+    behind |= track_reproject(o.extrinsic + 12 * v, o.intrinsic + 9 * v, c, static_cast<double>(pix % o.W) + 0.5,
+                              static_cast<double>(pix / o.W) + 0.5, X, du, dv);
     err = __dadd_rn(err, __dsqrt_rn(__dadd_rn(__dmul_rn(du, du), __dmul_rn(dv, dv))));
   }
   o.error[t] = behind ? __longlong_as_double(0x7ff0000000000000LL) : __ddiv_rn(err, cnt);

@@ -309,6 +309,7 @@ class OmniVGGT(nn.Module, PyTorchModelHubMixin):
     mesh = staticmethod(SC.mesh)
     matches = staticmethod(SC.matches)
     tracks = staticmethod(SC.tracks)
+    bundle_adjust = staticmethod(SC.bundle_adjust)
     _kept_views = staticmethod(SC._kept_views)          # their shared helpers, reached from the class as before
     _align = staticmethod(SC._align)
 

@@ -366,6 +366,36 @@ def sim3_apply(sim3: torch.Tensor, views: int, hw: int, points=(), depth=None, e
     L.check(L.lib().ovg_sim3_apply(sim3.data_ptr(), views, hw, *flat, L.stream()))
 
 
+BA_LOSSES = ("trivial", "cauchy")                 # OVG_BA_LOSS_TRIVIAL, OVG_BA_LOSS_CAUCHY
+
+
+def bundle_adjust(points, offsets, view, observations, extrinsic, intrinsic, *, iterations: int, refine_focal: bool,
+                  loss: str, loss_scale: float, trace: bool = False):
+    """ovg_bundle_adjust: points fp64 [n, 3], offsets int64 [n + 1], view int32 [m], observations fp64 [m, 2] (COLMAP pixel
+    frame), extrinsic fp32 [V, 3, 4], intrinsic fp32 [V, 3, 3], contiguous on one device.  Returns (points fp64 [n, 3],
+    extrinsic fp64 [V, 3, 4], intrinsic fp64 [V, 3, 3], error fp64 [n], cost fp64 [2], stats int64 [4] = steps, accepted,
+    PCG iterations, status, and with ``trace`` the cost after each step fp64 [iterations], NaN after the last).  No host read."""
+    n, m, V = points.shape[0], view.shape[0], extrinsic.shape[0]
+    for t, dtype, name, shape in ((points, torch.float64, "points", (n, 3)), (offsets, torch.int64, "offsets", (n + 1,)),
+                                  (view, torch.int32, "view", (m,)), (observations, torch.float64, "observations", (m, 2)),
+                                  (extrinsic, F32, "extrinsic", (V, 3, 4)), (intrinsic, F32, "intrinsic", (V, 3, 3))):
+        _chk(t, dtype, name)
+        assert t.is_contiguous() and tuple(t.shape) == shape, (name, tuple(t.shape), shape)
+    lib = L.lib()
+    dev = points.device
+    ws = torch.empty(lib.ovg_ba_workspace_bytes(V, n, m), device=dev, dtype=torch.uint8)
+    out = (torch.empty(n, 3, device=dev, dtype=torch.float64), torch.empty(V, 3, 4, device=dev, dtype=torch.float64),
+           torch.empty(V, 3, 3, device=dev, dtype=torch.float64), torch.empty(n, device=dev, dtype=torch.float64),
+           torch.empty(2, device=dev, dtype=torch.float64), torch.empty(4, device=dev, dtype=torch.int64))
+    tr = torch.empty(iterations, device=dev, dtype=torch.float64) if trace else None
+    L.check(lib.ovg_bundle_adjust(L.ptr(points) if n else None, offsets.data_ptr(), L.ptr(view) if m else None,
+                                  L.ptr(observations) if m else None, extrinsic.data_ptr(), intrinsic.data_ptr(), V, n, m,
+                                  int(iterations), int(bool(refine_focal)), BA_LOSSES.index(loss), float(loss_scale),
+                                  ws.data_ptr(), ws.numel(), *(t.data_ptr() if t.numel() else None for t in out), L.ptr(tr),
+                                  L.stream()))
+    return out + ((tr,) if trace else ())
+
+
 def host_read(t: torch.Tensor) -> torch.Tensor:
     """The device-to-host read of a matching or mesh call (its one synchronisation)."""
     return t.cpu()

@@ -1,8 +1,11 @@
 """A predictions dict on the device: its cameras and world points (``postprocess``), and the sky, point cloud, mesh,
-matches and tracks of one scene.  They read no weight; ``OmniVGGT`` exposes each under the same name.  Each checks its
-arguments before any library call (``_check_views``), then takes the scene's views from ``_kept_views``."""
+matches and tracks of one scene, and the bundle adjustment of those tracks.  They read no weight; ``OmniVGGT`` exposes each
+under the same name.  Each checks its arguments before any library call (``_check_views``), then takes the scene's views
+from ``_kept_views``."""
 from __future__ import annotations
 
+import math
+import numbers
 from typing import Dict, List, Optional
 
 import numpy as np
@@ -216,6 +219,70 @@ def tracks(predictions: Dict[str, object], pairs=None, *, source: str = "depth",
         raise ValueError("kept points must be finite (cKDTree: data must be finite, check for nan or inf values)")
     out = tr.gather(images, ext, intr, W, n, m)
     out.update(extrinsic=ext, intrinsic=intr)
+    return out
+
+
+_TRACK_KEYS = (("points", torch.float64, ("n", 3)), ("colors", torch.uint8, ("n", 3)), ("error", torch.float64, ("n",)),
+               ("offsets", torch.int64, ("n1",)), ("view", torch.int32, ("m",)), ("xy", torch.int64, ("m", 2)),
+               ("point2d", torch.int32, ("m",)), ("view_offsets", torch.int64, ("V1",)), ("view_track", torch.int32, ("m",)),
+               ("view_xy", torch.int64, ("m", 2)), ("extrinsic", torch.float32, ("V", 3, 4)),
+               ("intrinsic", torch.float32, ("V", 3, 3)))
+
+
+def _check_tracks(tracks) -> None:
+    """ValueError unless ``tracks`` has the keys, dtypes, shapes and one device of what ``tracks`` returns."""
+    if not isinstance(tracks, dict) or any(not torch.is_tensor(tracks.get(k)) for k, _, _ in _TRACK_KEYS):
+        raise ValueError("bundle_adjust needs the dict tracks() returns")
+    n, m, V = tracks["points"].shape[0], tracks["view"].shape[0], tracks["extrinsic"].shape[0]
+    sizes = {"n": n, "n1": n + 1, "m": m, "V": V, "V1": V + 1}
+    dev = tracks["points"].device
+    for k, dtype, shape in _TRACK_KEYS:
+        t = tracks[k]
+        want = tuple(sizes.get(d, d) for d in shape)
+        if t.dtype != dtype or tuple(t.shape) != want or t.device != dev:
+            raise ValueError(f"tracks[{k!r}]: expected {dtype} {want} on device {dev}, got {t.dtype} {tuple(t.shape)} on device "
+                             f"{t.device}")
+
+
+@torch.no_grad()
+def bundle_adjust(tracks: Dict[str, torch.Tensor], *, iterations: int = 100, refine_focal: bool = True,
+                  loss: str = "trivial", loss_scale: float = 1.0) -> Dict[str, object]:
+    """Bundle adjustment of the output of ``tracks`` on the device (libovg ovg_bundle_adjust); no counterpart in the reference.
+
+    COLMAP's default PINHOLE bundle adjustment: the residual of an observation is ``tracks``' error formula, (fx X/Z + cx +
+    0.5 - (x + 0.5), fy Y/Z + cy + 0.5 - (y + 0.5)) with (X, Y, Z) = R P + t, and the cost is 1/2 sum rho(|r|^2), rho(s) = s
+    (``loss="trivial"``) or c^2 log(1 + s/c^2) with c = ``loss_scale`` pixels (``"cauchy"``).  Robust losses weight the
+    normal equations by rho'(s) (IRLS) without Ceres' second-order correction: the minimiser is the same, the path to it may
+    differ.  Refined: every view's rotation and translation, fx and fy when ``refine_focal`` (the principal point stays), and
+    every track point.  The gauge keeps the predictions' frame and scale: view 0's pose and the largest coordinate of view 1's
+    baseline t1 - R1 R0^T t0 are held.  Tracks with one observation or seen behind a camera (``error`` +inf) are held and
+    left out of the cost.  Levenberg-Marquardt with a Schur complement and preconditioned conjugate gradients, at most
+    ``iterations`` steps; the rules are in include/ovg.h and INTEGRATION.md ("Bundle adjustment").
+
+    Returns a new dict with the keys of ``tracks``: ``points`` fp64 [n, 3], ``extrinsic`` fp64 [V, 3, 4] and ``intrinsic``
+    fp64 [V, 3, 3] refined, ``error`` recomputed with them, the other tensors of ``tracks`` as they are, and ``ba``: ``cost``
+    fp64 [2] (initial and final 1/2 sum rho), ``steps``, ``accepted`` and ``pcg_iterations`` int64, ``status`` int32 (0
+    converged, 1 ``iterations`` reached, 2 the trust region collapsed, 3 nothing to refine), all on the device.  No host read."""
+    if not geometry._is_int(iterations) or not 1 <= iterations <= 2 ** 31 - 1:
+        raise ValueError(f"iterations must be an integer in [1, 2^31 - 1], got {iterations!r}")
+    if loss not in ops.BA_LOSSES:
+        raise ValueError(f"loss must be 'trivial' or 'cauchy', got {loss!r}")
+    if not (isinstance(loss_scale, numbers.Real) and not isinstance(loss_scale, bool) and math.isfinite(loss_scale)
+            and loss_scale > 0):
+        raise ValueError(f"loss_scale must be a finite number > 0, got {loss_scale!r}")
+    _check_tracks(tracks)
+    V = tracks["extrinsic"].shape[0]
+    if not 2 <= V <= 256:
+        raise ValueError(f"bundle_adjust needs 2 to 256 views, got {V}")
+    obs = tracks["xy"].to(torch.float64) + 0.5                           # COLMAP's pixel centres
+    points, ext, intr, error, cost, stats = ops.bundle_adjust(
+        tracks["points"].contiguous(), tracks["offsets"].contiguous(), tracks["view"].contiguous(), obs,
+        tracks["extrinsic"].contiguous(), tracks["intrinsic"].contiguous(), iterations=iterations,
+        refine_focal=refine_focal, loss=loss, loss_scale=loss_scale)
+    out = dict(tracks)
+    out.update(points=points, extrinsic=ext, intrinsic=intr, error=error,
+               ba={"cost": cost, "steps": stats[0], "accepted": stats[1], "pcg_iterations": stats[2],
+                   "status": stats[3].to(torch.int32)})
     return out
 
 
