@@ -298,10 +298,9 @@ class Engine:
                 self.table(oc, hp, wp, W / H)
             self.table_xy(pk.feat // 2, hp * self.patch, wp * self.patch, W / H)
 
-    def _workspace(self, name: str, nbytes: int) -> torch.Tensor:
-        if nbytes < 0:
-            raise L.OvgError("libovg: workspace size query failed")
-        return self.ws.get(name, (nbytes,), torch.uint8)
+    def _workspace(self, name: str, query: str, *args) -> torch.Tensor:
+        """The named, reused uint8 buffer of ops.workspace_bytes(query, *args) bytes."""
+        return self.ws.get(name, (ops.workspace_bytes(query, *args),), torch.uint8)
 
     # ------------------------------------------------------------------------------------------ DINOv2 patchifier
     def dino_patchify(self, images: torch.Tensor, pos_embed: torch.Tensor, mean, std) -> torch.Tensor:
@@ -313,7 +312,7 @@ class Engine:
         pe = self.m.aggregator.patch_embed
         # [cls + pos0, registers, pos_patches]: the same for every frame; the patch-embedding GEMM adds on top
         base = torch.cat([pe.cls_token.float() + pos_embed[:, :1], pe.register_tokens.float(), pos_embed[:, 1:]], 1).contiguous()
-        wsb = self._workspace("dino_ws", lib.ovg_dino_workspace_bytes(self.h_dino, K, H, W))
+        wsb = self._workspace("dino_ws", "ovg_dino_workspace_bytes", self.h_dino, K, H, W)
         out = self.ws.get("dino_out", (K, P, self.C), F32)
         m3 = (C.c_float * 3)(*[float(v) for v in mean])
         s3 = (C.c_float * 3)(*[float(v) for v in std])
@@ -338,7 +337,18 @@ class Engine:
         T = hp * wp + R + 1
         if max(hp, wp) + 1 > 64:
             raise ValueError(f"{H}x{W} input: the fused RoPE epilogue holds 64 positions per axis (at most 882 px per side)")
-        assert tuple(keep) == self.keep or set(keep) == set(self.keep), "kept layers are fixed when the engine is built"
+        if tuple(keep) != self.keep and set(keep) != set(self.keep):
+            raise ValueError(f"kept layers {tuple(keep)}: they are fixed to {self.keep} when the engine is built")
+        if cp is not None and B != 1:
+            raise ValueError(f"context parallelism shards the views of one scene, got B = {B}")
+        if layers is not None:
+            if cp is not None:
+                raise ValueError("layer export runs without context parallelism")
+            if len(layers) != self.depth:
+                raise ValueError(f"layers: expected {self.depth} tensors (or None), got {len(layers)}")
+            for i, t in enumerate(layers):
+                if t is not None:
+                    ops.check_operand(t, f"layers[{i}]", F32, numel=K * T * 2 * Cc, contiguous=True)
         cos, sin = self.rope(max(hp, wp) + 1)
         Sd = len(depth_idx)
         idx = idx_loc = d32 = m32 = None
@@ -356,21 +366,17 @@ class Engine:
                 n_loc = len(loc)
                 if n_loc:
                     idx_loc = self.cached(("depth_idx", tuple(loc)), lambda: torch.tensor(loc, dtype=torch.int32))
-        wsb = self._workspace("agg_ws", lib.ovg_aggregator_workspace_bytes(self.h_agg, B, S, H, W, Sd))
+        wsb = self._workspace("agg_ws", "ovg_aggregator_workspace_bytes", self.h_agg, B, S, H, W, Sd)
         slot_t = [self.ws.get(f"slot{i}", (K, T, 2 * Cc)) for i in self.keep] if slots else []
         slot_p = (C.c_void_p * 4)(*[t.data_ptr() for t in slot_t])
         cam_out = self.ws.get("cam_out", (K, 2 * Cc), F32)
         pt, ij = patch_tokens.contiguous(), inj.contiguous()
         if layers is not None:
-            assert cp is None and len(layers) == self.depth
-            for t in layers:
-                assert t is None or (t.dtype == F32 and t.is_contiguous() and t.numel() == K * T * 2 * Cc)
             layer_p = (C.c_void_p * self.depth)(*[L.ptr(t) for t in layers])
             L.check(lib.ovg_aggregator_forward_layers(self.h_agg, pt.data_ptr(), ij.data_ptr(), L.ptr(d32), L.ptr(m32), L.ptr(idx), Sd,
                                                       cos.data_ptr(), sin.data_ptr(), cos.shape[0], B, S, H, W, wsb.data_ptr(),
                                                       wsb.numel(), slot_p, cam_out.data_ptr(), layer_p, L.stream()))
         elif cp is not None:
-            assert B == 1, "context parallelism shards the views of one scene"
             cd = cp.desc(self.heads, views_total * T, views_total)
             L.check(lib.ovg_aggregator_forward_cp(self.h_agg, C.byref(cd), pt.data_ptr(), ij.data_ptr(), L.ptr(d32), L.ptr(m32),
                                                   L.ptr(idx), Sd, L.ptr(idx_loc), n_loc, cos.data_ptr(), sin.data_ptr(),
@@ -387,7 +393,7 @@ class Engine:
         """cam_tokens fp32 [B*S, 2C] -> list of `iters` activated pose encodings fp32 [B, S, 9] (heads/camera_head.py:83-154)."""
         lib = L.lib()
         K = B * S
-        wsb = self._workspace("cam.ws", lib.ovg_camera_workspace_bytes(self.h_cam, K))
+        wsb = self._workspace("cam.ws", "ovg_camera_workspace_bytes", self.h_cam, K)
         out = torch.empty(iters, K, 9, device=self.device, dtype=F32)
         ct = cam_tokens.contiguous()
         L.check(lib.ovg_camera_forward(self.h_cam, ct.data_ptr(), B, S, iters, out.data_ptr(), wsb.data_ptr(), wsb.numel(), L.stream()))
@@ -417,7 +423,7 @@ class Engine:
         tab_p = (C.c_void_p * 4)(*[t.data_ptr() for t in tabs])
         tx, ty = self.table_xy(pk.feat // 2, hp * self.patch, wp * self.patch, W / H)
         fc_max = min(chunk, K)
-        wsb = self._workspace(name + ".ws", lib.ovg_dpt_workspace_bytes(self.h_dpt[name], fc_max, H, W))
+        wsb = self._workspace(name + ".ws", "ovg_dpt_workspace_bytes", self.h_dpt[name], fc_max, H, W)
         for f0 in range(0, K, chunk):
             L.check(forward(self.h_dpt[name], slot_p, T, nspecial, f0, min(chunk, K - f0), H, W, tab_p, tx.data_ptr(), ty.data_ptr(),
                             head_act, preds.data_ptr(), conf.data_ptr(), wsb.data_ptr(), wsb.numel(), L.stream()))

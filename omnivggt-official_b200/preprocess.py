@@ -137,7 +137,8 @@ def _resize_view(lib, st, im, nw: int, nh: int, crop: int, fh: int, out: torch.T
     set to fill.  Returns the staging tensors, which must stay alive until the launches have run."""
     h, w = int(im.shape[0]), int(im.shape[1])
     src = torch.as_tensor(np.array(im, dtype=np.uint8, copy=True) if isinstance(im, np.ndarray) else im, dtype=torch.uint8).to(dev).contiguous()
-    assert src.shape == (h, w, 3), "images are uint8 RGB [h, w, 3]"
+    if src.shape != (h, w, 3):
+        raise ValueError(f"images are uint8 RGB [h, w, 3], got {list(src.shape)}")
     hk = bicubic_taps(w, nw, dev) if w != nw else (None, None, None, 0)
     vk = bicubic_taps(h, nh, dev) if h != nh else (None, None, None, 0)
     tmp = torch.empty(h, nw, 3, device=dev, dtype=torch.uint8) if w != nw else None
