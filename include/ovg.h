@@ -354,6 +354,54 @@ int ovg_mesh_faces(const float* images, const void* colors, int color_bytes, int
 int ovg_mesh_compact(const float* points, const float* images, int F, int H, int W, const void* workspace,
                      long long workspace_bytes, float* positions, unsigned char* colors, int* indices, void* stream);
 
+/* Fused mesh: TSDF fusion of F posed depth maps into one voxel grid and its marching-cubes surface.  Reference lines: none,
+ * the reference has no fusion step (it replaces a host TSDF such as Open3D's ScalableTSDFVolume).  Call order on one stream:
+ * ovg_tsdf_bounds, one host read (the grid is derived from it), ovg_tsdf_integrate, ovg_tsdf_count, one host read (the
+ * output sizes), ovg_tsdf_extract: two host synchronisations per mesh, and a fixed number of kernel launches (56, 2, 3 and 2)
+ * whatever F and the content.  Every fp32 operation is explicitly rounded in the order given (oracle/tsdf_oracle.py restates
+ * it), every sum has a fixed order and no atomic decides a value or a slot: results are bit-identical from run to run.
+ * Bricks are 8 x 8 x 8 voxels, numbered row-major; the grid layout is [nz, ny, nx]; voxel (i, j, k) sits at (ox + i s,
+ * oy + j s, oz + k s) (one multiply and one add per axis).
+ * Workspace: ovg_tsdf_workspace_bytes(nx, ny, nz, F, H, W), 256-byte aligned, where either triple may be all zero.  Both
+ * phases carve it from its start: the bounds use the (F, H, W) part, the volume calls the (nx, ny, nz) part, and the bounds'
+ * scratch is dead once their results are read, so one buffer sized for both serves a whole mesh.  F H W < 2^31 and
+ * 3 nx ny nz < 2^31.
+ * ovg_tsdf_bounds: points fp32 [F H W, 3] and mask uint8 [F H W] (nonzero = kept).  bounds_out fp64 [8] = kept count,
+ *     numpy.percentile(kept coordinate a, 1) for a = x, y, z, the same at 99, and 1.0 if a kept coordinate is not finite
+ *     (else 0.0).  Each percentile is ovg_conf_percentile_mask's exact radix selection over the kept values, with its ranks
+ *     and weight computed on the device from the kept count: lo + (hi - lo) frac in fp32. */
+long long ovg_tsdf_workspace_bytes(int nx, int ny, int nz, int F, int H, int W);
+int ovg_tsdf_bounds(const float* points, const unsigned char* mask, int F, int H, int W, void* workspace,
+                    long long workspace_bytes, double* bounds_out, void* stream);
+/* ovg_tsdf_integrate: depth fp32 [F, H, W], mask uint8 [F, H, W], images fp32 [F, 3, H, W] in [0, 1], extrinsic fp32
+ *     [F, 3, 4] world-to-camera [R | t], intrinsic fp32 [F, 3, 3]; trunc > 0 the truncation.  Marks every brick that the box
+ *     of the two points at depths d -/+ trunc on the ray of a kept pixel with d > 0 touches, grown by one voxel (pixel (x, y)
+ *     -> ((x - cx) / fx, (y - cy) / fy)).  Then per voxel of a marked brick, for f = 0 .. F-1: X = ((R00 x + R01 y) + R02 z)
+ *     + t0 (likewise Y, Z), skipped unless Z > 0; pixel (floor(X / Z fx + cx + 0.5), floor(Y / Z fy + cy + 0.5)), skipped
+ *     outside the image, when not kept or when its depth is not > 0; sdf = d - Z, skipped when < -trunc, else min(1, sdf /
+ *     trunc).  tsdf fp32 [nz, ny, nx] = the mean of those values (their sum in view order over n), NaN (0x7fc00000) when n =
+ *     0 or in an unmarked brick; color uint8 [nz, ny, nx, 4] = ((sum of uint8(trunc(255 x))) + n / 2) / n per channel and
+ *     255, or all zero when unobserved. */
+int ovg_tsdf_integrate(const float* depth, const unsigned char* mask, const float* images, const float* extrinsic,
+                       const float* intrinsic, int F, int H, int W, int nx, int ny, int nz, float ox, float oy, float oz,
+                       float voxel, float trunc, void* workspace, long long workspace_bytes, float* tsdf, unsigned char* color,
+                       void* stream);
+/* ovg_tsdf_count: marching cubes on tsdf fp32 [nz, ny, nx] (NaN = unobserved; any volume, not only ovg_tsdf_integrate's).
+ *     A cube (corners numbered as in csrc/mc_table.h, case bit n set when tsdf(corner n) < 0) emits its table's triangles
+ *     iff its 8 corners are observed.  Voxel (i, j, k) owns its +x, +y and +z edges; an owned edge has a vertex iff both ends
+ *     are observed, their signs differ and one of the up-to-4 cubes around it emits.  Vertices go in brick-major order
+ *     (voxels row-major inside a brick), by axis x, y, z within a voxel; triangles by cube in the same order, then table
+ *     order.  counts_out: device int64 [2] = vertices, triangles: reading it back is the second host synchronisation. */
+int ovg_tsdf_count(const float* tsdf, int nx, int ny, int nz, void* workspace, long long workspace_bytes, long long* counts_out,
+                   void* stream);
+/* ovg_tsdf_extract: after ovg_tsdf_count on the same volume and workspace.  positions fp32 [vertices, 3]: along the edge
+ *     axis c0 + t s with t = f0 / (f0 - f1), the other coordinates the voxel's; colors uint8 [vertices, 3]: color's RGB of
+ *     the endpoint with the smaller |tsdf| (endpoint 0 on ties); indices int32 [triangles, 3], counter-clockwise seen from
+ *     the positive (free-space) side. */
+int ovg_tsdf_extract(const float* tsdf, const unsigned char* color, int nx, int ny, int nz, float ox, float oy, float oz,
+                     float voxel, void* workspace, long long workspace_bytes, float* positions, unsigned char* colors,
+                     int* indices, void* stream);
+
 /* Model-free sky segmentation: viz.py:357-393 (segment_sky) on F views of H x W at once, and the --mask_sky confidence of
  * visual_util.py:184-188.  Per view: u8 = the image (uint8), or uint8(trunc(255 * clamp(x, 0, 1))) in fp32; OpenCV's integer
  * BGR2HSV of u8 with channel 0 read as B; the colour test (H <= 30 && V >= 100) | (S < 10 && V > 150) | (S < 30 && V > 180) |

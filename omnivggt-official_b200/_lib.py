@@ -141,6 +141,11 @@ EXPORTS = {
     "ovg_mesh_count": (C.c_int, [_vp, _vp, _i, _i, _i, _i, _i, _vp, _ll, _vp, _vp]),
     "ovg_mesh_faces": (C.c_int, [_vp, _vp, _i, _i, _i, _i, _vp, _ll, _vp, _vp, _vp]),
     "ovg_mesh_compact": (C.c_int, [_vp, _vp, _i, _i, _i, _vp, _ll, _vp, _vp, _vp, _vp]),
+    "ovg_tsdf_workspace_bytes": (_ll, [_i, _i, _i, _i, _i, _i]),
+    "ovg_tsdf_bounds": (C.c_int, [_vp, _vp, _i, _i, _i, _vp, _ll, _vp, _vp]),
+    "ovg_tsdf_integrate": (C.c_int, [_vp, _vp, _vp, _vp, _vp, _i, _i, _i, _i, _i, _i, _f, _f, _f, _f, _f, _vp, _ll, _vp, _vp, _vp]),
+    "ovg_tsdf_count": (C.c_int, [_vp, _i, _i, _i, _vp, _ll, _vp, _vp]),
+    "ovg_tsdf_extract": (C.c_int, [_vp, _vp, _i, _i, _i, _f, _f, _f, _f, _vp, _ll, _vp, _vp, _vp, _vp]),
     "ovg_sky_workspace_bytes": (_ll, [_i, _i, _i]),
     "ovg_segment_sky": (C.c_int, [_vp, _i, _ll, _ll, _ll, _i, _i, _i, _vp, _vp, _ll, _vp, _vp, _vp]),
     "ovg_sky_mask_conf": (C.c_int, [_vp, _vp, _ll, _vp, _vp]),

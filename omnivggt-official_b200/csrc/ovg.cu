@@ -1,4 +1,5 @@
 // libovg C ABI (include/ovg.h): argument validation, TMA descriptor cache, kernel launches.
+#include <algorithm>
 #include <atomic>
 #include <cmath>
 #include <cstdlib>
@@ -19,6 +20,7 @@
 #include "tracks.cuh"
 #include "ba.cuh"
 #include "mesh.cuh"
+#include "tsdf.cuh"
 #include "sky.cuh"
 #include "fps.cuh"
 #include "rank.cuh"
@@ -668,6 +670,25 @@ int select_blocks(long long n) {
   return blocks < 1 ? 1 : static_cast<int>(blocks);
 }
 
+// The 4 x (histogram, decide) passes of a radix selection whose ranks an init launch has set in the workspace's state.
+int radix_select_passes(const float* v, long long n, void* workspace, float* out3, float frac, const std::string& what,
+                        cudaStream_t st) {
+  unsigned long long* state = reinterpret_cast<unsigned long long*>(workspace);
+  unsigned int* hist = reinterpret_cast<unsigned int*>(state + 6);
+  int rc = OVG_OK;
+  const int blocks = select_blocks(n);
+  for (int pass = 0; pass < 4; ++pass) {
+    ovg::SelectParams sp{v, n, state, hist, pass, out3, frac};
+    ovg::select_hist_kernel<<<blocks, 256, 0, st>>>(sp);
+    rc = post_launch((what + "(hist)").c_str());
+    if (rc) return rc;
+    ovg::select_decide_kernel<<<1, 32, 0, st>>>(sp);
+    rc = post_launch((what + "(decide)").c_str());
+    if (rc) return rc;
+  }
+  return OVG_OK;
+}
+
 // numpy.percentile(v[0, n), percent) (method "linear", exact) by radix select: one init launch, then 4 x (histogram, decide).
 // workspace: OVG_PERCENTILE_WORKSPACE_BYTES (6 x u64 state | 512 x u32 histograms | ...); out3: device float[3] = the two
 // neighbouring order statistics and the interpolated percentile.  count (optional) is zeroed by the init launch.
@@ -681,19 +702,8 @@ int radix_percentile(const float* v, long long n, float percent, void* workspace
   unsigned long long* state = reinterpret_cast<unsigned long long*>(workspace);
   unsigned int* hist = reinterpret_cast<unsigned int*>(state + 6);
   ovg::select_init_kernel<<<1, 128, 0, st>>>(state, hist, r0, r1, count);
-  int rc = post_launch((what + "(init)").c_str());
-  if (rc) return rc;
-  const int blocks = select_blocks(n);
-  for (int pass = 0; pass < 4; ++pass) {
-    ovg::SelectParams sp{v, n, state, hist, pass, out3, static_cast<float>(frac)};
-    ovg::select_hist_kernel<<<blocks, 256, 0, st>>>(sp);
-    rc = post_launch((what + "(hist)").c_str());
-    if (rc) return rc;
-    ovg::select_decide_kernel<<<1, 32, 0, st>>>(sp);
-    rc = post_launch((what + "(decide)").c_str());
-    if (rc) return rc;
-  }
-  return OVG_OK;
+  const int rc = post_launch((what + "(init)").c_str());
+  return rc ? rc : radix_select_passes(v, n, workspace, out3, static_cast<float>(frac), what, st);
 }
 
 struct Arena {
@@ -1325,6 +1335,167 @@ int ovg_mesh_compact(const float* points, const float* images, int F, int H, int
   if ((rc = post_launch("ovg_mesh_compact(vertices)"))) return rc;
   ovg::mesh_indices_kernel<<<dim3(p.tpv, F), ovg::COMPACT_THREADS, 0, st>>>(p);
   return post_launch("ovg_mesh_compact(indices)");
+}
+
+}  // extern "C"
+
+// -------------------------------------------------------------------------------------------------------------- fused mesh
+namespace {
+
+// TSDF workspace: the bounds part (F, H, W) and the volume part (nx, ny, nz) are both carved from the start, carved the
+// same way by the size query and by every entry point.
+struct TsdfWorkspace {
+  void* select;                      // OVG_PERCENTILE_WORKSPACE_BYTES
+  float* sel;                        // [6][3] selection results, in the order (axis, percentile)
+  float* frac;                       // [6] their interpolation weights
+  unsigned long long* count;
+  unsigned int* nonfinite;
+  float* cols;                       // [3, ld]
+  long long ld;
+  unsigned char* marked;             // [bricks]
+  unsigned int* tile_count;          // [2 bricks]
+  unsigned long long* tile_offset;   // [2 bricks + 1]
+  int* edge_vertex;                  // [nz, ny, nx, 3]
+  long long bricks, bytes;
+};
+
+TsdfWorkspace tsdf_workspace(void* base, int nx, int ny, int nz, int F, int H, int W) {
+  TsdfWorkspace w{};
+  Arena b(base, 0);
+  const long long n = static_cast<long long>(F) * H * W;
+  w.ld = (n + 3) / 4 * 4;
+  w.select = b.take(OVG_PERCENTILE_WORKSPACE_BYTES);
+  w.sel = b.get<float>(18);
+  w.frac = b.get<float>(6);
+  w.count = b.get<unsigned long long>(1);
+  w.nonfinite = b.get<unsigned int>(1);
+  w.cols = b.get<float>(3 * w.ld);
+  Arena v(base, 0);
+  w.bricks = static_cast<long long>((nx + 7) / 8) * ((ny + 7) / 8) * ((nz + 7) / 8);
+  w.marked = v.get<unsigned char>(w.bricks);
+  w.tile_count = v.get<unsigned int>(2 * w.bricks);
+  w.tile_offset = v.get<unsigned long long>(2 * w.bricks + 1);
+  w.edge_vertex = v.get<int>(3LL * nx * ny * nz);
+  w.bytes = std::max(n ? b.bytes() : 0LL, w.bricks ? v.bytes() : 0LL);
+  return w;
+}
+
+bool tsdf_triple(int a, int b, int c) { return (a > 0 && b > 0 && c > 0) || (a == 0 && b == 0 && c == 0); }
+
+int tsdf_grid(int nx, int ny, int nz, float ox, float oy, float oz, float voxel, float trunc, const void* workspace,
+              long long workspace_bytes, TsdfWorkspace* w, ovg::TsdfGrid* g) {
+  OVG_REQUIRE(nx > 0 && ny > 0 && nz > 0 && 3LL * nx * ny * nz < (1LL << 31), "need 0 < nx, ny, nz and 3 nx ny nz < 2^31");
+  OVG_REQUIRE(std::isfinite(ox) && std::isfinite(oy) && std::isfinite(oz) && std::isfinite(voxel) && voxel > 0.f &&
+                  std::isfinite(trunc) && trunc > 0.f,
+              "origin, voxel and trunc must be finite, voxel and trunc > 0");
+  *w = tsdf_workspace(const_cast<void*>(workspace), nx, ny, nz, 0, 0, 0);
+  OVG_REQUIRE(workspace_ok(workspace, workspace_bytes, w->bytes, 256),
+              "workspace must be 256-byte aligned and ovg_tsdf_workspace_bytes(nx, ny, nz, ...) long");
+  *g = ovg::TsdfGrid{nx, ny, nz, (nx + 7) / 8, (ny + 7) / 8, (nz + 7) / 8, ox, oy, oz, voxel, trunc};
+  return OVG_OK;
+}
+
+int tsdf_mesh(const float* tsdf, int nx, int ny, int nz, float ox, float oy, float oz, float voxel, const void* workspace,
+              long long workspace_bytes, ovg::TsdfMeshParams* p) {
+  OVG_REQUIRE(tsdf, "null tsdf");
+  TsdfWorkspace w;
+  *p = ovg::TsdfMeshParams{};
+  const int rc = tsdf_grid(nx, ny, nz, ox, oy, oz, voxel, 1.f, workspace, workspace_bytes, &w, &p->g);
+  if (rc) return rc;
+  p->tsdf = tsdf; p->bricks = w.bricks;
+  p->tile_count = w.tile_count; p->tile_offset = w.tile_offset; p->edge_vertex = w.edge_vertex;
+  return OVG_OK;
+}
+
+}  // namespace
+
+extern "C" {
+
+long long ovg_tsdf_workspace_bytes(int nx, int ny, int nz, int F, int H, int W) {
+  if (!tsdf_triple(nx, ny, nz) || !tsdf_triple(F, H, W) || (nx == 0 && F == 0)) return -1;
+  if (3LL * nx * ny * nz >= (1LL << 31) || static_cast<long long>(F) * H * W >= (1LL << 31)) return -1;
+  return tsdf_workspace(nullptr, nx, ny, nz, F, H, W).bytes;
+}
+
+int ovg_tsdf_bounds(const float* points, const unsigned char* mask, int F, int H, int W, void* workspace,
+                    long long workspace_bytes, double* bounds_out, void* stream) {
+  OVG_REQUIRE(points && mask && bounds_out, "null operand");
+  OVG_REQUIRE(F > 0 && H > 0 && W > 0 && static_cast<long long>(F) * H * W < (1LL << 31), "need F H W < 2^31");
+  const TsdfWorkspace w = tsdf_workspace(workspace, 0, 0, 0, F, H, W);
+  OVG_REQUIRE(workspace_ok(workspace, workspace_bytes, w.bytes, 256),
+              "workspace must be 256-byte aligned and ovg_tsdf_workspace_bytes(..., F, H, W) long");
+  cudaStream_t st = reinterpret_cast<cudaStream_t>(stream);
+  const long long n = static_cast<long long>(F) * H * W;
+  OVG_CUDA(cudaMemsetAsync(w.count, 0, sizeof(unsigned long long), st));
+  OVG_CUDA(cudaMemsetAsync(w.nonfinite, 0, sizeof(unsigned int), st));
+  const ovg::TsdfBoundsParams bp{points, mask, n, w.ld, w.cols, w.count, w.nonfinite};
+  ovg::tsdf_fill_kernel<<<select_blocks(n), 256, 0, st>>>(bp);
+  int rc = post_launch("ovg_tsdf_bounds(fill)");
+  if (rc) return rc;
+  unsigned long long* state = reinterpret_cast<unsigned long long*>(w.select);
+  for (int j = 0; j < 6; ++j) {          // j = 2 axis + (0: 1st percentile, 1: 99th)
+    ovg::tsdf_select_init_kernel<<<1, 128, 0, st>>>(state, reinterpret_cast<unsigned int*>(state + 6), w.count,
+                                                    (j & 1) ? 99.f : 1.f, w.frac + j);
+    if ((rc = post_launch("ovg_tsdf_bounds(init)"))) return rc;
+    // the decide step's own interpolation (frac 0) is unused: tsdf_bounds_kernel weighs the pair with the device's frac
+    if ((rc = radix_select_passes(w.cols + (j >> 1) * w.ld, n, w.select, w.sel + 3 * j, 0.f, "ovg_tsdf_bounds", st))) return rc;
+  }
+  ovg::tsdf_bounds_kernel<<<1, 32, 0, st>>>(w.sel, w.frac, w.count, w.nonfinite, bounds_out);
+  return post_launch("ovg_tsdf_bounds");
+}
+
+int ovg_tsdf_integrate(const float* depth, const unsigned char* mask, const float* images, const float* extrinsic,
+                       const float* intrinsic, int F, int H, int W, int nx, int ny, int nz, float ox, float oy, float oz,
+                       float voxel, float trunc, void* workspace, long long workspace_bytes, float* tsdf, unsigned char* color,
+                       void* stream) {
+  OVG_REQUIRE(depth && mask && images && extrinsic && intrinsic && tsdf && color, "null operand");
+  OVG_REQUIRE(F > 0 && H > 0 && W > 0 && static_cast<long long>(F) * H * W < (1LL << 31), "need F H W < 2^31");
+  TsdfWorkspace w;
+  ovg::TsdfIntegrateParams p{};
+  int rc = tsdf_grid(nx, ny, nz, ox, oy, oz, voxel, trunc, workspace, workspace_bytes, &w, &p.g);
+  if (rc) return rc;
+  OVG_REQUIRE((reinterpret_cast<uintptr_t>(color) & 3) == 0, "color must be 4-byte aligned");
+  p.depth = depth; p.mask = mask; p.images = images; p.ext = extrinsic; p.intr = intrinsic;
+  p.F = F; p.H = H; p.W = W;
+  p.marked = w.marked; p.tsdf = tsdf; p.color = color;
+  cudaStream_t st = reinterpret_cast<cudaStream_t>(stream);
+  OVG_CUDA(cudaMemsetAsync(w.marked, 0, w.bricks, st));
+  const long long n = static_cast<long long>(F) * H * W;
+  ovg::tsdf_mark_kernel<<<static_cast<unsigned>((n + 255) / 256), 256, 0, st>>>(p);
+  if ((rc = post_launch("ovg_tsdf_integrate(mark)"))) return rc;
+  ovg::tsdf_integrate_kernel<<<static_cast<unsigned>(w.bricks), ovg::TSDF_BRICK_VOXELS, 0, st>>>(p);
+  return post_launch("ovg_tsdf_integrate");
+}
+
+int ovg_tsdf_count(const float* tsdf, int nx, int ny, int nz, void* workspace, long long workspace_bytes, long long* counts_out,
+                   void* stream) {
+  ovg::TsdfMeshParams p;
+  int rc = tsdf_mesh(tsdf, nx, ny, nz, 0.f, 0.f, 0.f, 1.f, workspace, workspace_bytes, &p);
+  if (rc) return rc;
+  OVG_REQUIRE(counts_out, "null counts_out");
+  p.totals = counts_out;
+  cudaStream_t st = reinterpret_cast<cudaStream_t>(stream);
+  ovg::tsdf_count_kernel<<<static_cast<unsigned>(p.bricks), ovg::COMPACT_THREADS, 0, st>>>(p);
+  if ((rc = post_launch("ovg_tsdf_count"))) return rc;
+  ovg::tile_scan_kernel<<<1, 1024, 0, st>>>(p.tile_count, p.tile_offset, p.tile_offset + 2 * p.bricks, 2 * p.bricks);
+  if ((rc = post_launch("ovg_tsdf_count(scan)"))) return rc;
+  ovg::tsdf_totals_kernel<<<1, 32, 0, st>>>(p);
+  return post_launch("ovg_tsdf_count(totals)");
+}
+
+int ovg_tsdf_extract(const float* tsdf, const unsigned char* color, int nx, int ny, int nz, float ox, float oy, float oz,
+                     float voxel, void* workspace, long long workspace_bytes, float* positions, unsigned char* colors,
+                     int* indices, void* stream) {
+  ovg::TsdfMeshParams p;
+  int rc = tsdf_mesh(tsdf, nx, ny, nz, ox, oy, oz, voxel, workspace, workspace_bytes, &p);
+  if (rc) return rc;
+  OVG_REQUIRE(color && positions && colors && indices, "null operand");
+  p.color = color; p.positions = positions; p.colors = colors; p.indices = indices;
+  cudaStream_t st = reinterpret_cast<cudaStream_t>(stream);
+  ovg::tsdf_vertices_kernel<<<static_cast<unsigned>(p.bricks), ovg::COMPACT_THREADS, 0, st>>>(p);
+  if ((rc = post_launch("ovg_tsdf_extract(vertices)"))) return rc;
+  ovg::tsdf_triangles_kernel<<<static_cast<unsigned>(p.bricks), ovg::COMPACT_THREADS, 0, st>>>(p);
+  return post_launch("ovg_tsdf_extract(triangles)");
 }
 
 }  // extern "C"

@@ -310,6 +310,7 @@ class OmniVGGT(nn.Module, PyTorchModelHubMixin):
     matches = staticmethod(SC.matches)
     tracks = staticmethod(SC.tracks)
     bundle_adjust = staticmethod(SC.bundle_adjust)
+    fused_mesh = staticmethod(SC.fused_mesh)
     _kept_views = staticmethod(SC._kept_views)          # their shared helpers, reached from the class as before
     _align = staticmethod(SC._align)
 

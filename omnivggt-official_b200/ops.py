@@ -456,6 +456,77 @@ class Mesher:
         return pos[:n_used], cols[:n_used], idx[:n_fwd]
 
 
+def tsdf_bounds(points, mask):
+    """ovg_tsdf_bounds: points fp32 [F, H, W, 3] and mask uint8 [F, H, W], contiguous on the device.  Returns fp64 [8] on the
+    device = kept count, the 1st percentiles of the kept x, y, z, their 99th percentiles, and 1.0 if a kept point is not finite."""
+    check_operand(points, "points", F32, shape=(None, None, None, 3), contiguous=True)
+    F, H, W = points.shape[:3]
+    check_operand(mask, "mask", torch.uint8, shape=(F, H, W), contiguous=True)
+    ws = workspace(points.device, "ovg_tsdf_workspace_bytes", 0, 0, 0, F, H, W)
+    out = torch.empty(8, device=points.device, dtype=torch.float64)
+    L.check(L.lib().ovg_tsdf_bounds(points.data_ptr(), mask.data_ptr(), F, H, W, ws.data_ptr(), ws.numel(), out.data_ptr(),
+                                    L.stream()))
+    return out
+
+
+def tsdf_workspace(device, shape):
+    """The volume workspace of ovg_tsdf_integrate / count / extract for a grid of ``shape`` = (nz, ny, nx)."""
+    nz, ny, nx = shape
+    return workspace(device, "ovg_tsdf_workspace_bytes", nx, ny, nz, 0, 0, 0)
+
+
+def tsdf_integrate(depth, mask, images, extrinsic, intrinsic, shape, origin, voxel: float, trunc: float, ws):
+    """ovg_tsdf_integrate: depth fp32 [F, H, W], mask uint8 [F, H, W], images fp32 [F, 3, H, W], extrinsic fp32 [F, 3, 4],
+    intrinsic fp32 [F, 3, 3], contiguous on the device; the grid ``shape`` (nz, ny, nx), ``origin`` (3 floats), ``voxel`` and
+    ``trunc``; ``ws`` from tsdf_workspace.  Returns (tsdf fp32 [nz, ny, nx], NaN = unobserved; color uint8 [nz, ny, nx, 4])."""
+    check_operand(depth, "depth", F32, shape=(None, None, None), contiguous=True)
+    F, H, W = depth.shape
+    check_operand(mask, "mask", torch.uint8, shape=(F, H, W), contiguous=True)
+    check_operand(images, "images", F32, shape=(F, 3, H, W), contiguous=True)
+    check_operand(extrinsic, "extrinsic", F32, shape=(F, 3, 4), contiguous=True)
+    check_operand(intrinsic, "intrinsic", F32, shape=(F, 3, 3), contiguous=True)
+    check_operand(ws, "ws", torch.uint8, shape=(None,))
+    nz, ny, nx = shape
+    tsdf = torch.empty(nz, ny, nx, device=depth.device, dtype=F32)
+    color = torch.empty(nz, ny, nx, 4, device=depth.device, dtype=torch.uint8)
+    L.check(L.lib().ovg_tsdf_integrate(depth.data_ptr(), mask.data_ptr(), images.data_ptr(), extrinsic.data_ptr(),
+                                       intrinsic.data_ptr(), F, H, W, nx, ny, nz, *(float(o) for o in origin), float(voxel),
+                                       float(trunc), ws.data_ptr(), ws.numel(), tsdf.data_ptr(), color.data_ptr(), L.stream()))
+    return tsdf, color
+
+
+class TsdfMesher:
+    """Marching cubes (ovg_tsdf_count / ovg_tsdf_extract) of a volume tsdf fp32 [nz, ny, nx] (NaN = unobserved) on the device,
+    voxel (i, j, k) at origin + (i, j, k) voxel.  Counts on construction; ``totals`` int64 [2] (vertices, triangles) is read
+    by the caller, once."""
+
+    def __init__(self, tsdf: torch.Tensor, origin, voxel: float, ws: Optional[torch.Tensor] = None):
+        check_operand(tsdf, "tsdf", F32, shape=(None, None, None), contiguous=True)
+        self.tsdf, self.origin, self.voxel = tsdf, tuple(float(o) for o in origin), float(voxel)
+        self.shape = tuple(tsdf.shape)
+        if ws is None:
+            ws = tsdf_workspace(tsdf.device, self.shape)
+        check_operand(ws, "ws", torch.uint8, shape=(None,))
+        self.ws = ws
+        nz, ny, nx = self.shape
+        self.totals = torch.empty(2, device=tsdf.device, dtype=torch.int64)
+        L.check(L.lib().ovg_tsdf_count(tsdf.data_ptr(), nx, ny, nz, ws.data_ptr(), ws.numel(), self.totals.data_ptr(),
+                                       L.stream()))
+
+    def extract(self, color: torch.Tensor, m: int, k: int):
+        """(positions fp32 [m, 3], colors uint8 [m, 3], indices int32 [k, 3]) for the totals m, k; color uint8 [nz, ny, nx, 4]."""
+        check_operand(color, "color", torch.uint8, shape=self.shape + (4,), contiguous=True)
+        dev = self.tsdf.device
+        pos = torch.empty(max(m, 1), 3, device=dev, dtype=F32)             # >= 1 row: the library wants real pointers
+        cols = torch.empty(max(m, 1), 3, device=dev, dtype=torch.uint8)
+        idx = torch.empty(max(k, 1), 3, device=dev, dtype=torch.int32)
+        nz, ny, nx = self.shape
+        L.check(L.lib().ovg_tsdf_extract(self.tsdf.data_ptr(), color.data_ptr(), nx, ny, nz, *self.origin, self.voxel,
+                                         self.ws.data_ptr(), self.ws.numel(), pos.data_ptr(), cols.data_ptr(), idx.data_ptr(),
+                                         L.stream()))
+        return pos[:m], cols[:m], idx[:k]
+
+
 class Matcher:
     """Reciprocal nearest-neighbour matches (ovg_match_*) between the kept points of V views: points fp32 [V, cap, 3] and keep
     uint8 [V, cap] (or None: all rows), pairs int32 [P, 2] on the device.  Builds every view's index once (ovg_match_index), then

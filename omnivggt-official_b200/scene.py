@@ -1,5 +1,5 @@
 """A predictions dict on the device: its cameras and world points (``postprocess``), and the sky, point cloud, mesh,
-matches and tracks of one scene, and the bundle adjustment of those tracks.  They read no weight; ``OmniVGGT`` exposes each
+fused mesh, matches and tracks of one scene, and the bundle adjustment of those tracks.  They read no weight; ``OmniVGGT`` exposes each
 under the same name.  Each checks its arguments before any library call (``_check_views``), then takes the scene's views
 from ``_kept_views``."""
 from __future__ import annotations
@@ -386,3 +386,78 @@ def mesh(predictions: Dict[str, object], *, source: str = "depth", conf_percent:
     faces, face_colors = mesher.faces(n_ref)
     return {"vertices": points.view(-1, 3).clone(), "face_colors": face_colors, "faces": faces, "conf_threshold": thr,
             "align": align}
+
+
+def _fusion_grid(lo: np.ndarray, hi: np.ndarray, resolution: int):
+    """(origin fp32 [3], voxel fp32, trunc fp32, (nz, ny, nx)) from the kept points' 1st / 99th percentiles, in fp64 on the
+    host; None for a zero extent."""
+    L = float((hi - lo).max())
+    if not L > 0:
+        return None
+    margin = 0.05 * L
+    s = np.float32((L + 2 * margin) / resolution)
+    origin = (lo - margin).astype(np.float32)
+    n = [min(math.ceil((hi[a] - lo[a] + 2 * margin) / float(s)) + 1, resolution + 1) for a in range(3)]
+    return origin, s, np.float32(4.0 * float(s)), (n[2], n[1], n[0])
+
+
+def _fusion(predictions, resolution, conf_percent, conf_floor, scene, mask_sky):
+    """fused_mesh, and the volume it extracted from: (result, tsdf, color), both volumes None when the result is empty."""
+    _check_views(predictions, "depth", conf_percent, conf_floor, None, scene, mask_sky)
+    if not geometry._is_int(resolution) or not 16 <= resolution <= 512:
+        raise ValueError(f"resolution must be an integer in [16, 512], got {resolution!r}")
+    if "depth" not in predictions:
+        raise ValueError("fused_mesh needs the predictions' depth")
+    if not ("extrinsic" in predictions and "intrinsic" in predictions or "pose_enc" in predictions):
+        raise ValueError("fused_mesh needs extrinsic and intrinsic, or pose_enc to decode them from")
+    S = _of_scene(predictions["images"], 3, scene).shape[0]
+    H, W = predictions["images"].shape[-2:]
+    if S * H * W >= 2 ** 31:
+        raise ValueError(f"fused_mesh needs views * H * W < 2^31, got {S} x {H} x {W}")
+    images, (ext, intr), points, mask, thr, _ = _kept_views(predictions, "depth", conf_percent, conf_floor, None, scene,
+                                                           mask_sky, cameras="predictions")
+    dev = images.device
+    host = ops.host_read(torch.cat([ops.tsdf_bounds(points, mask), ext[0].double().reshape(-1)]))
+    if host[7]:
+        raise ValueError("kept points must be finite (cKDTree: data must be finite, check for nan or inf values)")
+    align = _align(host[8:].view(3, 4)).to(dev)
+    lo, hi = host[1:4].numpy(), host[4:7].numpy()
+    grid = _fusion_grid(lo, hi, resolution) if host[0] > 0 else None
+    out = {"positions": torch.empty(0, 3, device=dev), "colors": torch.empty(0, 3, device=dev, dtype=torch.uint8),
+           "indices": torch.empty(0, 3, device=dev, dtype=torch.int32), "conf_threshold": thr, "align": align,
+           "origin": torch.zeros(3, device=dev), "voxel_size": torch.zeros((), device=dev)}
+    if grid is None:
+        return out, None, None
+    origin, s, trunc, shape = grid
+    ws = ops.tsdf_workspace(dev, shape)
+    depth = _of_scene(predictions["depth"], 3, scene).float().reshape(S, H, W).contiguous()
+    tsdf, color = ops.tsdf_integrate(depth, mask, images, ext, intr, shape, origin, s, trunc, ws)
+    mc = ops.TsdfMesher(tsdf, origin, s, ws)
+    m, k = (int(v) for v in ops.host_read(mc.totals).tolist())
+    out.update(origin=torch.from_numpy(origin).to(dev), voxel_size=torch.tensor(s, device=dev))
+    if k:
+        out["positions"], out["colors"], out["indices"] = mc.extract(color, m, k)
+    return out, tsdf, color
+
+
+@torch.no_grad()
+def fused_mesh(predictions: Dict[str, object], *, resolution: int = 512, conf_percent: float = 50.0,
+               conf_floor: float = 1e-5, scene: int = 0, mask_sky=False) -> Dict[str, torch.Tensor]:
+    """One coloured surface of a scene: its depth maps fused into a truncated signed distance (TSDF) volume and the volume's
+    zero level set extracted by marching cubes, on the device (libovg ovg_tsdf_*); no counterpart in the reference.  Where
+    ``mesh`` gives every view its own sheet of triangles, each surface seen by several views appears once here.
+
+    Kept pixels are ``point_cloud``'s with ``source="depth"`` (``conf_percent``, ``conf_floor``, ``mask_sky``); the cameras are
+    the predictions' ``extrinsic`` / ``intrinsic``, decoded from ``pose_enc`` where missing, as ``tracks`` takes them.
+    Grid: per axis lo / hi = numpy.percentile(kept points, 1 / 99), L = max(hi - lo), margin = 0.05 L, voxel s = (L + 2 margin)
+    / ``resolution`` (an integer in [16, 512]), at most resolution + 1 voxels per axis, truncation 4 s.  Only the 8^3-voxel
+    bricks that some kept pixel's band d -/+ 4 s touches are integrated; a voxel's value is the mean over the views that see
+    it in front of the truncation band of min(1, (d - z) / 4 s), its colour the mean colour of those pixels.  Triangles face
+    the free space (the cameras).  The rules are in include/ovg.h and INTEGRATION.md ("Fused mesh").
+
+    Returns on the device ``positions`` fp32 [m, 3], ``colors`` uint8 [m, 3] and ``indices`` int32 [k, 3] for
+    ``glb.write_mesh_glb``, ``conf_threshold`` and ``align`` as ``point_cloud`` returns them, and the grid: ``origin`` fp32 [3]
+    (voxel (0, 0, 0)) and ``voxel_size`` (0-d fp32).  No kept pixel or a zero extent gives an empty mesh (origin 0, voxel
+    size 0).  Two host reads: the bounds with the first camera, then the mesh's sizes.  Kept points that are not finite raise
+    ValueError."""
+    return _fusion(predictions, resolution, conf_percent, conf_floor, scene, mask_sky)[0]
