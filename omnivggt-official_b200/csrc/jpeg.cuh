@@ -34,6 +34,7 @@
 #include <new>
 #include <thread>
 #include <vector>
+#include "arena.cuh"
 
 namespace ovg {
 namespace jpg {
@@ -938,17 +939,11 @@ struct Workspace {
   uint8_t* planes;
   uint8_t** out;
   int* changed;
-  long long bytes;
 };
 
-inline Workspace plan_workspace(const Plan* P, int nout, void* base) {
+inline Workspace plan_layout(Arena& ar, const Plan* P, int nout) {
   Workspace w;
-  long long o = 0;
-  auto take = [&](long long bytes) {
-    const long long at = o;
-    o = align_up(o + std::max<long long>(bytes, 1), 256);
-    return static_cast<uint8_t*>(base) + at;
-  };
+  auto take = [&](long long bytes) { return static_cast<uint8_t*>(ar.take(std::max<long long>(bytes, 1))); };
   const long long nsub_chunks = (P->nsub + SCAN_CHUNK - 1) / SCAN_CHUNK;
   const long long nblk_chunks = (P->nblocks + SCAN_CHUNK - 1) / SCAN_CHUNK;
   w.exits = reinterpret_cast<uint32_t*>(take(4 * P->nsub));
@@ -962,7 +957,6 @@ inline Workspace plan_workspace(const Plan* P, int nout, void* base) {
   w.planes = take(P->plane_bytes);
   w.out = reinterpret_cast<uint8_t**>(take(8LL * nout));
   w.changed = reinterpret_cast<int*>(take(4));
-  w.bytes = o;
   return w;
 }
 

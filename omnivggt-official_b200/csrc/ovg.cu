@@ -11,6 +11,7 @@
 #include <cudaTypedefs.h>
 
 #include "../../include/ovg.h"
+#include "arena.cuh"
 #include "attn.cuh"
 #include "camera.cuh"
 #include "elem.cuh"
@@ -55,6 +56,32 @@ int post_launch(const char* what) {
   cudaError_t e = cudaGetLastError();
   if (e != cudaSuccess) return fail(OVG_E_CUDA, std::string(what) + ": launch failed: " + cudaGetErrorString(e));
   g_launches.fetch_add(1, std::memory_order_relaxed);
+  return OVG_OK;
+}
+
+// ------------------------------------------------------------------------------ workspaces
+// Every component with a size query has one layout function, Bufs layout(Arena&, dims...).  Its size query answers
+// layout_bytes(layout, dims...) and its entry points take their buffers from carve(), so the two cannot disagree.
+using ovg::Arena;
+
+template <typename Bufs, typename... P, typename... A>
+long long layout_bytes(Bufs (*layout)(Arena&, P...), A... dims) {
+  Arena ar(nullptr);
+  layout(ar, dims...);
+  return ar.bytes();
+}
+
+// The caller's workspace, checked to be non-null, Align-byte aligned and layout_bytes() long, carved into *out.  A failure
+// names the entry point fn and the size query to call.
+template <uintptr_t Align = 256, typename Bufs, typename... P, typename... A>
+int carve(const char* fn, const char* query, const void* workspace, long long workspace_bytes, Bufs* out,
+          Bufs (*layout)(Arena&, P...), A... dims) {
+  if (!workspace || (reinterpret_cast<uintptr_t>(workspace) & (Align - 1)) != 0 ||
+      workspace_bytes < layout_bytes(layout, dims...))
+    return fail(OVG_E_INVALID, std::string(fn) + ": workspace must be " + std::to_string(Align) + "-byte aligned and " +
+                                   query + " long");
+  Arena ar(const_cast<void*>(workspace));
+  *out = layout(ar, dims...);
   return OVG_OK;
 }
 
@@ -670,15 +697,28 @@ int select_blocks(long long n) {
   return blocks < 1 ? 1 : static_cast<int>(blocks);
 }
 
+// The percentile's workspace of OVG_PERCENTILE_WORKSPACE_BYTES, packed (not carved at 256-byte boundaries):
+// 6 x u64 state | 512 x u32 histograms | 3 x f32 results.
+struct PercentileRegion {
+  unsigned long long* state;
+  unsigned int* hist;
+  float* res;
+};
+
+PercentileRegion percentile_region(void* workspace) {
+  unsigned long long* state = static_cast<unsigned long long*>(workspace);
+  unsigned int* hist = reinterpret_cast<unsigned int*>(state + 6);
+  return {state, hist, reinterpret_cast<float*>(hist + 512)};
+}
+
 // The 4 x (histogram, decide) passes of a radix selection whose ranks an init launch has set in the workspace's state.
 int radix_select_passes(const float* v, long long n, void* workspace, float* out3, float frac, const std::string& what,
                         cudaStream_t st) {
-  unsigned long long* state = reinterpret_cast<unsigned long long*>(workspace);
-  unsigned int* hist = reinterpret_cast<unsigned int*>(state + 6);
+  const PercentileRegion r = percentile_region(workspace);
   int rc = OVG_OK;
   const int blocks = select_blocks(n);
   for (int pass = 0; pass < 4; ++pass) {
-    ovg::SelectParams sp{v, n, state, hist, pass, out3, frac};
+    ovg::SelectParams sp{v, n, r.state, r.hist, pass, out3, frac};
     ovg::select_hist_kernel<<<blocks, 256, 0, st>>>(sp);
     rc = post_launch((what + "(hist)").c_str());
     if (rc) return rc;
@@ -690,8 +730,8 @@ int radix_select_passes(const float* v, long long n, void* workspace, float* out
 }
 
 // numpy.percentile(v[0, n), percent) (method "linear", exact) by radix select: one init launch, then 4 x (histogram, decide).
-// workspace: OVG_PERCENTILE_WORKSPACE_BYTES (6 x u64 state | 512 x u32 histograms | ...); out3: device float[3] = the two
-// neighbouring order statistics and the interpolated percentile.  count (optional) is zeroed by the init launch.
+// workspace: a percentile_region; out3: device float[3] = the two neighbouring order statistics and the interpolated
+// percentile.  count (optional) is zeroed by the init launch.
 int radix_percentile(const float* v, long long n, float percent, void* workspace, float* out3, unsigned long long* count,
                      const std::string& what, cudaStream_t st) {
   // virtual index p/100 * (n - 1), linear interpolation between its two neighbours
@@ -699,53 +739,27 @@ int radix_percentile(const float* v, long long n, float percent, void* workspace
   const unsigned long long r0 = static_cast<unsigned long long>(vi);
   const unsigned long long r1 = r0 + 1 < static_cast<unsigned long long>(n) ? r0 + 1 : r0;
   const double frac = vi - static_cast<double>(r0);
-  unsigned long long* state = reinterpret_cast<unsigned long long*>(workspace);
-  unsigned int* hist = reinterpret_cast<unsigned int*>(state + 6);
-  ovg::select_init_kernel<<<1, 128, 0, st>>>(state, hist, r0, r1, count);
+  const PercentileRegion r = percentile_region(workspace);
+  ovg::select_init_kernel<<<1, 128, 0, st>>>(r.state, r.hist, r0, r1, count);
   const int rc = post_launch((what + "(init)").c_str());
   return rc ? rc : radix_select_passes(v, n, workspace, out3, static_cast<float>(frac), what, st);
 }
 
-struct Arena {
-  char* base;
-  long long cap, off = 0;
-  bool dry;        // size query: no pointers are formed
-  Arena(void* b, long long c) : base(static_cast<char*>(b)), cap(c), dry(b == nullptr) {}
-  void* take(long long bytes) {
-    const long long at = (off + 255) & ~255LL;
-    off = at + bytes;
-    return dry ? nullptr : base + at;
-  }
-  template <typename T>
-  T* get(long long n) { return static_cast<T*>(take(n * static_cast<long long>(sizeof(T)))); }
-  bool ok() const { return dry || off <= cap; }
-  long long bytes() const { return (off + 255) & ~255LL; }   // the layout's size in whole 256-byte blocks
-};
-
-// A caller's workspace for a layout of `need` bytes: non-null, `align`-byte aligned and at least `need` bytes long.
-bool workspace_ok(const void* workspace, long long workspace_bytes, long long need, uintptr_t align) {
-  return workspace && (reinterpret_cast<uintptr_t>(workspace) & (align - 1)) == 0 && workspace_bytes >= need;
-}
-
-// Point-cloud workspace, carved the same way by the size query and by every entry point.
-struct CloudWorkspace {
+struct CloudBufs {
   void* select;                      // OVG_PERCENTILE_WORKSPACE_BYTES
   float* sel;                        // [6][3] selection results of the scale
   double* center_partial;            // [CLOUD_CENTER_BLOCKS][3]
   unsigned int* tile_count;          // [tiles]
   unsigned long long* tile_offset;   // [tiles]
-  long long bytes;
 };
 
-CloudWorkspace cloud_workspace(void* base, long long n) {
-  Arena ar(base, 0);
-  CloudWorkspace w;
+CloudBufs cloud_layout(Arena& ar, long long n) {
+  CloudBufs w;
   w.select = ar.take(OVG_PERCENTILE_WORKSPACE_BYTES);
   w.sel = ar.get<float>(18);
   w.center_partial = ar.get<double>(3LL * ovg::CLOUD_CENTER_BLOCKS);
   w.tile_count = ar.get<unsigned int>(ovg::compact_tiles(n));
   w.tile_offset = ar.get<unsigned long long>(ovg::compact_tiles(n));
-  w.bytes = ar.bytes();
   return w;
 }
 
@@ -761,8 +775,7 @@ int ovg_conf_percentile_mask(const float* conf, long long n, float percent, floa
                   (reinterpret_cast<uintptr_t>(workspace) & 15) == 0,
               "conf must be 16-byte, mask 4-byte, workspace 16-byte aligned");
   cudaStream_t st = reinterpret_cast<cudaStream_t>(stream);
-  // workspace: 6 x u64 state | 512 x u32 histograms | 3 x f32 results       (OVG_PERCENTILE_WORKSPACE_BYTES)
-  float* res = reinterpret_cast<float*>(reinterpret_cast<unsigned int*>(reinterpret_cast<unsigned long long*>(workspace) + 6) + 512);
+  float* res = percentile_region(workspace).res;
   int rc = radix_percentile(conf, n, percent, workspace, res, count_out, "ovg_conf_percentile_mask", st);
   if (rc) return rc;
   const int blocks = select_blocks(n);
@@ -772,19 +785,19 @@ int ovg_conf_percentile_mask(const float* conf, long long n, float percent, floa
   return post_launch("ovg_conf_percentile_mask");
 }
 
-long long ovg_point_cloud_workspace_bytes(long long n) { return n > 0 ? cloud_workspace(nullptr, n).bytes : -1; }
+long long ovg_point_cloud_workspace_bytes(long long n) { return n > 0 ? layout_bytes(cloud_layout, n) : -1; }
 
 }  // extern "C"
 
 namespace {
 
-int cloud_params(const unsigned char* conf_mask, const float* images, int F, int H, int W, int mask_black_bg, int mask_white_bg,
-                 void* workspace, long long workspace_bytes, ovg::CloudParams* p) {
-  OVG_REQUIRE(conf_mask && images && workspace && F > 0 && H > 0 && W > 0, "bad arguments");
+int cloud_params(const char* fn, const unsigned char* conf_mask, const float* images, int F, int H, int W, int mask_black_bg,
+                 int mask_white_bg, const void* workspace, long long workspace_bytes, ovg::CloudParams* p) {
+  OVG_REQUIRE(conf_mask && images && F > 0 && H > 0 && W > 0, "bad arguments");
   const long long n = static_cast<long long>(F) * H * W;
-  const CloudWorkspace w = cloud_workspace(workspace, n);
-  OVG_REQUIRE(workspace_ok(workspace, workspace_bytes, w.bytes, 16),
-              "workspace must be 16-byte aligned and ovg_point_cloud_workspace_bytes(F*H*W) long");
+  CloudBufs w;
+  const int rc = carve<16>(fn, "ovg_point_cloud_workspace_bytes(F*H*W)", workspace, workspace_bytes, &w, cloud_layout, n);
+  if (rc) return rc;
   OVG_REQUIRE(ovg::compact_tiles(n) < (1LL << 31), "too many pixels");
   *p = ovg::CloudParams{};
   p->conf_mask = conf_mask; p->images = images; p->n = n; p->hw = static_cast<long long>(H) * W;
@@ -803,7 +816,7 @@ int ovg_point_cloud_count(const unsigned char* conf_mask, const float* images, i
                           void* stream) {
   OVG_REQUIRE(count_out, "null count_out");
   ovg::CloudParams p;
-  int rc = cloud_params(conf_mask, images, F, H, W, mask_black_bg, mask_white_bg, workspace, workspace_bytes, &p);
+  int rc = cloud_params(__func__, conf_mask, images, F, H, W, mask_black_bg, mask_white_bg, workspace, workspace_bytes, &p);
   if (rc) return rc;
   cudaStream_t st = reinterpret_cast<cudaStream_t>(stream);
   ovg::cloud_count_kernel<<<p.tiles, ovg::COMPACT_THREADS, 0, st>>>(p);
@@ -819,8 +832,7 @@ int ovg_point_cloud_gather(const float* points, const unsigned char* conf_mask, 
                            void* stream) {
   OVG_REQUIRE(points && points_out && colors_out && frame_out && xyz, "null operand");
   ovg::CloudParams p;
-  int rc = cloud_params(conf_mask, images, F, H, W, mask_black_bg, mask_white_bg, const_cast<void*>(workspace),
-                        workspace_bytes, &p);
+  int rc = cloud_params(__func__, conf_mask, images, F, H, W, mask_black_bg, mask_white_bg, workspace, workspace_bytes, &p);
   if (rc) return rc;
   OVG_REQUIRE(ld >= 0 && (ld % 4) == 0 && (reinterpret_cast<uintptr_t>(xyz) & 15) == 0,
               "xyz must be 16-byte aligned with a column stride ld % 4 == 0");
@@ -832,14 +844,14 @@ int ovg_point_cloud_gather(const float* points, const unsigned char* conf_mask, 
 
 int ovg_point_cloud_center(const float* points, long long n, void* workspace, long long workspace_bytes, float* center_out,
                            void* stream) {
-  OVG_REQUIRE(points && workspace && center_out && n > 0, "bad arguments");
-  const CloudWorkspace w = cloud_workspace(workspace, n);
-  OVG_REQUIRE(workspace_ok(workspace, workspace_bytes, w.bytes, 16),
-              "workspace must be 16-byte aligned and ovg_point_cloud_workspace_bytes(n) long");
+  OVG_REQUIRE(points && center_out && n > 0, "bad arguments");
+  CloudBufs w;
+  int rc = carve<16>(__func__, "ovg_point_cloud_workspace_bytes(n)", workspace, workspace_bytes, &w, cloud_layout, n);
+  if (rc) return rc;
   cudaStream_t st = reinterpret_cast<cudaStream_t>(stream);
   ovg::CloudCenterParams p{points, n, w.center_partial, center_out};
   ovg::cloud_center_partial_kernel<<<ovg::CLOUD_CENTER_BLOCKS, 256, 0, st>>>(p);
-  int rc = post_launch("ovg_point_cloud_center");
+  rc = post_launch("ovg_point_cloud_center");
   if (rc) return rc;
   ovg::cloud_center_final_kernel<<<1, 32, 0, st>>>(p);
   return post_launch("ovg_point_cloud_center(final)");
@@ -847,16 +859,16 @@ int ovg_point_cloud_center(const float* points, long long n, void* workspace, lo
 
 int ovg_point_cloud_scale(const float* xyz, long long n_kept, long long ld, void* workspace, long long workspace_bytes,
                           float* scale_out, void* stream) {
-  OVG_REQUIRE(xyz && workspace && scale_out && n_kept > 0 && ld >= n_kept && ld % 4 == 0, "bad arguments");
+  OVG_REQUIRE(xyz && scale_out && n_kept > 0 && ld >= n_kept && ld % 4 == 0, "bad arguments");
   OVG_REQUIRE((reinterpret_cast<uintptr_t>(xyz) & 15) == 0, "xyz must be 16-byte aligned");
-  const CloudWorkspace w = cloud_workspace(workspace, 1);   // the scale uses only the fixed-size head of the workspace
-  OVG_REQUIRE(workspace_ok(workspace, workspace_bytes, w.bytes, 16),
-              "workspace must be 16-byte aligned and ovg_point_cloud_workspace_bytes() long");
+  CloudBufs w;     // the scale uses only the fixed-size head of the workspace: the layout of one point
+  int rc = carve<16>(__func__, "ovg_point_cloud_workspace_bytes()", workspace, workspace_bytes, &w, cloud_layout, 1LL);
+  if (rc) return rc;
   cudaStream_t st = reinterpret_cast<cudaStream_t>(stream);
   for (int q = 0; q < 2; ++q)
     for (int a = 0; a < 3; ++a) {
-      const int rc = radix_percentile(xyz + a * ld, n_kept, q ? 95.f : 5.f, w.select, w.sel + (q * 3 + a) * 3, nullptr,
-                                      "ovg_point_cloud_scale", st);
+      rc = radix_percentile(xyz + a * ld, n_kept, q ? 95.f : 5.f, w.select, w.sel + (q * 3 + a) * 3, nullptr,
+                            "ovg_point_cloud_scale", st);
       if (rc) return rc;
     }
   ovg::cloud_scale_kernel<<<1, 32, 0, st>>>(w.sel, scale_out);
@@ -868,16 +880,13 @@ int ovg_point_cloud_scale(const float* xyz, long long n_kept, long long ld, void
 // ------------------------------------------------------------------------------------------------------- reciprocal matches
 namespace {
 
-// Match workspace, carved the same way by the size query and by every entry point.
-struct MatchWorkspace {
+struct MatchBufs {
   ovg::MatchParams p;
   int passes;          // 8-bit radix-sort passes over the cell ids
-  long long bytes;
 };
 
-MatchWorkspace match_workspace(void* base, int V, long long cap, int P) {
-  Arena ar(base, 0);
-  MatchWorkspace w;
+MatchBufs match_layout(Arena& ar, int V, long long cap, int P) {
+  MatchBufs w;
   ovg::MatchParams& p = w.p;
   p = ovg::MatchParams{};
   p.V = V; p.cap = cap; p.P = P;
@@ -907,18 +916,17 @@ MatchWorkspace match_workspace(void* base, int V, long long cap, int P) {
   p.pair_tile_count = ar.get<unsigned int>(static_cast<long long>(P) * p.ptiles);
   p.pair_tile_offset = ar.get<unsigned long long>(static_cast<long long>(P) * p.ptiles);
   p.total = ar.get<unsigned long long>(1);
-  w.bytes = ar.bytes();
   return w;
 }
 
-int match_check(int V, long long cap, int P, const void* workspace, long long workspace_bytes, ovg::MatchParams* p,
-                int* passes = nullptr) {
+int match_check(const char* fn, int V, long long cap, int P, const void* workspace, long long workspace_bytes,
+                ovg::MatchParams* p, int* passes = nullptr) {
   // cap < 2^30 keeps the cell ids (cells_cap = 2 cap + 64) and the slots inside a view in int range
   OVG_REQUIRE(V > 0 && V <= 65535 && cap > 0 && cap < (1LL << 30) && P > 0 && 2LL * P <= 65535, "bad sizes");
   OVG_REQUIRE(static_cast<long long>(V) * cap < (1LL << 40), "too many points");
-  const MatchWorkspace w = match_workspace(const_cast<void*>(workspace), V, cap, P);
-  OVG_REQUIRE(workspace_ok(workspace, workspace_bytes, w.bytes, 256),
-              "workspace must be 256-byte aligned and ovg_match_workspace_bytes(V, cap, P) long");
+  MatchBufs w;
+  const int rc = carve(fn, "ovg_match_workspace_bytes(V, cap, P)", workspace, workspace_bytes, &w, match_layout, V, cap, P);
+  if (rc) return rc;
   *p = w.p;
   if (passes) *passes = w.passes;
   return OVG_OK;
@@ -935,14 +943,14 @@ int match_blocks(long long cap) {
 extern "C" {
 
 long long ovg_match_workspace_bytes(int V, long long cap, int P) {
-  return (V > 0 && cap > 0 && P > 0) ? match_workspace(nullptr, V, cap, P).bytes : -1;
+  return (V > 0 && cap > 0 && P > 0) ? layout_bytes(match_layout, V, cap, P) : -1;
 }
 
 int ovg_match_index(const float* points, const unsigned char* keep, int V, long long cap, int P, void* workspace,
                     long long workspace_bytes, void* stream) {
   ovg::MatchParams p;
   int passes = 0;
-  int rc = match_check(V, cap, P, workspace, workspace_bytes, &p, &passes);
+  int rc = match_check(__func__, V, cap, P, workspace, workspace_bytes, &p, &passes);
   if (rc) return rc;
   OVG_REQUIRE(points, "null points");
   p.points = points;
@@ -983,7 +991,7 @@ int ovg_match_index(const float* points, const unsigned char* keep, int V, long 
 int ovg_match_query(const int* pairs, int P, int V, long long cap, void* workspace, long long workspace_bytes, long long* counts_out,
                     void* stream) {
   ovg::MatchParams p;
-  int rc = match_check(V, cap, P, workspace, workspace_bytes, &p);
+  int rc = match_check(__func__, V, cap, P, workspace, workspace_bytes, &p);
   if (rc) return rc;
   OVG_REQUIRE(pairs && counts_out, "null pairs / counts_out");
   OVG_REQUIRE(static_cast<long long>(P) * p.ptiles < (1LL << 31), "too many pairs");
@@ -1005,7 +1013,7 @@ int ovg_match_query(const int* pairs, int P, int V, long long cap, void* workspa
 int ovg_match_gather(const int* pairs, int P, int V, long long cap, int W, const void* workspace, long long workspace_bytes,
                      long long* xy_i, long long* xy_j, void* stream) {
   ovg::MatchParams p;
-  int rc = match_check(V, cap, P, workspace, workspace_bytes, &p);
+  int rc = match_check(__func__, V, cap, P, workspace, workspace_bytes, &p);
   if (rc) return rc;
   OVG_REQUIRE(pairs && xy_i && xy_j && W > 0, "bad arguments");
   p.pairs = pairs;
@@ -1017,7 +1025,7 @@ int ovg_match_gather(const int* pairs, int P, int V, long long cap, int W, const
 int ovg_match_pair(const int* pairs, int P, int V, long long cap, int pair, const void* workspace, long long workspace_bytes,
                    unsigned char* reciprocal, long long* nn, void* stream) {
   ovg::MatchParams p;
-  int rc = match_check(V, cap, P, workspace, workspace_bytes, &p);
+  int rc = match_check(__func__, V, cap, P, workspace, workspace_bytes, &p);
   if (rc) return rc;
   OVG_REQUIRE(pairs && reciprocal && nn && pair >= 0 && pair < P, "bad arguments");
   p.pairs = pairs;
@@ -1031,31 +1039,30 @@ int ovg_match_pair(const int* pairs, int P, int V, long long cap, int pair, cons
 // ------------------------------------------------------------------------------------------------------------- star tracks
 namespace {
 
-// Track workspace, carved the same way by the size query and by both entry points.
-long long tracks_workspace(void* base, int V, long long cap, ovg::TrackParams* p) {
-  Arena ar(base, 0);
+ovg::TrackParams tracks_layout(Arena& ar, int V, long long cap) {
+  ovg::TrackParams p{};
   const long long nodes = V * cap;
   const long long tiles = ovg::compact_tiles(cap) * (V > 2 ? V : 2);
-  p->claim = ar.get<int>(nodes);
-  p->rank = ar.get<int>(nodes);
-  p->obs = ar.get<int>(nodes);
-  p->track_start = ar.get<int>(nodes);
-  p->tile_count = ar.get<unsigned int>(tiles);
-  p->tile_offset = ar.get<unsigned long long>(tiles);
-  p->scan_total = ar.get<unsigned long long>(1);
-  p->totals = ar.get<unsigned long long>(4);
-  return ar.bytes();
+  p.claim = ar.get<int>(nodes);
+  p.rank = ar.get<int>(nodes);
+  p.obs = ar.get<int>(nodes);
+  p.track_start = ar.get<int>(nodes);
+  p.tile_count = ar.get<unsigned int>(tiles);
+  p.tile_offset = ar.get<unsigned long long>(tiles);
+  p.scan_total = ar.get<unsigned long long>(1);
+  p.totals = ar.get<unsigned long long>(4);
+  return p;
 }
 
-int tracks_check(int V, long long cap, int P, const void* match_ws, long long match_ws_bytes, void* workspace,
+int tracks_check(const char* fn, int V, long long cap, int P, const void* match_ws, long long match_ws_bytes, void* workspace,
                  long long workspace_bytes, ovg::TrackParams* p) {
   OVG_REQUIRE(V > 0 && cap > 0 && static_cast<long long>(V) * cap < (1LL << 31), "V * cap must be below 2^31");
-  int rc = match_check(V, cap, P, match_ws, match_ws_bytes, &p->m);
+  ovg::MatchParams m;
+  int rc = match_check(fn, V, cap, P, match_ws, match_ws_bytes, &m);
   if (rc) return rc;
-  OVG_REQUIRE(workspace_ok(workspace, workspace_bytes, tracks_workspace(nullptr, V, cap, p), 256),
-              "workspace must be 256-byte aligned and ovg_tracks_workspace_bytes(V, cap) long");
-  tracks_workspace(workspace, V, cap, p);
-  return OVG_OK;
+  rc = carve(fn, "ovg_tracks_workspace_bytes(V, cap)", workspace, workspace_bytes, p, tracks_layout, V, cap);
+  p->m = m;
+  return rc;
 }
 
 }  // namespace
@@ -1063,15 +1070,14 @@ int tracks_check(int V, long long cap, int P, const void* match_ws, long long ma
 extern "C" {
 
 long long ovg_tracks_workspace_bytes(int V, long long cap) {
-  ovg::TrackParams p{};
-  return (V > 0 && cap > 0) ? tracks_workspace(nullptr, V, cap, &p) : -1;
+  return (V > 0 && cap > 0) ? layout_bytes(tracks_layout, V, cap) : -1;
 }
 
 int ovg_tracks_assign(const int* pairs, const int* pair_off, int P, int V, long long cap, int min_views, const void* match_workspace,
                       long long match_workspace_bytes, void* workspace, long long workspace_bytes, long long* counts_out,
                       void* stream) {
   ovg::TrackParams p{};
-  int rc = tracks_check(V, cap, P, match_workspace, match_workspace_bytes, workspace, workspace_bytes, &p);
+  int rc = tracks_check(__func__, V, cap, P, match_workspace, match_workspace_bytes, workspace, workspace_bytes, &p);
   if (rc) return rc;
   OVG_REQUIRE(pairs && pair_off && counts_out, "null pairs / pair_off / counts_out");
   OVG_REQUIRE(min_views >= 1 && min_views <= V, "min_views must be in [1, V]");
@@ -1100,7 +1106,7 @@ int ovg_tracks_gather(const float* images, const float* extrinsic, const float* 
                       long long* offsets, int* view, long long* xy, int* point2d, long long* view_offsets, int* view_track,
                       long long* view_xy, void* stream) {
   ovg::TrackParams p{};
-  int rc = tracks_check(V, cap, P, match_workspace, match_workspace_bytes, workspace, workspace_bytes, &p);
+  int rc = tracks_check(__func__, V, cap, P, match_workspace, match_workspace_bytes, workspace, workspace_bytes, &p);
   if (rc) return rc;
   OVG_REQUIRE(W > 0 && cap % W == 0, "cap must be H * W");
   OVG_REQUIRE(n_tracks >= 0 && n_tracks <= n_obs && n_obs <= static_cast<long long>(V) * cap, "bad track counts");
@@ -1131,35 +1137,34 @@ int ovg_tracks_gather(const float* images, const float* extrinsic, const float* 
 // ------------------------------------------------------------------------------------------------------- bundle adjustment
 namespace {
 
-// Bundle-adjustment workspace, carved the same way by the size query and by the entry point.
-long long ba_workspace(void* base, int V, long long n, long long m, ovg::BaParams* p) {
-  Arena ar(base, 0);
-  p->tblocks = static_cast<int>(std::max(1LL, (n + ovg::BA_THREADS - 1) / ovg::BA_THREADS));
-  p->vtiles = static_cast<int>(std::max(1LL, ovg::compact_tiles(m)));
-  p->st = ar.get<ovg::BaState>(1);
-  p->cam = ar.get<double>(2LL * V * ovg::BA_CAM);
-  p->mask = ar.get<double>(static_cast<long long>(V) * ovg::BA_NP);
-  p->dcam = ar.get<double>(static_cast<long long>(V) * ovg::BA_NP);
-  p->pts = ar.get<double>(6 * n);
-  p->dp = ar.get<double>(3 * n);
-  p->vinv = ar.get<double>(9 * n);
-  p->y = ar.get<double>(3 * n);
-  p->gp = ar.get<double>(3 * n);
-  p->zt = ar.get<double>(3 * n);
-  p->incl = ar.get<unsigned char>(n);
-  p->ob = ar.get<ovg::BaObs>(m);
-  p->obs_track = ar.get<int>(m);
-  p->view_obs = ar.get<int>(m);
-  p->view_off = ar.get<long long>(V + 1);
-  p->gmax = ar.get<double>(p->tblocks);
-  p->vpart = ar.get<double>(static_cast<long long>(V) * ovg::BA_BLOCK_CHUNKS * ovg::BA_ENTRIES);
-  p->vsum = ar.get<double>(static_cast<long long>(V) * ovg::BA_ENTRIES);
-  p->bpart = ar.get<double>(static_cast<long long>(V) * ovg::BA_PCG_CHUNKS * ovg::BA_NP);
-  p->epart = ar.get<double>(static_cast<long long>(p->tblocks) * ovg::BA_EVAL);
-  p->tile_count = ar.get<unsigned int>(static_cast<long long>(V) * p->vtiles);
-  p->tile_offset = ar.get<unsigned long long>(static_cast<long long>(V) * p->vtiles);
-  p->scan_total = ar.get<unsigned long long>(1);
-  return ar.bytes();
+ovg::BaParams ba_layout(Arena& ar, int V, long long n, long long m) {
+  ovg::BaParams p{};
+  p.tblocks = static_cast<int>(std::max(1LL, (n + ovg::BA_THREADS - 1) / ovg::BA_THREADS));
+  p.vtiles = static_cast<int>(std::max(1LL, ovg::compact_tiles(m)));
+  p.st = ar.get<ovg::BaState>(1);
+  p.cam = ar.get<double>(2LL * V * ovg::BA_CAM);
+  p.mask = ar.get<double>(static_cast<long long>(V) * ovg::BA_NP);
+  p.dcam = ar.get<double>(static_cast<long long>(V) * ovg::BA_NP);
+  p.pts = ar.get<double>(6 * n);
+  p.dp = ar.get<double>(3 * n);
+  p.vinv = ar.get<double>(9 * n);
+  p.y = ar.get<double>(3 * n);
+  p.gp = ar.get<double>(3 * n);
+  p.zt = ar.get<double>(3 * n);
+  p.incl = ar.get<unsigned char>(n);
+  p.ob = ar.get<ovg::BaObs>(m);
+  p.obs_track = ar.get<int>(m);
+  p.view_obs = ar.get<int>(m);
+  p.view_off = ar.get<long long>(V + 1);
+  p.gmax = ar.get<double>(p.tblocks);
+  p.vpart = ar.get<double>(static_cast<long long>(V) * ovg::BA_BLOCK_CHUNKS * ovg::BA_ENTRIES);
+  p.vsum = ar.get<double>(static_cast<long long>(V) * ovg::BA_ENTRIES);
+  p.bpart = ar.get<double>(static_cast<long long>(V) * ovg::BA_PCG_CHUNKS * ovg::BA_NP);
+  p.epart = ar.get<double>(static_cast<long long>(p.tblocks) * ovg::BA_EVAL);
+  p.tile_count = ar.get<unsigned int>(static_cast<long long>(V) * p.vtiles);
+  p.tile_offset = ar.get<unsigned long long>(static_cast<long long>(V) * p.vtiles);
+  p.scan_total = ar.get<unsigned long long>(1);
+  return p;
 }
 
 bool ba_sizes_ok(int V, long long n, long long m) {
@@ -1171,8 +1176,7 @@ bool ba_sizes_ok(int V, long long n, long long m) {
 extern "C" {
 
 long long ovg_ba_workspace_bytes(int V, long long n_tracks, long long n_obs) {
-  ovg::BaParams p{};
-  return ba_sizes_ok(V, n_tracks, n_obs) ? ba_workspace(nullptr, V, n_tracks, n_obs, &p) : -1;
+  return ba_sizes_ok(V, n_tracks, n_obs) ? layout_bytes(ba_layout, V, n_tracks, n_obs) : -1;
 }
 
 int ovg_bundle_adjust(const double* points, const long long* offsets, const int* view, const double* observations,
@@ -1187,10 +1191,10 @@ int ovg_bundle_adjust(const double* points, const long long* offsets, const int*
   OVG_REQUIRE(offsets && extrinsic && intrinsic && extrinsic_out && intrinsic_out && cost_out && stats_out, "null operand");
   OVG_REQUIRE(n_tracks == 0 || (points && points_out && error_out), "null points / points_out / error_out");
   OVG_REQUIRE(n_obs == 0 || (view && observations), "null view / observations");
-  ovg::BaParams p{};
-  OVG_REQUIRE(workspace_ok(workspace, workspace_bytes, ba_workspace(nullptr, V, n_tracks, n_obs, &p), 256),
-              "workspace must be 256-byte aligned and ovg_ba_workspace_bytes(V, n_tracks, n_obs) long");
-  ba_workspace(workspace, V, n_tracks, n_obs, &p);
+  ovg::BaParams p;
+  int rc = carve(__func__, "ovg_ba_workspace_bytes(V, n_tracks, n_obs)", workspace, workspace_bytes, &p, ba_layout, V, n_tracks,
+                 n_obs);
+  if (rc) return rc;
   p.V = V; p.n = n_tracks; p.m = n_obs; p.iterations = iterations; p.refine_focal = refine_focal ? 1 : 0;
   p.cauchy = loss == OVG_BA_LOSS_CAUCHY; p.c2 = loss_scale * loss_scale;
   p.points = points; p.offsets = offsets; p.view = view; p.obs = observations; p.ext = extrinsic; p.intr = intrinsic;
@@ -1198,7 +1202,7 @@ int ovg_bundle_adjust(const double* points, const long long* offsets, const int*
   p.cost_out = cost_out; p.stats_out = stats_out; p.trace = trace_out;
   // the PCG spins on the other CTAs: launched cooperatively with the grid the occupancy query allows
   const int smem = ovg::BA_VIEW_SMEM * V * static_cast<int>(sizeof(double));
-  int rc = allow_dynamic_smem<ovg::ba_pcg_kernel>(ovg::BA_VIEW_SMEM * ovg::BA_MAX_VIEWS * static_cast<int>(sizeof(double)));
+  rc = allow_dynamic_smem<ovg::ba_pcg_kernel>(ovg::BA_VIEW_SMEM * ovg::BA_MAX_VIEWS * static_cast<int>(sizeof(double)));
   if (rc) return rc;
   int per_sm = 0;
   OVG_CUDA(cudaOccupancyMaxActiveBlocksPerMultiprocessor(&per_sm, ovg::ba_pcg_kernel, ovg::BA_PCG_THREADS, smem));
@@ -1248,9 +1252,7 @@ int ovg_bundle_adjust(const double* points, const long long* offsets, const int*
 // -------------------------------------------------------------------------------------------------------------- triangle mesh
 namespace {
 
-// Mesh workspace, carved the same way by the size query and by every entry point.
-ovg::MeshParams mesh_workspace(void* base, int F, int H, int W, long long* bytes) {
-  Arena ar(base, 0);
+ovg::MeshParams mesh_layout(Arena& ar, int F, int H, int W) {
   ovg::MeshParams p{};
   p.H = H; p.W = W;
   p.hw = static_cast<long long>(H) * W;
@@ -1261,18 +1263,13 @@ ovg::MeshParams mesh_workspace(void* base, int F, int H, int W, long long* bytes
   p.remap = ar.get<int>(p.n);
   p.tile_count = ar.get<unsigned int>(static_cast<long long>(ovg::MESH_STREAMS) * p.T);
   p.tile_offset = ar.get<unsigned long long>(static_cast<long long>(ovg::MESH_STREAMS) * p.T + 1);
-  *bytes = ar.bytes();
   return p;
 }
 
-int mesh_check(int F, int H, int W, const void* workspace, long long workspace_bytes, ovg::MeshParams* p) {
+int mesh_check(const char* fn, int F, int H, int W, const void* workspace, long long workspace_bytes, ovg::MeshParams* p) {
   OVG_REQUIRE(F > 0 && F <= 65535 && H > 0 && W > 0, "bad sizes");
   OVG_REQUIRE(static_cast<long long>(F) * H * W < (1LL << 31), "F*H*W must be below 2^31");
-  long long bytes = 0;
-  *p = mesh_workspace(const_cast<void*>(workspace), F, H, W, &bytes);
-  OVG_REQUIRE(workspace_ok(workspace, workspace_bytes, bytes, 256),
-              "workspace must be 256-byte aligned and ovg_mesh_workspace_bytes(F, H, W) long");
-  return OVG_OK;
+  return carve(fn, "ovg_mesh_workspace_bytes(F, H, W)", workspace, workspace_bytes, p, mesh_layout, F, H, W);
 }
 
 }  // namespace
@@ -1280,16 +1277,13 @@ int mesh_check(int F, int H, int W, const void* workspace, long long workspace_b
 extern "C" {
 
 long long ovg_mesh_workspace_bytes(int F, int H, int W) {
-  if (F <= 0 || H <= 0 || W <= 0) return -1;
-  long long bytes = 0;
-  mesh_workspace(nullptr, F, H, W, &bytes);
-  return bytes;
+  return (F > 0 && H > 0 && W > 0) ? layout_bytes(mesh_layout, F, H, W) : -1;
 }
 
 int ovg_mesh_count(const unsigned char* conf_mask, const float* images, int F, int H, int W, int mask_black_bg,
                    int mask_white_bg, void* workspace, long long workspace_bytes, long long* counts_out, void* stream) {
   ovg::MeshParams p;
-  int rc = mesh_check(F, H, W, workspace, workspace_bytes, &p);
+  int rc = mesh_check(__func__, F, H, W, workspace, workspace_bytes, &p);
   if (rc) return rc;
   OVG_REQUIRE(conf_mask && counts_out, "null conf_mask / counts_out");
   OVG_REQUIRE(images || !(mask_black_bg || mask_white_bg), "the background masks need images");
@@ -1311,7 +1305,7 @@ int ovg_mesh_count(const unsigned char* conf_mask, const float* images, int F, i
 int ovg_mesh_faces(const float* images, const void* colors, int color_bytes, int F, int H, int W, const void* workspace,
                    long long workspace_bytes, long long* faces, void* face_colors, void* stream) {
   ovg::MeshParams p;
-  int rc = mesh_check(F, H, W, workspace, workspace_bytes, &p);
+  int rc = mesh_check(__func__, F, H, W, workspace, workspace_bytes, &p);
   if (rc) return rc;
   OVG_REQUIRE(faces && face_colors, "null faces / face_colors");
   OVG_REQUIRE(images || (colors && (color_bytes == 1 || color_bytes == 2 || color_bytes == 4 || color_bytes == 8)),
@@ -1325,7 +1319,7 @@ int ovg_mesh_faces(const float* images, const void* colors, int color_bytes, int
 int ovg_mesh_compact(const float* points, const float* images, int F, int H, int W, const void* workspace,
                      long long workspace_bytes, float* positions, unsigned char* colors, int* indices, void* stream) {
   ovg::MeshParams p;
-  int rc = mesh_check(F, H, W, workspace, workspace_bytes, &p);
+  int rc = mesh_check(__func__, F, H, W, workspace, workspace_bytes, &p);
   if (rc) return rc;
   OVG_REQUIRE(points && images && positions && colors && indices, "null operand");
   p.points = points; p.images = images;
@@ -1342,9 +1336,9 @@ int ovg_mesh_compact(const float* points, const float* images, int F, int H, int
 // -------------------------------------------------------------------------------------------------------------- fused mesh
 namespace {
 
-// TSDF workspace: the bounds part (F, H, W) and the volume part (nx, ny, nz) are both carved from the start, carved the
-// same way by the size query and by every entry point.
-struct TsdfWorkspace {
+// The TSDF workspace holds two parts, each carved from its start: the bounds part of F*H*W points and the volume part of an
+// nx x ny x nz grid.  ovg_tsdf_workspace_bytes is the larger of the two.
+struct TsdfBoundsBufs {
   void* select;                      // OVG_PERCENTILE_WORKSPACE_BYTES
   float* sel;                        // [6][3] selection results, in the order (axis, percentile)
   float* frac;                       // [6] their interpolation weights
@@ -1352,55 +1346,56 @@ struct TsdfWorkspace {
   unsigned int* nonfinite;
   float* cols;                       // [3, ld]
   long long ld;
+};
+
+TsdfBoundsBufs tsdf_bounds_layout(Arena& ar, long long n) {
+  TsdfBoundsBufs w;
+  w.ld = (n + 3) / 4 * 4;
+  w.select = ar.take(OVG_PERCENTILE_WORKSPACE_BYTES);
+  w.sel = ar.get<float>(18);
+  w.frac = ar.get<float>(6);
+  w.count = ar.get<unsigned long long>(1);
+  w.nonfinite = ar.get<unsigned int>(1);
+  w.cols = ar.get<float>(3 * w.ld);
+  return w;
+}
+
+struct TsdfVolumeBufs {
   unsigned char* marked;             // [bricks]
   unsigned int* tile_count;          // [2 bricks]
   unsigned long long* tile_offset;   // [2 bricks + 1]
   int* edge_vertex;                  // [nz, ny, nx, 3]
-  long long bricks, bytes;
+  long long bricks;
 };
 
-TsdfWorkspace tsdf_workspace(void* base, int nx, int ny, int nz, int F, int H, int W) {
-  TsdfWorkspace w{};
-  Arena b(base, 0);
-  const long long n = static_cast<long long>(F) * H * W;
-  w.ld = (n + 3) / 4 * 4;
-  w.select = b.take(OVG_PERCENTILE_WORKSPACE_BYTES);
-  w.sel = b.get<float>(18);
-  w.frac = b.get<float>(6);
-  w.count = b.get<unsigned long long>(1);
-  w.nonfinite = b.get<unsigned int>(1);
-  w.cols = b.get<float>(3 * w.ld);
-  Arena v(base, 0);
+TsdfVolumeBufs tsdf_volume_layout(Arena& ar, int nx, int ny, int nz) {
+  TsdfVolumeBufs w;
   w.bricks = static_cast<long long>((nx + 7) / 8) * ((ny + 7) / 8) * ((nz + 7) / 8);
-  w.marked = v.get<unsigned char>(w.bricks);
-  w.tile_count = v.get<unsigned int>(2 * w.bricks);
-  w.tile_offset = v.get<unsigned long long>(2 * w.bricks + 1);
-  w.edge_vertex = v.get<int>(3LL * nx * ny * nz);
-  w.bytes = std::max(n ? b.bytes() : 0LL, w.bricks ? v.bytes() : 0LL);
+  w.marked = ar.get<unsigned char>(w.bricks);
+  w.tile_count = ar.get<unsigned int>(2 * w.bricks);
+  w.tile_offset = ar.get<unsigned long long>(2 * w.bricks + 1);
+  w.edge_vertex = ar.get<int>(3LL * nx * ny * nz);
   return w;
 }
 
 bool tsdf_triple(int a, int b, int c) { return (a > 0 && b > 0 && c > 0) || (a == 0 && b == 0 && c == 0); }
 
-int tsdf_grid(int nx, int ny, int nz, float ox, float oy, float oz, float voxel, float trunc, const void* workspace,
-              long long workspace_bytes, TsdfWorkspace* w, ovg::TsdfGrid* g) {
+int tsdf_grid(const char* fn, int nx, int ny, int nz, float ox, float oy, float oz, float voxel, float trunc,
+              const void* workspace, long long workspace_bytes, TsdfVolumeBufs* w, ovg::TsdfGrid* g) {
   OVG_REQUIRE(nx > 0 && ny > 0 && nz > 0 && 3LL * nx * ny * nz < (1LL << 31), "need 0 < nx, ny, nz and 3 nx ny nz < 2^31");
   OVG_REQUIRE(std::isfinite(ox) && std::isfinite(oy) && std::isfinite(oz) && std::isfinite(voxel) && voxel > 0.f &&
                   std::isfinite(trunc) && trunc > 0.f,
               "origin, voxel and trunc must be finite, voxel and trunc > 0");
-  *w = tsdf_workspace(const_cast<void*>(workspace), nx, ny, nz, 0, 0, 0);
-  OVG_REQUIRE(workspace_ok(workspace, workspace_bytes, w->bytes, 256),
-              "workspace must be 256-byte aligned and ovg_tsdf_workspace_bytes(nx, ny, nz, ...) long");
   *g = ovg::TsdfGrid{nx, ny, nz, (nx + 7) / 8, (ny + 7) / 8, (nz + 7) / 8, ox, oy, oz, voxel, trunc};
-  return OVG_OK;
+  return carve(fn, "ovg_tsdf_workspace_bytes(nx, ny, nz, ...)", workspace, workspace_bytes, w, tsdf_volume_layout, nx, ny, nz);
 }
 
-int tsdf_mesh(const float* tsdf, int nx, int ny, int nz, float ox, float oy, float oz, float voxel, const void* workspace,
-              long long workspace_bytes, ovg::TsdfMeshParams* p) {
+int tsdf_mesh(const char* fn, const float* tsdf, int nx, int ny, int nz, float ox, float oy, float oz, float voxel,
+              const void* workspace, long long workspace_bytes, ovg::TsdfMeshParams* p) {
   OVG_REQUIRE(tsdf, "null tsdf");
-  TsdfWorkspace w;
+  TsdfVolumeBufs w;
   *p = ovg::TsdfMeshParams{};
-  const int rc = tsdf_grid(nx, ny, nz, ox, oy, oz, voxel, 1.f, workspace, workspace_bytes, &w, &p->g);
+  const int rc = tsdf_grid(fn, nx, ny, nz, ox, oy, oz, voxel, 1.f, workspace, workspace_bytes, &w, &p->g);
   if (rc) return rc;
   p->tsdf = tsdf; p->bricks = w.bricks;
   p->tile_count = w.tile_count; p->tile_offset = w.tile_offset; p->edge_vertex = w.edge_vertex;
@@ -1414,28 +1409,28 @@ extern "C" {
 long long ovg_tsdf_workspace_bytes(int nx, int ny, int nz, int F, int H, int W) {
   if (!tsdf_triple(nx, ny, nz) || !tsdf_triple(F, H, W) || (nx == 0 && F == 0)) return -1;
   if (3LL * nx * ny * nz >= (1LL << 31) || static_cast<long long>(F) * H * W >= (1LL << 31)) return -1;
-  return tsdf_workspace(nullptr, nx, ny, nz, F, H, W).bytes;
+  return std::max(F ? layout_bytes(tsdf_bounds_layout, static_cast<long long>(F) * H * W) : 0LL,
+                  nx ? layout_bytes(tsdf_volume_layout, nx, ny, nz) : 0LL);
 }
 
 int ovg_tsdf_bounds(const float* points, const unsigned char* mask, int F, int H, int W, void* workspace,
                     long long workspace_bytes, double* bounds_out, void* stream) {
   OVG_REQUIRE(points && mask && bounds_out, "null operand");
   OVG_REQUIRE(F > 0 && H > 0 && W > 0 && static_cast<long long>(F) * H * W < (1LL << 31), "need F H W < 2^31");
-  const TsdfWorkspace w = tsdf_workspace(workspace, 0, 0, 0, F, H, W);
-  OVG_REQUIRE(workspace_ok(workspace, workspace_bytes, w.bytes, 256),
-              "workspace must be 256-byte aligned and ovg_tsdf_workspace_bytes(..., F, H, W) long");
-  cudaStream_t st = reinterpret_cast<cudaStream_t>(stream);
   const long long n = static_cast<long long>(F) * H * W;
+  TsdfBoundsBufs w;
+  int rc = carve(__func__, "ovg_tsdf_workspace_bytes(..., F, H, W)", workspace, workspace_bytes, &w, tsdf_bounds_layout, n);
+  if (rc) return rc;
+  cudaStream_t st = reinterpret_cast<cudaStream_t>(stream);
   OVG_CUDA(cudaMemsetAsync(w.count, 0, sizeof(unsigned long long), st));
   OVG_CUDA(cudaMemsetAsync(w.nonfinite, 0, sizeof(unsigned int), st));
   const ovg::TsdfBoundsParams bp{points, mask, n, w.ld, w.cols, w.count, w.nonfinite};
   ovg::tsdf_fill_kernel<<<select_blocks(n), 256, 0, st>>>(bp);
-  int rc = post_launch("ovg_tsdf_bounds(fill)");
+  rc = post_launch("ovg_tsdf_bounds(fill)");
   if (rc) return rc;
-  unsigned long long* state = reinterpret_cast<unsigned long long*>(w.select);
+  const PercentileRegion r = percentile_region(w.select);
   for (int j = 0; j < 6; ++j) {          // j = 2 axis + (0: 1st percentile, 1: 99th)
-    ovg::tsdf_select_init_kernel<<<1, 128, 0, st>>>(state, reinterpret_cast<unsigned int*>(state + 6), w.count,
-                                                    (j & 1) ? 99.f : 1.f, w.frac + j);
+    ovg::tsdf_select_init_kernel<<<1, 128, 0, st>>>(r.state, r.hist, w.count, (j & 1) ? 99.f : 1.f, w.frac + j);
     if ((rc = post_launch("ovg_tsdf_bounds(init)"))) return rc;
     // the decide step's own interpolation (frac 0) is unused: tsdf_bounds_kernel weighs the pair with the device's frac
     if ((rc = radix_select_passes(w.cols + (j >> 1) * w.ld, n, w.select, w.sel + 3 * j, 0.f, "ovg_tsdf_bounds", st))) return rc;
@@ -1450,9 +1445,9 @@ int ovg_tsdf_integrate(const float* depth, const unsigned char* mask, const floa
                        void* stream) {
   OVG_REQUIRE(depth && mask && images && extrinsic && intrinsic && tsdf && color, "null operand");
   OVG_REQUIRE(F > 0 && H > 0 && W > 0 && static_cast<long long>(F) * H * W < (1LL << 31), "need F H W < 2^31");
-  TsdfWorkspace w;
+  TsdfVolumeBufs w;
   ovg::TsdfIntegrateParams p{};
-  int rc = tsdf_grid(nx, ny, nz, ox, oy, oz, voxel, trunc, workspace, workspace_bytes, &w, &p.g);
+  int rc = tsdf_grid(__func__, nx, ny, nz, ox, oy, oz, voxel, trunc, workspace, workspace_bytes, &w, &p.g);
   if (rc) return rc;
   OVG_REQUIRE((reinterpret_cast<uintptr_t>(color) & 3) == 0, "color must be 4-byte aligned");
   p.depth = depth; p.mask = mask; p.images = images; p.ext = extrinsic; p.intr = intrinsic;
@@ -1470,7 +1465,7 @@ int ovg_tsdf_integrate(const float* depth, const unsigned char* mask, const floa
 int ovg_tsdf_count(const float* tsdf, int nx, int ny, int nz, void* workspace, long long workspace_bytes, long long* counts_out,
                    void* stream) {
   ovg::TsdfMeshParams p;
-  int rc = tsdf_mesh(tsdf, nx, ny, nz, 0.f, 0.f, 0.f, 1.f, workspace, workspace_bytes, &p);
+  int rc = tsdf_mesh(__func__, tsdf, nx, ny, nz, 0.f, 0.f, 0.f, 1.f, workspace, workspace_bytes, &p);
   if (rc) return rc;
   OVG_REQUIRE(counts_out, "null counts_out");
   p.totals = counts_out;
@@ -1487,7 +1482,7 @@ int ovg_tsdf_extract(const float* tsdf, const unsigned char* color, int nx, int 
                      float voxel, void* workspace, long long workspace_bytes, float* positions, unsigned char* colors,
                      int* indices, void* stream) {
   ovg::TsdfMeshParams p;
-  int rc = tsdf_mesh(tsdf, nx, ny, nz, ox, oy, oz, voxel, workspace, workspace_bytes, &p);
+  int rc = tsdf_mesh(__func__, tsdf, nx, ny, nz, ox, oy, oz, voxel, workspace, workspace_bytes, &p);
   if (rc) return rc;
   OVG_REQUIRE(color && positions && colors && indices, "null operand");
   p.color = color; p.positions = positions; p.colors = colors; p.indices = indices;
@@ -1503,9 +1498,7 @@ int ovg_tsdf_extract(const float* tsdf, const unsigned char* color, int nx, int 
 // ------------------------------------------------------------------------------------------------------- sky segmentation
 namespace {
 
-// Sky workspace, carved the same way by the size query and by the entry point.
-ovg::SkyParams sky_workspace(void* base, int F, int H, int W, long long* bytes) {
-  Arena ar(base, 0);
+ovg::SkyParams sky_layout(Arena& ar, int F, int H, int W) {
   ovg::SkyParams p{};
   p.F = F; p.H = H; p.W = W;
   p.hw = static_cast<long long>(H) * W;
@@ -1514,7 +1507,6 @@ ovg::SkyParams sky_workspace(void* base, int F, int H, int W, long long* bytes) 
   p.label = ar.get<int>(p.n);
   p.area = ar.get<int>(p.n);
   p.view_max = ar.get<int>(F);
-  *bytes = ar.bytes();
   return p;
 }
 
@@ -1523,10 +1515,7 @@ ovg::SkyParams sky_workspace(void* base, int F, int H, int W, long long* bytes) 
 extern "C" {
 
 long long ovg_sky_workspace_bytes(int F, int H, int W) {
-  if (F <= 0 || H <= 0 || W <= 0) return -1;
-  long long bytes = 0;
-  sky_workspace(nullptr, F, H, W, &bytes);
-  return bytes;
+  return (F > 0 && H > 0 && W > 0) ? layout_bytes(sky_layout, F, H, W) : -1;
 }
 
 int ovg_segment_sky(const void* image, int image_u8, long long view_stride, long long pixel_stride, long long channel_stride,
@@ -1535,17 +1524,16 @@ int ovg_segment_sky(const void* image, int image_u8, long long view_stride, long
   OVG_REQUIRE(F > 0 && F <= 65535 && H > 0 && W > 0, "bad sizes");
   OVG_REQUIRE(static_cast<long long>(F) * H * W < (1LL << 31), "F*H*W must be below 2^31");
   OVG_REQUIRE(image && sky_out && (conf == nullptr) == (conf_out == nullptr), "null image / sky_out, or conf without conf_out");
-  long long bytes = 0;
-  ovg::SkyParams p = sky_workspace(workspace, F, H, W, &bytes);
-  OVG_REQUIRE(workspace_ok(workspace, workspace_bytes, bytes, 256),
-              "workspace must be 256-byte aligned and ovg_sky_workspace_bytes(F, H, W) long");
+  ovg::SkyParams p;
+  int rc = carve(__func__, "ovg_sky_workspace_bytes(F, H, W)", workspace, workspace_bytes, &p, sky_layout, F, H, W);
+  if (rc) return rc;
   p.image = image; p.u8 = image_u8 ? 1 : 0;
   p.view_stride = view_stride; p.pixel_stride = pixel_stride; p.channel_stride = channel_stride;
   p.conf = conf; p.conf_out = conf_out; p.sky = sky_out;
   cudaStream_t st = reinterpret_cast<cudaStream_t>(stream);
   const int tiles = p.tiles_x * ((H + ovg::SKY_TILE - 1) / ovg::SKY_TILE);
   ovg::sky_open_kernel<<<dim3(tiles, F), ovg::SKY_THREADS, 0, st>>>(p);
-  int rc = post_launch("ovg_segment_sky(colour test, opening)");
+  rc = post_launch("ovg_segment_sky(colour test, opening)");
   if (rc) return rc;
   const unsigned blocks = static_cast<unsigned>((p.n + 255) / 256);
   ovg::sky_merge_kernel<<<blocks, 256, 0, st>>>(p);
@@ -1570,15 +1558,12 @@ int ovg_sky_mask_conf(const float* conf, const unsigned char* sky, long long n, 
 // -------------------------------------------------------------------------------------------------- farthest point sampling
 namespace {
 
-// FPS workspace, carved the same way by the size query and by the entry point.
-ovg::FpsParams fps_workspace(void* base, int B, long long N, long long* bytes) {
-  Arena ar(base, 0);
+ovg::FpsParams fps_layout(Arena& ar, int B, long long N) {
   ovg::FpsParams p{};
   p.B = B; p.N = N;
   p.arrive = ar.get<unsigned>(B);
   p.slots = ar.get<ovg::FpsSlot>(2LL * ovg::FPS_MAX_CTAS);
   p.dist = ar.get<float>(static_cast<long long>(B) * N);
-  *bytes = ar.bytes();
   return p;
 }
 
@@ -1587,10 +1572,7 @@ ovg::FpsParams fps_workspace(void* base, int B, long long N, long long* bytes) {
 extern "C" {
 
 long long ovg_fps_workspace_bytes(int B, long long N) {
-  if (B <= 0 || N <= 0) return -1;
-  long long bytes = 0;
-  fps_workspace(nullptr, B, N, &bytes);
-  return bytes;
+  return (B > 0 && N > 0) ? layout_bytes(fps_layout, B, N) : -1;
 }
 
 int ovg_farthest_point_sample(const float* xyz, int B, long long N, int npoint, const long long* start, int include_ends,
@@ -1600,21 +1582,20 @@ int ovg_farthest_point_sample(const float* xyz, int B, long long N, int npoint, 
   OVG_REQUIRE(npoint <= N, "npoint must be <= N");
   OVG_REQUIRE(static_cast<long long>(B) * N < (1LL << 40), "too many points");
   OVG_REQUIRE(xyz && inds_out && (start || include_ends), "null xyz / inds_out, or no start without include_ends");
-  long long bytes = 0;
-  ovg::FpsParams p = fps_workspace(workspace, B, N, &bytes);
-  OVG_REQUIRE(workspace_ok(workspace, workspace_bytes, bytes, 256),
-              "workspace must be 256-byte aligned and ovg_fps_workspace_bytes(B, N) long");
+  ovg::FpsParams p;
+  int rc = carve(__func__, "ovg_fps_workspace_bytes(B, N)", workspace, workspace_bytes, &p, fps_layout, B, N);
+  if (rc) return rc;
   p.xyz = xyz; p.start = start; p.inds = inds_out; p.npoint = npoint; p.ends = include_ends ? 1 : 0;
   cudaStream_t st = reinterpret_cast<cudaStream_t>(stream);
   if (N <= ovg::FPS_CTA_POINTS) {   // one CTA per batch, every point in its shared memory
-    int rc = allow_dynamic_smem<ovg::fps_cta_kernel>(ovg::FPS_SMEM_BYTES);
+    rc = allow_dynamic_smem<ovg::fps_cta_kernel>(ovg::FPS_SMEM_BYTES);
     if (rc) return rc;
     ovg::fps_cta_kernel<<<B, ovg::FPS_THREADS, static_cast<int>(N) * 16, st>>>(p);
     return post_launch("ovg_farthest_point_sample(cta)");
   }
   // The grid kernel spins on the other CTAs of its group: launched cooperatively, sized by the occupancy query, so the
   // launch fails rather than run with CTAs that are not co-resident.
-  int rc = allow_dynamic_smem<ovg::fps_grid_kernel>(ovg::FPS_SMEM_BYTES);
+  rc = allow_dynamic_smem<ovg::fps_grid_kernel>(ovg::FPS_SMEM_BYTES);
   if (rc) return rc;
   int per_sm = 0;
   OVG_CUDA(cudaOccupancyMaxActiveBlocksPerMultiprocessor(&per_sm, ovg::fps_grid_kernel, ovg::FPS_THREADS,
@@ -1635,17 +1616,14 @@ int ovg_farthest_point_sample(const float* xyz, int B, long long N, int npoint, 
 // ----------------------------------------------------------------------------------------------------------- image ranking
 namespace {
 
-// Ranking workspace, carved the same way by the size query and by the entry point: the packed operands, and on the grid
-// path one scratch of two key / index buffers per CTA.
-ovg::RankParams ranking_workspace(void* base, long long N, int out_f64, long long* bytes) {
-  Arena ar(base, 0);
+// The packed operands, and on the grid path one scratch of two key / index buffers per CTA.
+ovg::RankParams ranking_layout(Arena& ar, long long N, int out_f64) {
   ovg::RankParams p{};
   p.pose = ar.get<double>(N * 12);
   if (N > ovg::RANK_CTA_VIEWS) {
     p.scratch_stride = (N * (2 * (out_f64 ? 8 : 4) + 8) + 255) & ~255LL;
     p.scratch = ar.get<unsigned char>(ovg::RANK_GRID_CTAS * p.scratch_stride);
   }
-  *bytes = ar.bytes();
   return p;
 }
 
@@ -1667,10 +1645,7 @@ int launch_ranking(const ovg::RankParams& p, cudaStream_t st) {
 extern "C" {
 
 long long ovg_ranking_workspace_bytes(long long N, int out_f64) {
-  if (N <= 0 || N >= (1LL << 31)) return -1;
-  long long bytes = 0;
-  ranking_workspace(nullptr, N, out_f64, &bytes);
-  return bytes;
+  return (N > 0 && N < (1LL << 31)) ? layout_bytes(ranking_layout, N, out_f64) : -1;
 }
 
 int ovg_compute_ranking(const void* extrinsics, int in_f64, long long N, long long view_stride, long long row_stride,
@@ -1679,17 +1654,17 @@ int ovg_compute_ranking(const void* extrinsics, int in_f64, long long N, long lo
   OVG_REQUIRE(N > 0 && N < (1LL << 31), "N must be in [1, 2^31)");
   OVG_REQUIRE(k >= 1 && k <= N, "k must be in [1, N]");
   OVG_REQUIRE(extrinsics && ranking && dists, "null extrinsics / ranking / dists");
-  long long bytes = 0;
-  ovg::RankParams p = ranking_workspace(workspace, N, out_f64, &bytes);
-  OVG_REQUIRE(workspace_ok(workspace, workspace_bytes, bytes, 256),
-              "workspace must be 256-byte aligned and ovg_ranking_workspace_bytes(N, out_f64) long");
+  ovg::RankParams p;
+  int rc = carve(__func__, "ovg_ranking_workspace_bytes(N, out_f64)", workspace, workspace_bytes, &p, ranking_layout, N,
+                 out_f64);
+  if (rc) return rc;
   p.ext = extrinsics; p.s0 = view_stride; p.s1 = row_stride; p.s2 = col_stride;
   p.ranking = ranking; p.dists = dists; p.lambda = lambda_t;
   p.N = static_cast<int>(N); p.k = static_cast<int>(k);
   p.in_f64 = in_f64 ? 1 : 0; p.out_f64 = out_f64 ? 1 : 0; p.normalize = normalize ? 1 : 0;
   cudaStream_t st = reinterpret_cast<cudaStream_t>(stream);
   ovg::rank_prep_kernel<<<1, ovg::RANK_PREP_THREADS, 0, st>>>(p);
-  const int rc = post_launch("ovg_compute_ranking(prep)");
+  rc = post_launch("ovg_compute_ranking(prep)");
   if (rc) return rc;
   return p.out_f64 ? launch_ranking<double, unsigned long long>(p, st) : launch_ranking<float, unsigned>(p, st);
 }
@@ -1699,16 +1674,13 @@ int ovg_compute_ranking(const void* extrinsics, int in_f64, long long N, long lo
 // ------------------------------------------------------------------------------------------------------ Sim(3) alignment
 namespace {
 
-// Sim(3) workspace, carved the same way by the size query and by the entry point: the partials of the three passes and the
-// solved transform.  Its size does not depend on n.
-ovg::Sim3Params sim3_workspace(void* base, long long* bytes) {
-  Arena ar(base, 0);
+// The partials of the three passes and the solved transform.  Its size does not depend on n.
+ovg::Sim3Params sim3_layout(Arena& ar) {
   ovg::Sim3Params p{};
   p.part0 = ar.get<double>(ovg::SIM3_BLOCKS * ovg::SIM3_P0);
   p.part1 = ar.get<double>(ovg::SIM3_BLOCKS * ovg::SIM3_P1);
   p.part2 = ar.get<double>(ovg::SIM3_BLOCKS);
   p.solved = ar.get<double>(12);
-  *bytes = ar.bytes();
   return p;
 }
 
@@ -1717,10 +1689,7 @@ ovg::Sim3Params sim3_workspace(void* base, long long* bytes) {
 extern "C" {
 
 long long ovg_sim3_workspace_bytes(long long n) {
-  if (n < 0) return -1;
-  long long bytes = 0;
-  sim3_workspace(nullptr, &bytes);
-  return bytes;
+  return n >= 0 ? layout_bytes(sim3_layout) : -1;
 }
 
 int ovg_sim3_estimate(const float* src, const float* dst, const unsigned char* keep, long long n, void* workspace,
@@ -1728,14 +1697,13 @@ int ovg_sim3_estimate(const float* src, const float* dst, const unsigned char* k
   OVG_REQUIRE(n >= 0, "n must be >= 0");
   OVG_REQUIRE((src && dst) || n == 0, "null src / dst");
   OVG_REQUIRE(out_sim3 && out_stats, "null out_sim3 / out_stats");
-  long long bytes = 0;
-  ovg::Sim3Params p = sim3_workspace(workspace, &bytes);
-  OVG_REQUIRE(workspace_ok(workspace, workspace_bytes, bytes, 256),
-              "workspace must be 256-byte aligned and ovg_sim3_workspace_bytes(n) long");
+  ovg::Sim3Params p;
+  int rc = carve(__func__, "ovg_sim3_workspace_bytes(n)", workspace, workspace_bytes, &p, sim3_layout);
+  if (rc) return rc;
   p.src = src; p.dst = dst; p.keep = keep; p.n = n; p.sim3 = out_sim3; p.stats = out_stats;
   cudaStream_t st = reinterpret_cast<cudaStream_t>(stream);
   ovg::sim3_means_kernel<<<ovg::SIM3_BLOCKS, ovg::SIM3_THREADS, 0, st>>>(p);
-  int rc = post_launch("ovg_sim3_estimate(means)");
+  rc = post_launch("ovg_sim3_estimate(means)");
   if (rc) return rc;
   ovg::sim3_moments_kernel<<<ovg::SIM3_BLOCKS, ovg::SIM3_THREADS, 0, st>>>(p);
   if ((rc = post_launch("ovg_sim3_estimate(moments)"))) return rc;
@@ -1802,7 +1770,7 @@ long long ovg_jpeg_plan_segments(const ovg_jpeg_plan* plan) { return plan ? stat
 int ovg_jpeg_plan_rounds(const ovg_jpeg_plan* plan) { return plan ? plan->rounds : -1; }
 
 long long ovg_jpeg_plan_workspace_bytes(const ovg_jpeg_plan* plan) {
-  return plan ? ovg::jpg::plan_workspace(plan, static_cast<int>(plan->route.size()), nullptr).bytes : -1;
+  return plan ? layout_bytes(ovg::jpg::plan_layout, plan, static_cast<int>(plan->route.size())) : -1;
 }
 
 int ovg_jpeg_plan_segment(const ovg_jpeg_plan* plan, long long k, int* file, long long* offset, long long* nbytes, int* first_mcu,
@@ -1832,10 +1800,10 @@ int ovg_jpeg_decode(ovg_jpeg_plan* plan, const void* d_stream, unsigned char* co
   if (n) OVG_CUDA(cudaMemsetAsync(d_status, 0, sizeof(unsigned) * n, st));
   plan->rounds = 0;
   if (plan->files.empty()) return OVG_OK;
-  OVG_REQUIRE(d_stream && d_out && workspace && (reinterpret_cast<uintptr_t>(d_stream) & 255) == 0 &&
-              (reinterpret_cast<uintptr_t>(workspace) & 255) == 0, "stream and workspace must be 256-byte aligned");
-  const Workspace w = plan_workspace(plan, n, workspace);
-  OVG_REQUIRE(workspace_bytes >= w.bytes, "workspace smaller than ovg_jpeg_plan_workspace_bytes()");
+  OVG_REQUIRE(d_stream && d_out && (reinterpret_cast<uintptr_t>(d_stream) & 255) == 0, "stream must be 256-byte aligned");
+  Workspace w;
+  int rc = carve(__func__, "ovg_jpeg_plan_workspace_bytes()", workspace, workspace_bytes, &w, plan_layout, plan, n);
+  if (rc) return rc;
   for (const FileDev& f : plan->files) OVG_REQUIRE(d_out[f.out_index], "null output for a device-routed file");
   const uint8_t* base = static_cast<const uint8_t*>(d_stream);
   Params p;
@@ -1857,7 +1825,7 @@ int ovg_jpeg_decode(ovg_jpeg_plan* plan, const void* d_stream, unsigned char* co
   for (long long r = 0; r <= plan->nsub; ++r) {
     OVG_CUDA(cudaMemsetAsync(w.changed, 0, 4, st));
     jpeg_sync_kernel<<<sub_grid, 256, 0, st>>>(p);
-    int rc = post_launch("ovg_jpeg_decode(sync)");
+    rc = post_launch("ovg_jpeg_decode(sync)");
     if (rc) return rc;
     int changed = 0;
     OVG_CUDA(cudaMemcpyAsync(&changed, w.changed, 4, cudaMemcpyDeviceToHost, st));
@@ -1867,7 +1835,7 @@ int ovg_jpeg_decode(ovg_jpeg_plan* plan, const void* d_stream, unsigned char* co
   }
   const long long nsub_chunks = (plan->nsub + SCAN_CHUNK - 1) / SCAN_CHUNK;
   jpeg_count_scan_local_kernel<<<static_cast<unsigned>(nsub_chunks), SCAN_CHUNK, 0, st>>>(p);
-  int rc = post_launch("ovg_jpeg_decode(count scan)");
+  rc = post_launch("ovg_jpeg_decode(count scan)");
   if (rc) return rc;
   jpeg_count_scan_chunks_kernel<<<1, SCAN_CHUNK, 0, st>>>(w.chunk, nsub_chunks);
   if ((rc = post_launch("ovg_jpeg_decode(count scan chunks)"))) return rc;
