@@ -111,6 +111,8 @@ __host__ __device__ constexpr int ba_pk(int i, int j) { return i * (i + 1) / 2 +
 __device__ __forceinline__ double ba_rho(const BaParams& p, double s) { return p.cauchy ? p.c2 * log1p(s / p.c2) : s; }
 __device__ __forceinline__ double ba_weight(const BaParams& p, double s) { return p.cauchy ? 1.0 / (1.0 + s / p.c2) : 1.0; }
 __device__ __forceinline__ double ba_clamp(double d) { return fmin(fmax(d, 1e-6), 1e32); }
+// |g| for the gradient test, NaN as +inf: fmax drops a NaN, and a NaN gradient must not pass for a small one
+__device__ __forceinline__ double ba_gabs(double g) { return isnan(g) ? __longlong_as_double(0x7ff0000000000000LL) : fabs(g); }
 
 // Fixed-order sum of one value per thread over a block of BA_PCG_THREADS (or fewer, whole warps); every thread gets it.
 template <int T>
@@ -451,7 +453,7 @@ __global__ void __launch_bounds__(BA_THREADS) ba_track_kernel(const BaParams p) 
       inv[6] = Cc / det; inv[7] = D / det; inv[8] = F / det;
 #pragma unroll
       for (int r = 0; r < 3; ++r) y[r] = inv[3 * r] * g[0] + inv[3 * r + 1] * g[1] + inv[3 * r + 2] * g[2];
-      gm = fmax(fabs(g[0]), fmax(fabs(g[1]), fabs(g[2])));
+      gm = fmax(ba_gabs(g[0]), fmax(ba_gabs(g[1]), ba_gabs(g[2])));
     }
 #pragma unroll
     for (int k = 0; k < 9; ++k) p.vinv[9 * t + k] = inv[k];
@@ -607,7 +609,7 @@ __global__ void __launch_bounds__(BA_PCG_THREADS) ba_pcg_kernel(const BaParams p
   // gradient test: |g|inf over the points (per-block maxima) and the cameras
   double gm = 0.0;
   for (int i = threadIdx.x; i < p.tblocks; i += BA_PCG_THREADS) gm = fmax(gm, p.gmax[i]);
-  for (int i = threadIdx.x; i < V * BA_NP; i += BA_PCG_THREADS) gm = fmax(gm, fabs(p.vsum[(i / BA_NP) * BA_ENTRIES + 72 + i % BA_NP]));
+  for (int i = threadIdx.x; i < V * BA_NP; i += BA_PCG_THREADS) gm = fmax(gm, ba_gabs(p.vsum[(i / BA_NP) * BA_ENTRIES + 72 + i % BA_NP]));
   gm = ba_block_max<BA_PCG_THREADS>(gm, red);
   if (gm <= 1e-10) {
     if (blockIdx.x == 0 && threadIdx.x == 0) s->small = 1;

@@ -61,6 +61,11 @@ def inv3_sym(H):
     return out / det[:, None, None]
 
 
+def scatter(index, values, size):
+    """Sums of the rows of values [k, c] by index [k] into [size, c], each sum in row order (np.add.at's order, faster)."""
+    return np.stack([np.bincount(index, values[:, j], size) for j in range(values.shape[1])], 1)
+
+
 class Problem:
     """The fixed parts of one call: observations, the gauge mask and the refined tracks."""
 
@@ -138,7 +143,8 @@ def bundle_adjust(points, offsets, view, obs, ext, intr, iterations=100, refine_
         np.add.at(U, vo, w[:, None, None] * np.einsum("ori,orj->oij", jc, jc))
         gc = np.zeros((V, NP))
         np.add.at(gc, vo, w[:, None] * np.einsum("ori,or->oi", jc, r))
-        if max(np.abs(gp[pr.incl]).max(initial=0.0), np.abs(gc).max()) <= 1e-10:
+        g = np.abs(np.r_[gp[pr.incl].ravel(), gc.ravel()])
+        if not np.isnan(g).any() and g.max() <= 1e-10:           # a NaN gradient is not a small one
             res["status"] = 0
             break
         Dp = np.clip(np.diagonal(Hp, axis1=1, axis2=2), 1e-6, 1e32)
@@ -153,17 +159,16 @@ def bundle_adjust(points, offsets, view, obs, ext, intr, iterations=100, refine_
         b = -gc.copy()
         np.add.at(b, vo, np.einsum("oia,oa->oi", W, y[to]))
         Lc = np.linalg.cholesky(Svv)
+        LcT = np.swapaxes(Lc, 1, 2)
 
-        def precond(rv):
-            return np.stack([np.linalg.solve(Lc[v].T, np.linalg.solve(Lc[v], rv[v])) for v in range(V)])
+        def precond(rv):                                # per view, the same LAPACK solves as one call each
+            return np.linalg.solve(LcT, np.linalg.solve(Lc, rv[:, :, None]))[:, :, 0]
 
-        def apply_s(pv):
-            s = np.zeros((n, 3))
-            np.add.at(s, to, np.einsum("oia,oi->oa", W, pv[vo]))
-            z = np.einsum("pij,pj->pi", Vinv, s)
-            q = np.einsum("vij,vj->vi", Us, pv)
-            np.add.at(q, vo, -np.einsum("oia,oa->oi", W, z[to]))
-            return q
+        q_index = np.r_[np.arange(V), vo]
+
+        def apply_s(pv):                                # q = U* p, then each - W z term added in observation order
+            z = np.einsum("pij,pj->pi", Vinv, scatter(to, np.einsum("oia,oi->oa", W, pv[vo]), n))
+            return scatter(q_index, np.r_[np.einsum("vij,vj->vi", Us, pv), -np.einsum("oia,oa->oi", W, z[to])], V)
 
         x = np.zeros((V, NP))
         rr_ = b.copy()

@@ -219,6 +219,12 @@ def _oracle(inp, **kw):
 RTOL = 1e-7                   # final points and cameras, device against oracle, relative to each array's largest value
 
 
+def max_rel_diff(a, b):
+    """Largest |a - b| over the largest finite |b|; equal entries (equal infinities too) differ by 0, a NaN fails."""
+    d = np.where(a == b, 0.0, np.abs(a - b))
+    return d.max() / np.abs(b[np.isfinite(b)]).max(initial=0.0)
+
+
 def _assert_matches(got, want, iterations):
     pts, ext, intr, err, cost, stats, trace = (t.cpu().numpy() for t in got)
     steps, acc, pcg, status = stats.tolist()
@@ -229,7 +235,7 @@ def _assert_matches(got, want, iterations):
     assert np.isnan(trace[steps:]).all()
     np.testing.assert_allclose(cost, want["cost"], rtol=1e-9, atol=0)
     for a, b in ((pts, want["points"]), (ext, want["extrinsic"]), (intr, want["intrinsic"])):
-        assert np.abs(a - b).max() <= RTOL * np.abs(b).max(), np.abs(a - b).max() / np.abs(b).max()
+        assert max_rel_diff(a, b) <= RTOL, max_rel_diff(a, b)
     fin = np.isfinite(want["error"])
     assert np.array_equal(np.isfinite(err), fin)
     np.testing.assert_allclose(err[fin], want["error"][fin], rtol=1e-6, atol=1e-9)
