@@ -197,7 +197,11 @@ int ovg_pose_decode(const float* pose_enc, float* extrinsic, float* intrinsic, f
 int ovg_unproject_depth(const float* depth, const float* intrinsic, const float* cam2world, float* world, int K, int H, int W,
                         void* stream);
 
-/* ovg_conf_percentile_mask: threshold = numpy.percentile(conf, percent) (exact, linear interpolation),
+/* ovg_conf_percentile_mask: threshold = numpy.percentile(conf, percent) to the bit, as numpy >= 2 computes it for fp32 conf
+ * (method 'linear', every step rounded to fp32): q = percent / 100, vi = f32(n - 1) * q, lo / hi = the order statistics of
+ * ranks floor(vi) and floor(vi) + 1 (both n - 1 once vi >= f32(n - 1)), g = vi - floor(vi), d = hi - lo, threshold =
+ * g >= 0.5 ? hi - d (1 - g) : lo + d g (exact order statistics by radix select).  Any NaN in conf gives a NaN threshold,
+ * so the mask keeps nothing and the count is 0.
  * mask[i] = conf[i] >= threshold && conf[i] > floor (inference.py:132-133: floor = 0.1).  workspace: device scratch of
  * OVG_PERCENTILE_WORKSPACE_BYTES; threshold_out: device float; count_out: device u64 (kept elements) or NULL. */
 #define OVG_PERCENTILE_WORKSPACE_BYTES (6 * 8 + 512 * 4 + 4 * 4)
@@ -228,7 +232,7 @@ int ovg_point_cloud_gather(const float* points, const unsigned char* conf_mask, 
 int ovg_point_cloud_center(const float* points, long long n, void* workspace, long long workspace_bytes, float* center_out,
                            void* stream);
 /* ovg_point_cloud_scale: scale_out fp32 = || percentile(p, 95) - percentile(p, 5) || per axis over the n_kept columns of xyz
- * (visual_util.py:231-236), by the exact selection of ovg_conf_percentile_mask.  n_kept >= 1. */
+ * (visual_util.py:231-236), each percentile by ovg_conf_percentile_mask's selection and fp32 rule.  n_kept >= 1. */
 int ovg_point_cloud_scale(const float* xyz, long long n_kept, long long ld, void* workspace, long long workspace_bytes,
                           float* scale_out, void* stream);
 

@@ -698,27 +698,30 @@ int select_blocks(long long n) {
 }
 
 // The percentile's workspace of OVG_PERCENTILE_WORKSPACE_BYTES, packed (not carved at 256-byte boundaries):
-// 6 x u64 state | 512 x u32 histograms | 3 x f32 results.
+// 6 x u64 state | 512 x u32 histograms | 3 x f32 results | u32 NaN count.
 struct PercentileRegion {
   unsigned long long* state;
   unsigned int* hist;
   float* res;
+  unsigned int* nan;
 };
 
 PercentileRegion percentile_region(void* workspace) {
   unsigned long long* state = static_cast<unsigned long long*>(workspace);
   unsigned int* hist = reinterpret_cast<unsigned int*>(state + 6);
-  return {state, hist, reinterpret_cast<float*>(hist + 512)};
+  float* res = reinterpret_cast<float*>(hist + 512);
+  return {state, hist, res, reinterpret_cast<unsigned int*>(res + 3)};
 }
 
 // The 4 x (histogram, decide) passes of a radix selection whose ranks an init launch has set in the workspace's state.
-int radix_select_passes(const float* v, long long n, void* workspace, float* out3, float frac, const std::string& what,
+// nan: the region's NaN counter for a percentile (see ovg::SelectParams), or null for a bare selection.
+int radix_select_passes(const float* v, long long n, void* workspace, float* out3, unsigned int* nan, const std::string& what,
                         cudaStream_t st) {
   const PercentileRegion r = percentile_region(workspace);
   int rc = OVG_OK;
   const int blocks = select_blocks(n);
   for (int pass = 0; pass < 4; ++pass) {
-    ovg::SelectParams sp{v, n, r.state, r.hist, pass, out3, frac};
+    ovg::SelectParams sp{v, n, r.state, r.hist, pass, out3, nan};
     ovg::select_hist_kernel<<<blocks, 256, 0, st>>>(sp);
     rc = post_launch((what + "(hist)").c_str());
     if (rc) return rc;
@@ -729,20 +732,16 @@ int radix_select_passes(const float* v, long long n, void* workspace, float* out
   return OVG_OK;
 }
 
-// numpy.percentile(v[0, n), percent) (method "linear", exact) by radix select: one init launch, then 4 x (histogram, decide).
-// workspace: a percentile_region; out3: device float[3] = the two neighbouring order statistics and the interpolated
-// percentile.  count (optional) is zeroed by the init launch.
+// numpy.percentile(v[0, n), percent) (method "linear", numpy >= 2's fp32 rule, exact) by radix select: one init launch that
+// takes the ranks and weight on the device, then 4 x (histogram, decide).  workspace: a percentile_region; out3: device
+// float[3] = the two neighbouring order statistics and the interpolated percentile, NaN if any v is NaN.  count (optional)
+// is zeroed by the init launch.
 int radix_percentile(const float* v, long long n, float percent, void* workspace, float* out3, unsigned long long* count,
                      const std::string& what, cudaStream_t st) {
-  // virtual index p/100 * (n - 1), linear interpolation between its two neighbours
-  const double vi = static_cast<double>(percent) / 100.0 * static_cast<double>(n - 1);
-  const unsigned long long r0 = static_cast<unsigned long long>(vi);
-  const unsigned long long r1 = r0 + 1 < static_cast<unsigned long long>(n) ? r0 + 1 : r0;
-  const double frac = vi - static_cast<double>(r0);
   const PercentileRegion r = percentile_region(workspace);
-  ovg::select_init_kernel<<<1, 128, 0, st>>>(r.state, r.hist, r0, r1, count);
+  ovg::select_init_kernel<<<1, 128, 0, st>>>(r.state, r.hist, n, percent, out3 + 2, r.nan, count);
   const int rc = post_launch((what + "(init)").c_str());
-  return rc ? rc : radix_select_passes(v, n, workspace, out3, static_cast<float>(frac), what, st);
+  return rc ? rc : radix_select_passes(v, n, workspace, out3, r.nan, what, st);
 }
 
 struct CloudBufs {
@@ -1432,8 +1431,9 @@ int ovg_tsdf_bounds(const float* points, const unsigned char* mask, int F, int H
   for (int j = 0; j < 6; ++j) {          // j = 2 axis + (0: 1st percentile, 1: 99th)
     ovg::tsdf_select_init_kernel<<<1, 128, 0, st>>>(r.state, r.hist, w.count, (j & 1) ? 99.f : 1.f, w.frac + j);
     if ((rc = post_launch("ovg_tsdf_bounds(init)"))) return rc;
-    // the decide step's own interpolation (frac 0) is unused: tsdf_bounds_kernel weighs the pair with the device's frac
-    if ((rc = radix_select_passes(w.cols + (j >> 1) * w.ld, n, w.select, w.sel + 3 * j, 0.f, "ovg_tsdf_bounds", st))) return rc;
+    // a bare selection: tsdf_bounds_kernel weighs the pair with the device's frac
+    if ((rc = radix_select_passes(w.cols + (j >> 1) * w.ld, n, w.select, w.sel + 3 * j, nullptr, "ovg_tsdf_bounds", st)))
+      return rc;
   }
   ovg::tsdf_bounds_kernel<<<1, 32, 0, st>>>(w.sel, w.frac, w.count, w.nonfinite, bounds_out);
   return post_launch("ovg_tsdf_bounds");

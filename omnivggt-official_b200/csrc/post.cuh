@@ -153,15 +153,36 @@ struct SelectParams {
   unsigned long long* state;   // [0..1] target ranks, [2..3] prefixes (as u64), [4..5] residual ranks
   unsigned int* hist;          // [2][256]
   int pass;                    // 0..3
-  float* out;                  // [2] selected values (written after the last pass), [2] = interpolated threshold
-  float frac;                  // linear interpolation weight between the two order statistics (numpy 'linear')
+  float* out;                  // [2] selected values (written after the last pass), [2] see nan
+  unsigned int* nan;           // a percentile's NaN count (pass 0 counts), or null: a bare selection that leaves out[2] alone.
+                               // With it, out[2] holds the interpolation weight from select_init_kernel until the last pass
+                               // replaces it by the percentile.
 };
 
-// Ranks, empty prefixes, zeroed histograms and kept-counter: one tiny launch instead of host-side copies (graph-capturable).
-__global__ void select_init_kernel(unsigned long long* state, unsigned int* hist, unsigned long long r0, unsigned long long r1,
-                                   unsigned long long* count) {
+// numpy >= 2's np.percentile(v[0, n), percent) of fp32 values and an fp32 percent takes its ranks and weight in fp32 (NEP 50):
+// q = percent / 100, vi = f32(n - 1) * q, ranks floor(vi) and f32(floor(vi) + 1) with weight g = vi - floor(vi); once
+// vi >= f32(n - 1) both ranks are n - 1 (numpy's index -1) and g = vi - (-1), which only decides the sign of a zero result.
+// Computed here with explicitly rounded operations, so no host compiler or contraction changes them.
+// Also zeroes the histograms, the NaN counter and the optional kept-counter: one tiny launch instead of host-side copies
+// (graph-capturable).  g goes to *weight, the out[2] of the selection.
+__global__ void select_init_kernel(unsigned long long* state, unsigned int* hist, long long n, float percent, float* weight,
+                                   unsigned int* nan, unsigned long long* count) {
   if (threadIdx.x == 0) {
+    const float last = __ll2float_rn(n - 1);
+    const float vi = __fmul_rn(last, __fdiv_rn(percent, 100.0f));
+    unsigned long long r0 = static_cast<unsigned long long>(n - 1), r1 = r0;
+    float g = __fadd_rn(vi, 1.0f);
+    if (vi < last) {
+      r0 = __float2ull_rd(vi);
+      // numpy's floor(vi) + 1 is an fp32 sum: above 2^24 it rounds to even, to r0 or r0 + 2.  r0 + 2 can be n (first at
+      // n = 2^24 + 4), where numpy itself fails with 'kth out of bounds'; the last rank is taken there.
+      r1 = __float2ull_rd(__fadd_rn(__ull2float_rn(r0), 1.0f));
+      if (r1 > static_cast<unsigned long long>(n - 1)) r1 = n - 1;
+      g = __fsub_rn(vi, __ull2float_rn(r0));
+    }
     state[0] = r0; state[1] = r1; state[2] = 0; state[3] = 0; state[4] = r0; state[5] = r1;
+    *weight = g;
+    *nan = 0;
     if (count) *count = 0;
   }
   for (int i = threadIdx.x; i < 512; i += blockDim.x) hist[i] = 0;
@@ -178,6 +199,7 @@ __global__ void __launch_bounds__(256) select_hist_kernel(const SelectParams p) 
   const bool same = pre0 == pre1;
   const long long n4 = p.n / 4;
   const float4* v4 = reinterpret_cast<const float4*>(p.v);
+  unsigned int nan = 0;
   for (long long i = blockIdx.x * static_cast<long long>(blockDim.x) + threadIdx.x; i < n4;
        i += static_cast<long long>(gridDim.x) * blockDim.x) {
     const float4 f = v4[i];
@@ -185,6 +207,7 @@ __global__ void __launch_bounds__(256) select_hist_kernel(const SelectParams p) 
 #pragma unroll
     for (int j = 0; j < 4; ++j) {
       const uint32_t key = f32_key(e[j]);
+      nan += isnan(e[j]);
       if ((key & mask_hi) == pre0) atomicAdd(&sh[0][(key >> shift) & 255], 1u);
       if (!same && (key & mask_hi) == pre1) atomicAdd(&sh[1][(key >> shift) & 255], 1u);
     }
@@ -192,9 +215,15 @@ __global__ void __launch_bounds__(256) select_hist_kernel(const SelectParams p) 
   if (blockIdx.x == 0) {
     for (long long i = n4 * 4 + threadIdx.x; i < p.n; i += blockDim.x) {
       const uint32_t key = f32_key(p.v[i]);
+      nan += isnan(p.v[i]);
       if ((key & mask_hi) == pre0) atomicAdd(&sh[0][(key >> shift) & 255], 1u);
       if (!same && (key & mask_hi) == pre1) atomicAdd(&sh[1][(key >> shift) & 255], 1u);
     }
+  }
+  if (p.nan && p.pass == 0) {          // NaN keys sort below -inf or above +inf; numpy's percentile of them is NaN
+#pragma unroll
+    for (int o = 16; o > 0; o >>= 1) nan += __shfl_xor_sync(0xffffffffu, nan, o);
+    if ((threadIdx.x & 31) == 0 && nan) atomicAdd(p.nan, nan);
   }
   __syncthreads();
   if (sh[0][threadIdx.x]) atomicAdd(&p.hist[threadIdx.x], sh[0][threadIdx.x]);
@@ -222,10 +251,13 @@ __global__ void select_decide_kernel(const SelectParams p) {
   }
   __syncwarp();
   for (int i = threadIdx.x; i < 512; i += 32) p.hist[i] = 0;
-  if (p.pass == 3 && threadIdx.x == 0) {
+  if (p.nan && p.pass == 3 && threadIdx.x == 0) {
     __threadfence_block();
-    const float lo = p.out[0], hi = p.out[1];
-    p.out[2] = lo + (hi - lo) * p.frac;          // numpy.percentile(method='linear'): lerp between the neighbours
+    // numpy's _lerp, each operation rounded on its own: g >= 0.5 ? hi - d (1 - g) : lo + d g, d = hi - lo
+    const float lo = p.out[0], hi = p.out[1], g = p.out[2];
+    const float d = __fsub_rn(hi, lo);
+    const float t = g >= 0.5f ? __fsub_rn(hi, __fmul_rn(d, __fsub_rn(1.0f, g))) : __fadd_rn(lo, __fmul_rn(d, g));
+    p.out[2] = *p.nan ? __int_as_float(0x7fc00000) : t;
   }
 }
 

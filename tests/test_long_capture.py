@@ -285,11 +285,6 @@ def test_sim3_apply_is_fp64_rounded_once():
         assert np.array_equal(outs[3].cpu().numpy(), ref["ext"])
 
 
-def _device_threshold(pct):
-    from omnivggt_official_b200 import ops
-    return lambda conf: ops.conf_percentile_mask(torch.from_numpy(np.ascontiguousarray(conf)).cuda(), pct, 1e-5)[1].item()
-
-
 def _raw_chunk(m, inp, a, b, didx, cidx):
     """model(...) on views a..b-1 with the re-indexed aux lists, decoded and unprojected, as numpy."""
     from omnivggt_official_b200 import ops
@@ -325,7 +320,7 @@ def test_reconstruct_mini(S, overlap, aux, tmp_path):
     raws = {c: _raw_chunk(m, inp, *c, didx, cidx) for c in chunks}
     got = {k: out[k][0].cpu().numpy() for k in SO.POINT_KEYS + SO.COPY_KEYS + ("depth", "extrinsic")}
     sims = out["sim3"].cpu().numpy()
-    ref = SO.merge(lambda a, b: raws[(a, b)], S, chunk, overlap, threshold=_device_threshold(50.0))
+    ref = SO.merge(lambda a, b: raws[(a, b)], S, chunk, overlap)
     for k, ((a, b), (n0, n1)) in enumerate(zip(chunks, SO.new_views(chunks))):
         r, new = raws[(a, b)], slice(n0 - a, b - a)
         if k == 0:
@@ -365,8 +360,7 @@ def test_reconstruct_pointmap_source_and_single_chunk():
     inp = {k: v.cuda() for k, v in make_inputs(1, 13, 56, 56, seed=77).items()}
     out = m.reconstruct(**inp, chunk=8, overlap=3, source="pointmap", conf_percent=30.0)
     raws = {c: _raw_chunk(m, inp, *c, None, None) for c in out["chunks"]}
-    ref = SO.merge(lambda a, b: raws[(a, b)], 13, 8, 3, source="pointmap", conf_percent=30.0,
-                   threshold=_device_threshold(30.0))
+    ref = SO.merge(lambda a, b: raws[(a, b)], 13, 8, 3, source="pointmap", conf_percent=30.0)
     for k in range(1, len(out["chunks"])):
         assert _rel(out["sim3"][k].cpu().numpy(), ref["sim3"][k]) < 1e-9
     one = m.reconstruct(**{k: v[:, :6] for k, v in inp.items()}, chunk=8, overlap=3)      # S <= chunk: the plain forward

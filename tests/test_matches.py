@@ -13,6 +13,7 @@ import torch
 
 from conftest import GOLDEN
 from oracle import matches_oracle as MO
+from oracle import postprocess_oracle as PO
 from oracle.make_golden_matches import make_cases, surface_views
 from ovg_support import install, sha256
 
@@ -171,7 +172,7 @@ def test_two_518_views_against_ckdtree():
 def test_scene_all_pairs_equal_per_pair_calls():
     """S = 24: every pair of one batched call equals find_reciprocal_matches on the kept points of the two views; the call's
     kernel launches do not depend on the number of pairs."""
-    from omnivggt_official_b200 import OmniVGGT, _lib, ops
+    from omnivggt_official_b200 import OmniVGGT, _lib
     from omnivggt_official_b200.geometry import find_reciprocal_matches
     S, H, W = 24, 30, 40
     pred = {k: v.cuda() for k, v in _scene(S, H, W).items()}
@@ -182,8 +183,7 @@ def test_scene_all_pairs_equal_per_pair_calls():
     out = OmniVGGT.matches(pred, conf_percent=30.0)
     n2 = lib.ovg_launch_count()
     assert len(out) == S * (S - 1) // 2 and n2 - n1 == n1 - n0
-    mask, _, _ = ops.conf_percentile_mask(pred["depth_conf"][0].contiguous(), 30.0, 1e-5)
-    keep = mask.bool().view(S, -1)
+    keep = torch.from_numpy(PO.conf_percentile_mask(pred["depth_conf"][0].cpu().numpy(), 30.0, 1e-5)[0]).cuda().view(S, -1)
     pts = pred["world_points_from_depth"][0].reshape(S, -1, 3)
     grid = torch.from_numpy(MO.xy_grid(W, H).reshape(-1, 2)).cuda()
     pairs = [(i, j) for i in range(S) for j in range(i + 1, S)]
@@ -241,7 +241,6 @@ def test_identical_views_match_every_pixel_to_itself():
 @pytest.mark.gpu
 def test_model_matches_api():
     from test_model_gpu import model
-    from omnivggt_official_b200 import ops
     from oracle.synth import make_inputs
     m = model("mini_conv")
     inp = {k: v.cuda() for k, v in make_inputs(1, 3, 56, 56, seed=4).items()}
@@ -251,8 +250,7 @@ def test_model_matches_api():
         out = m.matches(pred, source=source, conf_percent=25.0)
         assert len(out) == 3
         key, ckey = ("world_points_from_depth", "depth_conf") if source == "depth" else ("world_points", "world_points_conf")
-        mask, _, _ = ops.conf_percentile_mask(pred[ckey][0].float().contiguous(), 25.0, 1e-5)    # the mask matches() uses
-        keep = mask.bool().cpu().numpy()
+        keep, _ = PO.conf_percentile_mask(pred[ckey][0].float().cpu().numpy(), 25.0, 1e-5)      # numpy's, to the bit
         ref = MO.scene_matches(pred[key][0].float().cpu().numpy(), keep, [(0, 1), (0, 2), (1, 2)])
         for o, r in zip(out, ref):
             assert o["count"] == r["count"]

@@ -194,16 +194,14 @@ def test_errors_before_any_device_work(dry):
 
 # ------------------------------------------------------------------------------------------------------------------ GPU
 def _check_device_against_oracle(d, world, conf, images, ext, pct, frame, black, white, layout):
-    """Bit-equal to the oracle at the device's threshold (within 1e-6 of numpy's; see test_point_cloud)."""
-    o = MO.mesh(world, conf, images, ext, pct, 1e-5, frame, black, white, layout=layout)
-    t_ref = float(o["conf_threshold"])
-    assert abs(float(d["conf_threshold"]) - t_ref) <= 1e-6 * abs(t_ref)
-    od = MO.mesh(world, conf, images, ext, pct, 1e-5, frame, black, white, layout=layout, threshold=d["conf_threshold"])
+    """numpy's threshold to the bit, and bit-equal to the oracle."""
+    od = MO.mesh(world, conf, images, ext, pct, 1e-5, frame, black, white, layout=layout)
+    assert float(d["conf_threshold"]) == float(od["conf_threshold"]), (d["conf_threshold"], od["conf_threshold"])
     keys = KEYS if layout == "reference" else ("positions", "colors", "indices")
     for k in keys:
         assert d[k].dtype == od[k].dtype and np.array_equal(d[k], od[k]), k
     assert np.abs(d["align"] - od["align"]).max() <= 1e-6
-    return od, float(d["conf_threshold"]) == t_ref
+    return od
 
 
 @pytest.mark.gpu
@@ -216,8 +214,8 @@ def test_device_mesh_matches_oracle_and_golden(i, layout):
     world, conf = _source(g, src)
     d = _np(OmniVGGT.mesh(_pred(g), source=src, conf_percent=pct, frame=frame, mask_black_bg=black, mask_white_bg=white,
                           layout=layout))
-    _, same_thr = _check_device_against_oracle(d, world, conf, g["images"], g["extrinsic"], pct, frame, black, white, layout)
-    if layout == "reference" and same_thr:
+    _check_device_against_oracle(d, world, conf, g["images"], g["extrinsic"], pct, frame, black, white, layout)
+    if layout == "reference":
         _check_golden(f"glb{i}", d)
 
 
@@ -314,7 +312,7 @@ def test_model_mesh_api_and_glb_bytes():
         assert torch.equal(ref[k], direct[k]), k
     _check_device_against_oracle(_np(ref), world, conf, images, ext, 25.0, None, True, False, "reference")
     glb = _np(m.mesh(pred, conf_percent=25.0, mask_black_bg=True, layout="glb"))
-    od, _ = _check_device_against_oracle(glb, world, conf, images, ext, 25.0, None, True, False, "glb")
+    od = _check_device_against_oracle(glb, world, conf, images, ext, 25.0, None, True, False, "glb")
     assert len(glb["indices"]) > 0
     assert mesh_glb_bytes(glb) == mesh_glb_bytes({**od, "align": glb["align"]})
     cloud = m.point_cloud(pred, conf_percent=25.0, mask_black_bg=True)

@@ -168,17 +168,9 @@ def _device_cloud(world, conf, images, extrinsic, **kw):
 
 
 def _check_against_oracle(d, world, conf, images, extrinsic, pct, floor, frame, black, white):
-    """Bit-equal points / colours / frames for the device threshold; that threshold within 1e-6 of numpy's, and the kept
-    set differing from numpy's only by elements that tie with it."""
-    o = PC.point_cloud(world, conf, images, extrinsic, pct, floor, frame, black, white)
-    t_ref = float(o["conf_threshold"])
-    assert abs(float(d["conf_threshold"]) - t_ref) <= 1e-6 * abs(t_ref)
-    od = PC.point_cloud(world, conf, images, extrinsic, pct, floor, frame, black, white, threshold=d["conf_threshold"])
-    if len(od["points"]) != len(o["points"]):
-        c = conf if frame is None else conf[frame]
-        c = c.reshape(-1)
-        flips = (c >= np.float32(d["conf_threshold"])) != (c >= o["conf_threshold"])
-        assert (np.abs(c[flips] - t_ref) <= 1e-6 * abs(t_ref)).all()
+    """numpy's threshold to the bit, and bit-equal points / colours / frames."""
+    od = PC.point_cloud(world, conf, images, extrinsic, pct, floor, frame, black, white)
+    assert float(d["conf_threshold"]) == float(od["conf_threshold"]), (d["conf_threshold"], od["conf_threshold"])
     assert np.array_equal(d["points"], od["points"]) and np.array_equal(d["colors"], od["colors"])
     assert np.array_equal(d["frame"], od["frame"]) and d["frame"].dtype == np.int32
     pts = world if frame is None else world[frame]
@@ -199,7 +191,8 @@ def test_point_cloud_kernels_match_golden(i):
     _check_against_oracle(d, world, conf, g["images"], g["extrinsic"], pct, 1e-5, frame, black, white)
     if len(d["points"]) == 0:
         assert float(d["scale"]) == 1.0 and d["colors"].shape == (0, 3)
-    elif float(d["conf_threshold"]) == float(g[f"glb{i}_thr"]):
+    else:
+        assert float(d["conf_threshold"]) == float(g[f"glb{i}_thr"])
         assert len(d["points"]) == int(g[f"glb{i}_count"])
         assert sha256(d["points"], hex=False) == g[f"glb{i}_points_sha256"].tobytes()
         assert sha256(d["colors"], hex=False) == g[f"glb{i}_colors_sha256"].tobytes()

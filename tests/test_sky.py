@@ -337,14 +337,11 @@ def test_point_cloud_mask_sky_matches_reference_golden(i):
     d = OmniVGGT.point_cloud(pred, source=src, conf_percent=pct, frame=frame, mask_black_bg=black, mask_white_bg=white,
                              mask_sky=True)
     sky = SO.sky_of_views(g["images"])
-    t_ref = float(GOLD[f"glb{i}_thr"])
-    assert abs(float(d["conf_threshold"]) - t_ref) <= 1e-6 * abs(t_ref)
-    o = SO.point_cloud(world, conf, g["images"], g["extrinsic"], sky, pct, 1e-5, frame, black, white,
-                       threshold=float(d["conf_threshold"]))
+    assert float(d["conf_threshold"]) == float(GOLD[f"glb{i}_thr"])
+    o = SO.point_cloud(world, conf, g["images"], g["extrinsic"], sky, pct, 1e-5, frame, black, white)
     for k in ("points", "colors", "frame"):
         assert np.array_equal(d[k].cpu().numpy(), o[k]), (i, k)
-    if float(d["conf_threshold"]) == t_ref:
-        _check_glb_golden(i, d["points"].cpu().numpy(), d["colors"].cpu().numpy())
+    _check_glb_golden(i, d["points"].cpu().numpy(), d["colors"].cpu().numpy())
     explicit = OmniVGGT.point_cloud(pred, source=src, conf_percent=pct, frame=frame, mask_black_bg=black, mask_white_bg=white,
                                     mask_sky=OmniVGGT.sky_mask(pred))
     for k in d:
@@ -363,7 +360,7 @@ def test_mesh_and_matches_mask_sky_match_oracle_composition():
         for frame in (None, 1):
             d = OmniVGGT.mesh(pred, conf_percent=30.0, frame=frame, mask_white_bg=True, layout=layout, mask_sky=True)
             o = SO.mesh(g["world_points_from_depth"], g["depth_conf"], g["images"], g["extrinsic"], sky, 30.0, 1e-5, frame,
-                        False, True, layout, threshold=float(d["conf_threshold"]))
+                        False, True, layout)
             for k in (("vertices", "face_colors", "faces") if layout == "reference" else ("positions", "colors", "indices")):
                 assert np.array_equal(d[k].cpu().numpy(), o[k]), (layout, frame, k)
             e = OmniVGGT.mesh(pred, conf_percent=30.0, frame=frame, mask_white_bg=True, layout=layout, mask_sky=sky_t[None])
@@ -413,7 +410,7 @@ def test_model_point_cloud_mask_sky():
     world = pred["world_points_from_depth"][0].cpu().numpy()
     conf = pred["depth_conf"][0].cpu().numpy()
     ext = pred["extrinsic"][0].cpu().numpy()
-    o = SO.point_cloud(world, conf, images, ext, sky.cpu().numpy(), 25.0, 0.1, threshold=float(d["conf_threshold"]))
+    o = SO.point_cloud(world, conf, images, ext, sky.cpu().numpy(), 25.0, 0.1)
     for k in ("points", "colors", "frame"):
         assert np.array_equal(d[k].cpu().numpy(), o[k]), k
     assert len(d["points"]) > 0 and not (d["frame"] < 0).any()
