@@ -143,10 +143,10 @@ __device__ __forceinline__ void acc_ld32(const float* src, uint32_t* r) {
 }
 
 // One 128 x BN accumulator tile: smem -> registers -> fused epilogue -> global.  `arow` is this thread's row of the fp32
-// accumulator tile, `m` its global row; this thread owns the column chunks cfirst, cfirst + cstep, ... of the row.
+// accumulator tile, `m` its global row; this thread owns every column of the row.
 template <int BN, int EPI>
 __device__ __forceinline__ void epilogue_tile(const GemmParams& p, const float* arow, const int m, const int n0,
-                                              const int cfirst, const int cstep, const float* s_rope) {
+                                              const float* s_rope) {
   if constexpr (EPI == EPI_QKV) {
     // ---- per-row RoPE position (reference omnivggt_aggregator.py:215-224; layers/rope.py:39-59)
     int py = 0, px = 0;
@@ -170,7 +170,7 @@ __device__ __forceinline__ void epilogue_tile(const GemmParams& p, const float* 
     const long long seq = m / p.ntok;
     const long long tok = m % p.ntok;
     const int heads = p.C >> 6;
-    for (int c = cfirst; c < BN / 64; c += cstep) {
+    for (int c = 0; c < BN / 64; ++c) {
       const int n = n0 + c * 64;
       if (n >= p.N) continue;                                   // warp-uniform
       if (m < p.M) {
@@ -285,7 +285,7 @@ __device__ __forceinline__ void epilogue_tile(const GemmParams& p, const float* 
         interior = (yy >= 1 && yy <= p.gh && xx >= 1 && xx <= p.gw);
       }
     }
-    for (int c = cfirst; c < BN / 32; c += cstep) {
+    for (int c = 0; c < BN / 32; ++c) {
       const int n = n0 + c * 32;
       if (n >= p.N || !row_ok) continue;
       uint32_t raw[32];
@@ -570,129 +570,8 @@ gemm_kernel(const __grid_constant__ CUtensorMap tmA, const __grid_constant__ CUt
       const int n0 = (tile % n_tiles) * BN;
       named_sync(GEMM_BAR_ACC_FULL, 384);
       if constexpr (EPI == EPI_RESID) epilogue_resid_tile<BN>(p, sAcc, m0, n0, r >> 5, lane);
-      else epilogue_tile<BN, EPI>(p, sAcc + r * Cfg::ACC_LD, m0 + r, n0, 0, 1, s_rope);
+      else epilogue_tile<BN, EPI>(p, sAcc + r * Cfg::ACC_LD, m0 + r, n0, s_rope);
       if (tile + static_cast<int>(gridDim.x) < num_tiles) named_arrive(GEMM_BAR_ACC_FREE, 384);
-    }
-  }
-}
-
-// DPT output tail at full resolution (heads/dpt_head.py:121-126,:255-260) for the shapes the fused tail (tail.cuh) does not take:
-// 3x3 conv 128 -> 32 over the zero-bordered NHWC map + ReLU + 1x1 conv + activations.  With N = 32 the generic 9-tap path is bound
-// by L2->SM traffic: it re-loads the 128 x 64 A tile for every tap (18 loads of 16 KB per 128 output pixels).  Here the three
-// horizontal taps of one kernel row read ONE smem block of 136 rows through row-shifted wgmma descriptors (start address +
-// kx * 128 B), so a tile needs 6 A loads instead of 18, and the 72 KB of weights are loaded once per CTA and stay resident.
-constexpr int HT_A_ROWS = 136;
-constexpr int HT_A_BYTES = HT_A_ROWS * 128;          // 17 408 = 17 swizzle atoms
-constexpr int HT_STAGES = 6;
-constexpr int HT_B_TILE = 32 * 128;                  // one [32 x 64] 16-bit weight tile
-constexpr int HT_B_BYTES = 18 * HT_B_TILE;           // 9 taps x 2 K blocks
-constexpr int HT_ACC_LD = 36;
-constexpr int HT_SMEM_BYTES = HT_STAGES * HT_A_BYTES + HT_B_BYTES + GEMM_BM * HT_ACC_LD * 4 + 1024 + 256;
-constexpr int HT_THREADS = 384;   // producer warpgroup + 2 wgmma warpgroups that also run the epilogue
-
-__global__ void __launch_bounds__(HT_THREADS, 1)
-headtail_kernel(const __grid_constant__ CUtensorMap tmA, const __grid_constant__ CUtensorMap tmB, const GemmParams p) {
-  extern __shared__ uint8_t smem_raw[];
-  uint8_t* smem = reinterpret_cast<uint8_t*>((reinterpret_cast<uintptr_t>(smem_raw) + 1023) & ~uintptr_t(1023));
-  uint8_t* sA = smem;
-  uint8_t* sB = smem + HT_STAGES * HT_A_BYTES;
-  float* sAcc = reinterpret_cast<float*>(sB + HT_B_BYTES);
-  uint64_t* bars = reinterpret_cast<uint64_t*>(sAcc + GEMM_BM * HT_ACC_LD);
-  uint64_t* full = bars;
-  uint64_t* empty = bars + HT_STAGES;
-  uint64_t* bfull = bars + 2 * HT_STAGES;
-
-  const int warp = threadIdx.x >> 5;
-  const int lane = threadIdx.x & 31;
-  const int num_tiles = (p.M + GEMM_BM - 1) / GEMM_BM;
-
-  if (threadIdx.x == 0) {
-    tma_prefetch_desc(&tmA);
-    tma_prefetch_desc(&tmB);
-    for (int i = 0; i < HT_STAGES; ++i) {
-      mbar_init(&full[i], 1);
-      mbar_init(&empty[i], 8);     // one arrive per consumer warp
-    }
-    mbar_init(bfull, 1);
-    fence_barrier_init();
-  }
-  __syncthreads();
-
-  if (warp < 4) {
-    // ===================== TMA producer: weights once, then 3 kernel rows x 2 K blocks of 136 A rows per tile =====================
-    reg_dealloc<40>();
-    if (threadIdx.x == 0) {
-      mbar_expect_tx(bfull, HT_B_BYTES);
-      for (int t = 0; t < 18; ++t) tma_load_2d(sB + t * HT_B_TILE, &tmB, bfull, t * GEMM_BK, 0);
-      int s = 0;
-      uint32_t ph = 0;
-      for (int tile = blockIdx.x; tile < num_tiles; tile += gridDim.x) {
-        const int m0 = tile * GEMM_BM;
-        for (int ky = 0; ky < 3; ++ky) {
-          const int row0 = m0 + p.tap_off[ky * 3 + 1] - 1;     // first row the kx = 0 tap reads
-          for (int kb = 0; kb < 2; ++kb) {
-            mbar_wait_quiet(&empty[s], ph ^ 1);
-            mbar_expect_tx(&full[s], HT_A_BYTES);
-            tma_load_2d(sA + s * HT_A_BYTES, &tmA, &full[s], kb * GEMM_BK, row0);
-            if (++s == HT_STAGES) {
-              s = 0;
-              ph ^= 1;
-            }
-          }
-        }
-      }
-    }
-  } else {
-    // ===================== wgmma (64 rows per warpgroup) + HEADTAIL epilogue =====================
-    reg_alloc<232>();
-    const int cw = (warp >> 2) - 1;
-    const int e = warp - 4;
-    const int r = (e & 3) * 32 + lane;
-    const int frow = cw * 64 + (warp & 3) * 16 + (lane >> 2);
-    const int fcol = 2 * (lane & 3);
-    mbar_wait_quiet(bfull, 0);
-    int s = 0;
-    uint32_t ph = 0;
-    float acc[16];
-    for (int tile = blockIdx.x; tile < num_tiles; tile += gridDim.x) {
-      const int m0 = tile * GEMM_BM;
-      int prev = -1;
-      for (int ky = 0; ky < 3; ++ky) {
-        for (int kb = 0; kb < 2; ++kb) {
-          mbar_wait_quiet(&full[s], ph);
-          const uint32_t a_atom = smem_u32(sA + s * HT_A_BYTES + cw * 64 * 128);
-          wgmma_fence();
-#pragma unroll
-          for (int kx = 0; kx < 3; ++kx) {
-            const uint64_t adesc = make_sw128_desc_rows(a_atom, kx);
-            const uint64_t bdesc = make_sw128_desc(smem_u32(sB + ((ky * 3 + kx) * 2 + kb) * HT_B_TILE));
-#pragma unroll
-            for (int k = 0; k < GEMM_BK / 16; ++k) {
-              if (p.f16) wgmma_ss<32, true>(acc, adesc + 2 * k, bdesc + 2 * k, (ky | kb | kx | k) != 0);
-              else wgmma_ss<32, false>(acc, adesc + 2 * k, bdesc + 2 * k, (ky | kb | kx | k) != 0);
-            }
-          }
-          wgmma_commit();
-          wgmma_wait<1>();               // the previous A stage has been read: release it
-          if (prev >= 0 && lane == 0) mbar_arrive(&empty[prev]);
-          prev = s;
-          if (++s == HT_STAGES) {
-            s = 0;
-            ph ^= 1;
-          }
-        }
-      }
-      wgmma_wait<0>();
-      fence_regs<16>(acc);
-      if (lane == 0) mbar_arrive(&empty[prev]);
-      named_sync(1, 256);
-#pragma unroll
-      for (int j = 0; j < 4; ++j) {
-        *reinterpret_cast<float2*>(sAcc + frow * HT_ACC_LD + 8 * j + fcol) = make_float2(acc[4 * j], acc[4 * j + 1]);
-        *reinterpret_cast<float2*>(sAcc + (frow + 8) * HT_ACC_LD + 8 * j + fcol) = make_float2(acc[4 * j + 2], acc[4 * j + 3]);
-      }
-      named_sync(1, 256);
-      epilogue_tile<32, EPI_HEADTAIL>(p, sAcc + r * HT_ACC_LD, m0 + r, 0, e >> 2, 2, nullptr);
     }
   }
 }

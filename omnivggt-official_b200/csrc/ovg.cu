@@ -333,23 +333,9 @@ int ovg_gemm(const ovg_gemm_args* a, void* stream) {
   switch (a->epi) {
     case OVG_EPI_BF16: return dispatch_bn<ovg::EPI_BF16>(bn, ta, tb, p, st);
     case OVG_EPI_RESID: return dispatch_bn<ovg::EPI_RESID>(bn, ta, tb, p, st);
-    case OVG_EPI_QKV: return dispatch_bn<ovg::EPI_QKV>(bn, ta, tb, p, st);
-    case OVG_EPI_HEADTAIL: {
-      // row-shift kernel: 3x3 taps in row-major order over a 128-channel map ((ky, kx) -> tap_off = (ky-1)*pitch + kx-1)
-      bool shape_ok = a->num_taps == 9 && a->a_cols == 128 && a->n == 32;
-      for (int ky = 0; ky < 3 && shape_ok; ++ky)
-        shape_ok = a->tap_off[ky * 3 + 1] - a->tap_off[ky * 3] == 1 && a->tap_off[ky * 3 + 2] - a->tap_off[ky * 3 + 1] == 1;
-      if (!shape_ok) return launch_gemm<32, ovg::EPI_HEADTAIL>(ta, tb, p, st);
-      CUtensorMap ta136;
-      rc = get_map(a->a, a->a_cols, a->a_rows, 0, a->lda, ovg::HT_A_ROWS, &ta136);
-      if (rc) return rc;
-      rc = allow_dynamic_smem<ovg::headtail_kernel>(ovg::HT_SMEM_BYTES);
-      if (rc) return rc;
-      const int tiles = (p.M + ovg::GEMM_BM - 1) / ovg::GEMM_BM;
-      const int grid = tiles < num_sms() ? tiles : num_sms();
-      ovg::headtail_kernel<<<grid, ovg::HT_THREADS, ovg::HT_SMEM_BYTES, st>>>(ta136, tb, p);
-      return post_launch("ovg_gemm(headtail)");
-    }
+    case OVG_EPI_QKV:   // bn is 64 or 128 (raised above)
+      return bn == 128 ? launch_gemm<128, ovg::EPI_QKV>(ta, tb, p, st) : launch_gemm<64, ovg::EPI_QKV>(ta, tb, p, st);
+    case OVG_EPI_HEADTAIL: return launch_gemm<32, ovg::EPI_HEADTAIL>(ta, tb, p, st);
     default: return fail(OVG_E_INVALID, "ovg_gemm: unknown epilogue");
   }
 }

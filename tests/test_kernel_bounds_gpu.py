@@ -297,7 +297,7 @@ def test_gemm_qkv_norm_rope_per_element(C, frames, hp, wp, bn):
 @pytest.mark.parametrize("dtype", [BF16, F16])
 @pytest.mark.parametrize("outc,act", [(2, 0), (4, 1)])
 def test_headtail_per_element(outc, act, dtype):
-    """EPI_HEADTAIL (row-shift kernel): 3x3 conv 128 -> 32 + ReLU + 1x1 + activations, fp32 outputs, against the bound."""
+    """EPI_HEADTAIL (gemm_kernel<32, EPI_HEADTAIL>): 3x3 conv 128 -> 32 + ReLU + 1x1 + activations, fp32 outputs, against the bound."""
     ops = ops_module()
     Fr, h, w, Cin = 2, 14, 28, 128
     x = randn(Fr, h + 2, w + 2, Cin, seed=1)

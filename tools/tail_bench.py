@@ -1,4 +1,6 @@
-"""DPT output tail at the product shape (8 frames, 296^2 -> 518^2, 128 channels): fused kernel vs upsample + HEADTAIL (GPU box)."""
+"""DPT output tail at the product shape (8 frames, 296^2 -> 518^2, 128 channels): the fused kernel (ovg_dpt_tail), next to the
+two-kernel composition it replaced, ovg_upsample_bilinear + the generic gemm_kernel<32, EPI_HEADTAIL> (GPU box).  The model takes
+the fused kernel at this shape; the two-kernel leg is a point of comparison, not a path the product runs."""
 import json, os, sys
 import torch
 ROOT = os.path.dirname(os.path.dirname(os.path.abspath(__file__)))
