@@ -22,7 +22,7 @@ extern "C" {
 #define OVG_E_NODEVICE (-3)
 
 /* Library / device ------------------------------------------------------------------------------------- */
-int ovg_version(void);               /* ABI version, currently 4 */
+int ovg_version(void);               /* ABI version, currently 5 */
 const char* ovg_last_error(void);    /* thread-local message of the last failing call */
 int ovg_device_check(void);          /* OVG_OK iff the current device is sm_90 (H100); OVG_E_NODEVICE otherwise */
 long long ovg_launch_count(void);    /* kernels launched by this library since load (bench.py "gpu_launches") */
@@ -561,22 +561,25 @@ typedef struct ovg_aggregator ovg_aggregator;
 int ovg_aggregator_create(const ovg_aggregator_desc* desc, ovg_aggregator** out);
 void ovg_aggregator_destroy(ovg_aggregator* h);
 long long ovg_aggregator_workspace_bytes(const ovg_aggregator* h, int B, int S, int H, int W, int n_depth);
+typedef struct ovg_context_parallel ovg_context_parallel;     /* below, with ovg_peer_barrier */
 /* patch_tokens fp32 [B*S, P, C]; inj fp32 [depth+1, B*S, C] (camera injection vectors, omnivggt_aggregator.py:172-179,:273-287);
  * depth / mask fp32 [B,S,H,W] and depth_idx device int[n_depth] (n_depth = 0: no depth aux); rope tables fp32 [maxpos, 16];
- * slots: host array of 4 device pointers, bf16 [B*S, T, 2C] each (frame half | global half); cam_out fp32 [B*S, 2C]. */
-int ovg_aggregator_forward(ovg_aggregator* h, const float* patch_tokens, const float* inj, const float* depth, const float* mask,
-                           const int* depth_idx, int n_depth, const float* rope_cos, const float* rope_sin, int maxpos, int B,
-                           int S, int H, int W, void* workspace, long long workspace_bytes, void* const* slots, float* cam_out,
-                           void* stream);
-/* As ovg_aggregator_forward, and additionally exports layers in fp32, as the reference's aggregator returns them
- * (models/omnivggt_aggregator.py:248-256: aggregated_tokens_list, one [B, S, T, 2C] tensor per layer, frame half | global half).
- * layers: host array of `depth` device pointers, fp32 [B*S, T, 2C] each; NULL entries are not exported.  Each layer is written in
- * the same pass that makes its bf16 snapshot.  Entries of slots may be NULL (that slot is not written); with all four NULL and no
- * layer exported, the call produces cam_out only (the input of the camera head, heads/camera_head.py:96-99). */
-int ovg_aggregator_forward_layers(ovg_aggregator* h, const float* patch_tokens, const float* inj, const float* depth,
-                                  const float* mask, const int* depth_idx, int n_depth, const float* rope_cos, const float* rope_sin,
-                                  int maxpos, int B, int S, int H, int W, void* workspace, long long workspace_bytes,
-                                  void* const* slots, float* cam_out, float* const* layers, void* stream);
+ * slots: host array of 4 device pointers, bf16 [B*S, T, 2C] each (frame half | global half); cam_out fp32 [B*S, 2C].  Entries of
+ * slots may be NULL (that slot is not written); with all four NULL and no layer exported, the call produces cam_out only (the
+ * input of the camera head, heads/camera_head.py:96-99).
+ * layers: NULL (no export), or a host array of `depth` device pointers, fp32 [B*S, T, 2C] each, NULL entries not exported: the
+ * layers as the reference's aggregator returns them (models/omnivggt_aggregator.py:248-256: aggregated_tokens_list, one
+ * [B, S, T, 2C] tensor per layer, frame half | global half).  Each layer is written in the same pass that makes its bf16 snapshot.
+ * cp: NULL on one GPU; depth_idx_local must then be NULL and n_depth_local 0.  Non-NULL: B = 1 and S = the LOCAL view count, except
+ * for the depth modality, whose normalisation is global over the scene: depth / mask are the FULL tensors [1, views_total, H, W],
+ * depth_idx lists ALL selected views (scene indices, n_depth of them) and depth_idx_local the selected views this rank owns (scene
+ * indices, n_depth_local of them); cam_out holds this rank's rows [S, 2C], the camera tokens of all views land in
+ * cp->cam_peers[rank].  cp and layers are refused together. */
+int ovg_aggregator_forward(ovg_aggregator* h, const ovg_context_parallel* cp, const float* patch_tokens, const float* inj,
+                           const float* depth, const float* mask, const int* depth_idx, int n_depth,
+                           const int* depth_idx_local, int n_depth_local, const float* rope_cos, const float* rope_sin,
+                           int maxpos, int B, int S, int H, int W, void* workspace, long long workspace_bytes,
+                           void* const* slots, float* cam_out, float* const* layers, void* stream);
 
 /* Frozen DINOv2 patchifier on the same kernels: reference layers/vision_transformer.py:214-271. */
 typedef struct ovg_dino_desc {
@@ -618,20 +621,16 @@ typedef struct ovg_dpt ovg_dpt;
 int ovg_dpt_create(const ovg_dpt_desc* desc, ovg_dpt** out);
 void ovg_dpt_destroy(ovg_dpt* h);
 long long ovg_dpt_workspace_bytes(const ovg_dpt* h, int Fc, int H, int W);
-/* One chunk of Fc frames starting at frame f0.  slots: host array of 4 device pointers, bf16 [K, T, C2]; tables: host array of 4
+/* One chunk of Fc frames starting at frame f0.  slots: host array of 4 device pointers, [K, T, C2] each, bf16 if slots_f32 is 0;
+ * if it is 1, fp32 -- the layers the DPT head selects from an aggregated_tokens_list (heads/dpt_head.py:128-183,:212-229;
+ * DPTHead.forward) -- and the first LayerNorm rounds each element to bf16 (nearest even) as it loads it, so the results equal the
+ * bf16 call on the bf16 rounding of the same layers bit for bit; any other slots_f32 is refused.  tables: host array of 4
  * device pointers, fp32 [P, oc[l]] UV position embeddings x0.1 (heads/dpt_head.py:262-272); tx fp32 [W, feat/4], ty fp32
  * [H, feat/4] separable embedding of the full-resolution stage; head_act 0: exp (depth), 1: inverse-log (points);
  * preds fp32 [K, H, W, outc-1], conf fp32 [K, H, W] (written for frames f0 .. f0+Fc-1). */
-int ovg_dpt_forward(ovg_dpt* h, const void* const* slots, int T, int nspecial, int f0, int Fc, int H, int W,
+int ovg_dpt_forward(ovg_dpt* h, const void* const* slots, int slots_f32, int T, int nspecial, int f0, int Fc, int H, int W,
                     const float* const* tables, const float* tx, const float* ty, int head_act, float* preds, float* conf,
                     void* workspace, long long workspace_bytes, void* stream);
-/* As ovg_dpt_forward on fp32 layers: layers is a host array of 4 device pointers, fp32 [K, T, C2] -- the layers the DPT head
- * selects from an aggregated_tokens_list (heads/dpt_head.py:128-183,:212-229; DPTHead.forward).  The first LayerNorm rounds each
- * element to bf16 (nearest even) as it loads it, so the results equal ovg_dpt_forward on the bf16 rounding of the same layers
- * bit for bit. */
-int ovg_dpt_forward_f32(ovg_dpt* h, const float* const* layers, int T, int nspecial, int f0, int Fc, int H, int W,
-                        const float* const* tables, const float* tx, const float* ty, int head_act, float* preds, float* conf,
-                        void* workspace, long long workspace_bytes, void* stream);
 
 /* Camera head: iterative pose refinement on the camera tokens; reference heads/camera_head.py:83-154.  The weight-streaming
  * GEMMs run on the wgmma GEMM; AdaLN, the S-token attention (head_dim D / heads) and the 9-wide pose update are small fp32
@@ -666,7 +665,7 @@ int ovg_peer_barrier(int* const* flag_peers, int* epoch_counter, int rank, int w
  * straight into every rank's full-length K / V buffer over NVLink (ovg_gemm_args.k_peers), a flag barrier follows, and the
  * rank's own queries attend to all keys (ovg_attention with nq < nkv).  No collective library call on the data path; K / V buffers are
  * double buffered so that one barrier per global block suffices. */
-typedef struct ovg_context_parallel {
+struct ovg_context_parallel {
   int rank; int world;
   int views_total;                    /* views of the whole scene; this rank holds views [rank*S, rank*S + S), S = views_total / world */
   void* k_peers[2][8];                /* [buffer][rank]: bf16 [heads, views_total*T, 64] in rank's memory, peer mapped */
@@ -675,15 +674,7 @@ typedef struct ovg_context_parallel {
   int* epoch_counter;                 /* private device int, zero-initialised once */
   float* cam_peers[8];                /* [rank]: fp32 [views_total, 2C] camera tokens of ALL views (the camera head attends across
                                          views, heads/camera_head.py:104-154); every rank stores its rows into every peer */
-} ovg_context_parallel;
-/* As ovg_aggregator_forward with B = 1 and S = the LOCAL view count, except for the depth modality, whose normalisation is
- * global over the scene: depth / mask are the FULL tensors [1, views_total, H, W], depth_idx lists ALL selected views (scene
- * indices, n_depth of them) and depth_idx_local the selected views this rank owns (scene indices, n_depth_local of them). */
-int ovg_aggregator_forward_cp(ovg_aggregator* h, const ovg_context_parallel* cp, const float* patch_tokens, const float* inj,
-                              const float* depth, const float* mask, const int* depth_idx, int n_depth,
-                              const int* depth_idx_local, int n_depth_local, const float* rope_cos, const float* rope_sin,
-                              int maxpos, int S, int H, int W, void* workspace, long long workspace_bytes, void* const* slots,
-                              float* cam_out, void* stream);   /* cam_out: this rank's rows [S, 2C]; all views: cp->cam_peers[rank] */
+};
 
 /* Timing hook for bench.py: when enabled, every global-attention launch of ovg_aggregator_forward is bracketed by CUDA events
  * on its stream; after a synchronize, ovg_runtime_attention_times() returns the elapsed ms of the launches since the enable. */

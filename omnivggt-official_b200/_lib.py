@@ -100,8 +100,6 @@ EXPORTS = {
     "ovg_attention": (C.c_int, [_vp, _vp, _vp, _vp, _i, _i, _i, _i, _vp, _ll, _vp]),
     "ovg_attention_scratch_bytes": (C.c_longlong, []),
     "ovg_peer_barrier": (C.c_int, [C.POINTER(_vp), _vp, _i, _i, _vp]),
-    "ovg_aggregator_forward_cp": (C.c_int, [_vp, C.POINTER(ContextParallelDesc), _vp, _vp, _vp, _vp, _vp, _i, _vp, _i, _vp, _vp, _i,
-                                            _i, _i, _i, _vp, _ll, _pp, _vp, _vp]),
     "ovg_layernorm": (C.c_int, [_vp, _i, _ll, _vp, _i, _ll, _i, _i, _vp, _vp, _f, _i, _i, _i, _vp]),
     "ovg_image_im2col": (C.c_int, [_vp, _vp, _vp, _vp, _i, _i, _i, _i, _i, _vp]),
     "ovg_assemble_tokens": (C.c_int, [_vp, _vp, _vp, _vp, _vp, _vp, _vp, _i, _i, _i, _i, _i, _i, _vp]),
@@ -171,9 +169,8 @@ EXPORTS = {
     "ovg_aggregator_create": (C.c_int, [C.POINTER(AggregatorDesc), _pp]),
     "ovg_aggregator_destroy": (None, [_vp]),
     "ovg_aggregator_workspace_bytes": (_ll, [_vp, _i, _i, _i, _i, _i]),
-    "ovg_aggregator_forward": (C.c_int, [_vp, _vp, _vp, _vp, _vp, _vp, _i, _vp, _vp, _i, _i, _i, _i, _i, _vp, _ll, _pp, _vp, _vp]),
-    "ovg_aggregator_forward_layers": (C.c_int, [_vp, _vp, _vp, _vp, _vp, _vp, _i, _vp, _vp, _i, _i, _i, _i, _i, _vp, _ll, _pp, _vp,
-                                                _pp, _vp]),
+    "ovg_aggregator_forward": (C.c_int, [_vp, C.POINTER(ContextParallelDesc), _vp, _vp, _vp, _vp, _vp, _i, _vp, _i, _vp, _vp, _i,
+                                         _i, _i, _i, _i, _vp, _ll, _pp, _vp, _pp, _vp]),
     "ovg_dino_create": (C.c_int, [C.POINTER(DinoDesc), _pp]),
     "ovg_dino_destroy": (None, [_vp]),
     "ovg_dino_workspace_bytes": (_ll, [_vp, _i, _i, _i]),
@@ -181,8 +178,7 @@ EXPORTS = {
     "ovg_dpt_create": (C.c_int, [C.POINTER(DptDesc), _pp]),
     "ovg_dpt_destroy": (None, [_vp]),
     "ovg_dpt_workspace_bytes": (_ll, [_vp, _i, _i, _i]),
-    "ovg_dpt_forward": (C.c_int, [_vp, _pp, _i, _i, _i, _i, _i, _i, _pp, _vp, _vp, _i, _vp, _vp, _vp, _ll, _vp]),
-    "ovg_dpt_forward_f32": (C.c_int, [_vp, _pp, _i, _i, _i, _i, _i, _i, _pp, _vp, _vp, _i, _vp, _vp, _vp, _ll, _vp]),
+    "ovg_dpt_forward": (C.c_int, [_vp, _pp, _i, _i, _i, _i, _i, _i, _i, _pp, _vp, _vp, _i, _vp, _vp, _vp, _ll, _vp]),
     "ovg_camera_create": (C.c_int, [C.POINTER(CameraDesc), _pp]),
     "ovg_camera_destroy": (None, [_vp]),
     "ovg_camera_workspace_bytes": (_ll, [_vp, _i]),

@@ -208,7 +208,7 @@ int dispatch_bn(int bn, const CUtensorMap& ta, const CUtensorMap& tb, const ovg:
 
 extern "C" {
 
-int ovg_version(void) { return 4; }
+int ovg_version(void) { return 5; }
 const char* ovg_last_error(void) { return g_err.c_str(); }
 long long ovg_launch_count(void) { return g_launches.load(); }
 
@@ -401,7 +401,7 @@ int ovg_attention(const void* q, const void* k, const void* v, void* out, int ba
   return post_launch("ovg_attention(merge)");
 }
 
-// in_mode: ovg::LN_IN_F32, LN_IN_BF16 or LN_IN_F32_AS_BF16 (the last is internal: ovg_dpt_forward_f32 reads fp32 layers with it)
+// in_mode: ovg::LN_IN_F32, LN_IN_BF16 or LN_IN_F32_AS_BF16 (the last is internal: ovg_dpt_forward reads fp32 slots with it)
 static int layernorm(const void* in, int in_mode, long long ld_in, void* out, int out_is_f32, long long ld_out, int rows, int C,
                      const float* w, const float* b, float eps, int grp_out, int grp_in, int grp_off, void* stream) {
   OVG_REQUIRE(in && out && rows > 0, "null operand");
@@ -458,7 +458,7 @@ int ovg_peer_barrier(int* const* flag_peers, int* epoch_counter, int rank, int w
   return post_launch("ovg_peer_barrier");
 }
 
-// layer: fp32 [K*T, 2C] export of the same half (ovg_aggregator_forward_layers), or NULL
+// layer: fp32 [K*T, 2C] export of the same half (ovg_aggregator_forward's layers), or NULL
 static int inject_snapshot(float* x, const float* inj, void* slot, float* layer, float* cam_out, int K, int T, int C, int coff,
                            void* stream) {
   OVG_REQUIRE(x && K > 0 && T > 0 && C % 4 == 0, "bad arguments");

@@ -164,10 +164,9 @@ class OmniVGGT(nn.Module, PyTorchModelHubMixin):
                                                         camera_gt_index)
         eng = self.engine()
         args = (images, extrinsics, intrinsics, depth, mask, depth_idx, cam_idx)
-        impl = self._forward_cp if self._cp is not None else self._forward_impl
         if self.use_cuda_graph and images.is_cuda and not torch.cuda.is_current_stream_capturing():
-            return self._forward_graphed(eng, impl, *args)
-        return impl(eng, *args)
+            return self._forward_graphed(eng, *args)
+        return self._forward_impl(eng, *args)
 
     def _check_inputs(self, images, extrinsics, intrinsics, depth, mask, depth_gt_index, camera_gt_index):
         if images.dim() == 4:
@@ -200,42 +199,6 @@ class OmniVGGT(nn.Module, PyTorchModelHubMixin):
         self._cp = ContextParallel(next(self.parameters()).device, group)
         return self
 
-    def _forward_cp(self, eng, images, extrinsics, intrinsics, depth, mask, depth_idx, cam_idx):
-        cp = self._cp
-        B, S, Cin, H, W = images.shape
-        if B != 1:
-            raise ValueError("context parallelism shards the views of ONE scene (B = 1); use scene-level data parallelism for batches")
-        v0, n = cp.local_views(S)
-        sl = slice(v0, v0 + n)
-        ag = self.aggregator
-        if eng.dino is None:
-            raise RuntimeError("context parallelism runs the DINOv2 patchifier on the libovg runtime (dino_backend='ovg')")
-        P = (H // self.patch_size) * (W // self.patch_size)
-        pos = TP.dino_pos_embed(ag.patch_embed, P, H, W, self.patch_size).float()
-        patch = eng.dino_patchify(images[0, sl].float().contiguous(), pos, _RESNET_MEAN, _RESNET_STD)
-        # camera aux: pose normalisation is global over the selected views (omnivggt_aggregator.py:85-105), the inputs are a
-        # few hundred bytes per view and replicated, so every rank computes all injection vectors and keeps its columns
-        pose = rows = None
-        if len(cam_idx):
-            ci = eng.cached(("cam_idx", tuple(cam_idx)), lambda: torch.tensor(cam_idx))
-            rows = eng.cached(("cam_rows", 1, S, tuple(cam_idx)), lambda: torch.tensor(cam_idx))
-            pose = TP.aux_pose_encoding(extrinsics.index_select(1, ci), intrinsics.index_select(1, ci), H, W)
-        inj = TP.injection_vectors(eng.inj_pack, pose, cam_idx, 1, S, rows)[:, sl].contiguous()
-        # depth aux: full tensors + scene indices (the masked-mean normalisation is over all selected views of the scene)
-        heads = self._dpt_heads()
-        slots, cam_loc = eng.aggregate(patch, inj, depth, mask, depth_idx, 1, n, H, W, set(self.dpt_layers), cp=cp, views_total=S,
-                                       slots=bool(heads))
-        out: Dict[str, object] = {}
-        if self.camera_head is not None:   # [S, 2C] gathered by peer stores: the camera head attends across all views
-            pose_list = self._camera(eng, cp.cam_all, 1, S)
-            out["pose_enc"], out["pose_enc_list"] = pose_list[-1], pose_list
-        eng.warm_tables(H, W)
-        for name, act in heads:
-            preds, conf = eng.dpt(name, slots, self.dpt_layers, n, H, W, head_act=act)
-            self._put_dpt(out, name, preds, conf, 1, n, H, W)
-        out["images"], out["view_range"] = images[:, sl], (v0, v0 + n)
-        return out
-
     @staticmethod
     def _put_dpt(out, name, preds, conf, B, S, H, W):
         key = "depth" if name == "depth_head" else "world_points"
@@ -256,7 +219,7 @@ class OmniVGGT(nn.Module, PyTorchModelHubMixin):
                          ) -> Tuple[List[torch.Tensor], int]:
         """All ``depth`` layers in fp32 [B, S, T, 2C] (frame half | global half) and patch_start_idx = 1 + registers, as
         ZeroAggregator.forward returns them (omnivggt_aggregator.py:248-256).  Same patchifier, injection and kernels as
-        forward(); the layers are written by the snapshot pass of the aggregator (ovg_aggregator_forward_layers)."""
+        forward(); the layers are written by the snapshot pass of the aggregator."""
         images, depth_idx, cam_idx = self._check_inputs(images, extrinsics, intrinsics, depth, mask, depth_gt_index,
                                                         camera_gt_index)
         eng = self._component_engine()
@@ -426,7 +389,7 @@ class OmniVGGT(nn.Module, PyTorchModelHubMixin):
         return sim3, stats
 
     # ---------------------------------------------------------------------------------------------- CUDA graph replay
-    def _forward_graphed(self, eng, impl, images, extrinsics, intrinsics, depth, mask, depth_idx, cam_idx):
+    def _forward_graphed(self, eng, images, extrinsics, intrinsics, depth, mask, depth_idx, cam_idx):
         """Same computation, launched from a captured CUDA graph (a forward is >1000 kernel launches; issuing them from
         Python costs about as much host time as the GPU needs to run them).  A graph is captured the third time a
         (shape, index-list) signature is seen; inputs are copied into static buffers, outputs are cloned."""
@@ -434,7 +397,7 @@ class OmniVGGT(nn.Module, PyTorchModelHubMixin):
         def sig(t):
             return None if t is None else (tuple(t.shape), t.dtype)
         heads = tuple(getattr(self, n) is not None for n in _HEADS)
-        key = (impl.__name__, sig(images), tuple(depth_idx), tuple(cam_idx), sig(extrinsics) if need_c else None,
+        key = (self._cp is not None, sig(images), tuple(depth_idx), tuple(cam_idx), sig(extrinsics) if need_c else None,
                sig(intrinsics) if need_c else None, sig(depth) if need_d else None, sig(mask) if need_d else None, heads)
         ent = self._graphs.pop(key, None)
         if ent is None:
@@ -444,7 +407,7 @@ class OmniVGGT(nn.Module, PyTorchModelHubMixin):
         self._graphs[key] = ent                             # most recently used last
         ent["calls"] += 1
         if ent["graph"] is None and (ent["calls"] < 3 or ent.get("failed")):
-            return impl(eng, images, extrinsics, intrinsics, depth, mask, depth_idx, cam_idx)
+            return self._forward_impl(eng, images, extrinsics, intrinsics, depth, mask, depth_idx, cam_idx)
         dyn = [images, extrinsics if need_c else None, intrinsics if need_c else None, depth if need_d else None,
                mask if need_d else None]
         if ent["graph"] is None or ent["ws_version"] != eng.ws.version:
@@ -453,11 +416,11 @@ class OmniVGGT(nn.Module, PyTorchModelHubMixin):
                 s = torch.cuda.Stream()
                 s.wait_stream(torch.cuda.current_stream())
                 with torch.cuda.stream(s):      # allocator warm-up on a side stream, as the capture API requires
-                    impl(eng, *static, depth_idx, cam_idx)
+                    self._forward_impl(eng, *static, depth_idx, cam_idx)
                 torch.cuda.current_stream().wait_stream(s)
                 g = torch.cuda.CUDAGraph()
                 with torch.cuda.graph(g):
-                    out = impl(eng, *static, depth_idx, cam_idx)
+                    out = self._forward_impl(eng, *static, depth_idx, cam_idx)
                 ent.update(graph=g, static=static, out=out, ws_version=eng.ws.version)
             except torch.cuda.OutOfMemoryError as ex:
                 # the only failure that is a property of the call, not a bug: the private pool of one more graph does not fit.
@@ -467,7 +430,7 @@ class OmniVGGT(nn.Module, PyTorchModelHubMixin):
                 warnings.warn(f"OmniVGGT: no memory for another CUDA graph ({ex}); this signature keeps eager launches")
                 torch.cuda.synchronize()
                 torch.cuda.empty_cache()
-                return impl(eng, images, extrinsics, intrinsics, depth, mask, depth_idx, cam_idx)
+                return self._forward_impl(eng, images, extrinsics, intrinsics, depth, mask, depth_idx, cam_idx)
         for st, t in zip(ent["static"], dyn):
             if st is not None:
                 st.copy_(t)
@@ -485,17 +448,24 @@ class OmniVGGT(nn.Module, PyTorchModelHubMixin):
             return eng.camera_head(cam_tokens, B, S)
         return TP.camera_head(self.camera_head, cam_tokens.view(B, S, -1), dtype=self.camera_dtype)
 
-    def _aggregate(self, eng, images, extrinsics, intrinsics, depth, mask, depth_idx, cam_idx, slots=True, layers=None):
-        """Patchifier, camera / depth injection and the aggregator: (bf16 slots of the kept layers, fp32 camera tokens [K, 2C])."""
+    def _aggregate(self, eng, images, extrinsics, intrinsics, depth, mask, depth_idx, cam_idx, slots=True, layers=None, sl=None):
+        """Patchifier, camera / depth injection and the aggregator on the views ``sl`` of each scene (default: all of them;
+        this rank's under context parallelism): (bf16 slots of the kept layers, fp32 camera tokens [B*S, 2C] of ALL S views).
+        Under context parallelism the camera tokens are the ones every rank gathered (cp.cam_all)."""
         B, S, Cin, H, W = images.shape
         ag = self.aggregator
-        K = B * S
+        cp = self._cp
+        sl = slice(0, S) if sl is None else sl
+        n = sl.stop - sl.start
+        K = B * n
 
         # ---- frozen patchifier (PyTorch): normalise, DINOv2 / conv patch embed       (omnivggt_aggregator.py:143-150)
         if eng.dino is not None:
             P = (H // self.patch_size) * (W // self.patch_size)
             pos = TP.dino_pos_embed(ag.patch_embed, P, H, W, self.patch_size).float()
-            patch = eng.dino_patchify(images.float().view(K, Cin, H, W), pos, _RESNET_MEAN, _RESNET_STD)
+            patch = eng.dino_patchify(images[:, sl].float().view(K, Cin, H, W), pos, _RESNET_MEAN, _RESNET_STD)
+        elif cp is not None:
+            raise RuntimeError("context parallelism runs the DINOv2 patchifier on the libovg runtime (dino_backend='ovg')")
         else:
             img = ((images.float() - self._resnet_mean) / self._resnet_std).view(K, Cin, H, W)
             if hasattr(ag.patch_embed, "blocks"):
@@ -506,6 +476,8 @@ class OmniVGGT(nn.Module, PyTorchModelHubMixin):
             patch = patch.float().contiguous()
 
         # ---- aux cameras -> pose encoding -> 25 injection vectors (tiny fp32 host math)  (:158-182,:273-287)
+        # The pose normalisation is global over the selected views of a scene (omnivggt_aggregator.py:85-105), and the inputs
+        # are a few hundred bytes per view, so the vectors are computed for all S views and the views of ``sl`` kept.
         pose = None
         rows = None
         if len(cam_idx):
@@ -514,17 +486,30 @@ class OmniVGGT(nn.Module, PyTorchModelHubMixin):
                               lambda: (torch.arange(B)[:, None] * S + torch.tensor(cam_idx)[None]).reshape(-1))
             pose = TP.aux_pose_encoding(extrinsics.index_select(1, ci), intrinsics.index_select(1, ci), H, W)
         inj = TP.injection_vectors(eng.inj_pack, pose, cam_idx, B, S, rows)
+        inj = inj.view(-1, B, S, inj.shape[-1])[:, :, sl].reshape(-1, K, inj.shape[-1])      # a view when sl is every view
 
-        # ---- hot path: aggregator on libovg
+        # ---- hot path: aggregator on libovg.  Under context parallelism depth / mask are the full tensors and depth_idx holds
+        # scene indices: the masked-mean normalisation of the depth modality is over all selected views of the scene.
         keep = set(self.dpt_layers)
-        return eng.aggregate(patch, inj, depth, mask, depth_idx, B, S, H, W, keep, slots=slots, layers=layers)
+        slots, cam_out = eng.aggregate(patch, inj, depth, mask, depth_idx, B, n, H, W, keep, cp=cp, views_total=S, slots=slots,
+                                       layers=layers)
+        return slots, (cp.cam_all if cp is not None else cam_out)
 
     def _forward_impl(self, eng, images, extrinsics, intrinsics, depth, mask, depth_idx, cam_idx):
         B, S, Cin, H, W = images.shape
-        K = B * S
+        sl = slice(0, S)
+        if self._cp is not None:
+            if B != 1:
+                raise ValueError("context parallelism shards the views of ONE scene (B = 1); use scene-level data parallelism for "
+                                 "batches")
+            v0, n = self._cp.local_views(S)
+            sl = slice(v0, v0 + n)
+        n = sl.stop - sl.start                    # views of each scene with dense outputs
+        K = B * n
         heads = self._dpt_heads()                 # the heads set to None are skipped, as the reference does (omnivggt.py:46-62)
         cam_on = self.camera_head is not None
-        slots, cam_tokens = self._aggregate(eng, images, extrinsics, intrinsics, depth, mask, depth_idx, cam_idx, slots=bool(heads))
+        slots, cam_tokens = self._aggregate(eng, images, extrinsics, intrinsics, depth, mask, depth_idx, cam_idx, slots=bool(heads),
+                                            sl=sl)
 
         # ---- heads.  The camera head and the two DPT heads only read the aggregator outputs: they run on three streams
         # (forked / joined with events, also inside a captured CUDA graph) so that their many small kernels -- 19^2 / 37^2
@@ -538,7 +523,7 @@ class OmniVGGT(nn.Module, PyTorchModelHubMixin):
             eng.dpt(name, slots, self.dpt_layers, K, H, W, head_act=act, out=outs[name])
 
         main = torch.cuda.current_stream() if images.is_cuda else None
-        if main is not None and self.head_streams and cam_on + len(heads) > 1:
+        if main is not None and self._cp is None and self.head_streams and cam_on + len(heads) > 1:
             if self._streams is None:
                 self._streams = (torch.cuda.Stream(), torch.cuda.Stream())
             side = list(self._streams)
@@ -569,6 +554,8 @@ class OmniVGGT(nn.Module, PyTorchModelHubMixin):
             predictions["pose_enc"] = pose_list[-1]
             predictions["pose_enc_list"] = pose_list
         for name, _ in heads:
-            self._put_dpt(predictions, name, *outs[name], B, S, H, W)
+            self._put_dpt(predictions, name, *outs[name], B, n, H, W)
         predictions["images"] = images
+        if self._cp is not None:
+            predictions["images"], predictions["view_range"] = images[:, sl], (sl.start, sl.stop)
         return predictions

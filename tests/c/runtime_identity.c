@@ -86,7 +86,8 @@ int main(void) {
   for (int i = 0; i < 4; ++i) slots[i] = dzero((size_t)K * T * 2 * C * 2);
   float* cam_out = dzero((size_t)K * 2 * C * 4);
   if (!patch || !inj || !ws || !cam_out || !slots[3]) { printf("allocation failed\n"); return 5; }
-  OK(ovg_aggregator_forward(agg, patch, inj, NULL, NULL, NULL, 0, cosd, sind, 3, B, S, H, W, ws, wsb, slots, cam_out, NULL));
+  OK(ovg_aggregator_forward(agg, NULL, patch, inj, NULL, NULL, NULL, 0, NULL, 0, cosd, sind, 3, B, S, H, W, ws, wsb, slots, cam_out,
+                            NULL, NULL));
   CK(cudaDeviceSynchronize());
 
   /* ---- check */

@@ -40,22 +40,24 @@ def test_engine_creates_no_dpt_handle_for_a_none_head(dry):
     assert dry.count("ovg_dpt_create") == 1 and dry.count("ovg_camera_create") == 1
 
 
-def test_pose_only_forward_writes_no_slot_and_runs_no_dpt(dry):
+def test_pose_only_forward_writes_no_slot_exports_no_layer_and_runs_no_dpt(dry):
     m = _model()
     m.depth_head = None
     m.point_head = None
     ready(m)
     out = m(**make_inputs(1, 3, 56, 56, seed=1), depth_gt_index=[1], camera_gt_index=[0])
     assert set(out) == {"pose_enc", "pose_enc_list", "images"} and out["pose_enc"].shape == (1, 3, 9)
-    assert dry.count("ovg_aggregator_forward") == 1 and dry.count("ovg_aggregator_forward_layers") == 0
-    slots = dry.args("ovg_aggregator_forward")[0][16]
+    assert dry.count("ovg_aggregator_forward") == 1
+    args = dry.args("ovg_aggregator_forward")[0]
+    assert args[1] is None and args[21] is None                             # one GPU, no layer export
+    slots = args[19]
     assert len(slots) == 4 and all(p is None for p in slots)
     assert dry.count("ovg_dpt_create") == 0 and dry.count("ovg_dpt_forward") == 0 and dry.count("ovg_camera_forward") == 1
     assert not any(k.startswith("slot") for k in m._engine.ws.bufs)
 
 
 @pytest.mark.parametrize("present", list(itertools.product([True, False], repeat=3)))
-def test_output_keys_follow_the_reference_gating(dry, present):
+def test_output_keys_and_library_calls_follow_the_reference_gating(dry, present):
     m = _model()
     for name, on in zip(HEADS, present):
         if not on:
@@ -68,8 +70,9 @@ def test_output_keys_follow_the_reference_gating(dry, present):
     assert out["images"].shape == (B, S, 3, H, W)
     n_dpt = sum(present[1:])
     assert dry.count("ovg_dpt_create") == n_dpt and dry.count("ovg_dpt_forward") == n_dpt
+    assert all(a[2] == 0 for a in dry.args("ovg_dpt_forward"))             # bf16 slots
     assert dry.count("ovg_camera_forward") == int(present[0])
-    slots = dry.args("ovg_aggregator_forward")[0][16]
+    slots = dry.args("ovg_aggregator_forward")[0][19]
     assert all(p is None for p in slots) == (n_dpt == 0)
     if present[1]:
         assert out["depth"].shape == (B, S, H, W, 1) and out["depth_conf"].shape == (B, S, H, W)
@@ -90,7 +93,7 @@ def test_setting_a_head_invalidates_the_engine(dry):
     assert "point_head" in ready(m).dpt_packs and eng is not m._engine
 
 
-def test_aggregator_component_exports_every_layer(dry):
+def test_aggregator_component_exports_every_layer_in_one_forward_call(dry):
     m = _model()
     ready(m)
     B, S, H, W = 2, 3, 42, 70
@@ -99,14 +102,15 @@ def test_aggregator_component_exports_every_layer(dry):
     T = (H // 14) * (W // 14) + 5
     assert ps == 5 and len(layers) == depth
     assert all(t.shape == (B, S, T, C2) and t.dtype == torch.float32 for t in layers)
-    assert dry.count("ovg_aggregator_forward_layers") == 1 and dry.count("ovg_aggregator_forward") == 0
-    args = dry.args("ovg_aggregator_forward_layers")[0]
-    assert all(p is None for p in args[16])                                 # no bf16 slot: no DPT head reads them
-    assert len(args[18]) == depth and list(args[18]) == [t.data_ptr() for t in layers]
+    assert dry.count("ovg_aggregator_forward") == 1
+    args = dry.args("ovg_aggregator_forward")[0]
+    assert args[1] is None                                                  # one GPU
+    assert all(p is None for p in args[19])                                 # no bf16 slot: no DPT head reads them
+    assert len(args[21]) == depth and list(args[21]) == [t.data_ptr() for t in layers]
     assert dry.count("ovg_dpt_forward") == 0 and dry.count("ovg_camera_forward") == 0
 
 
-def test_head_components_issue_the_fp32_entry_points(dry):
+def test_head_components_pass_fp32_slots(dry):
     m = _model()
     ready(m)
     B, S, H, W = 1, 9, 28, 42
@@ -116,9 +120,9 @@ def test_head_components_issue_the_fp32_entry_points(dry):
     d, dc = m.depth_head(tokens, images, 5)
     p, pc = m.point_head(tokens, images=images, patch_start_idx=5, frames_chunk_size=4)
     assert d.shape == (B, S, H, W, 1) and dc.shape == (B, S, H, W) and p.shape == (B, S, H, W, 3) and pc.shape == (B, S, H, W)
-    assert dry.count("ovg_dpt_forward_f32") == 2 + 3 and dry.count("ovg_dpt_forward") == 0     # chunks of 8, then of 4
-    first = dry.args("ovg_dpt_forward_f32")[0]
-    assert list(first[1]) == [t.data_ptr() for t in tokens] and first[2:4] == (T, 5)
+    dpt = dry.args("ovg_dpt_forward")
+    assert len(dpt) == 2 + 3 and all(a[2] == 1 for a in dpt)               # fp32 slots; chunks of 8, then of 4
+    assert list(dpt[0][1]) == [t.data_ptr() for t in tokens] and dpt[0][3:5] == (T, 5)
     poses = m.camera_head(tokens, num_iterations=3)
     assert len(poses) == 3 and poses[0].shape == (B, S, 9)
     ct = dry.args("ovg_camera_forward")[0]

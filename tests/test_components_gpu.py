@@ -3,7 +3,7 @@
   - model.aggregator / camera_head / depth_head / point_head compose to exactly what forward() returns (bit for bit, eager);
   - the exported fp32 layers against the reference's aggregated_tokens_list (goldens' agg_first / agg_last);
   - the reference's fp32 token list (CPU oracle) through these heads against the oracle's heads;
-  - the kernels: ovg_dpt_forward_f32 on fp32 layers equals ovg_dpt_forward on their bf16 rounding, and the fp32 export writes
+  - the kernels: ovg_dpt_forward on fp32 layers equals ovg_dpt_forward on their bf16 rounding, and the fp32 export writes
     the same values the bf16 snapshots and the camera tokens hold;
   - forward with heads set to None: the other outputs are unchanged, in eager and in CUDA-graph replay."""
 import json
@@ -153,7 +153,7 @@ def full_heads_model(dpt_dtype):
 
 @pytest.mark.parametrize("dpt_dtype", ["fp16", "bf16"])
 @pytest.mark.parametrize("name,act", [("depth_head", 0), ("point_head", 1)])
-def test_dpt_forward_f32_equals_bf16_slots(dpt_dtype, name, act):
+def test_dpt_forward_fp32_slots_equal_bf16_slots(dpt_dtype, name, act):
     from omnivggt_official_b200 import _lib as L
     m = full_heads_model(dpt_dtype)
     eng = m.engine()
@@ -174,9 +174,9 @@ def test_dpt_forward_f32_equals_bf16_slots(dpt_dtype, name, act):
 
 @pytest.mark.parametrize("variant", ["mini_conv", "full_width"])
 def test_layer_export_agrees_with_snapshots_and_camera_tokens(variant):
-    """One ovg_aggregator_forward_layers call writing slots and layers: every kept slot is the bf16 rounding of its layer; the
-    camera tokens are token 0 of the last layer; and ovg_aggregator_forward without layers writes the same slots and camera
-    tokens bit for bit (the export does not perturb the forward)."""
+    """One ovg_aggregator_forward call writing slots and layers: every kept slot is the bf16 rounding of its layer; the camera
+    tokens are token 0 of the last layer; and ovg_aggregator_forward without layers writes the same slots and camera tokens bit
+    for bit (the export does not perturb the forward)."""
     m = model(variant)
     eng = m.engine()
     B, S, H, W = (2, 3, 42, 70) if variant == "mini_conv" else (1, 3, 154, 210)

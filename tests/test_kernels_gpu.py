@@ -582,7 +582,7 @@ def test_dpt_tail_fused(Fr, h, w, H, W, outc, act, dtype):
 
 
 # ----------------------------------------------------------------------------------------------- C host
-def test_c_host_drives_the_runtime(tmp_path):
+def test_c_host_drives_the_aggregator_forward(tmp_path):
     """A plain C program (tests/c/runtime_identity.c: gcc, libovg + libcudart, no Python / torch in the process) runs the
     aggregator through the handle-level C ABI with raw device pointers; with zero block weights the kept intermediates must
     equal the assembled tokens bit for bit."""

@@ -61,9 +61,9 @@ def test_proxy_shapes_dtypes_poison_and_guards(poison):
 
 # ovg_* entry point -> positions of its workspace and output pointers (a ctypes array: every element)
 PTR_ARGS = {
-    "ovg_aggregator_forward": (14, 16, 17),     # workspace, slots, cam_out
+    "ovg_aggregator_forward": (17, 19, 20, 21), # workspace, slots, cam_out, layers
     "ovg_dino_forward": (8, 10),                # workspace, patch tokens
-    "ovg_dpt_forward": (12, 13, 14),            # preds, conf, workspace
+    "ovg_dpt_forward": (13, 14, 15),            # preds, conf, workspace
     "ovg_camera_forward": (5, 6),               # out, workspace
     "ovg_conf_percentile_mask": (4, 5, 6, 7),   # workspace, mask, threshold, count
     "ovg_point_cloud_count": (7, 9),            # workspace, count
@@ -94,7 +94,7 @@ def _coverage(rec, P, want):
     assert seen == want, seen ^ want
 
 
-def test_dry_run_forward_allocates_through_the_proxy(dry, poison):
+def test_dry_run_forward_allocates_every_pointer_through_the_proxy(dry, poison):
     """Forward of the DINOv2 variant with depth and camera aux and 9 views (DPT chunks of 8 and 1)."""
     from omnivggt_official_b200.engine import Engine
     m = mini_model("mini_dino").eval()

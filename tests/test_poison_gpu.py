@@ -15,7 +15,7 @@ Which launch first writes each stateful region, per entry point (read from csrc/
                reads them; depth im2col rows: depth_im2col_kernel (every column, including the padding columns).
   DINOv2       x and the patch-row list: dino_init_kernel; image im2col rows: image_im2col_kernel (padding columns zeroed).
   attention    KV-split partials (part_o, part_ml): the split CTAs of the same launch, before attn_merge_kernel.
-  DPT head     feat[l] zero borders: cudaMemsetAsync in dpt_run (the DENSE2PAD / PIXSHUF stores write the interior only);
+  DPT head     feat[l] zero borders: cudaMemsetAsync in ovg_dpt_forward (the DENSE2PAD / PIXSHUF stores write the interior only);
                lr, t, u, v, w, o1 borders: the ROWS_PAD epilogue writes border rows as zeros; xl[l] borders:
                upsample_rows_kernel / upsample_bilinear_kernel write rows 0 and H + 1 and the border columns as zeros;
                colsd: im2col3x3s2_kernel writes zeros for taps outside the map; tail scratch (gx, gy): tail_tables_kernel.

@@ -1,6 +1,7 @@
 """Workspace contract of every libovg entry point that carves a caller's workspace: a null workspace, a misaligned one and one a
 byte shorter than the call needs are each refused with OVG_E_INVALID before any launch.  The call needs what its size query
-answers, except where noted in cases().
+answers, except where noted in cases().  The argument combinations in MISUSE are refused the same way with a well-formed
+workspace.
 
 The operands are placeholder device pointers, so the calls run in a child process that sees no CUDA device: an entry point
 that wrongly accepted a workspace would fail with a CUDA error there instead of launching."""
@@ -130,38 +131,52 @@ def cases(lib, L):
         "ovg_sim3_estimate": (lambda ws, n: lib.ovg_sim3_estimate(PTR, PTR, None, 100, ws, n, PTR, PTR, None),
                               lib.ovg_sim3_workspace_bytes(100), 256),
         "ovg_aggregator_forward": (
-            lambda ws, n: lib.ovg_aggregator_forward(hs["aggregator"], PTR, PTR, None, None, None, 0, PTR, PTR, 64, 1, 2, 28, 28,
-                                                     ws, n, slots4, PTR, None),
+            lambda ws, n: lib.ovg_aggregator_forward(hs["aggregator"], None, PTR, PTR, None, None, None, 0, None, 0, PTR, PTR, 64, 1,
+                                                     2, 28, 28, ws, n, slots4, PTR, None, None),
             lib.ovg_aggregator_workspace_bytes(hs["aggregator"], 1, 2, 28, 28, 0), 256),
-        "ovg_aggregator_forward_layers": (
-            lambda ws, n: lib.ovg_aggregator_forward_layers(hs["aggregator"], PTR, PTR, None, None, None, 0, PTR, PTR, 64, 1, 2, 28,
-                                                            28, ws, n, slots4, PTR, slots1, None),
+        "ovg_aggregator_forward(layers)": (
+            lambda ws, n: lib.ovg_aggregator_forward(hs["aggregator"], None, PTR, PTR, None, None, None, 0, None, 0, PTR, PTR, 64, 1,
+                                                     2, 28, 28, ws, n, slots4, PTR, slots1, None),
             lib.ovg_aggregator_workspace_bytes(hs["aggregator"], 1, 2, 28, 28, 0), 256),
-        "ovg_aggregator_forward_cp": (
-            lambda ws, n: lib.ovg_aggregator_forward_cp(hs["aggregator"], C.byref(cp), PTR, PTR, None, None, None, 0, None, 0, PTR,
-                                                        PTR, 64, 2, 28, 28, ws, n, slots4, PTR, None),
+        "ovg_aggregator_forward(cp)": (
+            lambda ws, n: lib.ovg_aggregator_forward(hs["aggregator"], C.byref(cp), PTR, PTR, None, None, None, 0, None, 0, PTR,
+                                                     PTR, 64, 1, 2, 28, 28, ws, n, slots4, PTR, None, None),
             lib.ovg_aggregator_workspace_bytes(hs["aggregator"], 1, 2, 28, 28, 0), 256),
+        # refused whatever the workspace: MISUSE
+        "ovg_aggregator_forward(cp, layers)": (
+            lambda ws, n: lib.ovg_aggregator_forward(hs["aggregator"], C.byref(cp), PTR, PTR, None, None, None, 0, None, 0, PTR,
+                                                     PTR, 64, 1, 2, 28, 28, ws, n, slots4, PTR, slots1, None),
+            lib.ovg_aggregator_workspace_bytes(hs["aggregator"], 1, 2, 28, 28, 0), 256),
+        "ovg_aggregator_forward(depth_idx_local, no cp)": (
+            lambda ws, n: lib.ovg_aggregator_forward(hs["aggregator"], None, PTR, PTR, PTR, PTR, PTR, 1, PTR, 1, PTR, PTR, 64, 1, 2,
+                                                     28, 28, ws, n, slots4, PTR, None, None),
+            lib.ovg_aggregator_workspace_bytes(hs["aggregator"], 1, 2, 28, 28, 1), 256),
         "ovg_dino_forward": (lambda ws, n: lib.ovg_dino_forward(hs["dino"], PTR, PTR, mean3, mean3, 2, 28, 28, ws, n, PTR, None),
                              lib.ovg_dino_workspace_bytes(hs["dino"], 2, 28, 28), 256),
-        "ovg_dpt_forward": (lambda ws, n: lib.ovg_dpt_forward(hs["dpt"], slots4, 9, 5, 0, 2, 28, 28, slots4, PTR, PTR, 0, PTR, PTR,
-                                                              ws, n, None),
+        "ovg_dpt_forward": (lambda ws, n: lib.ovg_dpt_forward(hs["dpt"], slots4, 0, 9, 5, 0, 2, 28, 28, slots4, PTR, PTR, 0, PTR,
+                                                              PTR, ws, n, None),
                             lib.ovg_dpt_workspace_bytes(hs["dpt"], 2, 28, 28), 256),
-        "ovg_dpt_forward_f32": (lambda ws, n: lib.ovg_dpt_forward_f32(hs["dpt"], slots4, 9, 5, 0, 2, 28, 28, slots4, PTR, PTR, 0, PTR,
-                                                                      PTR, ws, n, None),
-                                lib.ovg_dpt_workspace_bytes(hs["dpt"], 2, 28, 28), 256),
+        "ovg_dpt_forward(f32)": (lambda ws, n: lib.ovg_dpt_forward(hs["dpt"], slots4, 1, 9, 5, 0, 2, 28, 28, slots4, PTR, PTR, 0,
+                                                                   PTR, PTR, ws, n, None),
+                                 lib.ovg_dpt_workspace_bytes(hs["dpt"], 2, 28, 28), 256),
+        "ovg_dpt_forward(slots_f32 = 2)": (lambda ws, n: lib.ovg_dpt_forward(hs["dpt"], slots4, 2, 9, 5, 0, 2, 28, 28, slots4, PTR,
+                                                                             PTR, 0, PTR, PTR, ws, n, None),
+                                           lib.ovg_dpt_workspace_bytes(hs["dpt"], 2, 28, 28), 256),
         "ovg_camera_forward": (lambda ws, n: lib.ovg_camera_forward(hs["camera"], PTR, 1, 2, 4, PTR, ws, n, None),
                                lib.ovg_camera_workspace_bytes(hs["camera"], 2), 256),
     }
 
 
 def outcomes():
-    """{case: {"need": bytes, "null" / "misaligned" / "short": [return code, launches made, last error]}}."""
+    """{case: {"need": bytes, "null" / "misaligned" / "short": [return code, launches made, last error]}}; the cases in MISUSE
+    get a well-formed workspace instead ("well-formed")."""
     from omnivggt_official_b200 import _lib as L
     lib = L.load()
     out = {}
     for name, (call, need, align) in cases(lib, L).items():
         res = {"need": need}
-        for what, ws, n in (("null", None, need), ("misaligned", PTR + align // 2, need), ("short", PTR, need - 1)):
+        bad = (("null", None, need), ("misaligned", PTR + align // 2, need), ("short", PTR, need - 1))
+        for what, ws, n in (("well-formed", PTR, need),) if name in MISUSE else bad:
             before = lib.ovg_launch_count()
             rc = call(ws, n)
             res[what] = [rc, lib.ovg_launch_count() - before, lib.ovg_last_error().decode()]
@@ -188,18 +203,28 @@ NAMES = ["ovg_point_cloud_count", "ovg_point_cloud_gather", "ovg_point_cloud_cen
          "ovg_tracks_gather", "ovg_tracks_gather(match)", "ovg_bundle_adjust", "ovg_mesh_count", "ovg_mesh_faces",
          "ovg_mesh_compact", "ovg_tsdf_bounds", "ovg_tsdf_integrate", "ovg_tsdf_count", "ovg_tsdf_extract", "ovg_segment_sky",
          "ovg_farthest_point_sample", "ovg_compute_ranking", "ovg_sim3_estimate", "ovg_aggregator_forward",
-         "ovg_aggregator_forward_layers", "ovg_aggregator_forward_cp", "ovg_dino_forward", "ovg_dpt_forward",
-         "ovg_dpt_forward_f32", "ovg_camera_forward"]
+         "ovg_aggregator_forward(layers)", "ovg_aggregator_forward(cp)", "ovg_dino_forward", "ovg_dpt_forward",
+         "ovg_dpt_forward(f32)", "ovg_camera_forward"]
+# argument combinations an entry point refuses before it looks at the workspace -> the reason it gives
+MISUSE = {"ovg_aggregator_forward(cp, layers)": "no layer export",
+          "ovg_aggregator_forward(depth_idx_local, no cp)": "need context parallelism",
+          "ovg_dpt_forward(slots_f32 = 2)": "slots_f32 must be 0"}
 
 
-def test_every_case_ran(refused):
-    assert sorted(refused) == sorted(NAMES)
+def test_every_case_and_misuse_ran(refused):
+    assert sorted(refused) == sorted(NAMES + list(MISUSE))
 
 
 @pytest.mark.parametrize("name", NAMES)
 @pytest.mark.parametrize("what", ["null", "misaligned", "short"])
-def test_bad_workspace_is_refused(refused, name, what):
+def test_bad_workspace_is_refused_before_any_launch(refused, name, what):
     r = refused[name]
     assert r["need"] > 0
     rc, launches, err = r[what]
     assert (rc, launches) == (OVG_E_INVALID, 0), err
+
+
+@pytest.mark.parametrize("name", list(MISUSE))
+def test_argument_misuse_is_refused(refused, name):
+    rc, launches, err = refused[name]["well-formed"]
+    assert (rc, launches) == (OVG_E_INVALID, 0) and MISUSE[name] in err, err
