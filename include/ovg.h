@@ -486,6 +486,59 @@ int ovg_sim3_apply(const double* sim3, int views, long long hw, const float* poi
                    const float* points2_in, float* points2_out, const float* depth_in, float* depth_out,
                    const float* ext_in, float* ext_out, void* stream);
 
+/* Evaluation of one scene against ground truth (scene.evaluate).  Cameras are world-to-camera fp32 [S, 3, 4] with intrinsics
+ * fp32 [S, 3, 3]; a view has a ground-truth camera when fx, fy > 0 and its extrinsic is finite.  Every sum is fp64 over a
+ * fixed grid, then in a fixed order, and every count is an integer: results are bit-identical from run to run.  The launch
+ * counts below do not depend on S, m or the number of pairs.  Workspaces are 256-byte aligned, of the size their query gives.
+ * ovg_eval_pose: the m <= 8192 distinct scene views views[m] (int32); the n of them with a ground-truth camera and a finite
+ *     prediction count, in that order.  Poses are camera-to-world P = [R^T | c], c = -R^T t, formed in fp64.
+ *     - The ATE alignment of vo_eval.py:190-199 (evo APE, translation part, align and correct_scale): ovg_sim3_estimate of the
+ *       predicted centres onto the ground-truth centres, each rounded once to fp32, over a keep mask of the n views.
+ *       sim3_out / stats_out are that call's outputs; stats_out[0] = n, stats_out[2] = the ATE (its RMS residual).
+ *     - RPE of vo_eval.py:201-236 (evo, delta 1 frame, all pairs, same alignment): the prediction after the fit is R_a R,
+ *       s R_a c + t_a; for k = 0 .. n-2, E = (Q_k^-1 Q_k+1)^-1 (P_k^-1 P_k+1); rpe_out fp64 [n - 1, 2] = |t(E)|,
+ *       angle(R(E)) in degrees, with angle(R) = atan2(|(R32 - R23, R13 - R31, R21 - R12)| / 2, (tr R - 1) / 2).
+ *     - Every pair i < j of the n views, in the order (0, 1), (0, 2), ..: R_ij = R_j R_i^T, t_ij = t_j - R_ij t_i;
+ *       RRE = angle(R_ij,gt^T R_ij,pred), RTE = the angle between t_ij,gt and t_ij,pred folded to min(e, 180 - e) (90 when
+ *       either is zero).  pairs_out int32 [n (n - 1) / 2, 2] = the scene views, pair_errors_out fp64 [.., 2] = RRE, RTE.
+ *     - scores_out fp64 [12] = ate, rpe_trans, rpe_rot (the RMS of rpe_out's columns; NaN when n < 2), auc, rra, rta at
+ *       tau = 5, 10, 30 degrees: auc = numpy's mean(cumsum(histogram(max(RRE, RTE), arange(tau + 1))[0]) / P), summed in
+ *       numpy's pairwise order; rra / rta the fractions with RRE / RTE < tau (NaN when there is no pair).
+ *     Outputs are sized for m views (n <= m).  Nine launches (five of them ovg_sim3_estimate's), no host synchronisation.
+ * ovg_eval_depth: gt, pred fp32 [S, hw]; mask uint8 [S, hw] or NULL; view_sel uint8 [S] (non-zero: scored).  A pixel counts
+ *     when its view is selected, its mask set, g > 0 and g and p finite.  s = median(g) / median(p) in fp64, each median
+ *     numpy.percentile(v, 50) of the fp32 values (exact radix selection); with sp = s p in fp64:
+ *     scores_out fp64 [10] = pixels, s, median(g), median(p), abs_rel = mean |sp - g| / g, sq_rel = mean (sp - g)^2 / g,
+ *     rmse = sqrt(mean (sp - g)^2), delta (3) = fractions with max(sp / g, g / sp) < 1.25, 1.25^2, 1.25^3; NaN when no pixel
+ *     counts.  Per view: view_abs_rel, view_delta1 fp64 [S] (NaN without pixels), view_pixels int64 [S].  21 launches.
+ * ovg_eval_points_keep: the inverse [R^T | -R^T t] of each ground-truth extrinsic (fp64, rounded once) into c2w_out fp32
+ *     [S, 3, 4], for ovg_unproject_depth of the ground-truth depth; and the pixel set shared by both clouds into both rows
+ *     of keep_out uint8 [2, S hw]: a selected view with a ground-truth camera, the mask set, g > 0 finite, and a finite
+ *     predicted point pred_points fp32 [S, hw, 3].  One launch.
+ * ovg_eval_points: after ovg_match_index / ovg_match_query with V = 2 (0: the aligned prediction, 1: the ground truth),
+ *     cap = S H W and the one pair (0, 1) over points fp32 [2, S H W, 3] and keep uint8 [2, S H W]; match_workspace is theirs.
+ *     Normals from the pixel grid: n = normalize((P[x+1, y] - P[x-1, y]) x (P[x, y+1] - P[x, y-1])) where the pixel and its
+ *     four neighbours are kept and the cross product is not zero.  acc_dist fp64 [n] = sqrt of the matcher's exact fp64
+ *     (d^2, lowest index) minimum from each kept predicted point to the ground truth, comp_dist fp64 [n] the other way, both
+ *     in kept (row-major) order; outputs are sized for S H W points.  scores_out fp64 [9] = n, acc, acc_median, comp,
+ *     comp_median, chamfer = (acc + comp) / 2, nc_acc, nc_comp (mean |n . n_nn| over the points where both have a normal; NaN
+ *     when none), nc = their mean.  Medians: numpy.percentile(50) of the distances rounded to fp32.  21 launches. */
+long long ovg_eval_pose_workspace_bytes(int m);
+int ovg_eval_pose(const float* gt_ext, const float* gt_intr, const float* pred_ext, const int* views, int m, void* workspace,
+                  long long workspace_bytes, double* sim3_out, double* stats_out, int* pairs_out, double* pair_errors_out,
+                  double* rpe_out, double* scores_out, void* stream);
+long long ovg_eval_depth_workspace_bytes(int S, long long hw);
+int ovg_eval_depth(const float* gt, const unsigned char* mask, const float* pred, const unsigned char* view_sel, int S,
+                   long long hw, void* workspace, long long workspace_bytes, double* scores_out, double* view_abs_rel,
+                   double* view_delta1, long long* view_pixels, void* stream);
+int ovg_eval_points_keep(const float* gt_ext, const float* gt_intr, const float* gt_depth, const unsigned char* mask,
+                         const float* pred_points, const unsigned char* view_sel, int S, long long hw, float* c2w_out,
+                         unsigned char* keep_out, void* stream);
+long long ovg_eval_points_workspace_bytes(int S, int H, int W);
+int ovg_eval_points(const float* points, const unsigned char* keep, int S, int H, int W, const void* match_workspace,
+                    long long match_workspace_bytes, void* workspace, long long workspace_bytes, double* acc_dist,
+                    double* comp_dist, double* scores_out, void* stream);
+
 /* Baseline JPEG decoding on the device, bit-identical to Pillow (libjpeg-turbo's default islow IDCT, fancy upsampling and
  * YCbCr -> RGB tables).  The plan is host code (no CUDA call): it parses every file, routes it to the device or to the host
  * (OVG_JPEG_* below: anything the device cannot decode exactly goes to the host), and builds the staging stream (tables plus the

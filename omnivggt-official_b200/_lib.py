@@ -154,6 +154,13 @@ EXPORTS = {
     "ovg_sim3_workspace_bytes": (_ll, [_ll]),
     "ovg_sim3_estimate": (C.c_int, [_vp, _vp, _vp, _ll, _vp, _ll, _vp, _vp, _vp]),
     "ovg_sim3_apply": (C.c_int, [_vp, _i, _ll, _vp, _vp, _vp, _vp, _vp, _vp, _vp, _vp, _vp]),
+    "ovg_eval_pose_workspace_bytes": (_ll, [_i]),
+    "ovg_eval_pose": (C.c_int, [_vp, _vp, _vp, _vp, _i, _vp, _ll, _vp, _vp, _vp, _vp, _vp, _vp, _vp]),
+    "ovg_eval_depth_workspace_bytes": (_ll, [_i, _ll]),
+    "ovg_eval_depth": (C.c_int, [_vp, _vp, _vp, _vp, _i, _ll, _vp, _ll, _vp, _vp, _vp, _vp, _vp]),
+    "ovg_eval_points_keep": (C.c_int, [_vp, _vp, _vp, _vp, _vp, _vp, _i, _ll, _vp, _vp, _vp]),
+    "ovg_eval_points_workspace_bytes": (_ll, [_i, _i, _i]),
+    "ovg_eval_points": (C.c_int, [_vp, _vp, _i, _i, _i, _vp, _ll, _vp, _ll, _vp, _vp, _vp, _vp]),
     "ovg_jpeg_plan_create": (C.c_int, [_pp, C.POINTER(_ll), _i, _i, _pp]),
     "ovg_jpeg_plan_destroy": (None, [_vp]),
     "ovg_jpeg_plan_file": (C.c_int, [_vp, _i, C.POINTER(_i), C.POINTER(_i), C.POINTER(_i), C.POINTER(_i)]),

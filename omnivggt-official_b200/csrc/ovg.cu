@@ -26,6 +26,7 @@
 #include "fps.cuh"
 #include "rank.cuh"
 #include "sim3.cuh"
+#include "eval.cuh"
 #include "tail.cuh"
 #include "pre.cuh"
 #include "jpeg.cuh"
@@ -1713,6 +1714,198 @@ int ovg_sim3_apply(const double* sim3, int views, long long hw, const float* poi
   if (blocks > num_sms() * 8LL) blocks = num_sms() * 8LL;          // grid-stride inside
   ovg::sim3_apply_kernel<<<static_cast<int>(blocks), 256, 0, reinterpret_cast<cudaStream_t>(stream)>>>(p);
   return post_launch("ovg_sim3_apply");
+}
+
+}  // extern "C"
+
+// -------------------------------------------------------------------------------------------------------------- evaluation
+namespace {
+
+struct EvalPoseBufs {
+  void* sim3;                        // ovg_sim3_workspace_bytes
+  ovg::EvalPoseParams p;
+};
+
+EvalPoseBufs eval_pose_layout(Arena& ar, int m) {
+  EvalPoseBufs w;
+  w.sim3 = ar.take(layout_bytes(sim3_layout));
+  ovg::EvalPoseParams& p = w.p;
+  p = ovg::EvalPoseParams{};
+  p.m = m;
+  p.keep = ar.get<unsigned char>(m);
+  p.centre_gt = ar.get<float>(3LL * m);
+  p.centre_pred = ar.get<float>(3LL * m);
+  p.count = ar.get<int>(1);
+  p.vidx = ar.get<int>(m);
+  p.pose_gt = ar.get<double>(15LL * m);
+  p.pose_pred = ar.get<double>(15LL * m);
+  p.pair_counts = ar.get<unsigned int>(static_cast<long long>(ovg::EVAL_PAIR_BLOCKS) * ovg::EVAL_PAIR_COUNTS);
+  return w;
+}
+
+// The selection region, the two medians' results and weights, and the partials of the depth group
+struct EvalDepthBufs {
+  void* select;                      // OVG_PERCENTILE_WORKSPACE_BYTES
+  ovg::EvalDepthParams p;
+};
+
+EvalDepthBufs eval_depth_layout(Arena& ar, int S, long long hw) {
+  EvalDepthBufs w;
+  ovg::EvalDepthParams& p = w.p;
+  p = ovg::EvalDepthParams{};
+  p.S = S; p.hw = hw;
+  p.tiles = static_cast<int>(ovg::compact_tiles(hw));
+  p.ld = (S * hw + 3) / 4 * 4;
+  w.select = ar.take(OVG_PERCENTILE_WORKSPACE_BYTES);
+  p.sel = ar.get<float>(6);
+  p.weight = ar.get<float>(2);
+  p.count = ar.get<unsigned long long>(1);
+  p.cols = ar.get<float>(2 * p.ld);
+  p.part = ar.get<double>(static_cast<long long>(S) * p.tiles * ovg::EVAL_DEPTH_P);
+  p.view_tot = ar.get<double>(static_cast<long long>(S) * ovg::EVAL_DEPTH_P);
+  return w;
+}
+
+struct EvalPointsBufs {
+  void* select;                      // OVG_PERCENTILE_WORKSPACE_BYTES
+  ovg::EvalPointsParams p;
+};
+
+EvalPointsBufs eval_points_layout(Arena& ar, int S, int H, int W) {
+  EvalPointsBufs w;
+  ovg::EvalPointsParams& p = w.p;
+  p = ovg::EvalPointsParams{};
+  p.S = S; p.H = H; p.W = W;
+  const long long n = static_cast<long long>(S) * H * W;
+  p.ld = (n + 3) / 4 * 4;
+  w.select = ar.take(OVG_PERCENTILE_WORKSPACE_BYTES);
+  p.sel = ar.get<float>(6);
+  p.weight = ar.get<float>(2);
+  p.count = ar.get<unsigned long long>(2);
+  p.normals = ar.get<double>(6 * n);
+  p.cols = ar.get<float>(2 * p.ld);
+  p.part = ar.get<double>(2LL * ovg::EVAL_DIST_BLOCKS * 3);
+  return w;
+}
+
+// The two medians of a group: numpy.percentile(cols[j, :count[j]], 50) for j = 0, 1, where every column holds +inf past its
+// values (so the ranks, which stay below the count, never reach them).  sel[3 j .. 3 j + 1] and weight[j] get the result.
+int eval_medians(const float* cols, long long ld, const unsigned long long* count, int count_stride, void* select, float* sel,
+                 float* weight, const char* what, cudaStream_t st) {
+  const PercentileRegion r = percentile_region(select);
+  for (int j = 0; j < 2; ++j) {
+    ovg::eval_select_init_kernel<<<1, 128, 0, st>>>(r.state, r.hist, count + j * count_stride, 50.f, weight + j);
+    int rc = post_launch((std::string(what) + "(median init)").c_str());
+    if (rc) return rc;
+    if ((rc = radix_select_passes(cols + j * ld, ld, select, sel + 3 * j, nullptr, what, st))) return rc;
+  }
+  return OVG_OK;
+}
+
+}  // namespace
+
+extern "C" {
+
+long long ovg_eval_pose_workspace_bytes(int m) {
+  return (m > 0 && m <= ovg::EVAL_MAX_VIEWS) ? layout_bytes(eval_pose_layout, m) : -1;
+}
+
+int ovg_eval_pose(const float* gt_ext, const float* gt_intr, const float* pred_ext, const int* views, int m, void* workspace,
+                  long long workspace_bytes, double* sim3_out, double* stats_out, int* pairs_out, double* pair_errors_out,
+                  double* rpe_out, double* scores_out, void* stream) {
+  OVG_REQUIRE(m > 0 && m <= ovg::EVAL_MAX_VIEWS, "m must be in [1, 8192]");
+  EvalPoseBufs w;
+  int rc = carve(__func__, "ovg_eval_pose_workspace_bytes(m)", workspace, workspace_bytes, &w, eval_pose_layout, m);
+  if (rc) return rc;
+  OVG_REQUIRE(gt_ext && gt_intr && pred_ext && views && sim3_out && stats_out && pairs_out && pair_errors_out && rpe_out &&
+                  scores_out, "null operand");
+  ovg::EvalPoseParams& p = w.p;
+  p.gt_ext = gt_ext; p.gt_intr = gt_intr; p.pred_ext = pred_ext; p.views = views;
+  p.sim3 = sim3_out; p.stats = stats_out; p.pairs_out = pairs_out; p.pair_err = pair_errors_out; p.rpe = rpe_out;
+  p.scores = scores_out;
+  cudaStream_t st = reinterpret_cast<cudaStream_t>(stream);
+  ovg::eval_pose_prep_kernel<<<1, 1024, 0, st>>>(p);
+  if ((rc = post_launch("ovg_eval_pose(prep)"))) return rc;
+  // the ATE alignment (vo_eval.py:190-199): Umeyama of the predicted centres onto the ground-truth ones
+  if ((rc = ovg_sim3_estimate(p.centre_pred, p.centre_gt, p.keep, m, w.sim3, layout_bytes(sim3_layout), sim3_out, stats_out,
+                              stream)))
+    return rc;
+  ovg::eval_rpe_kernel<<<(m + ovg::EVAL_THREADS - 1) / ovg::EVAL_THREADS, ovg::EVAL_THREADS, 0, st>>>(p);
+  if ((rc = post_launch("ovg_eval_pose(rpe)"))) return rc;
+  ovg::eval_pair_kernel<<<ovg::EVAL_PAIR_BLOCKS, ovg::EVAL_THREADS, 0, st>>>(p);
+  if ((rc = post_launch("ovg_eval_pose(pairs)"))) return rc;
+  ovg::eval_pose_finish_kernel<<<1, ovg::EVAL_THREADS, 0, st>>>(p);
+  return post_launch("ovg_eval_pose(finish)");
+}
+
+long long ovg_eval_depth_workspace_bytes(int S, long long hw) {
+  return (S > 0 && hw > 0 && S * hw < (1LL << 31)) ? layout_bytes(eval_depth_layout, S, hw) : -1;
+}
+
+int ovg_eval_depth(const float* gt, const unsigned char* mask, const float* pred, const unsigned char* view_sel, int S,
+                   long long hw, void* workspace, long long workspace_bytes, double* scores_out, double* view_abs_rel,
+                   double* view_delta1, long long* view_pixels, void* stream) {
+  OVG_REQUIRE(S > 0 && hw > 0 && S * hw < (1LL << 31), "need S > 0, hw > 0 and S hw < 2^31");
+  EvalDepthBufs w;
+  int rc = carve(__func__, "ovg_eval_depth_workspace_bytes(S, hw)", workspace, workspace_bytes, &w, eval_depth_layout, S, hw);
+  if (rc) return rc;
+  OVG_REQUIRE(gt && pred && view_sel && scores_out && view_abs_rel && view_delta1 && view_pixels, "null operand");
+  ovg::EvalDepthParams& p = w.p;
+  p.gt = gt; p.mask = mask; p.pred = pred; p.view_sel = view_sel;
+  p.scores = scores_out; p.view_abs_rel = view_abs_rel; p.view_delta1 = view_delta1; p.view_pixels = view_pixels;
+  cudaStream_t st = reinterpret_cast<cudaStream_t>(stream);
+  OVG_CUDA(cudaMemsetAsync(p.count, 0, sizeof(unsigned long long), st));
+  ovg::eval_depth_fill_kernel<<<select_blocks(p.ld), ovg::EVAL_THREADS, 0, st>>>(p);
+  if ((rc = post_launch("ovg_eval_depth(fill)"))) return rc;
+  if ((rc = eval_medians(p.cols, p.ld, p.count, 0, w.select, p.sel, p.weight,
+                         "ovg_eval_depth", st)))
+    return rc;
+  ovg::eval_depth_partial_kernel<<<dim3(p.tiles, S), ovg::EVAL_THREADS, 0, st>>>(p);
+  if ((rc = post_launch("ovg_eval_depth(partials)"))) return rc;
+  ovg::eval_depth_finish_kernel<<<1, ovg::EVAL_THREADS, 0, st>>>(p);
+  return post_launch("ovg_eval_depth(finish)");
+}
+
+int ovg_eval_points_keep(const float* gt_ext, const float* gt_intr, const float* gt_depth, const unsigned char* mask,
+                         const float* pred_points, const unsigned char* view_sel, int S, long long hw, float* c2w_out,
+                         unsigned char* keep_out, void* stream) {
+  OVG_REQUIRE(S > 0 && hw > 0 && S * hw < (1LL << 31), "need S > 0, hw > 0 and S hw < 2^31");
+  OVG_REQUIRE(gt_ext && gt_intr && gt_depth && pred_points && view_sel && c2w_out && keep_out, "null operand");
+  const ovg::EvalKeepParams p{gt_ext, gt_intr, gt_depth, mask, pred_points, view_sel, S, hw, c2w_out, keep_out};
+  ovg::eval_points_keep_kernel<<<select_blocks(S * hw), ovg::EVAL_THREADS, 0, reinterpret_cast<cudaStream_t>(stream)>>>(p);
+  return post_launch("ovg_eval_points_keep");
+}
+
+long long ovg_eval_points_workspace_bytes(int S, int H, int W) {
+  return (S > 0 && H > 0 && W > 0 && static_cast<long long>(S) * H * W < (1LL << 30))
+             ? layout_bytes(eval_points_layout, S, H, W) : -1;
+}
+
+int ovg_eval_points(const float* points, const unsigned char* keep, int S, int H, int W, const void* match_workspace,
+                    long long match_workspace_bytes, void* workspace, long long workspace_bytes, double* acc_dist,
+                    double* comp_dist, double* scores_out, void* stream) {
+  OVG_REQUIRE(S > 0 && H > 0 && W > 0 && static_cast<long long>(S) * H * W < (1LL << 30), "need S H W < 2^30");
+  const long long cap = static_cast<long long>(S) * H * W;
+  ovg::MatchParams m;
+  int rc = match_check(__func__, 2, cap, 1, match_workspace, match_workspace_bytes, &m);
+  if (rc) return rc;
+  EvalPointsBufs w;
+  rc = carve(__func__, "ovg_eval_points_workspace_bytes(S, H, W)", workspace, workspace_bytes, &w, eval_points_layout, S, H, W);
+  if (rc) return rc;
+  OVG_REQUIRE(points && keep && acc_dist && comp_dist && scores_out, "null operand");
+  ovg::EvalPointsParams& p = w.p;
+  p.m = m; p.points = points; p.keep = keep;
+  p.dist[0] = acc_dist; p.dist[1] = comp_dist; p.scores = scores_out;
+  cudaStream_t st = reinterpret_cast<cudaStream_t>(stream);
+  ovg::eval_normals_kernel<<<select_blocks(2 * cap), ovg::EVAL_THREADS, 0, st>>>(p);
+  if ((rc = post_launch("ovg_eval_points(normals)"))) return rc;
+  ovg::eval_points_dist_kernel<<<dim3(ovg::EVAL_DIST_BLOCKS, 2), ovg::EVAL_THREADS, 0, st>>>(p);
+  if ((rc = post_launch("ovg_eval_points(distances)"))) return rc;
+  if ((rc = eval_medians(p.cols, p.ld, p.count, 1, w.select, p.sel, p.weight,
+                         "ovg_eval_points", st)))
+    return rc;
+  ovg::eval_points_finish_kernel<<<1, 32, 0, st>>>(p);
+  return post_launch("ovg_eval_points(finish)");
 }
 
 }  // extern "C"

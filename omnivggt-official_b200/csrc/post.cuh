@@ -165,23 +165,36 @@ struct SelectParams {
 // Computed here with explicitly rounded operations, so no host compiler or contraction changes them.
 // Also zeroes the histograms, the NaN counter and the optional kept-counter: one tiny launch instead of host-side copies
 // (graph-capturable).  g goes to *weight, the out[2] of the selection.
+// The ranks and weight above into state[0..5] and *weight; n = 0 selects ranks 0 (callers ignore the result).
+__device__ __forceinline__ void select_init_ranks(long long n, float percent, unsigned long long* state, float* weight) {
+  if (n < 1) n = 1;
+  const float last = __ll2float_rn(n - 1);
+  const float vi = __fmul_rn(last, __fdiv_rn(percent, 100.0f));
+  unsigned long long r0 = static_cast<unsigned long long>(n - 1), r1 = r0;
+  float g = __fadd_rn(vi, 1.0f);
+  if (vi < last) {
+    r0 = __float2ull_rd(vi);
+    // numpy's floor(vi) + 1 is an fp32 sum: above 2^24 it rounds to even, to r0 or r0 + 2.  r0 + 2 can be n (first at
+    // n = 2^24 + 4), where numpy itself fails with 'kth out of bounds'; the last rank is taken there.
+    r1 = __float2ull_rd(__fadd_rn(__ull2float_rn(r0), 1.0f));
+    if (r1 > static_cast<unsigned long long>(n - 1)) r1 = n - 1;
+    g = __fsub_rn(vi, __ull2float_rn(r0));
+  }
+  state[0] = r0; state[1] = r1; state[2] = 0; state[3] = 0; state[4] = r0; state[5] = r1;
+  *weight = g;
+}
+
+// numpy's _lerp of the two order statistics, each operation rounded on its own: g >= 0.5 ? hi - d (1 - g) : lo + d g,
+// d = hi - lo
+__device__ __forceinline__ float select_lerp(float lo, float hi, float g) {
+  const float d = __fsub_rn(hi, lo);
+  return g >= 0.5f ? __fsub_rn(hi, __fmul_rn(d, __fsub_rn(1.0f, g))) : __fadd_rn(lo, __fmul_rn(d, g));
+}
+
 __global__ void select_init_kernel(unsigned long long* state, unsigned int* hist, long long n, float percent, float* weight,
                                    unsigned int* nan, unsigned long long* count) {
   if (threadIdx.x == 0) {
-    const float last = __ll2float_rn(n - 1);
-    const float vi = __fmul_rn(last, __fdiv_rn(percent, 100.0f));
-    unsigned long long r0 = static_cast<unsigned long long>(n - 1), r1 = r0;
-    float g = __fadd_rn(vi, 1.0f);
-    if (vi < last) {
-      r0 = __float2ull_rd(vi);
-      // numpy's floor(vi) + 1 is an fp32 sum: above 2^24 it rounds to even, to r0 or r0 + 2.  r0 + 2 can be n (first at
-      // n = 2^24 + 4), where numpy itself fails with 'kth out of bounds'; the last rank is taken there.
-      r1 = __float2ull_rd(__fadd_rn(__ull2float_rn(r0), 1.0f));
-      if (r1 > static_cast<unsigned long long>(n - 1)) r1 = n - 1;
-      g = __fsub_rn(vi, __ull2float_rn(r0));
-    }
-    state[0] = r0; state[1] = r1; state[2] = 0; state[3] = 0; state[4] = r0; state[5] = r1;
-    *weight = g;
+    select_init_ranks(n, percent, state, weight);
     *nan = 0;
     if (count) *count = 0;
   }
@@ -253,10 +266,7 @@ __global__ void select_decide_kernel(const SelectParams p) {
   for (int i = threadIdx.x; i < 512; i += 32) p.hist[i] = 0;
   if (p.nan && p.pass == 3 && threadIdx.x == 0) {
     __threadfence_block();
-    // numpy's _lerp, each operation rounded on its own: g >= 0.5 ? hi - d (1 - g) : lo + d g, d = hi - lo
-    const float lo = p.out[0], hi = p.out[1], g = p.out[2];
-    const float d = __fsub_rn(hi, lo);
-    const float t = g >= 0.5f ? __fsub_rn(hi, __fmul_rn(d, __fsub_rn(1.0f, g))) : __fadd_rn(lo, __fmul_rn(d, g));
+    const float t = select_lerp(p.out[0], p.out[1], p.out[2]);
     p.out[2] = *p.nan ? __int_as_float(0x7fc00000) : t;
   }
 }

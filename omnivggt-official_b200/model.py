@@ -274,6 +274,7 @@ class OmniVGGT(nn.Module, PyTorchModelHubMixin):
     tracks = staticmethod(SC.tracks)
     bundle_adjust = staticmethod(SC.bundle_adjust)
     fused_mesh = staticmethod(SC.fused_mesh)
+    evaluate = staticmethod(SC.evaluate)
     _kept_views = staticmethod(SC._kept_views)          # their shared helpers, reached from the class as before
     _align = staticmethod(SC._align)
 

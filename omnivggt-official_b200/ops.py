@@ -197,15 +197,18 @@ def pose_decode(pose_enc, H: int, W: int):
     return ext, intr, c2w
 
 
-def unproject_depth(depth, intrinsic, cam2world, H: int, W: int):
-    """depth fp32 [K, H, W], intrinsic fp32 [K, 3, 3], cam2world fp32 [K, 3, 4] -> world points fp32 [K, H, W, 3]."""
+def unproject_depth(depth, intrinsic, cam2world, H: int, W: int, out: Optional[torch.Tensor] = None):
+    """depth fp32 [K, H, W], intrinsic fp32 [K, 3, 3], cam2world fp32 [K, 3, 4] -> world points fp32 [K, H, W, 3], written
+    into ``out`` (contiguous, K H W 3 elements) when given."""
     check_operand(depth, "depth", F32)
     d = depth.contiguous()
     K = d.numel() // (H * W)
     intr, c2w = intrinsic.contiguous(), cam2world.contiguous()
     check_operand(intr, "intrinsic", F32, numel=K * 9)
     check_operand(c2w, "cam2world", F32, numel=K * 12)
-    world = torch.empty(K, H, W, 3, device=d.device, dtype=F32)
+    if out is not None:
+        check_operand(out, "out", F32, numel=K * H * W * 3, contiguous=True)
+    world = torch.empty(K, H, W, 3, device=d.device, dtype=F32) if out is None else out.view(K, H, W, 3)
     L.check(L.lib().ovg_unproject_depth(d.data_ptr(), intr.data_ptr(), c2w.data_ptr(), world.data_ptr(), K, H, W, L.stream()))
     return world
 
@@ -539,7 +542,7 @@ class Matcher:
         self.P = pairs.shape[0]
         if keep is not None:
             check_operand(keep, "keep", torch.uint8, numel=self.V * self.cap, contiguous=True)
-        self.pairs = pairs
+        self.points, self.keep, self.pairs = points, keep, pairs
         lib = L.lib()
         self.ws = workspace(points.device, "ovg_match_workspace_bytes", self.V, self.cap, self.P)
         self._counts = torch.zeros(self.P + 1, device=points.device, dtype=torch.int64)
@@ -615,3 +618,82 @@ class Tracker:
             mt.ws.numel(), self.ws.data_ptr(), self.ws.numel(), *(t.data_ptr() if t.numel() else None for t in out.values()),
             L.stream()))
         return out
+
+
+def eval_pose(gt_ext, gt_intr, pred_ext, views):
+    """ovg_eval_pose: gt_ext, pred_ext fp32 [S, 3, 4] world-to-camera, gt_intr fp32 [S, 3, 3], views int32 [m] (1 <= m <= 8192),
+    contiguous on the device.  Returns (sim3 fp64 [4, 4], stats fp64 [4], pairs int32 [P, 2], pair_errors fp64 [P, 2],
+    rpe fp64 [R, 2], scores fp64 [12]) with P = max(m (m - 1) / 2, 1) and R = max(m - 1, 1) rows, of which the n views with a
+    camera (stats[0]) fill the first n (n - 1) / 2 and n - 1.  Nine launches, no host read."""
+    check_operand(gt_ext, "gt_ext", F32, shape=(None, 3, 4), contiguous=True)
+    S = gt_ext.shape[0]
+    check_operand(gt_intr, "gt_intr", F32, shape=(S, 3, 3), contiguous=True)
+    check_operand(pred_ext, "pred_ext", F32, shape=(S, 3, 4), contiguous=True)
+    check_operand(views, "views", torch.int32, shape=(None,), contiguous=True)
+    m = views.shape[0]
+    dev = gt_ext.device
+    ws = workspace(dev, "ovg_eval_pose_workspace_bytes", m)
+    f64 = dict(device=dev, dtype=torch.float64)
+    out = (torch.empty(4, 4, **f64), torch.empty(4, **f64),
+           torch.empty(max(m * (m - 1) // 2, 1), 2, device=dev, dtype=torch.int32),
+           torch.empty(max(m * (m - 1) // 2, 1), 2, **f64), torch.empty(max(m - 1, 1), 2, **f64), torch.empty(12, **f64))
+    L.check(L.lib().ovg_eval_pose(gt_ext.data_ptr(), gt_intr.data_ptr(), pred_ext.data_ptr(), views.data_ptr(), m, ws.data_ptr(),
+                                  ws.numel(), *(t.data_ptr() for t in out), L.stream()))
+    return out
+
+
+def eval_depth(gt, mask, pred, view_sel):
+    """ovg_eval_depth: gt, pred fp32 [S, hw], mask uint8 [S, hw] or None, view_sel uint8 [S], contiguous on the device.
+    Returns (scores fp64 [10], view_abs_rel fp64 [S], view_delta1 fp64 [S], view_pixels int64 [S]).  No host read."""
+    check_operand(gt, "gt", F32, shape=(None, None), contiguous=True)
+    S, hw = gt.shape
+    check_operand(pred, "pred", F32, shape=(S, hw), contiguous=True)
+    if mask is not None:
+        check_operand(mask, "mask", torch.uint8, shape=(S, hw), contiguous=True)
+    check_operand(view_sel, "view_sel", torch.uint8, shape=(S,), contiguous=True)
+    dev = gt.device
+    ws = workspace(dev, "ovg_eval_depth_workspace_bytes", S, hw)
+    out = (torch.empty(10, device=dev, dtype=torch.float64), torch.empty(S, device=dev, dtype=torch.float64),
+           torch.empty(S, device=dev, dtype=torch.float64), torch.empty(S, device=dev, dtype=torch.int64))
+    L.check(L.lib().ovg_eval_depth(gt.data_ptr(), L.ptr(mask), pred.data_ptr(), view_sel.data_ptr(), S, hw, ws.data_ptr(),
+                                   ws.numel(), *(t.data_ptr() for t in out), L.stream()))
+    return out
+
+
+def eval_points_keep(gt_ext, gt_intr, gt_depth, mask, pred_points, view_sel):
+    """ovg_eval_points_keep: gt_ext fp32 [S, 3, 4], gt_intr fp32 [S, 3, 3], gt_depth fp32 [S, hw], mask uint8 [S, hw] or None,
+    pred_points fp32 [S, hw, 3], view_sel uint8 [S], contiguous on the device.  Returns (cam2world fp32 [S, 3, 4], keep uint8
+    [2, S hw], the shared pixel set once per cloud).  One launch."""
+    check_operand(gt_depth, "gt_depth", F32, shape=(None, None), contiguous=True)
+    S, hw = gt_depth.shape
+    check_operand(gt_ext, "gt_ext", F32, shape=(S, 3, 4), contiguous=True)
+    check_operand(gt_intr, "gt_intr", F32, shape=(S, 3, 3), contiguous=True)
+    if mask is not None:
+        check_operand(mask, "mask", torch.uint8, shape=(S, hw), contiguous=True)
+    check_operand(pred_points, "pred_points", F32, shape=(S, hw, 3), contiguous=True)
+    check_operand(view_sel, "view_sel", torch.uint8, shape=(S,), contiguous=True)
+    dev = gt_depth.device
+    c2w = torch.empty(S, 3, 4, device=dev, dtype=F32)
+    keep = torch.empty(2, S * hw, device=dev, dtype=torch.uint8)
+    L.check(L.lib().ovg_eval_points_keep(gt_ext.data_ptr(), gt_intr.data_ptr(), gt_depth.data_ptr(), L.ptr(mask),
+                                         pred_points.data_ptr(), view_sel.data_ptr(), S, hw, c2w.data_ptr(), keep.data_ptr(),
+                                         L.stream()))
+    return c2w, keep
+
+
+def eval_points(matcher: Matcher, S: int, H: int, W: int):
+    """ovg_eval_points over a Matcher of the two clouds (V = 2: the aligned prediction, the ground truth; cap = S H W; the one
+    pair (0, 1)), built from points fp32 [2, S H W, 3] and keep uint8 [2, S H W].  Returns (acc_dist fp64 [S H W], comp_dist
+    fp64 [S H W], of which the first n are set, scores fp64 [9]).  21 launches, no host read."""
+    if (matcher.V, matcher.cap, matcher.P) != (2, S * H * W, 1):
+        raise ValueError(f"eval_points needs a Matcher over 2 views of {S * H * W} points and one pair, got "
+                         f"{(matcher.V, matcher.cap, matcher.P)}")
+    check_operand(matcher.points, "points", F32, shape=(2, S * H * W, 3), contiguous=True)
+    check_operand(matcher.keep, "keep", torch.uint8, numel=2 * S * H * W, contiguous=True)
+    dev = matcher.ws.device
+    ws = workspace(dev, "ovg_eval_points_workspace_bytes", S, H, W)
+    out = (torch.empty(S * H * W, device=dev, dtype=torch.float64), torch.empty(S * H * W, device=dev, dtype=torch.float64),
+           torch.empty(9, device=dev, dtype=torch.float64))
+    L.check(L.lib().ovg_eval_points(matcher.points.data_ptr(), matcher.keep.data_ptr(), S, H, W, matcher.ws.data_ptr(),
+                                    matcher.ws.numel(), ws.data_ptr(), ws.numel(), *(t.data_ptr() for t in out), L.stream()))
+    return out

@@ -1,5 +1,6 @@
 """A predictions dict on the device: its cameras and world points (``postprocess``), and the sky, point cloud, mesh,
-fused mesh, matches and tracks of one scene, and the bundle adjustment of those tracks.  They read no weight; ``OmniVGGT`` exposes each
+fused mesh, matches and tracks of one scene, the bundle adjustment of those tracks, and the scores of a scene against its
+ground truth.  They read no weight; ``OmniVGGT`` exposes each
 under the same name.  Each checks its arguments before any library call (``_check_views``), then takes the scene's views
 from ``_kept_views``."""
 from __future__ import annotations
@@ -461,3 +462,166 @@ def fused_mesh(predictions: Dict[str, object], *, resolution: int = 512, conf_pe
     size 0).  Two host reads: the bounds with the first camera, then the mesh's sizes.  Kept points that are not finite raise
     ValueError."""
     return _fusion(predictions, resolution, conf_percent, conf_floor, scene, mask_sky)[0]
+
+
+EVAL_MAX_CAMERA_VIEWS = 8192          # pose group: at most 33.5 M pairs (537 MB of pair errors)
+
+
+def _gt_tensor(t, name: str, S: int, tail, device, scene: int, alt_tail=None) -> Optional[torch.Tensor]:
+    """A ground-truth tensor [B, S, *tail] or [S, *tail] (or *alt_tail) of the scene, checked: None stays None."""
+    if t is None:
+        return None
+    if not torch.is_tensor(t):
+        raise ValueError(f"{name} must be a tensor, got {type(t).__name__}")
+    shape = tuple(t.shape)
+    has_b = None
+    for tl in [tuple(tail)] + ([tuple(alt_tail)] if alt_tail is not None else []):
+        if shape == (S,) + tl:
+            has_b = False
+        elif len(shape) == len(tl) + 2 and shape[1:] == (S,) + tl and 0 <= scene < shape[0]:
+            has_b = True
+    if has_b is None:
+        tails = [tail] + ([alt_tail] if alt_tail is not None else [])
+        want = " or ".join(f"[B, {S}, {', '.join(map(str, tl))}] / [{S}, {', '.join(map(str, tl))}]" for tl in tails)
+        raise ValueError(f"{name} must have shape {want}, got {list(shape)}")
+    allowed = (torch.bool, torch.uint8) if name == "mask" else ()
+    if not (t.dtype.is_floating_point or t.dtype in allowed):
+        raise ValueError(f"{name} must be a floating tensor{' (or bool / uint8)' if allowed else ''}, got {t.dtype}")
+    if t.device != device:
+        raise ValueError(f"{name} is on {t.device}, the predictions on {device}")
+    return t[scene] if has_b else t
+
+
+def _check_eval_views(views, S: int) -> List[int]:
+    """The scored views, ascending: every view when None, else distinct integers in [0, S)."""
+    if views is None:
+        return list(range(S))
+    views = list(views)
+    if not all(geometry._is_int(v) for v in views):
+        raise ValueError(f"views must be integers, got {views!r}")
+    if any(not 0 <= v < S for v in views):
+        raise ValueError(f"views must be in [0, {S}), got {views!r}")
+    if len(set(int(v) for v in views)) != len(views):
+        raise ValueError(f"views must not repeat, got {views!r}")
+    if not views:
+        raise ValueError("views must not be empty")
+    return sorted(int(v) for v in views)
+
+
+@torch.no_grad()
+def evaluate(predictions: Dict[str, object], *, extrinsics=None, intrinsics=None, depth=None, mask=None, views=None,
+             source: str = "depth", scene: int = 0) -> Dict[str, Dict[str, torch.Tensor]]:
+    """Scores of one scene's predictions against its ground truth, on the device (libovg ovg_eval_*).  The reference scores
+    trajectories only, on the host through evo (vo_eval.py:163-246 eval_metrics); the definitions are in include/ovg.h and
+    INTEGRATION.md ("Evaluation").
+
+    Ground truth in the layout ``preprocess.load_images_and_cameras`` returns and the forward takes, with or without B:
+    ``extrinsics`` world-to-camera [B, S, 3, 4] / [B, S, 4, 4], ``intrinsics`` [B, S, 3, 3], ``depth`` [B, S, H, W(, 1)] at
+    the model's resolution, ``mask`` [B, S, H, W] (non-zero: valid; default every pixel).  A view has a ground-truth camera
+    when fx, fy > 0 and its extrinsic is finite (the loader's zero placeholders have none); a pixel has ground-truth depth
+    when its mask is set and the depth is > 0 and finite.  ``views`` (default: all) restricts every metric to those views,
+    e.g. the ones whose ground truth did not go into the forward.
+
+    Predictions: cameras ``extrinsic`` (decoded from ``pose_enc`` where missing, as ``tracks`` takes them), depth ``depth``,
+    points ``world_points_from_depth`` (``source="depth"``; unprojected through the decoded cameras when missing) or
+    ``world_points`` (``"pointmap"``).  A group is computed when its ground truth is given:
+      "pose" (extrinsics and intrinsics): ``ate``, ``rpe_trans``, ``rpe_rot`` (evo's APE / RPE after the Umeyama Sim(3) of
+          the camera centres, as vo_eval.py:190-236), ``auc`` / ``rra`` / ``rta`` fp64 [3] at 5, 10, 30 degrees (the
+          pairwise protocol of the VGGT family), ``sim3`` fp64 [4, 4], ``views`` (the count n), ``pairs`` int32 [P, 2],
+          ``pair_errors`` fp64 [P, 2] (RRE, RTE in degrees), ``rpe_errors`` fp64 [n - 1, 2] (|t|, degrees).
+      "depth" (depth): ``abs_rel``, ``sq_rel``, ``rmse``, ``delta`` fp64 [3] after per-scene median scaling ``scale``, with
+          ``pixels``, ``view_abs_rel``, ``view_delta1``, ``view_pixels`` [S].  No valid pixel gives NaN and 0 pixels.
+      "points" (depth and cameras): ``acc``, ``acc_median``, ``comp``, ``comp_median``, ``chamfer`` (nearest-neighbour
+          distances between the Umeyama-aligned prediction and the ground-truth points, exact), ``nc_acc``, ``nc_comp``, ``nc``
+          (normal consistency with grid normals, not Open3D's k-NN normals), ``pixels``, ``sim3``, ``acc_dist`` /
+          ``comp_dist`` fp64 [pixels].
+    Every value is a device tensor.  Host reads: the pose fit's status (``ovg_eval_pose``), the point fit's status
+    (``ovg_sim3_estimate``) and the matcher's non-finite flag (``ovg_match_query``): at most three.  ValueError before any
+    device work for wrong shapes or dtypes, bad ``views``, ``source="pointmap"`` without ``world_points``, no ground truth,
+    more than 8192 scored views with cameras and S H W >= 2^31; after a read, for fewer than 3 views or pixels to align, or
+    collinear ones."""
+    if source not in ("depth", "pointmap"):
+        raise ValueError(f"source must be 'depth' or 'pointmap', got {source!r}")
+    images = predictions["images"]
+    S, _, H, W = _of_scene(images, 3, scene).shape
+    dev = images.device
+    if S * H * W >= 2 ** 31:
+        raise ValueError(f"evaluate needs views * H * W < 2^31, got {S} x {H} x {W}")
+    gext = _gt_tensor(extrinsics, "extrinsics", S, (3, 4), dev, scene, alt_tail=(4, 4))
+    gint = _gt_tensor(intrinsics, "intrinsics", S, (3, 3), dev, scene)
+    gdep = _gt_tensor(depth, "depth", S, (H, W), dev, scene, alt_tail=(H, W, 1))
+    gmask = _gt_tensor(mask, "mask", S, (H, W), dev, scene)
+    if (gext is None) != (gint is None):
+        raise ValueError("ground-truth cameras need both extrinsics and intrinsics")
+    cams = gext is not None
+    if not cams and gdep is None:
+        raise ValueError("evaluate needs ground truth: extrinsics and intrinsics, depth, or both")
+    if gmask is not None and gdep is None:
+        raise ValueError("mask needs depth")
+    sel = _check_eval_views(views, S)
+    if cams and len(sel) > EVAL_MAX_CAMERA_VIEWS:
+        raise ValueError(f"the pose group scores at most {EVAL_MAX_CAMERA_VIEWS} views, got {len(sel)}")
+    if cams and not ("extrinsic" in predictions or "pose_enc" in predictions):
+        raise ValueError("the pose group needs the predictions' extrinsic, or pose_enc to decode it from")
+    if gdep is not None and "depth" not in predictions:
+        raise ValueError("the depth group needs the predictions' depth")
+    if cams and gdep is not None:
+        if source == "pointmap" and "world_points" not in predictions:
+            raise ValueError("source='pointmap' needs the predictions' world_points")
+        if source == "depth" and "world_points_from_depth" not in predictions and "pose_enc" not in predictions:
+            raise ValueError("source='depth' needs world_points_from_depth, or pose_enc and depth to compute it")
+
+    out: Dict[str, Dict[str, torch.Tensor]] = {}
+    hw = H * W
+    view_sel = torch.zeros(S, dtype=torch.uint8)
+    view_sel[sel] = 1
+    view_sel = view_sel.to(dev)
+    if cams:
+        gext = gext[..., :3, :4].float().contiguous()
+        gint = gint.float().contiguous()
+        if "extrinsic" in predictions:
+            pext = _of_scene(predictions["extrinsic"], 2, scene).float().contiguous()
+        else:
+            pext, _, _ = decode_cameras(_of_scene(predictions["pose_enc"], 1, scene), None, H, W)
+        sim3, stats, pairs, perr, rpe, sc = ops.eval_pose(gext, gint, pext, torch.tensor(sel, dtype=torch.int32).to(dev))
+        n_views, status = (int(v) for v in ops.host_read(stats[:2]).tolist())
+        if status:
+            raise ValueError(f"evaluate: the pose alignment is degenerate: {geometry.SIM3_STATUS[status]}")
+        P = n_views * (n_views - 1) // 2
+        out["pose"] = {"ate": sc[0], "rpe_trans": sc[1], "rpe_rot": sc[2], "auc": sc[3:6], "rra": sc[6:9], "rta": sc[9:12],
+                       "sim3": sim3, "views": stats[0].long(), "pairs": pairs[:P], "pair_errors": perr[:P],
+                       "rpe_errors": rpe[:n_views - 1]}
+    if gdep is not None:
+        gd = gdep.float().reshape(S, hw).contiguous()
+        pd = _of_scene(predictions["depth"], 3, scene).float().reshape(S, hw).contiguous()
+        m8 = None if gmask is None else (gmask != 0).to(torch.uint8).reshape(S, hw).contiguous()
+        sc, var, vd1, vpix = ops.eval_depth(gd, m8, pd, view_sel)
+        out["depth"] = {"pixels": sc[0].long(), "scale": sc[1], "median_gt": sc[2], "median_pred": sc[3], "abs_rel": sc[4],
+                        "sq_rel": sc[5], "rmse": sc[6], "delta": sc[7:10], "view_abs_rel": var, "view_delta1": vd1,
+                        "view_pixels": vpix}
+    if cams and gdep is not None:
+        if source == "pointmap":
+            pts = _of_scene(predictions["world_points"], 3, scene)
+        elif "world_points_from_depth" in predictions:
+            pts = _of_scene(predictions["world_points_from_depth"], 3, scene)
+        else:
+            _, _, pts = decode_cameras(_of_scene(predictions["pose_enc"], 1, scene), _of_scene(predictions["depth"], 3, scene),
+                                       H, W)
+        pts = pts.float().reshape(S, hw, 3).contiguous()
+        c2w, keep = ops.eval_points_keep(gext, gint, gd, m8, pts, view_sel)
+        clouds = torch.empty(2, S * hw, 3, device=dev, dtype=torch.float32)
+        ops.unproject_depth(gd.view(S, H, W), gint, c2w, H, W, out=clouds[1])
+        sim3p, stp = ops.sim3_estimate(pts.view(-1, 3), clouds[1], keep[0])
+        n_pix, status = (int(v) for v in ops.host_read(stp[:2]).tolist())
+        if status:
+            raise ValueError(f"evaluate: the point alignment is degenerate: {geometry.SIM3_STATUS[status]}")
+        ops.sim3_apply(sim3p, S, hw, points=((pts.view(-1, 3), clouds[0]),))
+        mt = ops.Matcher(clouds, keep, torch.tensor([[0, 1]], dtype=torch.int32).to(dev))
+        _, nonfinite = mt.counts()
+        if nonfinite:
+            raise ValueError("evaluate: an aligned or ground-truth point is not finite")
+        acc, comp, sc = ops.eval_points(mt, S, H, W)
+        out["points"] = {"pixels": sc[0].long(), "acc": sc[1], "acc_median": sc[2], "comp": sc[3], "comp_median": sc[4],
+                         "chamfer": sc[5], "nc_acc": sc[6], "nc_comp": sc[7], "nc": sc[8], "sim3": sim3p,
+                         "acc_dist": acc[:n_pix], "comp_dist": comp[:n_pix]}
+    return out
