@@ -192,7 +192,8 @@ int ovg_prepare_cameras(const float* c2w, const float* kin, const float* geom, c
 int ovg_pose_decode(const float* pose_enc, float* extrinsic, float* intrinsic, float* cam2world, int K, int H, int W,
                     void* stream);
 
-/* ovg_unproject_depth: world[k,v,u,:] = R_c2w ((u-cu) d/fu, (v-cv) d/fv, d) + t_c2w; depth fp32 [K,H,W], world fp32 [K,H,W,3].
+/* ovg_unproject_depth: world[k,v,u,:] = R_c2w ((u-cu) d/fu, (v-cv) d/fv, d) + t_c2w; depth fp32 [K,H,W], world fp32 [K,H,W,3],
+ * both 16-byte aligned; K <= 65535.
  * utils/geometry.py:151-180 (unproject_depth_map_to_point_map), :183-264; visual_util.py:42-73. */
 int ovg_unproject_depth(const float* depth, const float* intrinsic, const float* cam2world, float* world, int K, int H, int W,
                         void* stream);
@@ -491,7 +492,8 @@ int ovg_sim3_apply(const double* sim3, int views, long long hw, const float* poi
  * fixed grid, then in a fixed order, and every count is an integer: results are bit-identical from run to run.  The launch
  * counts below do not depend on S, m or the number of pairs.  Workspaces are 256-byte aligned, of the size their query gives.
  * ovg_eval_pose: the m <= 8192 distinct scene views views[m] (int32); the n of them with a ground-truth camera and a finite
- *     prediction count, in that order.  Poses are camera-to-world P = [R^T | c], c = -R^T t, formed in fp64.
+ *     prediction whose two centres are finite in fp32 count, in that order.  Poses are camera-to-world P = [R^T | c],
+ *     c = -R^T t, formed in fp64.
  *     - The ATE alignment of vo_eval.py:190-199 (evo APE, translation part, align and correct_scale): ovg_sim3_estimate of the
  *       predicted centres onto the ground-truth centres, each rounded once to fp32, over a keep mask of the n views.
  *       sim3_out / stats_out are that call's outputs; stats_out[0] = n, stats_out[2] = the ATE (its RMS residual).
@@ -510,7 +512,8 @@ int ovg_sim3_apply(const double* sim3, int views, long long hw, const float* poi
  *     numpy.percentile(v, 50) of the fp32 values (exact radix selection); with sp = s p in fp64:
  *     scores_out fp64 [10] = pixels, s, median(g), median(p), abs_rel = mean |sp - g| / g, sq_rel = mean (sp - g)^2 / g,
  *     rmse = sqrt(mean (sp - g)^2), delta (3) = fractions with max(sp / g, g / sp) < 1.25, 1.25^2, 1.25^3; NaN when no pixel
- *     counts.  Per view: view_abs_rel, view_delta1 fp64 [S] (NaN without pixels), view_pixels int64 [S].  21 launches.
+ *     counts.  Per view: view_abs_rel, view_delta1 fp64 [S] (NaN without pixels), view_pixels int64 [S].  Any S with
+ *     S hw < 2^31.  21 launches.
  * ovg_eval_points_keep: the inverse [R^T | -R^T t] of each ground-truth extrinsic (fp64, rounded once) into c2w_out fp32
  *     [S, 3, 4], for ovg_unproject_depth of the ground-truth depth; and the pixel set shared by both clouds into both rows
  *     of keep_out uint8 [2, S hw]: a selected view with a ground-truth camera, the mask set, g > 0 finite, and a finite
@@ -522,7 +525,8 @@ int ovg_sim3_apply(const double* sim3, int views, long long hw, const float* poi
  *     (d^2, lowest index) minimum from each kept predicted point to the ground truth, comp_dist fp64 [n] the other way, both
  *     in kept (row-major) order; outputs are sized for S H W points.  scores_out fp64 [9] = n, acc, acc_median, comp,
  *     comp_median, chamfer = (acc + comp) / 2, nc_acc, nc_comp (mean |n . n_nn| over the points where both have a normal; NaN
- *     when none), nc = their mean.  Medians: numpy.percentile(50) of the distances rounded to fp32.  21 launches. */
+ *     when none), nc = their mean.  Medians: numpy.percentile(50) of the distances rounded to fp32.  S H W < 2^30 (the
+ *     matcher's limit); the ground truth's unprojection further needs S <= 65535.  21 launches. */
 long long ovg_eval_pose_workspace_bytes(int m);
 int ovg_eval_pose(const float* gt_ext, const float* gt_intr, const float* pred_ext, const int* views, int m, void* workspace,
                   long long workspace_bytes, double* sim3_out, double* stats_out, int* pairs_out, double* pair_errors_out,

@@ -108,16 +108,19 @@ __global__ void __launch_bounds__(1024) eval_pose_prep_kernel(const EvalPosePara
     const int v = p.views[k];
     const float* Eg = p.gt_ext + 12LL * v;
     const float* Ep = p.pred_ext + 12LL * v;
-    const bool ok = eval_camera_ok(Eg, p.gt_intr + 9LL * v) && eval_finite12(Ep);
-    p.keep[k] = ok ? 1 : 0;
+    bool ok = eval_camera_ok(Eg, p.gt_intr + 9LL * v) && eval_finite12(Ep);
     double Pg[12], Pp[12];
     eval_c2w(Eg, Pg);
     eval_c2w(Ep, Pp);
 #pragma unroll
     for (int a = 0; a < 3; ++a) {
-      p.centre_gt[3 * k + a] = static_cast<float>(Pg[9 + a]);
-      p.centre_pred[3 * k + a] = static_cast<float>(Pp[9 + a]);
+      const float cg = static_cast<float>(Pg[9 + a]), cp = static_cast<float>(Pp[9 + a]);
+      p.centre_gt[3 * k + a] = cg;
+      p.centre_pred[3 * k + a] = cp;
+      // a finite extrinsic whose centre overflows fp32 would be dropped by the fit (sim3_pair) but not here: drop it here
+      ok = ok && isfinite(cg) && isfinite(cp);
     }
+    p.keep[k] = ok ? 1 : 0;
   }
   __syncthreads();
   __shared__ int base;
@@ -400,29 +403,31 @@ __device__ __forceinline__ double eval_depth_scale(const EvalDepthParams& p, flo
   return __ddiv_rn(static_cast<double>(mg), static_cast<double>(mp));
 }
 
-// grid (tiles, S)
+// grid (tiles, min(S, 65535)): the y blocks stride over the views, so any S launches; each (view, tile) partial is the same
 __global__ void __launch_bounds__(EVAL_THREADS) eval_depth_partial_kernel(const EvalDepthParams p) {
-  const int v = blockIdx.y;
   float mg, mp;
   const double s = eval_depth_scale(p, mg, mp);
-  double acc[EVAL_DEPTH_P] = {0.0, 0.0, 0.0, 0.0, 0.0, 0.0, 0.0};
   const long long base = static_cast<long long>(blockIdx.x) * COMPACT_TILE;
-  for (int it = 0; it < COMPACT_ITERS; ++it) {
-    const long long i = base + it * COMPACT_THREADS + threadIdx.x;
-    float g, d;
-    if (i < p.hw && eval_depth_valid(p, v * p.hw + i, g, d)) {
-      const double gd = g, sp = __dmul_rn(s, static_cast<double>(d)), e = __dsub_rn(sp, gd), e2 = __dmul_rn(e, e);
-      acc[0] = __dadd_rn(acc[0], __ddiv_rn(fabs(e), gd));
-      acc[1] = __dadd_rn(acc[1], __ddiv_rn(e2, gd));
-      acc[2] = __dadd_rn(acc[2], e2);
-      acc[3] += 1.0;
-      const double r = fmax(__ddiv_rn(sp, gd), __ddiv_rn(gd, sp));
-      acc[4] += r < 1.25 ? 1.0 : 0.0;
-      acc[5] += r < 1.5625 ? 1.0 : 0.0;
-      acc[6] += r < 1.953125 ? 1.0 : 0.0;
+  for (int v = blockIdx.y; v < p.S; v += gridDim.y) {
+    double acc[EVAL_DEPTH_P] = {0.0, 0.0, 0.0, 0.0, 0.0, 0.0, 0.0};
+    for (int it = 0; it < COMPACT_ITERS; ++it) {
+      const long long i = base + it * COMPACT_THREADS + threadIdx.x;
+      float g, d;
+      if (i < p.hw && eval_depth_valid(p, v * p.hw + i, g, d)) {
+        const double gd = g, sp = __dmul_rn(s, static_cast<double>(d)), e = __dsub_rn(sp, gd), e2 = __dmul_rn(e, e);
+        acc[0] = __dadd_rn(acc[0], __ddiv_rn(fabs(e), gd));
+        acc[1] = __dadd_rn(acc[1], __ddiv_rn(e2, gd));
+        acc[2] = __dadd_rn(acc[2], e2);
+        acc[3] += 1.0;
+        const double r = fmax(__ddiv_rn(sp, gd), __ddiv_rn(gd, sp));
+        acc[4] += r < 1.25 ? 1.0 : 0.0;
+        acc[5] += r < 1.5625 ? 1.0 : 0.0;
+        acc[6] += r < 1.953125 ? 1.0 : 0.0;
+      }
     }
+    sim3_block_sum<EVAL_DEPTH_P>(acc, p.part + (static_cast<long long>(v) * p.tiles + blockIdx.x) * EVAL_DEPTH_P);
+    __syncthreads();                // the block sum's shared partials are read before the next view writes them
   }
-  sim3_block_sum<EVAL_DEPTH_P>(acc, p.part + (static_cast<long long>(v) * p.tiles + blockIdx.x) * EVAL_DEPTH_P);
 }
 
 // one CTA of EVAL_THREADS: each view's tiles in order, then the views in order
@@ -432,7 +437,7 @@ __global__ void __launch_bounds__(EVAL_THREADS) eval_depth_finish_kernel(const E
     double t[EVAL_DEPTH_P] = {0.0, 0.0, 0.0, 0.0, 0.0, 0.0, 0.0};
     for (int b = 0; b < p.tiles; ++b)
       for (int k = 0; k < EVAL_DEPTH_P; ++k) t[k] = __dadd_rn(t[k], p.part[(static_cast<long long>(v) * p.tiles + b) * EVAL_DEPTH_P + k]);
-    for (int k = 0; k < EVAL_DEPTH_P; ++k) p.view_tot[v * EVAL_DEPTH_P + k] = t[k];
+    for (int k = 0; k < EVAL_DEPTH_P; ++k) p.view_tot[static_cast<long long>(v) * EVAL_DEPTH_P + k] = t[k];
     p.view_pixels[v] = static_cast<long long>(t[3]);
     p.view_abs_rel[v] = t[3] > 0.0 ? __ddiv_rn(t[0], t[3]) : nan;
     p.view_delta1[v] = t[3] > 0.0 ? __ddiv_rn(t[4], t[3]) : nan;
@@ -441,7 +446,7 @@ __global__ void __launch_bounds__(EVAL_THREADS) eval_depth_finish_kernel(const E
   if (threadIdx.x != 0) return;
   double t[EVAL_DEPTH_P] = {0.0, 0.0, 0.0, 0.0, 0.0, 0.0, 0.0};
   for (int v = 0; v < p.S; ++v)
-    for (int k = 0; k < EVAL_DEPTH_P; ++k) t[k] = __dadd_rn(t[k], p.view_tot[v * EVAL_DEPTH_P + k]);
+    for (int k = 0; k < EVAL_DEPTH_P; ++k) t[k] = __dadd_rn(t[k], p.view_tot[static_cast<long long>(v) * EVAL_DEPTH_P + k]);
   const double n = t[3];
   float mg, mp;
   const double s = eval_depth_scale(p, mg, mp);

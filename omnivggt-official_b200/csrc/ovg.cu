@@ -1860,7 +1860,7 @@ int ovg_eval_depth(const float* gt, const unsigned char* mask, const float* pred
   if ((rc = eval_medians(p.cols, p.ld, p.count, 0, w.select, p.sel, p.weight,
                          "ovg_eval_depth", st)))
     return rc;
-  ovg::eval_depth_partial_kernel<<<dim3(p.tiles, S), ovg::EVAL_THREADS, 0, st>>>(p);
+  ovg::eval_depth_partial_kernel<<<dim3(p.tiles, S < 65535 ? S : 65535), ovg::EVAL_THREADS, 0, st>>>(p);
   if ((rc = post_launch("ovg_eval_depth(partials)"))) return rc;
   ovg::eval_depth_finish_kernel<<<1, ovg::EVAL_THREADS, 0, st>>>(p);
   return post_launch("ovg_eval_depth(finish)");

@@ -465,6 +465,8 @@ def fused_mesh(predictions: Dict[str, object], *, resolution: int = 512, conf_pe
 
 
 EVAL_MAX_CAMERA_VIEWS = 8192          # pose group: at most 33.5 M pairs (537 MB of pair errors)
+EVAL_MAX_POINT_PIXELS = 2 ** 30       # points group: S H W below the matcher's limit
+EVAL_MAX_POINT_VIEWS = 65535          # points group: the unprojection's views
 
 
 def _gt_tensor(t, name: str, S: int, tail, device, scene: int, alt_tail=None) -> Optional[torch.Tensor]:
@@ -538,8 +540,9 @@ def evaluate(predictions: Dict[str, object], *, extrinsics=None, intrinsics=None
     Every value is a device tensor.  Host reads: the pose fit's status (``ovg_eval_pose``), the point fit's status
     (``ovg_sim3_estimate``) and the matcher's non-finite flag (``ovg_match_query``): at most three.  ValueError before any
     device work for wrong shapes or dtypes, bad ``views``, ``source="pointmap"`` without ``world_points``, no ground truth,
-    more than 8192 scored views with cameras and S H W >= 2^31; after a read, for fewer than 3 views or pixels to align, or
-    collinear ones."""
+    more than 8192 scored views with cameras, S H W >= 2^31, and, when both cameras and depth are given (the points group),
+    S H W >= 2^30 or S > 65535 views; after a read, for fewer than 3 views or pixels to align, or collinear ones.  S H W need
+    not be a multiple of 4, and the ground truth may be a view at any storage offset."""
     if source not in ("depth", "pointmap"):
         raise ValueError(f"source must be 'depth' or 'pointmap', got {source!r}")
     images = predictions["images"]
@@ -566,6 +569,9 @@ def evaluate(predictions: Dict[str, object], *, extrinsics=None, intrinsics=None
     if gdep is not None and "depth" not in predictions:
         raise ValueError("the depth group needs the predictions' depth")
     if cams and gdep is not None:
+        if S * H * W >= EVAL_MAX_POINT_PIXELS or S > EVAL_MAX_POINT_VIEWS:
+            raise ValueError(f"the points group needs views * H * W < 2^30 and at most {EVAL_MAX_POINT_VIEWS} views, got "
+                             f"{S} x {H} x {W}")
         if source == "pointmap" and "world_points" not in predictions:
             raise ValueError("source='pointmap' needs the predictions' world_points")
         if source == "depth" and "world_points_from_depth" not in predictions and "pose_enc" not in predictions:
@@ -610,7 +616,13 @@ def evaluate(predictions: Dict[str, object], *, extrinsics=None, intrinsics=None
         pts = pts.float().reshape(S, hw, 3).contiguous()
         c2w, keep = ops.eval_points_keep(gext, gint, gd, m8, pts, view_sel)
         clouds = torch.empty(2, S * hw, 3, device=dev, dtype=torch.float32)
-        ops.unproject_depth(gd.view(S, H, W), gint, c2w, H, W, out=clouds[1])
+        # ovg_unproject_depth wants 16-byte aligned depth and points: a depth view at an odd offset is copied, and when S H W
+        # is not a multiple of 4 (clouds[1] starts S H W 12 bytes in) the points go through a fresh tensor (same values)
+        gdu = gd if gd.data_ptr() % 16 == 0 else gd.clone()
+        if clouds[1].data_ptr() % 16 == 0:
+            ops.unproject_depth(gdu.view(S, H, W), gint, c2w, H, W, out=clouds[1])
+        else:
+            clouds[1].copy_(ops.unproject_depth(gdu.view(S, H, W), gint, c2w, H, W).view(S * hw, 3))
         sim3p, stp = ops.sim3_estimate(pts.view(-1, 3), clouds[1], keep[0])
         n_pix, status = (int(v) for v in ops.host_read(stp[:2]).tolist())
         if status:

@@ -50,13 +50,21 @@ def umeyama(src, dst):
     return A, t, c, float(np.sqrt((r ** 2).sum(1).mean()))
 
 
-def pose_metrics(gt_ext, gt_intr, pred_ext, views=None, sim3=None):
-    """The pose group over ``views`` (default all, ascending) with a ground-truth camera and a finite prediction.  ``sim3``
-    (fp64 [4, 4]) replaces the oracle's own Umeyama fit in the RPE, to check the later stages given the device's fit."""
+def centres_ok(ext):
+    """[S] bool: the camera centre -R^T t of world-to-camera ext [S, 3, 4], rounded to fp32, is finite."""
+    with np.errstate(all="ignore"):
+        return np.isfinite(cam_to_world(ext)[1].astype(np.float32)).all(1)
+
+
+def pose_metrics(gt_ext, gt_intr, pred_ext, views=None, sim3=None, chunk=None):
+    """The pose group over ``views`` (default all, ascending) with a ground-truth camera and a finite prediction whose fp32
+    centres are both finite.  ``sim3`` (fp64 [4, 4]) replaces the oracle's own Umeyama fit in the RPE, to check the later
+    stages given the device's fit.  ``chunk``: pairs per step of ``pair_errors``, to bound memory at many views."""
     gt_ext, pred_ext = np.asarray(gt_ext, np.float32)[:, :3, :4], np.asarray(pred_ext, np.float32)[:, :3, :4]
     S = len(gt_ext)
     views = sorted(range(S) if views is None else views)
     ok = camera_ok(gt_ext, gt_intr) & np.isfinite(pred_ext).all(axis=(1, 2))
+    ok &= centres_ok(gt_ext) & centres_ok(pred_ext)
     idx = np.array([v for v in views if ok[v]], dtype=np.int64)
     n = len(idx)
     Rg, cg = cam_to_world(gt_ext[idx])
@@ -73,7 +81,7 @@ def pose_metrics(gt_ext, gt_intr, pred_ext, views=None, sim3=None):
     Rpa = Ra @ Rp                                   # R_a R (camera-to-world rotations)
     cpa = cp @ A.T + t                              # s R_a c + t_a
     rpe = rpe_errors(Rg, cg, Rpa, cpa)
-    pairs, rre, rte = pair_errors(gt_ext[idx], pred_ext[idx])
+    pairs, rre, rte = pair_errors(gt_ext[idx], pred_ext[idx], chunk)
     out = {"n": n, "views": idx, "sim3": fit, "ate": ate, "rpe": rpe,
            "rpe_trans": float(np.sqrt((rpe[:, 0] ** 2).mean())) if n >= 2 else np.nan,
            "rpe_rot": float(np.sqrt((rpe[:, 1] ** 2).mean())) if n >= 2 else np.nan,
@@ -93,20 +101,26 @@ def rpe_errors(Rq, cq, Rp, cp):
     return np.stack([np.linalg.norm(tE, axis=-1), angle(RE)], -1).reshape(-1, 2)
 
 
-def pair_errors(gt_ext, pred_ext):
-    """(pairs [P, 2] of positions i < j, RRE [P], RTE [P]) in degrees; relative poses R_ij = R_j R_i^T, t_ij = t_j - R_ij t_i."""
+def pair_errors(gt_ext, pred_ext, chunk=None):
+    """(pairs [P, 2] of positions i < j, RRE [P], RTE [P]) in degrees; relative poses R_ij = R_j R_i^T, t_ij = t_j - R_ij t_i.
+    ``chunk``: at most that many pairs per step (each pair's values are computed on their own either way)."""
     n = len(gt_ext)
     ii, jj = np.triu_indices(n, 1)
-    rel = []
-    for e in (np.asarray(gt_ext, np.float64), np.asarray(pred_ext, np.float64)):
-        R, t = e[:, :3, :3], e[:, :3, 3]
-        Rij = R[jj] @ np.swapaxes(R[ii], 1, 2)
-        rel.append((Rij, t[jj] - np.einsum("pij,pj->pi", Rij, t[ii])))
-    (Rg, tg), (Rp, tp) = rel
-    rre = angle(np.swapaxes(Rg, 1, 2) @ Rp)
-    ng, np_ = np.linalg.norm(tg, axis=-1), np.linalg.norm(tp, axis=-1)
-    e = np.degrees(np.arctan2(np.linalg.norm(np.cross(tg, tp), axis=-1), (tg * tp).sum(-1)))
-    rte = np.where((ng > 0) & (np_ > 0), np.minimum(e, 180.0 - e), 90.0)
+    gt, pred = np.asarray(gt_ext, np.float64), np.asarray(pred_ext, np.float64)
+    step = max(len(ii), 1) if chunk is None else int(chunk)
+    rre, rte = np.empty(len(ii)), np.empty(len(ii))
+    for a in range(0, len(ii), step):
+        i, j = ii[a:a + step], jj[a:a + step]
+        rel = []
+        for e in (gt, pred):
+            R, t = e[:, :3, :3], e[:, :3, 3]
+            Rij = R[j] @ np.swapaxes(R[i], 1, 2)
+            rel.append((Rij, t[j] - np.einsum("pij,pj->pi", Rij, t[i])))
+        (Rg, tg), (Rp, tp) = rel
+        rre[a:a + step] = angle(np.swapaxes(Rg, 1, 2) @ Rp)
+        ng, np_ = np.linalg.norm(tg, axis=-1), np.linalg.norm(tp, axis=-1)
+        e = np.degrees(np.arctan2(np.linalg.norm(np.cross(tg, tp), axis=-1), (tg * tp).sum(-1)))
+        rte[a:a + step] = np.where((ng > 0) & (np_ > 0), np.minimum(e, 180.0 - e), 90.0)
     return np.stack([ii, jj], -1), rre, rte
 
 
@@ -134,8 +148,9 @@ def depth_valid(gt, pred, mask=None, views=None):
     return ok
 
 
-def depth_metrics(gt, pred, mask=None, views=None):
-    """The depth group of gt, pred fp32 [S, H, W] after per-scene median scaling, in fp64; per view too."""
+def depth_metrics(gt, pred, mask=None, views=None, chunk=None):
+    """The depth group of gt, pred fp32 [S, H, W] after per-scene median scaling, in fp64; per view too.  ``chunk``: the fp64
+    per-pixel terms of that many views at a time, summed view by view, to bound memory at many pixels."""
     gt, pred = np.asarray(gt, np.float32), np.asarray(pred, np.float32)
     ok = depth_valid(gt, pred, mask, views)
     S = len(gt)
@@ -148,6 +163,8 @@ def depth_metrics(gt, pred, mask=None, views=None):
         return out
     mg, mp = np.percentile(gt[ok], 50), np.percentile(pred[ok], 50)
     s = np.float64(mg) / np.float64(mp)
+    if chunk is not None:
+        return _depth_chunked(gt, pred, ok, s, mg, mp, int(chunk), out)
     g = gt.astype(np.float64)
     sp = s * pred.astype(np.float64)
     with np.errstate(all="ignore"):
@@ -163,6 +180,33 @@ def depth_metrics(gt, pred, mask=None, views=None):
     with np.errstate(all="ignore"):
         out["view_abs_rel"] = np.where(ok, are, 0).reshape(S, -1).sum(1) / np.where(vp > 0, vp, np.nan)
         out["view_delta1"] = d[0].reshape(S, -1).sum(1) / np.where(vp > 0, vp, np.nan)
+    out["view_pixels"] = vp
+    return out
+
+
+def _depth_chunked(gt, pred, ok, s, mg, mp, chunk, out):
+    """depth_metrics' sums per view, ``chunk`` views at a time, then over the views in order."""
+    S = len(gt)
+    tot = np.zeros((S, 7))                                   # sum |e| / g, sum e^2 / g, sum e^2, pixels, delta counts (3)
+    for a in range(0, S, chunk):
+        k = ok[a:a + chunk].reshape(min(chunk, S - a), -1)
+        g = gt[a:a + chunk].reshape(k.shape).astype(np.float64)
+        sp = s * pred[a:a + chunk].reshape(k.shape).astype(np.float64)
+        with np.errstate(all="ignore"):
+            e = sp - g
+            r = np.maximum(sp / g, g / sp)
+            terms = [np.abs(e) / g, e * e / g, e * e]
+        tot[a:a + chunk, :3] = np.stack([np.where(k, t, 0).sum(1) for t in terms], 1)
+        tot[a:a + chunk, 3] = k.sum(1)
+        tot[a:a + chunk, 4:] = np.stack([((r < 1.25 ** q) & k).sum(1) for q in (1, 2, 3)], 1)
+    n = tot[:, 3].sum()
+    vp = tot[:, 3].astype(np.int64)
+    counts = tot[:, 4:].sum(0).astype(np.int64)
+    out.update(scale=s, median_gt=mg, median_pred=mp, abs_rel=tot[:, 0].sum() / n, sq_rel=tot[:, 1].sum() / n,
+               rmse=np.sqrt(tot[:, 2].sum() / n), delta_counts=counts, delta=counts / n)
+    with np.errstate(all="ignore"):
+        out["view_abs_rel"] = tot[:, 0] / np.where(vp > 0, vp, np.nan)
+        out["view_delta1"] = tot[:, 4] / np.where(vp > 0, vp, np.nan)
     out["view_pixels"] = vp
     return out
 
